@@ -5,6 +5,8 @@
     python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's CUDA path
     python bench.py --impl reference [--steps K] [--warmup W]      # the reference's CPU path
     python bench.py --config {3,4,5} ...                           # the other BASELINE.json configs (bench_configs.py)
+    python bench.py ... --dump-outputs DIR                         # also write the last timed step's results
+
 
 A "step" is one complete pass of the hot path: every (candidate, fold) column fitted with
 the batched L-BFGS solver and scored on its held-out rows.  `value` is measured with
@@ -12,7 +14,9 @@ the batched L-BFGS solver and scored on its held-out rows.  `value` is measured 
 (DistGridSearchCV.fit on HOST numpy arrays: H2D staging, fits, scoring, D2H of results; refit
 excluded as SURVEY.md section 8d defines the metric).  Under torchrun (N > 1) columns are dealt
 round-robin to ranks ("weak": the per-rank batch shrinks, total work is fixed -> "strong").
-One JSON line is printed by rank 0.
+One JSON line is printed by rank 0.  With --dump-outputs DIR (single process only), the arrays the
+last timed step returned are also written as DIR/<name>.npy (float32 / float64, at most 64 MB in all);
+the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -45,8 +49,12 @@ def parse():
     p.add_argument("--candidates", type=int, default=512)
     p.add_argument("--folds", type=int, default=5)
     p.add_argument("--cpu-sample", type=int, default=40, help="fits timed for cpu_baseline / compared for parity (0 = skip)")
-    p.add_argument("--kernel", type=int, default=0, help="0 auto, 1 SIMT fp32, 2 tcgen05")
+    p.add_argument("--kernel", type=int, default=0, help="0 auto, 1 SIMT fp32, 2 tensor cores (wgmma)")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write the arrays the last timed step returned as DIR/<name>.npy")
     a = p.parse_args()
+    if a.dump_outputs and int(os.environ.get("WORLD_SIZE", 1)) > 1:
+        p.error("--dump-outputs writes the results a single process computes: run it with --gpus 1")
     if a.config == 2:
         a.n = a.n or 1_000_000
         a.d = a.d or 256
@@ -59,7 +67,59 @@ def peaks():
         j = json.load(open(path))
         return {"bf16_burst": j["bf16_tflops"], "bf16_sustained": j.get("bf16_tflops_sustained", j["bf16_tflops"]),
                 "hbm": j["hbm_gbs"], "src": "measured"}
-    return {"bf16_burst": 1590.0, "bf16_sustained": 1400.0, "hbm": 6650.0, "src": "fallback"}
+    # NVIDIA's H100 SXM data sheet (dense BF16, HBM3): an upper bound, not a measured rate
+    return {"bf16_burst": 989.0, "bf16_sustained": 989.0, "hbm": 3350.0, "src": "H100 SXM data sheet"}
+
+
+DUMP_LIMIT = 64 << 20
+NPY_HEADER = 256          # upper bound of the header np.save writes before an array's data
+
+
+def _numeric_arrays(prefix, obj, out):
+    """The numeric arrays of a step's result (nested dicts / tuples flattened into name_key / name_i);
+    timings are not results and are left out."""
+    if isinstance(obj, dict):
+        for k, v in obj.items():
+            if k == "gpu_seconds":
+                continue
+            _numeric_arrays("%s_%s" % (prefix, k) if prefix else str(k), v, out)
+    elif isinstance(obj, (tuple, list)):
+        for i, v in enumerate(obj):
+            _numeric_arrays("%s_%d" % (prefix, i), v, out)
+    else:
+        v = np.asarray(obj)
+        if v.dtype.kind in "biuf" and v.dtype.names is None:
+            out[prefix] = v.astype(np.float32 if v.dtype == np.float32 else np.float64)
+        elif v.dtype.names is not None:          # structured arrays (tree nodes): one array per field
+            for f in v.dtype.names:
+                _numeric_arrays("%s_%s" % (prefix, f), v[f], out)
+    return out
+
+
+def dump_outputs(path, result):
+    """Write the numeric arrays of `result` as path/<name>.npy, at most DUMP_LIMIT bytes of files in all.
+    Over the limit, the arrays with the same number of leading rows keep one fixed, seeded sample of those
+    rows, written once as path/sample_rows_<rows>.npy."""
+    arrays = _numeric_arrays("", result, {})
+    lengths = sorted({len(v) for v in arrays.values() if v.ndim > 0 and len(v) > 1})
+    full = sum(NPY_HEADER + v.nbytes for v in arrays.values())
+    keep = {}
+    if full > DUMP_LIMIT:
+        # bytes per kept row of each length: its rows in every array of that length + one float64 row id
+        per_row = {n: 8 + sum(v.nbytes // n for v in arrays.values() if v.ndim > 0 and len(v) == n) for n in lengths}
+        fixed = NPY_HEADER * (len(arrays) + len(lengths)) + sum(
+            v.nbytes for v in arrays.values() if not (v.ndim > 0 and len(v) > 1))
+        frac = max(0.0, DUMP_LIMIT - fixed) / sum(n * per_row[n] for n in lengths)
+        rng = np.random.default_rng(0)
+        for n in lengths:
+            keep[n] = np.sort(rng.choice(n, max(1, int(n * frac)), replace=False))
+    os.makedirs(path, exist_ok=True)
+    for n, rows in keep.items():
+        np.save(os.path.join(path, "sample_rows_%d.npy" % n), rows.astype(np.float64))
+    for name, v in arrays.items():
+        if v.ndim > 0 and len(v) in keep:
+            v = v[keep[len(v)]]
+        np.save(os.path.join(path, name + ".npy"), v)
 
 
 class ClockSampler:
@@ -262,7 +322,7 @@ def main():
         import bench_configs
         if a.impl == "reference":
             return bench_configs.run_reference(a)
-        return bench_configs.run(a, ClockSampler, peaks)
+        return bench_configs.run(a, ClockSampler, peaks, dump_outputs)
     if a.impl == "reference":
         return run_reference(a)
 
@@ -332,6 +392,8 @@ def main():
     prof = eng.profile(0)
     c1 = eng.counters()
     clocks = sampler.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, {"fit": res, "correct": correct, "count": count})
     # device time between the two events, max over ranks
     tt = torch.tensor([wall], dtype=torch.float64, device="cuda")
     if world > 1:
@@ -369,7 +431,7 @@ def main():
             "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload_name(a), "inputs": "exceed L2 (X is %.2f GB)" % (X.nbytes / 1e9),
                        "parallelism": "blocks of 128 same-fold columns dealt over %d rank(s) (longest first, by C), X replicated" % world,
-                       "kernel": {0: "auto", 1: "simt-fp32", 2: "tcgen05"}[a.kernel],
+                       "kernel": {0: "auto", 1: "simt-fp32", 2: "tensor-core"}[a.kernel],
                        "mean_test_score_best": float(np.max(gs.cv_results_["mean_test_score"])),
                        "best_C": float(gs.best_params_["C"]),
                        "rounds_per_step": prof["rounds"] / max(1, a.steps)},
@@ -387,14 +449,6 @@ def main():
                          # fp32-grade accuracy costs 3 fp16 MMA passes per algorithmic FLOP
                          "mma_passes": 3, "tensor_issue_frac": 3 * achieved / pk["bf16_sustained"]},
         }
-        # DRAM traffic of the dominant kernel comes from the committed ncu capture (bench.py never runs
-        # under a profiler); only reported for the workload it was captured on
-        tpath = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "roofline_traffic.json")
-        if os.path.exists(tpath) and (a.n, a.d, a.candidates, a.folds, a.kernel) == (1_000_000, 256, 512, 5, 0):
-            with open(tpath) as f:
-                tj = json.load(f)
-            line["roofline"]["traffic"] = tj["dram_bytes_per_launch"]
-            line["roofline"]["traffic_source"] = tj["source"]
         if world == 1 and a.cpu_sample > 0:
             cores = os.cpu_count() or 1
             tasks = cpu_tasks(a.candidates, a.folds, a.cpu_sample)

@@ -9,7 +9,7 @@
 time from CUDA events on the library's stream, max over ranks.  `e2e`: the public estimator's
 `fit` on HOST numpy arrays (staging, fits, results back, sklearn objects built), wall clock, max over
 ranks.  `roofline`: SURVEY.md section 8(d)'s algorithmic bytes / flops of the whole call over its
-device time (per-kernel shares: the ncu launch lists under profiles/).  `cpu_baseline` and
+device time.  `cpu_baseline` and
 `--impl reference`: scikit-learn's own estimator (what every reference task runs) fanned out over the
 host cores with joblib, one bounded wave.
 """
@@ -130,7 +130,7 @@ def run_reference(a):
 # ---------------------------------------------------------------------------------------------
 # device arms
 # ---------------------------------------------------------------------------------------------
-def run(a, ClockSampler, peaks):
+def run(a, ClockSampler, peaks, dump_outputs):
     import torch
     import torch.distributed as dist
     world = int(os.environ.get("WORLD_SIZE", 1))
@@ -218,6 +218,8 @@ def run(a, ClockSampler, peaks):
     sampler.end()
     c1 = eng.counters()
     clocks = sampler.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, res_box)
     tt = torch.tensor([dev_s], dtype=torch.float64, device="cuda")
     if world > 1:
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
@@ -291,7 +293,7 @@ def run(a, ClockSampler, peaks):
         roof = {"bound": "tensor", "achieved": achieved, "peak": pk["bf16_sustained"], "unit": "TFLOP/s",
                 "frac": achieved / pk["bf16_sustained"], "traffic": None,
                 "algorithmic_flops": "4 * n * d per label column per epoch x the epochs every column ran",
-                "kernel": "whole sgd_fit_batch call (screening products on tcgen05 + ordered scan); per-kernel shares in profiles/"}
+                "kernel": "whole sgd_fit_batch call (screening products on the tensor cores + ordered scan)"}
         extra["epochs_min_mean_max"] = [int(np.min(r["n_iter"])), float(np.mean(r["n_iter"])), int(np.max(r["n_iter"]))]
     elif a.config == 4:
         trees = res_box["r"]

@@ -1,4 +1,4 @@
-/* skdist_b200.h -- C-ABI of libskdist_b200.so (hand-written sm_100a CUDA, no torch types).
+/* skdist_b200.h -- C-ABI of libskdist_b200.so (hand-written sm_90a CUDA, no torch types).
  *
  * This is the drop-in boundary for the hot path of Ibotta/sk-dist (reference v0.1.9):
  * the per-task fits that skdist.distribute fans out over Spark executors.  The
@@ -265,7 +265,7 @@ int skd_forest_predict(skd_ctx* ctx, const float* Xnew, int64_t m, int64_t d, in
  * skdist/distribute/predict.py:160-179 (model.predict over row batches). */
 int skd_linear_decision(skd_ctx* ctx, int32_t B, const float* coef, float* out);
 
-/* Which evaluation kernel skd_logreg_fit_batch uses: 0 = auto, 1 = SIMT fp32, 2 = tcgen05
+/* Which evaluation kernel skd_logreg_fit_batch uses: 0 = auto, 1 = SIMT fp32, 2 = tensor-core (wgmma)
  * (fp16x2-split, fp32 accumulate).  Returns the previous value. */
 int skd_set_kernel(skd_ctx* ctx, int32_t which);
 

@@ -22,10 +22,11 @@ Pinning status (see DESIGN.md "Oracle"):
   ``tests/golden/search_logreg_digits10_{raw,scaled}.npz`` hold the scores of the reference's
   unmodified ``_fit_and_score`` plus its own run-to-run envelope; ``logreg_oracle.fit_multinomial_lbfgs``
   reproduces the stored fp32 coefficients bit for bit (``tests/test_oracle.py``).
-* Live pins that need /root/reference (skipped where it is absent): the multi-model search
-  against the reference's ``_raw_sampler`` / ``_fit_one_fold`` / ``_get_results``
-  (``tests/test_search_host.py``) and the feature eliminator against its ``_fit_and_score_one`` /
-  ``_drop_col`` (``tests/test_eliminate_host.py``).
+* Pins of reference functions the tests cannot run: ``tests/golden/make_reference_pins.py`` runs the
+  unmodified reference once (multi-model search ``_raw_sampler`` / ``_fit_one_fold`` / ``_get_results``,
+  the feature eliminator's ``_fit_and_score_one``, ``_negatives_mask``, ``_build_trees``, ``get_oof``, the
+  one-vs-rest SGD fit, the constructor / method surface) and stores the results in
+  ``tests/golden/reference_pins.npz`` and ``tests/golden/reference_surface.json``, which the tests read.
 * The SGD (``sgd_oracle.py``), logistic (``logreg_oracle.py``) and ridge (``ridge_oracle.py``)
   restatements are bit-identical to the installed scikit-learn estimators (``tests/test_oracle.py``,
   ``tests/test_multiclass_host.py``); trees are checked against scikit-learn directly, which the

@@ -1,4 +1,4 @@
-"""Drop-in alias: ``import skdist`` resolves to the B200-native implementation
+"""Drop-in alias: ``import skdist`` resolves to the H100-native implementation
 (package ``skdist_b200``), keeping the reference's import paths
 (``skdist.distribute.search.DistGridSearchCV`` ...)."""
 __version__ = "0.1.9+b200"

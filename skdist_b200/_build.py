@@ -1,4 +1,4 @@
-"""Build libskdist_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libskdist_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 import os
 import shutil
 import subprocess
@@ -10,7 +10,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIBPATH = os.path.join(LIBDIR, "libskdist_b200.so")
 SOURCES = ["api.cu", "logreg_simt.cu", "lbfgs_dev.cu", "logreg_multi.cu", "auc.cu", "logreg_tc.cu", "ridge.cu", "predict.cu", "sgd.cu", "sgd_tc.cu", "forest.cu", "forest_fast.cu", "bootstrap.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
 ]

@@ -1,6 +1,6 @@
 """ctypes binding of libskdist_b200.so (the C-ABI in include/skdist_b200.h).
 
-There is NO CPU fallback: if the library is missing or no B200 is visible the
+There is NO CPU fallback: if the library is missing or no H100 is visible the
 calls raise.  The library is built in-tree by ``skdist_b200._build`` /
 ``__graft_entry__.build()``.
 """

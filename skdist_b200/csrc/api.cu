@@ -35,7 +35,7 @@ struct skd_lbfgs {
 
 static inline int64_t round_up(int64_t a, int64_t b) { return (a + b - 1) / b * b; }
 
-// Which evaluation kernel serves this batch (SIMT fp32 now; tcgen05 once it lands).
+// Which evaluation kernel serves this batch: the tensor-core kernel (logreg_tc.cu) or SIMT fp32.
 static int eval_dispatch(Ctx* c, LogregWork& w, int n_act, int* nz_used) {
   if (w.use_tc) return tc_eval(c, w, n_act, nz_used);
   return simt_eval(c, w, n_act, nz_used);
@@ -52,7 +52,7 @@ static bool want_tc(const Ctx* c) {
 static int alloc_eval_buffers(Ctx* c, Scratch& sx, LogregWork& w, int B, int slot_cap = 0) {
   const int64_t n = c->n, ldx = c->ldx;
   if (c->kernel_choice == 2 && !tc_supported(c))
-    return fail(c, "tcgen05 path requested but the staged shape is unsupported (needs d <= 256)");
+    return fail(c, "tensor-core path requested but the staged shape is unsupported (needs d <= 256)");
   w.use_tc = want_tc(c);
   if (slot_cap < B) slot_cap = B;
   w.slot_cap = slot_cap;
@@ -79,8 +79,15 @@ static int alloc_eval_buffers(Ctx* c, Scratch& sx, LogregWork& w, int B, int slo
     w.ldw = (int)ldx;
     w.gscale = nullptr;
     w.ldg = (int)round_up(B, 64);
-    if ((double)n * w.ldg * 4.0 > 120e9)
-      return fail(c, "skd_logreg_fit_batch: batch too large for one SIMT call (n * B * 4 bytes > 120 GB); split the batch");
+    // the n x B gradient-factor matrix must leave room for X and the solver state: at most 3/4 of the device
+    size_t free_b = 0, total_b = 0;
+    SKD_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+    if ((double)n * w.ldg * 4.0 > 0.75 * (double)total_b) {
+      char b[200];
+      snprintf(b, sizeof(b), "skd_logreg_fit_batch: batch too large for one SIMT call (n * B * 4 bytes > %.0f GB, "
+               "3/4 of the device); split the batch", 0.75 * (double)total_b / 1e9);
+      return fail(c, b);
+    }
     SKD_CUDA(c, sx.alloc(&w.Wact, (size_t)B * ldx + B));
     SKD_CUDA(c, sx.alloc(&w.G, (size_t)n * w.ldg));
     SKD_CUDA(c, sx.alloc(&w.gradp, (size_t)w.cap_sc * ldx));
@@ -132,9 +139,9 @@ int skd_ctx_create(int device, skd_ctx** out) {
   SKD_CUDA(nullptr, cudaSetDevice(device));
   cudaDeviceProp prop;
   SKD_CUDA(nullptr, cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10) {
+  if (prop.major != 9 || prop.minor != 0) {   // sm_90a code runs on compute capability 9.0 only
     char b[256];
-    snprintf(b, sizeof(b), "skd_ctx_create: device %d is sm_%d%d; this library is built for sm_100a only",
+    snprintf(b, sizeof(b), "skd_ctx_create: device %d is sm_%d%d; this library is built for sm_90a only",
              device, prop.major, prop.minor);
     return fail(nullptr, b);
   }
@@ -937,7 +944,7 @@ int skd_linear_score_batch(skd_ctx* ctx, int32_t B, const float* coef, const int
   SKD_CUDA(c, cudaMemsetAsync(dcorrect, 0, B * sizeof(int64_t), c->stream));
   SKD_CUDA(c, cudaMemsetAsync(dcount, 0, B * sizeof(int64_t), c->stream));
   if (c->kernel_choice == 2 && !tc_supported(c))
-    return fail(c, "tcgen05 path requested but the staged shape is unsupported (needs d <= 256)");
+    return fail(c, "tensor-core path requested but the staged shape is unsupported (needs d <= 256)");
   if (want_tc(c)) {
     // tensor-core GEMM1-only pass with a counting epilogue (logreg_tc.cu, TC_SCORE)
     if (tc_prepare(c)) return 1;
@@ -1158,7 +1165,7 @@ int skd_linear_r2_batch(skd_ctx* ctx, int32_t B, const float* coef, const int32_
   SKD_CUDA(c, cudaMemsetAsync(dsse, 0, B * sizeof(double), c->stream));
   SKD_CUDA(c, cudaMemsetAsync(dcount, 0, B * sizeof(int64_t), c->stream));
   if (c->kernel_choice == 2 && !tc_supported(c))
-    return fail(c, "tcgen05 path requested but the staged shape is unsupported (needs d <= 256)");
+    return fail(c, "tensor-core path requested but the staged shape is unsupported (needs d <= 256)");
   if (want_tc(c)) {
     if (tc_prepare(c)) return 1;
     LogregWork w;

@@ -17,7 +17,7 @@
 // sums are added in chunk order, so a candidate's result does not depend on what else is in the
 // batch.  Held-out rows of a candidate get a zero pointwise gradient (fold mask, no copies of X).
 //
-// First CUDA path of this objective: fp32 CUDA cores (the binary objective's tcgen05 kernel does
+// First CUDA path of this objective: fp32 CUDA cores (the binary objective's tensor-core kernel does
 // not cover it yet, DESIGN.md "multinomial").
 #include <string.h>
 

@@ -1,6 +1,6 @@
 // logreg_simt.cu -- fp32 CUDA-core evaluation of the batched logistic objective.
 //
-// General-shape path (any d, any B) and the accuracy reference for the tcgen05 path.
+// General-shape path (any d, any B) and the accuracy reference for the tensor-core path.
 // Replaces, per L-BFGS evaluation and for all active columns at once,
 //   SK/linear_model/_linear_loss.py:291-379  LinearModelLoss.loss_gradient
 //     raw = X @ w32 + b32                         (:219)   -> fwd_kernel K-loop (fp32 FMA)

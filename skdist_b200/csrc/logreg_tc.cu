@@ -1,12 +1,12 @@
-// logreg_tc.cu -- fused batched logistic loss + gradient on the 5th-gen tensor cores (sm_100a).
+// logreg_tc.cu -- fused batched logistic loss + gradient on the Hopper tensor cores (sm_90a wgmma).
 //
 // One launch evaluates f, g of every active (candidate x fold) column, i.e. replaces, for all
 // columns at once, the two fp32 sgemv passes + pointwise loop that each reference task runs per
 // L-BFGS evaluation (SK/linear_model/_linear_loss.py:291-379; ref search.py:230):
 //
-//     Z  = W  X^T     (slots x rows)   GEMM1   tcgen05.mma, accumulators in TMEM
-//     G  = dloss(Z, y) masked by fold  epilogue (CUDA cores): tcgen05.ld -> math -> tcgen05.st
-//     dW = G  X       (slots x d)      GEMM2   tcgen05.mma, A operand = G straight from TMEM
+//     Z  = W  X^T     (slots x rows)   GEMM1   wgmma, A = W from shared memory, accumulators in registers
+//     G  = dloss(Z, y) masked by fold  epilogue on the accumulator registers (CUDA cores)
+//     dW = G  X       (slots x d)      GEMM2   wgmma, A operand = G straight from registers
 //
 // X is read ONCE per tile by TMA into 128B-swizzled shared memory and used by both GEMMs: as
 // the K-major B operand of GEMM1 (K = features) and, through a second descriptor over the same
@@ -16,14 +16,12 @@
 // numbers, v = hi + lo (22+ mantissa bits after exact power-of-two pre-scaling per feature /
 // per column), and each product is three MMAs hi*hi + hi*lo + lo*hi accumulated in fp32.
 //
-// Work decomposition: a group = 128 slots (MMA M, the TMEM lanes); its rows are cut into P parts;
-// one persistent CTA per (group, part) item.  Per CTA: W_hi stationary in shared memory, W_lo
-// stationary in TMEM, gradient accumulators (128 x d fp32) stationary in TMEM, X streamed in
-// tiles of 64 rows through a ring of 5 half-tile (hi or lo) slots.
-//   warp 0      : TMA producer        warp 1 : MMA issuer (+ TMEM allocation)
-//   warps 2..17 : epilogue, four warps per TMEM lane quadrant (lane = slot), 16 rows of the tile each
-// TMEM columns : [0,256) grad accumulator | [256,384) W_lo (packed fp16 pairs) |
-//                [384,448) Z/G buffer 0 | [448,512) Z/G buffer 1
+// Work decomposition: a group = 128 slots, two warpgroups of 64 slots each (wgmma M = 64); its
+// rows are cut into TC_NCH chunks; one persistent CTA per run of (group, chunk) items.  Per CTA:
+// W_hi and W_lo stationary in shared memory, the gradient accumulators (64 x d fp32 per
+// warpgroup) stationary in registers, X streamed in sub-tiles of 32 rows (hi and lo halves) through
+// a TMA ring that thread 0 keeps filled.  The accumulator fragment of a 16-row block of Z is the
+// register A fragment of one k16 step of GEMM2, so G never leaves the registers.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -37,20 +35,14 @@
 namespace skd {
 
 constexpr int TC_BC = 128;       // slots per group
-constexpr int TC_R = 64;         // rows per tile
-constexpr int TC_NS = 5;         // ring slots (half tiles)
-constexpr int TC_NCH = 147;      // fixed row chunks per group (one partial sum per (chunk, slot)); 147 = 3 * 7 * 7
-                                 // divides evenly over 7 / 21 / 49 CTAs per group (20, 7 or 3 groups per GPU)
-constexpr int TC_EPI_WARPS = 16;    // four per TMEM lane quadrant
-constexpr int TC_EPI_THREADS = TC_EPI_WARPS * 32;
-constexpr int TC_THREADS = 64 + TC_EPI_THREADS;
-constexpr uint32_t TM_GRAD = 0, TM_WLO = 256, TM_Z0 = 384;
+constexpr int TC_R = 64;         // rows per tile (the unit of the tile lists and row bit matrices)
+constexpr int TC_SUB = 32;       // rows per ring sub-tile (wgmma N of GEMM1, K of GEMM2)
+constexpr int TC_NCH = 132;      // fixed row chunks per group (one partial sum per (chunk, slot)); 132 = 4 * 3 * 11
+                                 // divides evenly over 132 / 66 / 44 / 33 / 22 CTAs per group (1, 2, 3, 4, 6 groups per GPU)
+constexpr int TC_THREADS = 256;  // two warpgroups
+constexpr uint32_t TC_SMEM_MAX = 232448;   // 227 KB of opt-in shared memory per block
 constexpr float XSCALE_TARGET_EXP = 13.f;   // column max scaled into [2^13, 2^14)
 constexpr float GSCALE = 16384.f;           // 2^14
-
-__device__ __forceinline__ void epi_bar_sync() {   // named barrier 1: the epilogue warps only
-  asm volatile("bar.sync 1, %0;" ::"n"(TC_EPI_THREADS) : "memory");
-}
 
 // ---------------------------------------------------------------------------------------------
 // data preparation kernels
@@ -194,7 +186,6 @@ tc_export_kernel(const double* __restrict__ vec, size_t vec_stride, const SlotMe
 // the fused kernel
 // ---------------------------------------------------------------------------------------------
 struct TcParams {
-  const __half* Wl;          // [slots_pad x dpad]
   const TcSlotParam* sp;     // [slots]
   const uint32_t* rowmeta;   // [npad]
   const float* yreal;        // [npad] regression targets (TC_R2)
@@ -217,64 +208,69 @@ struct TcParams {
   const uint32_t* mbits;     // TC_FIT: per-column training-row bits (nullptr: every row of the training folds)
   long long rb_words;
   int g_passes;              // MMA passes of the gradient product: 3 = G_hi X_hi + G_lo X_hi + G_hi X_lo, 2 = without G_lo X_hi
-  int debug;                 // SKDIST_B200_TC_DEBUG (timing experiments only): 2 = no GEMM2, 3 = no MMAs, 4 = no epilogue work
-};
-
-struct __align__(8) TcBarriers {
-  uint64_t full[TC_NS];
-  uint64_t empty[TC_NS];
-  uint64_t z_full[2];
-  uint64_t g_full[2];
-  uint64_t w_full;
-  uint64_t w_free;      // committed by the MMA warp when it leaves a group: W_hi may be overwritten
-  uint64_t wl_full;
-  uint64_t acc_done;
-  uint64_t acc_free;
-  uint32_t tmem_base;
-  uint32_t pad;
 };
 
 // TC_FIT_UNI: fit where every slot of a group shares (held-out fold, positive class): the row's
 // sign/mask comes from a precomputed per-fold array instead of being decoded per element
 enum { TC_FIT = 0, TC_SCORE = 1, TC_R2 = 2, TC_FIT_UNI = 3 };
 
+// shared memory of one CTA: W_hi, W_lo [NCHUNK][128 slots x 64 fp16] + the ring of sub-tiles
+template <int NCHUNK>
+struct TcSmem {
+  static constexpr uint32_t W_CHUNK = TC_BC * 128;
+  static constexpr uint32_t X_CHUNK = TC_SUB * 128;
+  static constexpr uint32_t W_BYTES = 2 * NCHUNK * W_CHUNK;
+  static constexpr uint32_t STAGE = 2 * NCHUNK * X_CHUNK;          // [X_hi chunks | X_lo chunks]
+  static constexpr int NS_FIT = (int)((TC_SMEM_MAX - 1024 - 256 - W_BYTES) / STAGE);
+  static constexpr int NS = NS_FIT < 8 ? NS_FIT : 8;
+  static constexpr size_t BYTES = 1024 + (size_t)W_BYTES + (size_t)NS * STAGE + 256;
+  static_assert(NS >= 2, "ring too small");
+};
+
+struct __align__(8) TcBarriers {
+  uint64_t full[8];
+  uint64_t empty[8];
+  uint64_t w_full;
+};
+
+template <int NCHUNK>
+__device__ __forceinline__ void wgmma_grad(float (&d)[NCHUNK * 32], const uint32_t (&a)[4], uint64_t b) {
+  if constexpr (NCHUNK == 1) wgmma_m64n64_rs_tb(d, a, b);
+  else if constexpr (NCHUNK == 2) wgmma_m64n128_rs_tb(d, a, b);
+  else if constexpr (NCHUNK == 3) wgmma_m64n192_rs_tb(d, a, b);
+  else wgmma_m64n256_rs_tb(d, a, b);
+}
+
+__device__ __forceinline__ void two_sum_add(float& hi, float& lo, float v) {
+  const float s = hi + v, bb = s - hi;
+  lo += (hi - (s - bb)) + (v - bb);
+  hi = s;
+}
+
 template <int NCHUNK, int MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant__ CUtensorMap map_xl,
-               const __grid_constant__ CUtensorMap map_wh, const TcParams prm) {
+               const __grid_constant__ CUtensorMap map_wh, const __grid_constant__ CUtensorMap map_wl,
+               const TcParams prm) {
   constexpr bool IS_FIT = MODE == TC_FIT || MODE == TC_FIT_UNI;
+  using SM = TcSmem<NCHUNK>;
+  constexpr int NS = SM::NS;
   extern __shared__ uint8_t smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // carve shared memory (1024-byte aligned for the 128B swizzle atoms)
+  const int wg = threadIdx.x >> 7;                 // warpgroup: slots [64 wg, 64 wg + 64) of the group
+  const bool wg_leader = (threadIdx.x & 127) == 0;
   uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  constexpr uint32_t WH_CHUNK = TC_BC * 128;     // [128 slots x 64 fp16]
-  constexpr uint32_t X_CHUNK = TC_R * 128;       // [64 rows x 64 fp16]
-  constexpr uint32_t SLOT_BYTES = NCHUNK * X_CHUNK;
   uint8_t* s_wh = base;
-  uint8_t* s_ring = s_wh + NCHUNK * WH_CHUNK;
-  TcBarriers* bars = reinterpret_cast<TcBarriers*>(s_ring + TC_NS * SLOT_BYTES);
+  uint8_t* s_wl = base + NCHUNK * SM::W_CHUNK;
+  uint8_t* s_ring = base + SM::W_BYTES;
+  TcBarriers* bars = reinterpret_cast<TcBarriers*>(s_ring + NS * SM::STAGE);
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < TC_NS; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&bars->z_full[i], 1); mbar_init(&bars->g_full[i], TC_EPI_THREADS); }
+    for (int i = 0; i < NS; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], 2); }
     mbar_init(&bars->w_full, 1);
-    mbar_init(&bars->w_free, 1);
-    mbar_init(&bars->wl_full, TC_EPI_THREADS);
-    mbar_init(&bars->acc_done, 1);
-    mbar_init(&bars->acc_free, TC_EPI_THREADS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(&bars->tmem_base)),
-                 "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
 
   // Work split.  A group's tile list (all tiles, or the tiles with training rows of the group's
   // fold) is cut into TC_NCH fixed chunks; a unit = (group, chunk); the groups * TC_NCH units are
@@ -302,414 +298,283 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
     }
     it.t0 = (int)((long long)cnt * it.z / TC_NCH);
     it.t1 = (int)((long long)cnt * (it.z + 1) / TC_NCH);
-    return it.t1 > it.t0;       // empty chunks (fewer tiles than chunks) are skipped by every role alike
+    return it.t1 > it.t0;       // empty chunks (fewer tiles than chunks) are skipped
   };
 
-  if (warp == 0) {
-    // ================================ TMA producer ==========================================
-    if (lane == 0) {
-      uint32_t h = 0;  // running half-tile counter (ring position), persists across items
-      int it_local = 0, g_prev = -1, w_loads = 0;
-      for (long long u = u_begin; u < u_end; ++u) {
-        TcItem it;
-        if (!get_item(u, it)) continue;
-        const int g = it.g, t0 = it.t0, t1 = it.t1;
-        const int32_t* tlist = it.tl;
-        if (g != g_prev) {
-          // W_hi of a new group: the MMA warp signals w_free once per group it leaves, after all its
-          // MMAs on that group (one phase per reload, so the parity wait cannot alias; acc_done
-          // completes one phase per ITEM and this thread may be several one-tile items ahead)
-          if (w_loads > 0) mbar_wait(&bars->w_free, (w_loads - 1) & 1, 100);
-          ++w_loads;
-          mbar_expect_tx(&bars->w_full, NCHUNK * WH_CHUNK);
+  // accumulator fragments (wgmma m64nN): register i of a thread holds row 16 (warp & 3) + lane / 4
+  // + 8 ((i >> 1) & 1) of its warpgroup's 64 slots and column 8 (i >> 2) + 2 (lane & 3) + (i & 1)
+  const int slot_in_wg = (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  constexpr float INV_G = 1.f / GSCALE;
+  const uint64_t desc_w = make_desc(smem_u32(s_wh), 16, 1024) + (uint64_t)((wg * 64 * 128) >> 4);
+  const uint64_t desc_k = make_desc(smem_u32(s_ring), 16, 1024);              // X as K-major (GEMM1)
+  const uint64_t desc_mn = make_desc(smem_u32(s_ring), SM::X_CHUNK, 1024);    // X as MN-major (GEMM2)
+  constexpr uint32_t WL_OFF = (NCHUNK * SM::W_CHUNK) >> 4;
+  constexpr uint32_t XL_OFF = (NCHUNK * SM::X_CHUNK) >> 4;
+
+  uint32_t h = 0;          // running sub-tile counter (ring position), identical in every thread
+  int w_loads = 0, g_prev = -1;
+  for (long long u = u_begin; u < u_end; ++u) {
+    TcItem it;
+    if (!get_item(u, it)) continue;
+    const int g = it.g, z_part = it.z;
+    const int nsub = 2 * (it.t1 - it.t0);
+    const int32_t* tlist = it.tl;
+    auto sub_row0 = [&](int j) -> int {
+      const int t = tlist ? tlist[it.t0 + (j >> 1)] : it.t0 + (j >> 1);
+      return t * TC_R + (j & 1) * TC_SUB;
+    };
+    // sub-tile k (global count) goes to slot k % NS once both warpgroups are done with sub-tile k - NS
+    auto issue = [&](uint32_t k, int j) {
+      const uint32_t sl = k % NS;
+      if (k >= (uint32_t)NS) mbar_wait(&bars->empty[sl], ((k / NS) - 1) & 1, 100);
+      mbar_expect_tx(&bars->full[sl], SM::STAGE);
+      const int r0 = sub_row0(j);
+      uint8_t* dst = s_ring + sl * SM::STAGE;
 #pragma unroll
-          for (int c = 0; c < NCHUNK; ++c)
-            tma_load_2d(s_wh + c * WH_CHUNK, &map_wh, c * 64, g * TC_BC, &bars->w_full);
-          g_prev = g;
-        }
-        ++it_local;
-        for (int t = t0; t < t1; ++t) {
-          const int tile = tlist ? tlist[t] : t;
+      for (int c = 0; c < NCHUNK; ++c) {
+        tma_load_2d(dst + c * SM::X_CHUNK, &map_xh, c * 64, r0, &bars->full[sl]);
+        tma_load_2d(dst + (NCHUNK + c) * SM::X_CHUNK, &map_xl, c * 64, r0, &bars->full[sl]);
+      }
+    };
+    const bool new_group = g != g_prev;
+    if (new_group) {
+      // weights of a new group: every wgmma of the previous group has completed (each sub-tile ends
+      // in wgmma_wait_all), the barrier makes sure both warpgroups are past them
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        mbar_expect_tx(&bars->w_full, SM::W_BYTES);
 #pragma unroll
-          for (int half = 0; half < 2; ++half, ++h) {
-            const uint32_t sl = h % TC_NS, ph = (h / TC_NS) & 1;
-            mbar_wait(&bars->empty[sl], ph ^ 1, 101);
-            mbar_expect_tx(&bars->full[sl], SLOT_BYTES);
-            const CUtensorMap* mp = half == 0 ? &map_xh : &map_xl;
-#pragma unroll
-            for (int c = 0; c < NCHUNK; ++c)
-              tma_load_2d(s_ring + sl * SLOT_BYTES + c * X_CHUNK, mp, c * 64, tile * TC_R, &bars->full[sl]);
-          }
+        for (int c = 0; c < NCHUNK; ++c) {
+          tma_load_2d(s_wh + c * SM::W_CHUNK, &map_wh, c * 64, g * TC_BC, &bars->w_full);
+          tma_load_2d(s_wl + c * SM::W_CHUNK, &map_wl, c * 64, g * TC_BC, &bars->w_full);
         }
       }
+      g_prev = g;
     }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ============================================
-    // The whole warp runs the control flow (waits, counters) with warp-uniform values; the MMAs of
-    // a tile are issued inside one `elect.sync` branch, which lets ptxas keep the descriptor
-    // arithmetic in the uniform datapath (one UIADD3 per MMA instead of an elect/broadcast loop).
-    {
-      constexpr uint32_t idesc1 = make_idesc(TC_BC, TC_R, 0);            // GEMM1: N = 64 rows
-      constexpr uint32_t idesc2 = make_idesc(TC_BC, NCHUNK * 64, 1);     // GEMM2: N = dpad, B MN-major
-      constexpr int KS1 = NCHUNK * 4;                                    // K = dpad, 16 per MMA
-      // descriptors: only the start-address field (low word, >>4 units) changes between MMAs
-      const uint64_t a_base = make_desc(smem_u32(s_wh), 16, 1024);
-      const uint64_t bk_base = make_desc(smem_u32(s_ring), 16, 1024);          // K-major view
-      const uint64_t bmn_base = make_desc(smem_u32(s_ring), X_CHUNK, 1024);    // MN-major view
-      uint32_t h = 0;       // half-tile counter, mirrors the producer
-      uint32_t tcount = 0;  // tile counter (Z buffer = tcount & 1)
-      int it_local = 0, w_loads = 0, g_prev = -1;
-      for (long long u = u_begin; u < u_end; ++u, ++it_local) {
-        TcItem it;
-        if (!get_item(u, it)) { --it_local; continue; }
-        const int nt = it.t1 - it.t0;
-        if (it.g != g_prev) {       // weights of a new group (W_hi by TMA, W_lo staged by the epilogue warps)
-          if (g_prev >= 0) {        // every MMA issued so far belongs to earlier groups: their completion frees W_hi
-            if (elect_one()) tc_commit(&bars->w_free);
-            __syncwarp();
-          }
-          mbar_wait(&bars->w_full, w_loads & 1, 200);
-          mbar_wait(&bars->wl_full, w_loads & 1, 201);
-          ++w_loads;
-          g_prev = it.g;
-        }
-        if (it_local > 0) mbar_wait(&bars->acc_free, (it_local - 1) & 1, 202);
-        tc_fence_after();
+    if (threadIdx.x == 0)
+      for (int j = 0; j < nsub && j < NS; ++j) issue(h + j, j);
+    __syncwarp();
+    if (new_group) mbar_wait(&bars->w_full, (w_loads++) & 1, 200);
 
-        auto issue_g1 = [&](uint32_t hh, uint32_t tc) {
-          const uint32_t zcol = tmem + TM_Z0 + (tc & 1) * 64;
-          {  // X_hi half tile: W_hi * X_hi + W_lo * X_hi
-            const uint32_t sl = hh % TC_NS, ph = (hh / TC_NS) & 1;
-            mbar_wait(&bars->full[sl], ph, 210);
-            tc_fence_after();
-            const uint64_t bb = bk_base + (uint64_t)((sl * SLOT_BYTES) >> 4);
-            if (elect_one()) {
-              if (prm.debug != 3) {
+    // the two slots of this thread
+    TcSlotParam sp[2];
+    bool valid[2];
+    int slot[2];
 #pragma unroll
-              for (int ks = 0; ks < KS1; ++ks) {
-                const uint32_t aoff = ((ks >> 2) * WH_CHUNK + (ks & 3) * 32) >> 4;
-                const uint32_t boff = ((ks >> 2) * X_CHUNK + (ks & 3) * 32) >> 4;
-                mma_ss(zcol, a_base + aoff, bb + boff, idesc1, ks > 0 ? 1u : 0u);
-                mma_ts(zcol, tmem + TM_WLO + ks * 8, bb + boff, idesc1, 1u);
-              }
-              }
-            }
-            __syncwarp();
-          }
-          {  // X_lo half tile: W_hi * X_lo
-            const uint32_t sl = (hh + 1) % TC_NS, ph = ((hh + 1) / TC_NS) & 1;
-            mbar_wait(&bars->full[sl], ph, 211);
-            tc_fence_after();
-            const uint64_t bb = bk_base + (uint64_t)((sl * SLOT_BYTES) >> 4);
-            if (elect_one()) {
-              if (prm.debug != 3) {
+    for (int s = 0; s < 2; ++s) {
+      slot[s] = g * TC_BC + wg * 64 + slot_in_wg + 8 * s;
+      valid[s] = slot[s] < n_live;
+      sp[s].inv_t = 1.f; sp[s].bias = 0.f; sp[s].fold = -1; sp[s].pos = -1; sp[s].neg1 = 0; sp[s].col = -1;
+      if (valid[s]) sp[s] = prm.sp[slot[s]];
+    }
+    // fit: work on z / 2^14 so that (row sign * 2^14) * z' = +-z and (row sign * 2^14) * sigma is
+    // the scaled gradient entry; all power-of-two factors, results identical to the unscaled form
+    float zi[2], zb0[2];
 #pragma unroll
-              for (int ks = 0; ks < KS1; ++ks) {
-                const uint32_t aoff = ((ks >> 2) * WH_CHUNK + (ks & 3) * 32) >> 4;
-                const uint32_t boff = ((ks >> 2) * X_CHUNK + (ks & 3) * 32) >> 4;
-                mma_ss(zcol, a_base + aoff, bb + boff, idesc1, 1u);
-              }
-              }
-              tc_commit(&bars->z_full[tc & 1]);
-              if (!IS_FIT) {  // no GEMM2: the ring slots are free once GEMM1 has read them
-                tc_commit(&bars->empty[hh % TC_NS]);
-                tc_commit(&bars->empty[(hh + 1) % TC_NS]);
-              }
-            }
-            __syncwarp();
-          }
-        };
-        auto issue_g2 = [&](uint32_t hh, uint32_t tc, bool first_tile) {
-          const uint32_t gcol = tmem + TM_Z0 + (tc & 1) * 64;
-          mbar_wait(&bars->g_full[tc & 1], (tc >> 1) & 1, 220);
-          tc_fence_after();
-          const uint32_t sl_h = hh % TC_NS, sl_l = (hh + 1) % TC_NS;
-          // B operand MN-major: N (features) contiguous within a chunk, chunks LBO apart;
-          // K (rows) in groups of 8 rows SBO = 1024 B apart; one MMA covers 16 rows = 2048 B
-          const uint64_t bh = bmn_base + (uint64_t)((sl_h * SLOT_BYTES) >> 4);
-          const uint64_t bl = bmn_base + (uint64_t)((sl_l * SLOT_BYTES) >> 4);
-          if (elect_one()) {
-            if (prm.debug < 2) {
+    for (int s = 0; s < 2; ++s) {
+      zi[s] = IS_FIT ? sp[s].inv_t * INV_G : sp[s].inv_t;
+      zb0[s] = IS_FIT ? sp[s].bias * INV_G : sp[s].bias;
+    }
+    const float* rsg = nullptr;
+    if (MODE == TC_FIT_UNI) {
+      const int f = prm.sp[g * TC_BC].fold;
+      const int li = (f >= 0 && f < prm.n_lists - 1) ? f : prm.n_lists - 1;
+      rsg = prm.rowsg + (size_t)li * prm.rowsg_ld;
+    }
+    float grad[IS_FIT ? NCHUNK * 32 : 1];
 #pragma unroll
-            for (int ks = 0; ks < TC_R / 16; ++ks) {
-              mma_ts(tmem + TM_GRAD, gcol + ks * 16, bh + ks * 128, idesc2, (first_tile && ks == 0) ? 0u : 1u);
-              if (prm.g_passes >= 3) mma_ts(tmem + TM_GRAD, gcol + ks * 16 + 8, bh + ks * 128, idesc2, 1u);
-            }
-            }
-            tc_commit(&bars->empty[sl_h]);
-            if (prm.debug < 2) {
-#pragma unroll
-            for (int ks = 0; ks < TC_R / 16; ++ks)
-              mma_ts(tmem + TM_GRAD, gcol + ks * 16, bl + ks * 128, idesc2, 1u);
-            }
-            tc_commit(&bars->empty[sl_l]);
-          }
-          __syncwarp();
-        };
+    for (int i = 0; i < (IS_FIT ? NCHUNK * 32 : 1); ++i) grad[i] = 0.f;
+    // per-item sums as compensated fp32 pairs (TwoSum)
+    float ls_hi[2] = {0.f, 0.f}, ls_lo[2] = {0.f, 0.f}, gs_hi[2] = {0.f, 0.f}, gs_lo[2] = {0.f, 0.f};
+    unsigned long long n_ok[2] = {0, 0}, n_all[2] = {0, 0};
 
-        if (IS_FIT) {
-          if (nt > 0) issue_g1(h, tcount);
-          for (int i = 0; i < nt; ++i) {
-            if (i + 1 < nt) issue_g1(h + 2 * (i + 1), tcount + i + 1);
-            issue_g2(h + 2 * i, tcount + i, i == 0);
-          }
+    for (int j = 0; j < nsub; ++j) {
+      const uint32_t hh = h + j, sl = hh % NS, ph = (hh / NS) & 1;
+      const int r0 = sub_row0(j);
+      // per-row data of this thread's 8 rows (columns of the Z fragment), loaded before the wait
+      uint32_t rm[8];
+      float yv[8];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int r = r0 + 8 * q + cq;
+        if (MODE == TC_FIT_UNI) {
+          const float2 v = __ldg(reinterpret_cast<const float2*>(rsg + r));
+          rm[2 * q] = __float_as_uint(v.x); rm[2 * q + 1] = __float_as_uint(v.y);
         } else {
-          // score: GEMM1 only; Z buffer b may be overwritten once the epilogue has consumed it
-          for (int i = 0; i < nt; ++i) {
-            const uint32_t tc = tcount + i;
-            if (tc >= 2) { mbar_wait(&bars->g_full[tc & 1], ((tc >> 1) - 1) & 1, 230); tc_fence_after(); }
-            issue_g1(h + 2 * i, tc);
+          const uint2 v = __ldg(reinterpret_cast<const uint2*>(prm.rowmeta + r));
+          rm[2 * q] = v.x; rm[2 * q + 1] = v.y;
+        }
+        if (MODE == TC_R2) {
+          const float2 v = __ldg(reinterpret_cast<const float2*>(prm.yreal + r));
+          yv[2 * q] = v.x; yv[2 * q + 1] = v.y;
+        }
+      }
+      uint32_t ybw[2] = {0u, 0u}, mbw[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
+      if (MODE == TC_FIT && (prm.ybits || prm.mbits)) {
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          if (sp[s].col < 0) continue;
+          const size_t wi = (size_t)sp[s].col * prm.rb_words + (size_t)(r0 / 32);   // one word = the 32 rows of this sub-tile
+          if (prm.ybits) ybw[s] = __ldg(prm.ybits + wi);
+          if (prm.mbits) mbw[s] = __ldg(prm.mbits + wi);
+        }
+      }
+      mbar_wait(&bars->full[sl], ph, 210);
+
+      // GEMM1: Z = W_hi X_hi + W_lo X_hi + W_hi X_lo   [64 slots x 32 rows per warpgroup]
+      float zf[16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) zf[i] = 0.f;
+      const uint64_t bx = desc_k + (uint64_t)((sl * SM::STAGE) >> 4);
+      reg_fence(zf);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < NCHUNK * 4; ++ks) {
+        const uint32_t aoff = ((ks >> 2) * SM::W_CHUNK + (ks & 3) * 32) >> 4;
+        const uint32_t boff = ((ks >> 2) * SM::X_CHUNK + (ks & 3) * 32) >> 4;
+        wgmma_m64n32_ss(zf, desc_w + aoff, bx + boff, ks > 0 ? 1u : 0u);
+        wgmma_m64n32_ss(zf, desc_w + WL_OFF + aoff, bx + boff, 1u);
+        wgmma_m64n32_ss(zf, desc_w + aoff, bx + XL_OFF + boff, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait_all();
+      reg_fence(zf);
+
+      if constexpr (IS_FIT) {
+        float lt[2] = {0.f, 0.f}, gt[2] = {0.f, 0.f};
+        float gv[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int s = (i >> 1) & 1;
+          const int rr = 2 * (i >> 2) + (i & 1);        // index into rm: row r0 + 8 (i >> 2) + cq + (i & 1)
+          float sg;                       // -y * 2^14 for a training row, 0 otherwise
+          if (MODE == TC_FIT_UNI) {
+            sg = __uint_as_float(rm[rr]);
+          } else {
+            const uint32_t m = rm[rr];
+            const int fr = (int)(m >> 24);
+            const int cls = (int)(m & 0x00FFFFFFu);
+            bool yb = cls == sp[s].pos;
+            bool train = (fr != 0xFF) && (fr != sp[s].fold) && (sp[s].neg1 == 0 || yb || cls == sp[s].neg1 - 1);
+            if (MODE == TC_FIT) {             // staged row bit matrices (multilabel targets, sampled negatives)
+              const int bit = 8 * (i >> 2) + cq + (i & 1);
+              if (prm.ybits) yb = (ybw[s] >> bit) & 1u;
+              if (prm.mbits) train = train && ((mbw[s] >> bit) & 1u);
+            }
+            sg = train ? (yb ? -GSCALE : GSCALE) : 0.f;
+          }
+          const float zp = fmaf(zf[i], zi[s], zb0[s]);
+          const float uu = sg * zp;       // = -y * z
+          const float e = ex2_approx(-fabsf(uu) * 1.4426950408889634f);
+          const float s1 = 1.f + e;
+          const float loss = fmaf(lg2_approx(s1), 0.6931471805599453f, fmaxf(uu, 0.f));
+          const float r = rcp_approx(s1);
+          const float sig = (uu >= 0.f) ? r : e * r;
+          gv[i] = sg * sig;               // 2^14 * dloss/dz
+          lt[s] = fmaf(fabsf(sg), loss, lt[s]);   // 2^14 * loss
+          gt[s] += gv[i];
+        }
+#pragma unroll
+        for (int s = 0; s < 2; ++s) { two_sum_add(ls_hi[s], ls_lo[s], lt[s]); two_sum_add(gs_hi[s], gs_lo[s], gt[s]); }
+        // G as the A operand of GEMM2 (k = the sub-tile's rows): the accumulator fragment of a
+        // 16-column block is the A fragment of one k16 step; split into fp16 hi + lo
+        uint32_t ahi[2][4], alo[2][4];
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) {
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int i = ks * 8 + (q >> 1) * 4 + (q & 1) * 2;
+            const uint32_t hi = pack_f16x2(gv[i], gv[i + 1]);
+            const float2 hf = unpack_f16x2(hi);
+            ahi[ks][q] = hi;
+            alo[ks][q] = pack_f16x2(gv[i] - hf.x, gv[i + 1] - hf.y);
           }
         }
-        h += 2 * nt;
-        tcount += nt;
-        if (elect_one()) tc_commit(&bars->acc_done);
-        __syncwarp();
+        // GEMM2: dW += G_hi X_hi + G_lo X_hi + G_hi X_lo   [64 slots x dpad per warpgroup]
+        const uint64_t bm = desc_mn + (uint64_t)((sl * SM::STAGE) >> 4);
+        reg_fence(grad);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) {
+          const uint64_t bh = bm + (uint64_t)((ks * 16 * 128) >> 4);
+          wgmma_grad<NCHUNK>(grad, ahi[ks], bh);
+          if (prm.g_passes >= 3) wgmma_grad<NCHUNK>(grad, alo[ks], bh);
+          wgmma_grad<NCHUNK>(grad, ahi[ks], bh + XL_OFF);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        reg_fence(grad);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int s = (i >> 1) & 1;
+          const int rr = 2 * (i >> 2) + (i & 1);
+          const uint32_t m = rm[rr];
+          const float zv = fmaf(zf[i], zi[s], zb0[s]);
+          const int fr = (int)(m >> 24);
+          // fold code: f >= 0 rows of fold f; -2 all rows; -3-f rows NOT in fold f
+          const bool in = (fr != 0xFF) && (sp[s].fold == -2 || (sp[s].fold >= 0 && fr == sp[s].fold) ||
+                                           (sp[s].fold <= -3 && fr != (-3 - sp[s].fold)));
+          if (MODE == TC_R2) {
+            const float r = yv[rr] - zv;
+            if (in) two_sum_add(ls_hi[s], ls_lo[s], r * r);
+          } else {
+            const bool yb = (int)(m & 0x00FFFFFFu) == sp[s].pos;
+            n_ok[s] += (in && ((zv > 0.f) == yb)) ? 1 : 0;
+          }
+          n_all[s] += in ? 1 : 0;
+        }
       }
+      if (wg_leader) mbar_arrive(&bars->empty[sl]);
+      if (threadIdx.x == 0 && j + NS < nsub) issue(hh + NS, j + NS);
       __syncwarp();
     }
-  } else {
-    // ================================ epilogue warps ========================================
-    // 16 warps: warps with the same (warp & 3) share TMEM lane quadrant q and take one 16-row
-    // chunk of the tile each (qt = 0..3).  Four warps per scheduler hide the MUFU / TMEM latency;
-    // the per-element instruction count, not the tensor pipe, was the limiter with 8 warps.
-    const int q = warp & 3;                       // TMEM lane quadrant this warp may access
-    const int qt = (warp - 2) >> 2;               // 16-row chunk of every tile
-    const int lane_in_group = q * 32 + lane;      // slot within the group == TMEM lane
-    const uint32_t tl = tmem + ((uint32_t)(q * 32) << 16);
-    constexpr float INV_G = 1.f / GSCALE;
-    uint32_t tcount = 0;
-    int it_local = 0, g_prev = -1;
-    for (long long u = u_begin; u < u_end; ++u, ++it_local) {
-      TcItem it;
-      if (!get_item(u, it)) { --it_local; continue; }
-      const int g = it.g, t0 = it.t0, t1 = it.t1;
-      const int32_t* tlist = it.tl;
-      const int nt = t1 - t0;
-      const int z_part = it.z;
-      const bool new_group = g != g_prev;
-      g_prev = g;
-      const int slot = g * TC_BC + lane_in_group;
-      const bool valid = slot < n_live;
-      TcSlotParam sp;
-      sp.inv_t = 1.f; sp.bias = 0.f; sp.fold = -1; sp.pos = -1; sp.neg1 = 0; sp.col = -1;
-      if (valid) sp = prm.sp[slot];
-      // fit: work on z / 2^14 so that (row sign * 2^14) * z' = +-z and (row sign * 2^14) * sigma is
-      // the scaled gradient entry; all power-of-two factors, results identical to the unscaled form
-      const float zi = IS_FIT ? sp.inv_t * INV_G : sp.inv_t;
-      const float zb0 = IS_FIT ? sp.bias * INV_G : sp.bias;
-      const float* rsg = nullptr;
-      if (MODE == TC_FIT_UNI) {
-        const int f = prm.sp[g * TC_BC].fold;
-        const int li = (f >= 0 && f < prm.n_lists - 1) ? f : prm.n_lists - 1;
-        rsg = prm.rowsg + (size_t)li * prm.rowsg_ld;
-      }
-      if (new_group) {  // W_lo row of this slot -> TMEM (packed fp16 pairs), 16 columns (32 values) at a time.
-         // The previous item's MMAs are done with W_lo: its acc_done was waited for below.
-        const uint32_t* src = reinterpret_cast<const uint32_t*>(prm.Wl + (size_t)slot * (NCHUNK * 64));
-#pragma unroll 1
-        for (int c16 = qt; c16 < NCHUNK * 2; c16 += 4) {
-          uint32_t r[16];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint4 v = valid ? __ldg(reinterpret_cast<const uint4*>(src + c16 * 16) + j) : make_uint4(0, 0, 0, 0);
-            r[4 * j] = v.x; r[4 * j + 1] = v.y; r[4 * j + 2] = v.z; r[4 * j + 3] = v.w;
-          }
-          tmem_st16(tl + TM_WLO + c16 * 16, r);
-        }
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(&bars->wl_full);
-      }
-      // per-item sums as compensated fp32 pairs (TwoSum): the fp64 pipe is slow enough that two
-      // DADDs per tile showed up as 16 % of the epilogue's stall samples
-      float ls_hi = 0.f, ls_lo = 0.f, gs_hi = 0.f, gs_lo = 0.f;
-      unsigned long long n_ok = 0, n_all = 0;
-      for (int i = 0; i < nt; ++i, ++tcount) {
-        const int t = tlist ? tlist[t0 + i] : t0 + i;
-        const uint32_t zb = tl + TM_Z0 + (tcount & 1) * 64;
-        // per-row data of this warp's 16 rows: issue the loads before waiting for the MMA so their
-        // latency is hidden behind the wait
-        uint32_t rm[16];
-        {
-          const uint4* rm4 = MODE == TC_FIT_UNI
-                                 ? reinterpret_cast<const uint4*>(rsg + (size_t)t * TC_R + qt * 16)
-                                 : reinterpret_cast<const uint4*>(prm.rowmeta + (size_t)t * TC_R + qt * 16);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint4 v = __ldg(rm4 + j);
-            rm[4 * j] = v.x; rm[4 * j + 1] = v.y; rm[4 * j + 2] = v.z; rm[4 * j + 3] = v.w;
-          }
-        }
-        float yv[16];
-        if (MODE == TC_R2) {
-          const float4* y4 = reinterpret_cast<const float4*>(prm.yreal + (size_t)t * TC_R + qt * 16);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float4 v = __ldg(y4 + j);
-            yv[4 * j] = v.x; yv[4 * j + 1] = v.y; yv[4 * j + 2] = v.z; yv[4 * j + 3] = v.w;
-          }
-        }
-        uint32_t yb16 = 0, mb16 = 0xFFFFu;
-        if (MODE == TC_FIT && (prm.ybits || prm.mbits) && sp.col >= 0) {
-          const size_t wi = (size_t)sp.col * prm.rb_words + (size_t)t * 2 + (qt >> 1);
-          const unsigned sh = (qt & 1) * 16;
-          if (prm.ybits) yb16 = (__ldg(prm.ybits + wi) >> sh) & 0xFFFFu;
-          if (prm.mbits) mb16 = (__ldg(prm.mbits + wi) >> sh) & 0xFFFFu;
-        }
-        mbar_wait(&bars->z_full[tcount & 1], (tcount >> 1) & 1, 300);
-        tc_fence_after();
-        if (prm.debug == 4) { tc_fence_before(); mbar_arrive(&bars->g_full[tcount & 1]); continue; }
-        float lt = 0.f, gt = 0.f;
-        int ok_t = 0, all_t = 0;
-        uint32_t zr[16];
-        tmem_ld16(zb + qt * 16, zr);
-        tmem_wait_ld();
-        if (IS_FIT) {
-          float gv[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float sg;                       // -y * 2^14 for a training row, 0 otherwise
-            if (MODE == TC_FIT_UNI) {
-              sg = __uint_as_float(rm[j]);
-            } else {
-              const uint32_t m = rm[j];
-              const int fr = (int)(m >> 24);
-              const int cls = (int)(m & 0x00FFFFFFu);
-              bool yb = cls == sp.pos;
-              bool train = (fr != 0xFF) && (fr != sp.fold) && (sp.neg1 == 0 || yb || cls == sp.neg1 - 1);
-              if (MODE == TC_FIT) {             // staged row bit matrices (multilabel targets, sampled negatives)
-                if (prm.ybits) yb = (yb16 >> j) & 1u;
-                if (prm.mbits) train = train && ((mb16 >> j) & 1u);
-              }
-              sg = train ? (yb ? -GSCALE : GSCALE) : 0.f;
-            }
-            const float zp = fmaf(__uint_as_float(zr[j]), zi, zb0);
-            const float u = sg * zp;        // = -y * z
-            const float e = ex2_approx(-fabsf(u) * 1.4426950408889634f);
-            const float s1 = 1.f + e;
-            const float loss = fmaf(lg2_approx(s1), 0.6931471805599453f, fmaxf(u, 0.f));
-            const float r = rcp_approx(s1);
-            const float sig = (u >= 0.f) ? r : e * r;
-            gv[j] = sg * sig;               // 2^14 * dloss/dz
-            lt = fmaf(fabsf(sg), loss, lt); // 2^14 * loss
-            gt += gv[j];
-          }
-          uint32_t out[16];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float a = gv[2 * j], b = gv[2 * j + 1];
-            const uint32_t hi = pack_f16x2(a, b);
-            const float2 hf2 = unpack_f16x2(hi);
-            out[j] = hi;
-            out[8 + j] = pack_f16x2(a - hf2.x, b - hf2.y);
-          }
-          tmem_st16(zb + qt * 16, out);
-        } else if (MODE == TC_R2) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const uint32_t m = rm[j];
-            const float z = fmaf(__uint_as_float(zr[j]), zi, zb0);
-            const int fr = (int)(m >> 24);
-            const bool in = (fr != 0xFF) && (sp.fold == -2 || (sp.fold >= 0 && fr == sp.fold) ||
-                                             (sp.fold <= -3 && fr != (-3 - sp.fold)));
-            const float r = yv[j] - z;
-            lt += in ? r * r : 0.f;
-            all_t += in ? 1 : 0;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const uint32_t m = rm[j];
-            const float z = fmaf(__uint_as_float(zr[j]), zi, zb0);
-            const int fr = (int)(m >> 24);
-            const bool yb = (int)(m & 0x00FFFFFFu) == sp.pos;
-            // fold code: f >= 0 rows of fold f; -2 all rows; -3-f rows NOT in fold f
-            const bool in = (fr != 0xFF) && (sp.fold == -2 || (sp.fold >= 0 && fr == sp.fold) ||
-                                             (sp.fold <= -3 && fr != (-3 - sp.fold)));
-            ok_t += (in && ((z > 0.f) == yb)) ? 1 : 0;
-            all_t += in ? 1 : 0;
-          }
-        }
-        if (IS_FIT) tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(&bars->g_full[tcount & 1]);
-        {
-          float sl = ls_hi + lt, bb = sl - ls_hi;
-          ls_lo += (ls_hi - (sl - bb)) + (lt - bb);
-          ls_hi = sl;
-          float sg2 = gs_hi + gt, cc = sg2 - gs_hi;
-          gs_lo += (gs_hi - (sg2 - cc)) + (gt - cc);
-          gs_hi = sg2;
-        }
-        n_ok += ok_t;
-        n_all += all_t;
-      }
-      // end of item: all MMAs done -> flush
-      mbar_wait(&bars->acc_done, it_local & 1, 310);
-      tc_fence_after();
-      if (IS_FIT || MODE == TC_R2) {
-        // the four warps of a quadrant hold partial sums of the same slots: exchange them through
-        // the (now idle) Z buffer and let warp qt = 0 add them in a fixed order (deterministic)
-        uint32_t v4[4] = {__float_as_uint(ls_hi), __float_as_uint(ls_lo), __float_as_uint(gs_hi),
-                          __float_as_uint(gs_lo)};
-        tmem_st4(tl + TM_Z0 + qt * 4, v4);
-        tmem_wait_st();
-        tc_fence_before();
-        epi_bar_sync();
-        tc_fence_after();
-      }
-      if (IS_FIT) {
-        float* dst = prm.gradp + ((size_t)z_part * prm.n_act + slot) * prm.ldw;
-#pragma unroll 1
-        for (int c16 = qt; c16 < NCHUNK * 4; c16 += 4) {
-          uint32_t r[16];
-          tmem_ld16(tl + TM_GRAD + c16 * 16, r);
-          tmem_wait_ld();
-          if (valid && nt > 0) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              *reinterpret_cast<uint4*>(dst + c16 * 16 + 4 * j) =
-                  make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-          }
-        }
-      }
-      if ((IS_FIT || MODE == TC_R2) && qt == 0) {
-        uint32_t r[16];
-        tmem_ld16(tl + TM_Z0, r);
-        tmem_wait_ld();
-        double ls = 0.0, gs = 0.0;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          ls += (double)__uint_as_float(r[4 * k]) + (double)__uint_as_float(r[4 * k + 1]);
-          gs += (double)__uint_as_float(r[4 * k + 2]) + (double)__uint_as_float(r[4 * k + 3]);
-        }
-        if (IS_FIT) {
-          if (valid && nt > 0) {   // partial (z_part, slot) has exactly one writer
-            prm.lossp[(size_t)z_part * prm.n_act + slot] = ls * (double)INV_G;
-            prm.gsump[(size_t)z_part * prm.n_act + slot] = gs * (double)INV_G;
-          }
-        } else if (valid && nt > 0) {
-          atomicAdd(prm.lossp + slot, ls);   // sum of squared residuals (parts add up)
-        }
-      }
-      if (MODE == TC_R2) {
-        if (valid && n_all > 0) atomicAdd(prm.count + slot, n_all);
-      } else if (MODE == TC_SCORE && valid && n_all > 0) {
-        atomicAdd(prm.correct + slot, n_ok);
-        atomicAdd(prm.count + slot, n_all);
-      }
-      tc_fence_before();
-      mbar_arrive(&bars->acc_free);
-    }
-  }
+    h += nsub;
 
-  // teardown
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
+    // end of item: the four lanes sharing a slot hold partial sums of it; combine them in a fixed
+    // order (deterministic) and write this chunk's partial
+    if (IS_FIT || MODE == TC_R2) {
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        double ls = (double)ls_hi[s] + (double)ls_lo[s];
+        double gs = (double)gs_hi[s] + (double)gs_lo[s];
+        ls += __shfl_xor_sync(0xffffffffu, ls, 1);
+        gs += __shfl_xor_sync(0xffffffffu, gs, 1);
+        ls += __shfl_xor_sync(0xffffffffu, ls, 2);
+        gs += __shfl_xor_sync(0xffffffffu, gs, 2);
+        if ((lane & 3) == 0 && valid[s]) {
+          if (IS_FIT) {   // partial (z_part, slot) has exactly one writer
+            prm.lossp[(size_t)z_part * prm.n_act + slot[s]] = ls * (double)INV_G;
+            prm.gsump[(size_t)z_part * prm.n_act + slot[s]] = gs * (double)INV_G;
+          } else {
+            atomicAdd(prm.lossp + slot[s], ls);   // sum of squared residuals (parts add up)
+          }
+        }
+      }
+    }
+    if (IS_FIT) {
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        if (!valid[s]) continue;
+        float* dst = prm.gradp + ((size_t)z_part * prm.n_act + slot[s]) * prm.ldw + cq;
+#pragma unroll
+        for (int b = 0; b < NCHUNK * 8; ++b)
+          *reinterpret_cast<float2*>(dst + 8 * b) = make_float2(grad[4 * b + 2 * s], grad[4 * b + 2 * s + 1]);
+      }
+    }
+    if (MODE == TC_R2 || MODE == TC_SCORE) {
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        unsigned long long a = n_all[s], o = n_ok[s];
+        a += __shfl_xor_sync(0xffffffffu, a, 1); o += __shfl_xor_sync(0xffffffffu, o, 1);
+        a += __shfl_xor_sync(0xffffffffu, a, 2); o += __shfl_xor_sync(0xffffffffu, o, 2);
+        if ((lane & 3) == 0 && valid[s] && a > 0) {
+          if (MODE == TC_SCORE) atomicAdd(prm.correct + slot[s], o);
+          atomicAdd(prm.count + slot[s], a);
+        }
+      }
+    }
   }
 }
 
@@ -799,8 +664,8 @@ int tc_prepare(Ctx* c) {
     SKD_CUDA(c, cudaGetLastError());
     SKD_CUDA(c, cudaStreamSynchronize(c->stream));
     cudaFree(colmax);
-    if (tc_make_map_2d(c, &t.map_xh, t.Xh, (uint64_t)npad, (uint64_t)dpad, TC_R)) return 1;
-    if (tc_make_map_2d(c, &t.map_xl, t.Xl, (uint64_t)npad, (uint64_t)dpad, TC_R)) return 1;
+    if (tc_make_map_2d(c, &t.map_xh, t.Xh, (uint64_t)npad, (uint64_t)dpad, TC_SUB)) return 1;
+    if (tc_make_map_2d(c, &t.map_xl, t.Xl, (uint64_t)npad, (uint64_t)dpad, TC_SUB)) return 1;
     t.x_valid = true;
     t.meta_valid = false;
   }
@@ -859,19 +724,20 @@ size_t tc_slot_param_bytes() { return sizeof(TcSlotParam); }
 int tc_partials_per_slot() { return TC_NCH; }
 
 template <int MODE>
-static cudaError_t tc_launch(int nchunk, int grid, size_t smem, cudaStream_t st, const CUtensorMap& xh,
-                             const CUtensorMap& xl, const CUtensorMap& wh, const TcParams& prm) {
+static cudaError_t tc_launch(int nchunk, int grid, cudaStream_t st, const CUtensorMap& xh, const CUtensorMap& xl,
+                             const CUtensorMap& wh, const CUtensorMap& wl, const TcParams& prm) {
   switch (nchunk) {
 #define TC_CASE(N)                                                                                   \
   case N: {                                                                                          \
+    constexpr size_t smem = TcSmem<N>::BYTES;                                                        \
     static bool attr = false;                                                                        \
     if (!attr) {                                                                                     \
       cudaError_t e = cudaFuncSetAttribute(tc_eval_kernel<N, MODE>,                                  \
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);     \
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);  \
       if (e != cudaSuccess) return e;                                                                \
       attr = true;                                                                                   \
     }                                                                                                \
-    tc_eval_kernel<N, MODE><<<grid, TC_THREADS, smem, st>>>(xh, xl, wh, prm);                        \
+    tc_eval_kernel<N, MODE><<<grid, TC_THREADS, smem, st>>>(xh, xl, wh, wl, prm);                    \
     break;                                                                                           \
   }
     TC_CASE(1) TC_CASE(2) TC_CASE(3) TC_CASE(4)
@@ -909,10 +775,10 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
       SKD_CUDA(c, cudaMemsetAsync(w.gradp, 0, (size_t)nz * n_act * w.ldw * sizeof(float), c->stream));
     }
   }
-  CUtensorMap map_wh;
+  CUtensorMap map_wh, map_wl;
   if (tc_make_map_2d(c, &map_wh, w.Wh, (uint64_t)w.slots_pad_cap, (uint64_t)t.dpad, TC_BC)) return 1;
+  if (tc_make_map_2d(c, &map_wl, w.Wl, (uint64_t)w.slots_pad_cap, (uint64_t)t.dpad, TC_BC)) return 1;
   TcParams prm;
-  prm.Wl = (const __half*)w.Wl;
   prm.sp = (const TcSlotParam*)w.sp;
   prm.rowmeta = t.rowmeta;
   prm.yreal = t.yreal_pad;
@@ -926,7 +792,6 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
   prm.groups = groups;
   prm.n_tiles = n_tiles;
   prm.ldw = w.ldw;
-  { const char* dbg = getenv("SKDIST_B200_TC_DEBUG"); prm.debug = dbg ? atoi(dbg) : 0; }
   { const char* gp = getenv("SKDIST_B200_TC_GPASSES"); prm.g_passes = gp ? atoi(gp) : 3; }
   prm.ybits = mode == TC_FIT ? w.ybits : nullptr;
   prm.mbits = mode == TC_FIT ? w.mbits : nullptr;
@@ -948,13 +813,11 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
   prm.tilecnt = lists ? t.tilecnt : nullptr;
   prm.n_lists = t.n_lists;
   prm.n_tiles_ld = n_tiles;
-  const size_t smem = 1024 + (size_t)nchunk * (TC_BC * 128) + (size_t)TC_NS * nchunk * (TC_R * 128) +
-                      sizeof(TcBarriers) + 64;
   if (mode == TC_R2 && !t.yreal_pad) return fail(c, "tc_r2: targets not staged");
-  cudaError_t e = uni ? tc_launch<TC_FIT_UNI>(nchunk, grid, smem, c->stream, t.map_xh, t.map_xl, map_wh, prm)
-                  : mode == TC_FIT ? tc_launch<TC_FIT>(nchunk, grid, smem, c->stream, t.map_xh, t.map_xl, map_wh, prm)
-                  : mode == TC_SCORE ? tc_launch<TC_SCORE>(nchunk, grid, smem, c->stream, t.map_xh, t.map_xl, map_wh, prm)
-                                     : tc_launch<TC_R2>(nchunk, grid, smem, c->stream, t.map_xh, t.map_xl, map_wh, prm);
+  cudaError_t e = uni ? tc_launch<TC_FIT_UNI>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)
+                  : mode == TC_FIT ? tc_launch<TC_FIT>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)
+                  : mode == TC_SCORE ? tc_launch<TC_SCORE>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)
+                                     : tc_launch<TC_R2>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm);
   c->launches += 1;
   if (e != cudaSuccess) return fail(c, std::string("tc_eval launch: ") + cudaGetErrorString(e));
   if (nz_used) *nz_used = nz;

@@ -12,8 +12,8 @@
 // and a violator j inside the block changes later margins of its column by q_j * (x_j . x_t),
 // one entry of the block's Gram matrix
 //     G = X_T X_T^T      [T x T]   (shared by all columns).
-// Both run on tcgen05 tensor cores in fp16 (sgd_gemm_kernel: TMA -> 128B-swizzled shared memory ->
-// tcgen05.mma 128x128x16 with a TMEM accumulator), X permuted into the epoch's shuffled order and
+// Both run on the tensor cores in fp16 (sgd_gemm_kernel: TMA -> 128B-swizzled shared memory ->
+// wgmma 64x128x16, two warpgroups per 128 x 128 tile, fp32 accumulators in registers), X permuted into the epoch's shuffled order and
 // scaled by a power of two once per epoch.  They are used for SCREENING only: sgd_scan_kernel (one
 // warp per column, its float32 weights in registers like sgd.cu) walks the block in order and
 // declares a sample a non-violator only if its approximate margin clears 1 by more than a rigorous
@@ -48,8 +48,9 @@ constexpr int ST_VMAX = 96;          // in-block violators a column can log befo
 constexpr float ST_KAPPA = 0.001953125f;   // 2^-9
 
 // ------------------------------------------------------------------------------------------
-// C = A B^T for fp16 row-major operands [rows x K] (K-major), fp32 accumulation in TMEM.
-// One 128 x 128 output tile per CTA.  warp 0: TMA producer, warp 1: MMA issuer, warps 2..5: epilogue.
+// C = A B^T for fp16 row-major operands [rows x K] (K-major), fp32 accumulation in registers.
+// One 128 x 128 output tile per CTA, two warpgroups of 64 output rows each (wgmma m64n128k16);
+// thread 0 also streams the K chunks through a TMA ring of ST_STAGES slots.
 // Tiles [0, n_s): S tile (sample tile mi, column group ni), stored transposed S[col][sample];
 // tiles [n_s, n_s + n_g): Gram tile (mi <= ni) stored G[j][t].
 // ------------------------------------------------------------------------------------------
@@ -66,33 +67,25 @@ struct SgdGemmParams {
 struct __align__(8) SgdGemmBars {
   uint64_t full[ST_STAGES];
   uint64_t empty[ST_STAGES];
-  uint64_t acc_done;
-  uint32_t tmem_base;
-  uint32_t pad;
 };
 
-__global__ void __launch_bounds__(192, 1)
+constexpr int ST_THREADS = 256;
+
+__global__ void __launch_bounds__(ST_THREADS, 1)
 sgd_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
                 const SgdGemmParams prm) {
   extern __shared__ uint8_t smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;                   // warpgroup: output rows [64 wg, 64 wg + 64) of the tile
   uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   constexpr uint32_t CHUNK = ST_TILE * 128;          // 128 rows x 64 fp16
   constexpr uint32_t STAGE = 2 * CHUNK;
   SgdGemmBars* bars = reinterpret_cast<SgdGemmBars*>(base + ST_STAGES * STAGE);
   if (threadIdx.x == 0) {
-    for (int i = 0; i < ST_STAGES; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], 1); }
-    mbar_init(&bars->acc_done, 1);
+    for (int i = 0; i < ST_STAGES; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars->tmem_base)), "r"(128u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
 
   const int tile = blockIdx.x;
   const bool is_g = tile >= prm.n_s;
@@ -103,62 +96,55 @@ sgd_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
   const int brow = is_g ? prm.row0 + ni * ST_TILE : ni * ST_TILE;
   const CUtensorMap* bmap = is_g ? &map_x : &map_w;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int kc = 0; kc < prm.kchunks; ++kc) {
-        const uint32_t sl = kc % ST_STAGES, ph = (kc / ST_STAGES) & 1;
-        mbar_wait(&bars->empty[sl], ph ^ 1, 500);
-        mbar_expect_tx(&bars->full[sl], STAGE);
-        tma_load_2d(base + sl * STAGE, &map_x, kc * 64, arow, &bars->full[sl]);
-        tma_load_2d(base + sl * STAGE + CHUNK, bmap, kc * 64, brow, &bars->full[sl]);
-      }
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc(ST_TILE, ST_TILE, 0);
-    const uint64_t d0 = make_desc(smem_u32(base), 16, 1024);
-    for (int kc = 0; kc < prm.kchunks; ++kc) {
-      const uint32_t sl = kc % ST_STAGES, ph = (kc / ST_STAGES) & 1;
-      mbar_wait(&bars->full[sl], ph, 510);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t a = d0 + (uint64_t)((sl * STAGE) >> 4);
-        const uint64_t b = d0 + (uint64_t)((sl * STAGE + CHUNK) >> 4);
+  // chunk kc goes to slot kc % ST_STAGES once both warpgroups are done with chunk kc - ST_STAGES
+  auto issue = [&](int kc) {
+    const uint32_t sl = kc % ST_STAGES;
+    if (kc >= ST_STAGES) mbar_wait(&bars->empty[sl], ((kc / ST_STAGES) - 1) & 1, 500);
+    mbar_expect_tx(&bars->full[sl], STAGE);
+    tma_load_2d(base + sl * STAGE, &map_x, kc * 64, arow, &bars->full[sl]);
+    tma_load_2d(base + sl * STAGE + CHUNK, bmap, kc * 64, brow, &bars->full[sl]);
+  };
+  if (threadIdx.x == 0)
+    for (int kc = 0; kc < prm.kchunks && kc < ST_STAGES; ++kc) issue(kc);
+  __syncwarp();
+
+  float acc[64];
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks)
-          mma_ss(tmem, a + ks * 2, b + ks * 2, idesc, (kc > 0 || ks > 0) ? 1u : 0u);
-        tc_commit(&bars->empty[sl]);
-        if (kc == prm.kchunks - 1) tc_commit(&bars->acc_done);
-      }
-      __syncwarp();
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  const uint64_t d0 = make_desc(smem_u32(base), 16, 1024);
+  for (int kc = 0; kc < prm.kchunks; ++kc) {
+    const uint32_t sl = kc % ST_STAGES, ph = (kc / ST_STAGES) & 1;
+    mbar_wait(&bars->full[sl], ph, 510);
+    const uint64_t a = d0 + (uint64_t)((sl * STAGE + wg * 64 * 128) >> 4);
+    const uint64_t b = d0 + (uint64_t)((sl * STAGE + CHUNK) >> 4);
+    reg_fence(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) wgmma_m64n128_ss(acc, a + ks * 2, b + ks * 2, 1u);
+    wgmma_commit();
+    wgmma_wait_all();
+    reg_fence(acc);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&bars->empty[sl]);
+    if (threadIdx.x == 0 && kc + ST_STAGES < prm.kchunks) issue(kc + ST_STAGES);
+    __syncwarp();
+  }
+  // accumulator fragment: acc[i] is (row 64 wg + 16 (warp & 3) + lane / 4 + 8 ((i >> 1) & 1),
+  //                                   column 8 (i >> 2) + 2 (lane & 3) + (i & 1))
+  const int m0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int c0 = 2 * (lane & 3);
+  if (!is_g) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      const int m = m0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + c0 + (i & 1);
+      prm.S[(size_t)(ni * ST_TILE + col) * ST_T + mi * ST_TILE + m] = acc[i];
     }
   } else {
-    const int q = warp & 3;                           // TMEM lane quadrant of this warp
-    const int m = q * 32 + lane;                      // row of the tile
-    mbar_wait(&bars->acc_done, 0, 520);
-    tc_fence_after();
-    const uint32_t tl = tmem + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-    for (int c16 = 0; c16 < ST_TILE / 16; ++c16) {
-      uint32_t r[16];
-      tmem_ld16(tl + c16 * 16, r);
-      tmem_wait_ld();
-      if (!is_g) {
-        float* dst = prm.S + (size_t)(ni * ST_TILE + c16 * 16) * ST_T + mi * ST_TILE + m;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) dst[(size_t)j * ST_T] = __uint_as_float(r[j]);
-      } else {
-        float* dst = prm.G + (size_t)(mi * ST_TILE + m) * ST_T + ni * ST_TILE + c16 * 16;
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          *reinterpret_cast<uint4*>(dst + 4 * j) = make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-      }
+    for (int i = 0; i < 64; i += 2) {
+      const int m = m0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + c0;
+      *reinterpret_cast<float2*>(prm.G + (size_t)(mi * ST_TILE + m) * ST_T + ni * ST_TILE + col) = make_float2(acc[i], acc[i + 1]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(128u) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------
@@ -672,7 +658,7 @@ int sgd_fit_batch_tc(Ctx* c, int B, const int32_t* col_pos, double alpha, int fi
       SgdGemmParams gg;
       gg.S = S; gg.G = G[b & 1]; gg.row0 = b * ST_T; gg.n_colgroups = 1; gg.n_s = 0;
       gg.n_g = (int)hg.size(); gg.gtiles = gtiles; gg.kchunks = dpad / 64;
-      sgd_gemm_kernel<<<gg.n_g, 192, gemm_smem, sB>>>(map_x, map_w, gg);
+      sgd_gemm_kernel<<<gg.n_g, ST_THREADS, gemm_smem, sB>>>(map_x, map_w, gg);
       cudaEventRecord(ev_g[b & 1], sB);
     };
     launch_g(0);
@@ -686,7 +672,7 @@ int sgd_fit_batch_tc(Ctx* c, int B, const int32_t* col_pos, double alpha, int fi
       gp.n_g = 0; gp.gtiles = gtiles; gp.kchunks = dpad / 64;
       const bool tb = trace && (epoch == 1 || epoch == 20) && b >= 8 && b < 24;    // kernel split of 16 blocks
       if (tb) cudaEventRecord(ev_t[0], c->stream);
-      sgd_gemm_kernel<<<gp.n_s, 192, gemm_smem, c->stream>>>(map_x, map_w, gp);
+      sgd_gemm_kernel<<<gp.n_s, ST_THREADS, gemm_smem, c->stream>>>(map_x, map_w, gp);
       if (tb) cudaEventRecord(ev_t[1], c->stream);
       SKD_CUDA(c, cudaStreamWaitEvent(c->stream, ev_g[b & 1], 0));
       SgdScanParams sp;

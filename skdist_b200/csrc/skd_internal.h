@@ -66,8 +66,8 @@ struct Ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
   std::string err;
-  int sm_count = 148;
-  int kernel_choice = 0;  // 0 auto, 1 simt, 2 tcgen05
+  int sm_count = 132;
+  int kernel_choice = 0;  // 0 auto, 1 simt, 2 tensor cores (wgmma)
   // staged data
   float* X = nullptr;       // [n x ldx] fp32 row-major
   int64_t n = 0, d = 0, ldx = 0;

@@ -1,4 +1,4 @@
-"""Distributed feature elimination on B200s.
+"""Distributed feature elimination on H100 GPUs.
 
 Counterpart of /root/reference/skdist/distribute/eliminate.py (`DistFeatureEliminator`, :47-284).
 The reference ranks the features by the squared coefficients of one fit on all features, builds

@@ -1,4 +1,4 @@
-"""Distributed tree ensembles on B200s.
+"""Distributed tree ensembles on H100 GPUs.
 
 Drop-in for /root/reference/skdist/distribute/ensemble.py (class name, constructor signature with
 ``sc`` FIRST, fitted attributes).  The reference fans `_build_trees` (ensemble.py:68-109) out over
@@ -399,7 +399,7 @@ class _DistForestClassifier(_ScParamMixin):
 
 
 class DistRandomForestClassifier(_DistForestClassifier, RandomForestClassifier):
-    __doc__ = """Same as sklearn `RandomForestClassifier` with every tree built on a B200.
+    __doc__ = """Same as sklearn `RandomForestClassifier` with every tree built on an H100.
     Constructor mirrors ref ensemble.py:378-422 (``sc`` is the FIRST positional argument).""" + _LIMITS
 
     _splitter = 0
@@ -417,7 +417,7 @@ class DistRandomForestClassifier(_DistForestClassifier, RandomForestClassifier):
 
 
 class DistExtraTreesClassifier(_DistForestClassifier, ExtraTreesClassifier):
-    __doc__ = """Same as sklearn `ExtraTreesClassifier` with every tree built on a B200 (random splitter:
+    __doc__ = """Same as sklearn `ExtraTreesClassifier` with every tree built on an H100 (random splitter:
     one uniformly drawn threshold per drawn feature, no bootstrap by default).
     Constructor mirrors ref ensemble.py:437-478 (``sc`` is the FIRST positional argument).""" + _LIMITS
 
@@ -461,7 +461,7 @@ class _DistForestRegressor(_DistForestClassifier):
 
 
 class DistRandomForestRegressor(_DistForestRegressor, RandomForestRegressor):
-    __doc__ = """Same as sklearn `RandomForestRegressor` with every tree built on a B200.
+    __doc__ = """Same as sklearn `RandomForestRegressor` with every tree built on an H100.
     Constructor mirrors ref ensemble.py:531-572 (``sc`` FIRST; criterion "mse" = squared error).""" + _LIMITS
 
     _splitter = 0
@@ -477,7 +477,7 @@ class DistRandomForestRegressor(_DistForestRegressor, RandomForestRegressor):
 
 
 class DistExtraTreesRegressor(_DistForestRegressor, ExtraTreesRegressor):
-    __doc__ = """Same as sklearn `ExtraTreesRegressor` with every tree built on a B200.
+    __doc__ = """Same as sklearn `ExtraTreesRegressor` with every tree built on an H100.
     Constructor mirrors ref ensemble.py:584-616.""" + _LIMITS
 
     _splitter = 1
@@ -493,7 +493,7 @@ class DistExtraTreesRegressor(_DistForestRegressor, ExtraTreesRegressor):
 
 
 class DistRandomTreesEmbedding(_DistForestRegressor, RandomTreesEmbedding):
-    __doc__ = """Same as sklearn `RandomTreesEmbedding` with every tree built on a B200: totally random trees
+    __doc__ = """Same as sklearn `RandomTreesEmbedding` with every tree built on an H100: totally random trees
     (`ExtraTreeRegressor`, one drawn feature per node, uniformly drawn threshold) fitted on uniform random
     targets, then the one-hot code of the leaf every row lands in.  Constructor and `fit` / `fit_transform` /
     `transform` mirror ref ensemble.py:619-708 (``sc`` is the FIRST positional argument).  With one feature

@@ -1,4 +1,4 @@
-"""Distributed multiclass strategies on B200s.
+"""Distributed multiclass strategies on H100 GPUs.
 
 Drop-in for /root/reference/skdist/distribute/multiclass.py (class names, constructor
 signatures, fitted attributes).  The reference ships one dense 0/1 label vector per class to a

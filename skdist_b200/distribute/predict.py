@@ -1,4 +1,4 @@
-"""Batched model inference on B200s.
+"""Batched model inference on H100 GPUs.
 
 Counterpart of /root/reference/skdist/distribute/predict.py.  The reference wraps
 ``model.predict`` / ``model.predict_proba`` in a Spark pandas UDF that is called once per Arrow

@@ -1,4 +1,4 @@
-"""Distributed hyper-parameter search meta-estimators on B200s.
+"""Distributed hyper-parameter search meta-estimators on H100 GPUs.
 
 Drop-in for /root/reference/skdist/distribute/search.py (class names, constructor
 signatures incl. positional order, fitted attributes).  The reference fans
@@ -235,7 +235,7 @@ class DistBaseSearchCV(_ScParamMixin):
 
 
 class DistGridSearchCV(DistBaseSearchCV, GridSearchCV):
-    """Same as sklearn `GridSearchCV` but with the fits batched on B200s.
+    """Same as sklearn `GridSearchCV` but with the fits batched on H100 GPUs.
     Constructor mirrors ref search.py:608-641 (``sc`` is the 3rd positional argument)."""
 
     def __init__(self, estimator, param_grid, sc=None, partitions="auto", preds=False,
@@ -263,7 +263,7 @@ class DistGridSearchCV(DistBaseSearchCV, GridSearchCV):
 
 
 class DistRandomizedSearchCV(DistBaseSearchCV, RandomizedSearchCV):
-    """Same as sklearn `RandomizedSearchCV` but with the fits batched on B200s.
+    """Same as sklearn `RandomizedSearchCV` but with the fits batched on H100 GPUs.
     Constructor mirrors ref search.py:671-708."""
 
     def __init__(self, estimator, param_distributions, sc=None, partitions="auto", preds=False,

@@ -6,12 +6,12 @@ from sklearn.utils.validation import check_is_fitted
 
 def _check_estimator(estimator, verbose=False):
     """Print backend awareness (ref validation.py:14-20: spark vs local).  Here the
-    backend is always the B200 engine; ``sc`` is accepted and ignored."""
+    backend is always the H100 engine; ``sc`` is accepted and ignored."""
     if verbose:
         from .. import parallel
         rank, world, _ = parallel.dist_info()
         if rank == 0:
-            print("skdist_b200: running on %d B200 process(es); sc=%s is ignored"
+            print("skdist_b200: running on %d H100 process(es); sc=%s is ignored"
                   % (world, "None" if getattr(estimator, "sc", None) is None else "given"))
 
 

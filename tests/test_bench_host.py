@@ -42,3 +42,30 @@ def test_parity_block_against_the_cpu_leg(fake_engine):
     ci, f = tasks[4]
     bad["split%d_test_score" % f][ci] -= 3 / 1000
     assert bench.parity_block(bad, tasks, scores, fold, Cs, 3)["max_flips_per_fold"] == 3
+
+
+def test_dump_outputs_writes_float_arrays_within_the_limit(tmp_path, monkeypatch):
+    import bench
+    res = {"fit": {"coef": np.arange(12, dtype=np.float32).reshape(4, 3), "n_iter": np.array([3, 4, 5, 6], np.int32)},
+           "correct": np.array([1, 2, 3, 4], np.int64)}
+    bench.dump_outputs(str(tmp_path / "a"), res)
+    coef = np.load(tmp_path / "a" / "fit_coef.npy")
+    assert coef.dtype == np.float32 and np.array_equal(coef, res["fit"]["coef"])
+    assert np.load(tmp_path / "a" / "fit_n_iter.npy").dtype == np.float64
+    assert np.array_equal(np.load(tmp_path / "a" / "correct.npy"), [1, 2, 3, 4])
+    # over the limit: every file counted; arrays of the same length share one seeded row sample
+    monkeypatch.setattr(bench, "DUMP_LIMIT", 8192)
+    big = {"x": np.arange(4000, dtype=np.float64).reshape(1000, 4), "y": np.arange(1000, dtype=np.float32),
+           "z": np.arange(300, dtype=np.int32), "s": 3.5}
+    for d in ("b", "c"):
+        bench.dump_outputs(str(tmp_path / d), big)
+        assert sum(f.stat().st_size for f in (tmp_path / d).iterdir()) <= 8192
+    rows = np.load(tmp_path / "b" / "sample_rows_1000.npy").astype(int)
+    assert 0 < len(rows) < 1000 and not (tmp_path / "b" / "x_rows.npy").exists()
+    np.testing.assert_array_equal(np.load(tmp_path / "b" / "x.npy"), big["x"][rows])
+    np.testing.assert_array_equal(np.load(tmp_path / "b" / "y.npy"), big["y"][rows])
+    zrows = np.load(tmp_path / "b" / "sample_rows_300.npy").astype(int)
+    np.testing.assert_array_equal(np.load(tmp_path / "b" / "z.npy"), big["z"][zrows])
+    assert float(np.load(tmp_path / "b" / "s.npy")) == 3.5
+    for f in (tmp_path / "b").iterdir():
+        np.testing.assert_array_equal(np.load(f), np.load(tmp_path / "c" / f.name))

@@ -1,5 +1,8 @@
 """DistFeatureEliminator host logic on the test-double engine, pinned against the UNMODIFIED
-reference class where /root/reference is present (joblib branch, ref eliminate.py:163-184)."""
+reference's task function (joblib branch, ref eliminate.py:163-184), whose scores
+tests/golden/make_reference_pins.py recorded."""
+import os
+
 import numpy as np
 import pytest
 from sklearn.linear_model import LogisticRegression
@@ -21,15 +24,10 @@ def test_eliminator_matches_reference_task_function(fake_engine):
     positional arguments, eliminate.py:125), so the pin is on what every task executes: the
     UNMODIFIED `_fit_and_score_one` / `_drop_col` (eliminate.py:22-38) for each (feature set, fold),
     with the feature sets built as eliminate.py:131-154 builds them."""
-    from oracle import refshim
-    if not refshim.available():
-        pytest.skip("reference tree not present")
-    ref_elim = refshim.load_module("skdist.distribute.eliminate")
-    from sklearn.metrics import check_scoring
-    from sklearn.model_selection import StratifiedKFold
+    pins = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_pins.npz"))
     X, y = _data()
     d = X.shape[1]
-    for step, n_cv, min_keep in ((2, 3, d // 2), (3, 4, 3)):
+    for i, (step, n_cv, min_keep) in enumerate(((2, 3, d // 2), (3, 4, 3))):
         base = LogisticRegression(C=0.3)
         ours = DistFeatureEliminator(base, None, step=step, cv=n_cv, min_features_to_select=min_keep).fit(X, y)
         coefs = LogisticRegression(C=0.3).fit(X, y).coef_
@@ -38,9 +36,8 @@ def test_eliminator_matches_reference_task_function(fake_engine):
         while k < d - min_keep:
             k += step
             sets.append(ranks[:k])
-        scorer = check_scoring(base, scoring=None)
-        ref_scores = [np.mean([ref_elim._fit_and_score_one(idx, base, X, y, scorer, tr, te, False, {})
-                               for tr, te in StratifiedKFold(n_cv).split(X, y)]) for idx in sets]
+        ref_scores = pins["eliminate_scores_%d" % i]
+        assert len(ref_scores) == len(sets)
         np.testing.assert_allclose(ours.scores_, ref_scores, atol=1e-12)
         best = int(np.argmax(ref_scores))
         exp_keep = np.delete(range(d), sets[best].astype(int)) if len(sets[best]) else np.arange(d)

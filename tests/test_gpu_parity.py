@@ -1,4 +1,4 @@
-"""CUDA path vs the oracle / golden fixtures, through the C-ABI (run with -m gpu on a B200).
+"""CUDA path vs the oracle / golden fixtures, through the C-ABI (run with -m gpu on an H100).
 
 Tolerances.  Integer work (accuracy counts for given coefficients) is exact.  The logistic
 objective is fp32 arithmetic (sklearn: fp32 sgemv + float64 pointwise, ours: fp32 FMA or
@@ -28,7 +28,8 @@ FLIPS = 2
 
 @pytest.fixture(scope="module", params=[1, 2], ids=["simt", "tcgen05"])
 def eng(request):
-    """Every parity test runs on both evaluation kernels: 1 = SIMT fp32, 2 = tcgen05 fp16x2-split."""
+    """Every parity test runs on both evaluation kernels: 1 = SIMT fp32, 2 = tensor-core (wgmma) fp16x2-split.
+    The ids are the names these tests are known by: "tcgen05" selects the tensor-core kernel."""
     from skdist_b200.engine import Engine, set_engine_factory
     e = Engine(0)
     e.set_kernel(request.param)
@@ -75,7 +76,7 @@ def test_loss_grad_matches_oracle(eng):
         m = np.ones(len(y), bool) if cf[j] < 0 else fold != cf[j]
         fo, go = lo.loss_gradient(W[j], X[m], y[m].astype(np.float32), 1.0 / (C[j] * m.sum()))
         assert abs(f[j] - fo) <= 2e-6 * abs(fo)
-        # tcgen05: fp32 accumulation in the tensor core rounds toward zero -> ~1e-5 relative bias
+        # tensor cores: fp32 accumulation in the tensor core rounds toward zero -> ~1e-5 relative bias
         # on large same-sign sums (random W); vanishes near an optimum
         tol = 3e-6 if eng.kernel == 1 else 5e-5
         np.testing.assert_allclose(g[j], go, rtol=0, atol=tol * np.abs(go).max())
@@ -145,7 +146,7 @@ def test_fit_batch_vs_golden(eng, name):
 def test_fit_batch_vs_golden_midsize(eng):
     """G1 200 000 x 256, 32 C x 5 folds (the headline workload's generator, feature count and fold
     layout at 1/5 of its rows) against the scores of the reference's unmodified `_fit_and_score`
-    (tests/golden/make_golden.py --mid-only), on the fp32 CUDA-core kernels (1) and on the tcgen05
+    (tests/golden/make_golden.py --mid-only), on the fp32 CUDA-core kernels (1) and on the tensor-core
     kernel (2) separately.  At this size the reference is far from reproducing itself on the
     weakly regularised columns (fixture: up to 28 predictions per 40 000-row fold and 4 % in the
     coefficients between 1 BLAS thread / all threads / permuted rows); the device path is held to
@@ -158,7 +159,7 @@ def test_fit_batch_vs_golden_midsize(eng):
     Cs = g["C"]
     C = np.repeat(Cs, cv)
     cf = np.tile(np.arange(cv, dtype=np.int32), len(Cs))
-    kernel = eng.kernel            # the fixture runs the test on the fp32 CUDA-core kernels (1) and on tcgen05 (2)
+    kernel = eng.kernel            # the fixture runs the test on the fp32 CUDA-core kernels (1) and on the tensor cores (2)
     res = eng.logreg_fit_batch(C, cf, np.ones(len(C), np.int32))
     correct, count = eng.linear_score_batch(res["coef"], cf, np.ones(len(C), np.int32))
     gold_scores = np.stack([g["split%d_test_score" % i] for i in range(cv)], 1).ravel()
@@ -169,8 +170,8 @@ def test_fit_batch_vs_golden_midsize(eng):
     print("kernel %d: flips max %d mean %.2f (reference envelope max %d mean %.2f); excess over envelope max %d"
           % (kernel, flips.max(), flips.mean(), nf.max(), nf.mean(), np.max(flips - nf)))
     # The fixture's per-column envelope comes from only three perturbed runs of the reference and
-    # underestimates a column's spread (measured on the B200: 38 of 160 columns of the fp32 CUDA-core
-    # kernels -- the reference's own arithmetic class -- exceed their column's envelope, 43 on tcgen05),
+    # underestimates a column's spread (dozens of the 160 columns exceed their column's envelope on the
+    # fp32 CUDA-core kernels -- the reference's own arithmetic class -- as well as on the tensor cores),
     # so the comparison is made on the distribution: no more differing predictions than the reference
     # shows against itself, on average and at the maximum.
     assert flips.mean() <= nf.mean() + 1.0, (flips.mean(), nf.mean())
@@ -187,7 +188,7 @@ def test_fit_batch_vs_golden_midsize(eng):
     assert np.all(flips[stable] <= 1)
     gc = g["coef"].reshape(len(C), -1)
     rel = np.abs(res["coef"] - gc).max(1) / np.abs(gc).max(1)
-    assert np.all(rel[same_path] <= 5e-4), rel[same_path].max()      # measured: 1.2e-4 (fp32 kernels), 3.5e-4 (tcgen05)
+    assert np.all(rel[same_path] <= 5e-4), rel[same_path].max()
     assert np.all(rel[stable] <= 2e-2), rel[stable].max()
     scores = (correct / count).reshape(len(Cs), cv)
     mean = np.average(scores, axis=1, weights=count[:cv])
@@ -362,7 +363,7 @@ def test_ovr_sgd_exact_order_on_device(eng):
 
 @pytest.mark.parametrize("n,d,k,alpha", [(9000, 40, 7, 1e-4), (5000, 100, 5, 1e-4), (6000, 24, 4, 100.0)])
 def test_ovr_sgd_tensor_core_path_bit_identical(eng, monkeypatch, n, d, k, alpha):
-    """The blocked-exact tensor-core path (csrc/sgd_tc.cu: fp16 tcgen05 products S = X_T W^T and
+    """The blocked-exact tensor-core path (csrc/sgd_tc.cu: fp16 tensor-core products S = X_T W^T and
     G = X_T X_T^T screen the margins of 2048-sample blocks, every sample that does not clear 1 by the
     error bound gets the exact dot product) gives the same coefficients, intercepts, n_iter_ and t_
     as scikit-learn bit for bit.  alpha = 100 makes the lazy scale fall below 1e-6 (at the first sample and
@@ -529,7 +530,7 @@ def test_feature_eliminator_on_device(eng):
 
 
 def test_tc_column_result_independent_of_batch():
-    """tcgen05 path: partial sums are formed over fixed row chunks, so a (C, fold) column gets the
+    """Tensor-core path: partial sums are formed over fixed row chunks, so a (C, fold) column gets the
     same bits whether it is fitted alone, in a small batch or among hundreds of columns (and hence
     on however many GPUs the columns are dealt to)."""
     from skdist_b200.engine import Engine
@@ -616,7 +617,7 @@ def test_reference_toy_cases_on_device(eng):
 
 def test_tc_more_groups_than_sms():
     """20 480 columns = 160 groups of 128 (more groups than SMs): the (group, chunk) units are simply
-    dealt over 148 CTAs.  Columns must still equal their small-batch results bit for bit."""
+    dealt over one CTA per SM.  Columns must still equal their small-batch results bit for bit."""
     from skdist_b200.engine import Engine
     e = Engine(0)
     try:

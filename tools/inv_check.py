@@ -1,5 +1,5 @@
 """Batch invariance of the tensor-core fit: one (C, fold) column fitted alone and inside batches of
-1 / 32 / 148 / 160 groups of 128 columns must give bit-identical coefficients (more groups than SMs
+4 / 32 / 148 / 160 groups of 128 columns must give bit-identical coefficients (more groups than SMs
 exercises the weight reload of a CTA that spans several groups)."""
 import os, sys
 import numpy as np

@@ -1,5 +1,5 @@
 """Predictions that differ from the reference (`flips` per held-out fold) on every logistic fixture,
-for the fp32 CUDA-core kernels and for the tcgen05 kernel separately, next to the reference's own
+for the fp32 CUDA-core kernels and for the tensor-core kernel separately, next to the reference's own
 run-to-run envelope stored with the fixture.  One JSON line per (fixture, kernel); DESIGN.md section 4
 quotes them.   python tools/parity_report.py [--gpasses 2]"""
 import json, os, sys
@@ -19,7 +19,7 @@ for name in ["search_logreg_g1_4000x16", "search_logreg_g1_20000x64", "search_lo
     nf = g["noise_flips"].ravel(); nc = g["noise_coef"].ravel(); gi = g["n_iter"].ravel()
     gc = g["coef"].reshape(len(C), -1)
     stable = (nf == 0) & (nc < 1e-4) & (gi < 100)
-    for kernel, kname in ((1, "simt-fp32"), (2, "tcgen05")):
+    for kernel, kname in ((1, "simt-fp32"), (2, "tensor-core")):
         eng.set_kernel(kernel)
         res = eng.logreg_fit_batch(C, cf, np.ones(len(C), np.int32))
         correct, count = eng.linear_score_batch(res["coef"], cf, np.ones(len(C), np.int32))

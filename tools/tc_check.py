@@ -1,4 +1,4 @@
-"""tcgen05 path vs oracle: objective / gradient at random points, several shapes."""
+"""Tensor-core (wgmma) path vs oracle: objective / gradient at random points, several shapes."""
 import os, sys, time
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
