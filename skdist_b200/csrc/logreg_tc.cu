@@ -16,12 +16,14 @@
 // numbers, v = hi + lo (22+ mantissa bits after exact power-of-two pre-scaling per feature /
 // per column), and each product is three MMAs hi*hi + hi*lo + lo*hi accumulated in fp32.
 //
-// Work decomposition: a group = 128 slots, two warpgroups of 64 slots each (wgmma M = 64); its
-// rows are cut into TC_NCH chunks; one persistent CTA per run of (group, chunk) items.  Per CTA:
-// W_hi and W_lo stationary in shared memory, the gradient accumulators (64 x d fp32 per
+// Work decomposition: a group = 128 slots, two consumer warpgroups of 64 slots each (wgmma M = 64);
+// its rows are cut into TC_NCH chunks; one persistent CTA per run of (group, chunk) items.  Per CTA:
+// W_hi and W_lo stationary in shared memory, the gradient accumulators (64 x d fp32 per consumer
 // warpgroup) stationary in registers, X streamed in sub-tiles of 32 rows (hi and lo halves) through
-// a TMA ring that thread 0 keeps filled.  The accumulator fragment of a 16-row block of Z is the
-// register A fragment of one k16 step of GEMM2, so G never leaves the registers.
+// a TMA ring that a producer warpgroup keeps filled.  The accumulator fragment of a 16-row block of Z
+// is the register A fragment of one k16 step of GEMM2, so G never leaves the registers.  The two
+// consumers take turns on the tensor cores, so that one runs its epilogue while the products of the
+// other are in flight.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -39,7 +41,10 @@ constexpr int TC_R = 64;         // rows per tile (the unit of the tile lists an
 constexpr int TC_SUB = 32;       // rows per ring sub-tile (wgmma N of GEMM1, K of GEMM2)
 constexpr int TC_NCH = 132;      // fixed row chunks per group (one partial sum per (chunk, slot)); 132 = 4 * 3 * 11
                                  // divides evenly over 132 / 66 / 44 / 33 / 22 CTAs per group (1, 2, 3, 4, 6 groups per GPU)
-constexpr int TC_THREADS = 256;  // two warpgroups
+constexpr int TC_THREADS = 384;  // producer warpgroup + two consumer warpgroups
+// register split of the warpgroups (setmaxnreg): 128 * 24 + 256 * 240 = 64 512 of the SM's 65 536
+constexpr uint32_t TC_PRODUCER_REGS = 24;
+constexpr uint32_t TC_CONSUMER_REGS = 240;
 constexpr uint32_t TC_SMEM_MAX = 232448;   // 227 KB of opt-in shared memory per block
 constexpr float XSCALE_TARGET_EXP = 13.f;   // column max scaled into [2^13, 2^14)
 constexpr float GSCALE = 16384.f;           // 2^14
@@ -228,9 +233,10 @@ struct TcSmem {
 };
 
 struct __align__(8) TcBarriers {
-  uint64_t full[8];
-  uint64_t empty[8];
-  uint64_t w_full;
+  uint64_t full[8];    // stage loaded (TMA transaction count)
+  uint64_t empty[8];   // stage consumed by both consumer warpgroups
+  uint64_t w_full;     // W_hi / W_lo of the current group loaded
+  uint64_t w_free;     // both consumers are done with the previous group's W
 };
 
 template <int NCHUNK>
@@ -257,7 +263,10 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
   constexpr int NS = SM::NS;
   extern __shared__ uint8_t smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int wg = threadIdx.x >> 7;                 // warpgroup: slots [64 wg, 64 wg + 64) of the group
+  // warpgroup: 0 producer, 1 and 2 consumers (read from lane 0, so the compiler knows it is warp-uniform
+  // and keeps the descriptors built from it in uniform registers)
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
+  const int cw = wg - 1;                           // consumer cw: slots [64 cw, 64 cw + 64) of the group
   const bool wg_leader = (threadIdx.x & 127) == 0;
   uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* s_wh = base;
@@ -268,9 +277,10 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
   if (threadIdx.x == 0) {
     for (int i = 0; i < NS; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], 2); }
     mbar_init(&bars->w_full, 1);
+    mbar_init(&bars->w_free, 2);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
+  __syncthreads();   // the last block-wide barrier: the roles part here
 
   // Work split.  A group's tile list (all tiles, or the tiles with training rows of the group's
   // fold) is cut into TC_NCH fixed chunks; a unit = (group, chunk); the groups * TC_NCH units are
@@ -300,62 +310,88 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
     it.t1 = (int)((long long)cnt * (it.z + 1) / TC_NCH);
     return it.t1 > it.t0;       // empty chunks (fewer tiles than chunks) are skipped
   };
+  auto sub_row0 = [&](const TcItem& it, int j) -> int {   // first row of sub-tile j of an item
+    const int t = it.tl ? it.tl[it.t0 + (j >> 1)] : it.t0 + (j >> 1);
+    return t * TC_R + (j & 1) * TC_SUB;
+  };
+
+  // Producer: one thread walks the same item sequence as the consumers (same skips, same sub-tile
+  // order) and keeps the ring full across item boundaries.  Sub-tile k (running count) goes to stage
+  // k % NS once both consumers are done with sub-tile k - NS; a new group's W is loaded once both
+  // consumers are done with the previous group's.
+  if (wg == 0) {
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
+      uint32_t k = 0;
+      int w_loads = 0, g_prev = -1;
+      for (long long u = u_begin; u < u_end; ++u) {
+        TcItem it;
+        if (!get_item(u, it)) continue;
+        if (it.g != g_prev) {
+          if (w_loads > 0) mbar_wait(&bars->w_free, (w_loads - 1) & 1, 120);
+          mbar_expect_tx(&bars->w_full, SM::W_BYTES);
+#pragma unroll
+          for (int c = 0; c < NCHUNK; ++c) {
+            tma_load_2d(s_wh + c * SM::W_CHUNK, &map_wh, c * 64, it.g * TC_BC, &bars->w_full);
+            tma_load_2d(s_wl + c * SM::W_CHUNK, &map_wl, c * 64, it.g * TC_BC, &bars->w_full);
+          }
+          ++w_loads;
+          g_prev = it.g;
+        }
+        const int nsub = 2 * (it.t1 - it.t0);
+        for (int j = 0; j < nsub; ++j, ++k) {
+          const uint32_t sl = k % NS;
+          if (k >= (uint32_t)NS) mbar_wait(&bars->empty[sl], ((k / NS) - 1) & 1, 100);
+          mbar_expect_tx(&bars->full[sl], SM::STAGE);
+          const int r0 = sub_row0(it, j);
+          uint8_t* dst = s_ring + sl * SM::STAGE;
+#pragma unroll
+          for (int c = 0; c < NCHUNK; ++c) {
+            tma_load_2d(dst + c * SM::X_CHUNK, &map_xh, c * 64, r0, &bars->full[sl]);
+            tma_load_2d(dst + (NCHUNK + c) * SM::X_CHUNK, &map_xl, c * 64, r0, &bars->full[sl]);
+          }
+        }
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<TC_CONSUMER_REGS>();
+
+  // Consumers take turns on the tensor cores (named barriers 1 and 2, one per consumer): a turn is
+  // the issue of one sub-tile's products (see the sub-tile loop) and hands over to the other consumer,
+  // so one consumer's epilogue runs while the other's products are in flight.  Both consumers walk
+  // the same sub-tiles, so they take the same number of turns; consumer 0 takes the first.
+  const uint32_t bar_mine = 1 + cw, bar_other = 2 - cw;
+  auto turn_begin = [&] { named_bar_sync(bar_mine, 256); };
+  auto turn_end = [&] { named_bar_arrive(bar_other, 256); };
+  if (cw == 1) named_bar_arrive(1, 256);
 
   // accumulator fragments (wgmma m64nN): register i of a thread holds row 16 (warp & 3) + lane / 4
   // + 8 ((i >> 1) & 1) of its warpgroup's 64 slots and column 8 (i >> 2) + 2 (lane & 3) + (i & 1)
   const int slot_in_wg = (warp & 3) * 16 + (lane >> 2);
   const int cq = 2 * (lane & 3);
   constexpr float INV_G = 1.f / GSCALE;
-  const uint64_t desc_w = make_desc(smem_u32(s_wh), 16, 1024) + (uint64_t)((wg * 64 * 128) >> 4);
+  const uint64_t desc_w = make_desc(smem_u32(s_wh), 16, 1024) + (uint64_t)((cw * 64 * 128) >> 4);
   const uint64_t desc_k = make_desc(smem_u32(s_ring), 16, 1024);              // X as K-major (GEMM1)
   const uint64_t desc_mn = make_desc(smem_u32(s_ring), SM::X_CHUNK, 1024);    // X as MN-major (GEMM2)
   constexpr uint32_t WL_OFF = (NCHUNK * SM::W_CHUNK) >> 4;
   constexpr uint32_t XL_OFF = (NCHUNK * SM::X_CHUNK) >> 4;
+  const bool g3 = prm.g_passes >= 3;
 
-  uint32_t h = 0;          // running sub-tile counter (ring position), identical in every thread
+  uint32_t h = 0;          // running sub-tile counter (ring position), identical in both consumers
   int w_loads = 0, g_prev = -1;
   for (long long u = u_begin; u < u_end; ++u) {
     TcItem it;
     if (!get_item(u, it)) continue;
     const int g = it.g, z_part = it.z;
     const int nsub = 2 * (it.t1 - it.t0);
-    const int32_t* tlist = it.tl;
-    auto sub_row0 = [&](int j) -> int {
-      const int t = tlist ? tlist[it.t0 + (j >> 1)] : it.t0 + (j >> 1);
-      return t * TC_R + (j & 1) * TC_SUB;
-    };
-    // sub-tile k (global count) goes to slot k % NS once both warpgroups are done with sub-tile k - NS
-    auto issue = [&](uint32_t k, int j) {
-      const uint32_t sl = k % NS;
-      if (k >= (uint32_t)NS) mbar_wait(&bars->empty[sl], ((k / NS) - 1) & 1, 100);
-      mbar_expect_tx(&bars->full[sl], SM::STAGE);
-      const int r0 = sub_row0(j);
-      uint8_t* dst = s_ring + sl * SM::STAGE;
-#pragma unroll
-      for (int c = 0; c < NCHUNK; ++c) {
-        tma_load_2d(dst + c * SM::X_CHUNK, &map_xh, c * 64, r0, &bars->full[sl]);
-        tma_load_2d(dst + (NCHUNK + c) * SM::X_CHUNK, &map_xl, c * 64, r0, &bars->full[sl]);
-      }
-    };
-    const bool new_group = g != g_prev;
-    if (new_group) {
-      // weights of a new group: every wgmma of the previous group has completed (each sub-tile ends
-      // in wgmma_wait_all), the barrier makes sure both warpgroups are past them
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        mbar_expect_tx(&bars->w_full, SM::W_BYTES);
-#pragma unroll
-        for (int c = 0; c < NCHUNK; ++c) {
-          tma_load_2d(s_wh + c * SM::W_CHUNK, &map_wh, c * 64, g * TC_BC, &bars->w_full);
-          tma_load_2d(s_wl + c * SM::W_CHUNK, &map_wl, c * 64, g * TC_BC, &bars->w_full);
-        }
-      }
+    if (g != g_prev) {
+      // every product of the previous group has completed (each sub-tile ends in wgmma_wait_all):
+      // release its W, then wait for this group's
+      if (g_prev >= 0 && wg_leader) mbar_arrive(&bars->w_free);
+      mbar_wait(&bars->w_full, (w_loads++) & 1, 200);
       g_prev = g;
     }
-    if (threadIdx.x == 0)
-      for (int j = 0; j < nsub && j < NS; ++j) issue(h + j, j);
-    __syncwarp();
-    if (new_group) mbar_wait(&bars->w_full, (w_loads++) & 1, 200);
 
     // the two slots of this thread
     TcSlotParam sp[2];
@@ -363,7 +399,7 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
     int slot[2];
 #pragma unroll
     for (int s = 0; s < 2; ++s) {
-      slot[s] = g * TC_BC + wg * 64 + slot_in_wg + 8 * s;
+      slot[s] = g * TC_BC + cw * 64 + slot_in_wg + 8 * s;
       valid[s] = slot[s] < n_live;
       sp[s].inv_t = 1.f; sp[s].bias = 0.f; sp[s].fold = -1; sp[s].pos = -1; sp[s].neg1 = 0; sp[s].col = -1;
       if (valid[s]) sp[s] = prm.sp[slot[s]];
@@ -389,10 +425,61 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
     float ls_hi[2] = {0.f, 0.f}, ls_lo[2] = {0.f, 0.f}, gs_hi[2] = {0.f, 0.f}, gs_lo[2] = {0.f, 0.f};
     unsigned long long n_ok[2] = {0, 0}, n_all[2] = {0, 0};
 
+    // GEMM1 of a sub-tile: Z = W_hi X_hi + W_lo X_hi + W_hi X_lo   [64 slots x 32 rows per warpgroup]
+    auto gemm1 = [&](float (&zf)[16], uint32_t stage) {
+      const uint64_t bx = desc_k + (uint64_t)((stage * SM::STAGE) >> 4);
+#pragma unroll
+      for (int ks = 0; ks < NCHUNK * 4; ++ks) {
+        const uint32_t aoff = ((ks >> 2) * SM::W_CHUNK + (ks & 3) * 32) >> 4;
+        const uint32_t boff = ((ks >> 2) * SM::X_CHUNK + (ks & 3) * 32) >> 4;
+        wgmma_m64n32_ss(zf, desc_add(desc_w, aoff), desc_add(bx, boff), ks > 0 ? 1u : 0u);
+        wgmma_m64n32_ss(zf, desc_add(desc_w, WL_OFF + aoff), desc_add(bx, boff), 1u);
+        wgmma_m64n32_ss(zf, desc_add(desc_w, aoff), desc_add(bx, XL_OFF + boff), 1u);
+      }
+      wgmma_commit();
+    };
+    // GEMM2 of a sub-tile: dW += G_hi X_hi + G_lo X_hi + G_hi X_lo   [64 slots x dpad per warpgroup],
+    // one batch with every A fragment formed beforehand
+    auto gemm2 = [&](const uint32_t (&ahi)[2][4], const uint32_t (&alo)[2][4], uint32_t stage, bool three) {
+      if constexpr (IS_FIT) {
+        const uint64_t bm = desc_mn + (uint64_t)((stage * SM::STAGE) >> 4);
+        const uint64_t bh0 = bm, bh1 = bm + (uint64_t)((16 * 128) >> 4);
+        wgmma_grad<NCHUNK>(grad, ahi[0], bh0);
+        if (three) wgmma_grad<NCHUNK>(grad, alo[0], bh0);
+        wgmma_grad<NCHUNK>(grad, ahi[0], bh0 + XL_OFF);
+        wgmma_grad<NCHUNK>(grad, ahi[1], bh1);
+        if (three) wgmma_grad<NCHUNK>(grad, alo[1], bh1);
+        wgmma_grad<NCHUNK>(grad, ahi[1], bh1 + XL_OFF);
+        wgmma_commit();
+      }
+    };
+    // Fit modes keep GEMM2 of sub-tile j - 1 in flight through the epilogue of sub-tile j: one turn
+    // issues GEMM1 of j, then GEMM2 of j - 1 (A fragments and stage of j - 1 held in pa / pl / psl);
+    // wgmma_wait_one waits for GEMM1 only.  The stage of j - 1 is released after the epilogue of j,
+    // and the last GEMM2 of an item is issued in one more turn after the loop.
+    uint32_t pa[2][4], pl[2][4], psl = 0;
     for (int j = 0; j < nsub; ++j) {
       const uint32_t hh = h + j, sl = hh % NS, ph = (hh / NS) & 1;
-      const int r0 = sub_row0(j);
-      // per-row data of this thread's 8 rows (columns of the Z fragment), loaded before the wait
+      const int r0 = sub_row0(it, j);
+      mbar_wait(&bars->full[sl], ph, 210);
+
+      float zf[16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) zf[i] = 0.f;
+      const uint32_t slu = __shfl_sync(0xffffffffu, sl, 0);   // warp-uniform copy: uniform-register descriptors
+      reg_fence(zf);
+      reg_fence(grad);
+      turn_begin();
+      // straight-line issue in every branch (no control flow between a wgmma_fence and its products,
+      // so ptxas needs no warpgroup.arrive between the instructions)
+      if (IS_FIT && j > 0) {
+        if (g3) { wgmma_fence(); gemm1(zf, slu); gemm2(pa, pl, psl, true); }
+        else { wgmma_fence(); gemm1(zf, slu); gemm2(pa, pl, psl, false); }
+      } else {
+        wgmma_fence(); gemm1(zf, slu);
+      }
+      turn_end();
+      // per-row data of this thread's 8 rows (columns of the Z fragment), loaded while GEMM1 runs
       uint32_t rm[8];
       float yv[8];
 #pragma unroll
@@ -420,25 +507,8 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
           if (prm.mbits) mbw[s] = __ldg(prm.mbits + wi);
         }
       }
-      mbar_wait(&bars->full[sl], ph, 210);
-
-      // GEMM1: Z = W_hi X_hi + W_lo X_hi + W_hi X_lo   [64 slots x 32 rows per warpgroup]
-      float zf[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) zf[i] = 0.f;
-      const uint64_t bx = desc_k + (uint64_t)((sl * SM::STAGE) >> 4);
-      reg_fence(zf);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < NCHUNK * 4; ++ks) {
-        const uint32_t aoff = ((ks >> 2) * SM::W_CHUNK + (ks & 3) * 32) >> 4;
-        const uint32_t boff = ((ks >> 2) * SM::X_CHUNK + (ks & 3) * 32) >> 4;
-        wgmma_m64n32_ss(zf, desc_w + aoff, bx + boff, ks > 0 ? 1u : 0u);
-        wgmma_m64n32_ss(zf, desc_w + WL_OFF + aoff, bx + boff, 1u);
-        wgmma_m64n32_ss(zf, desc_w + aoff, bx + XL_OFF + boff, 1u);
-      }
-      wgmma_commit();
-      wgmma_wait_all();
+      if (IS_FIT && j > 0) wgmma_wait_one();
+      else wgmma_wait_all();
       reg_fence(zf);
 
       if constexpr (IS_FIT) {
@@ -491,20 +561,19 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
             alo[ks][q] = pack_f16x2(gv[i] - hf.x, gv[i + 1] - hf.y);
           }
         }
-        // GEMM2: dW += G_hi X_hi + G_lo X_hi + G_hi X_lo   [64 slots x dpad per warpgroup]
-        const uint64_t bm = desc_mn + (uint64_t)((sl * SM::STAGE) >> 4);
-        reg_fence(grad);
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) {
-          const uint64_t bh = bm + (uint64_t)((ks * 16 * 128) >> 4);
-          wgmma_grad<NCHUNK>(grad, ahi[ks], bh);
-          if (prm.g_passes >= 3) wgmma_grad<NCHUNK>(grad, alo[ks], bh);
-          wgmma_grad<NCHUNK>(grad, ahi[ks], bh + XL_OFF);
+        // GEMM2 of j - 1 has completed: release its stage, keep this sub-tile's fragments for the next turn
+        if (j > 0) {
+          wgmma_wait_all();
+          reg_fence(grad);
+          reg_hold(pa);
+          reg_hold(pl);
+          if (wg_leader) mbar_arrive(&bars->empty[psl]);
         }
-        wgmma_commit();
-        wgmma_wait_all();
-        reg_fence(grad);
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) { pa[ks][q] = ahi[ks][q]; pl[ks][q] = alo[ks][q]; }
+        psl = slu;
       } else {
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
@@ -525,12 +594,22 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
           }
           n_all[s] += in ? 1 : 0;
         }
+        if (wg_leader) mbar_arrive(&bars->empty[sl]);
       }
-      if (wg_leader) mbar_arrive(&bars->empty[sl]);
-      if (threadIdx.x == 0 && j + NS < nsub) issue(hh + NS, j + NS);
-      __syncwarp();
     }
     h += nsub;
+    if constexpr (IS_FIT) {   // the item's last GEMM2 (nsub >= 2: empty chunks are skipped)
+      reg_fence(grad);
+      turn_begin();
+      if (g3) { wgmma_fence(); gemm2(pa, pl, psl, true); }
+      else { wgmma_fence(); gemm2(pa, pl, psl, false); }
+      turn_end();
+      wgmma_wait_all();
+      reg_fence(grad);
+      reg_hold(pa);
+      reg_hold(pl);
+      if (wg_leader) mbar_arrive(&bars->empty[psl]);
+    }
 
     // end of item: the four lanes sharing a slot hold partial sums of it; combine them in a fixed
     // order (deterministic) and write this chunk's partial
@@ -576,6 +655,9 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
       }
     }
   }
+  // consumer 1's last hand-over (or its opening one, if there was no work) is still pending on
+  // consumer 0's barrier
+  if (cw == 0) named_bar_sync(1, 256);
 }
 
 // ---------------------------------------------------------------------------------------------

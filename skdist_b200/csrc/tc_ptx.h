@@ -93,14 +93,45 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_b
   return d;
 }
 
+// named barriers (id 0 is __syncthreads): `count` threads in all, counted per arriving thread
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+// per-warpgroup register budget of a warp-specialised kernel (every warp of the warpgroup executes it)
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// descriptor + offset (16-byte units): the start address field (bits 0-13) holds every shared-memory
+// address below 256 KB, so the sum never carries out of the low word
+__device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t off) {
+  return (d & 0xFFFFFFFF00000000ull) | (uint32_t)((uint32_t)d + off);
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// every committed group but the newest has completed
+__device__ __forceinline__ void wgmma_wait_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 // keeps the compiler from moving accesses to accumulator registers across wgmma_commit / wgmma_wait_all
 template <int N>
 __device__ __forceinline__ void reg_fence(float (&d)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// the A fragments of an in-flight wgmma: call after its wait, so that the compiler keeps them in their
+// registers until then (their last use in the program is the wgmma, which reads them asynchronously)
+template <int M, int N>
+__device__ __forceinline__ void reg_hold(uint32_t (&a)[M][N]) {
+#pragma unroll
+  for (int i = 0; i < M; ++i)
+#pragma unroll
+    for (int j = 0; j < N; ++j) asm volatile("" : "+r"(a[i][j])::"memory");
 }
 
 // D[64 x 32] (+)= A[smem, K-major] * B[smem, K-major]^T, fp16 in, fp32 accumulators in registers
