@@ -8,28 +8,23 @@
 //
 // SGD is sequential in the samples but independent across label columns, and every column
 // sees the same shuffled sample order (same seed).  One WARP owns one column: its d float32
-// weights live in registers (d/32 per lane) for the whole epoch, the warp walks the shuffled
-// rows (next row prefetched while the current one is processed), and reproduces the reference's
-// arithmetic operation by operation -- float32 products accumulated in float64, float32 lazy
-// scale `wscale`, float64 intercept / objective, weight update w = float(double(w) + double(x)*q)
-// -- so hinge-loss fits are bit-identical to scikit-learn.  No tensor cores: the work per sample
-// is two length-d vector operations per column, bound by the FP64 pipe and L2 latency.
+// weights live in registers (d/32 per lane) for the whole epoch and the warp walks the shuffled
+// rows, reproducing the reference's arithmetic operation by operation (sgd_replay.h), so fits are
+// bit-identical to scikit-learn.  No tensor cores: the work per sample is two length-d vector
+// operations per column, bound by the FP64 pipe and L2 latency.  Large hinge problems run their
+// epochs on the tensor cores instead (sgd_tc.cu); sgd_fit_batch below drives both.
 #include <math.h>
 #include <stdio.h>
 
 #include <chrono>
+#include <memory>
 #include <stdlib.h>
 
-#include "skd_internal.h"
+#include "sgd_replay.h"
 
 namespace skd {
 
-struct SgdState {
-  double wscale, sq_norm, intercept, best_objective, t;
-  int32_t no_improve, done, n_iter, status;
-};
-
-enum { SGD_HINGE = 0, SGD_LOG = 1 };
+enum { SGD_HINGE = 0 };
 
 // per-sample learning rate and weight-decay factor of one epoch (class independent)
 __global__ void sgd_schedule_kernel(int64_t n, double t0, double alpha, double optimal_init,
@@ -46,13 +41,8 @@ __global__ void sgd_schedule_kernel(int64_t n, double t0, double alpha, double o
   cfac[i] = (float)fmax(0.0, __dsub_rn(1.0, __dmul_rn(e, alpha)));  // w.scale(max(0, 1 - eta*alpha)) arg as float
 }
 
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-template <int DPL, int LOSS>
+// log_loss, one sample at a time
+template <int DPL>
 __global__ void __launch_bounds__(128)
 sgd_epoch_kernel(const float* __restrict__ X, int ldx, int d, const int32_t* __restrict__ ycls,
                  const int32_t* __restrict__ order, const double* __restrict__ eta,
@@ -92,7 +82,7 @@ sgd_epoch_kernel(const float* __restrict__ X, int ldx, int d, const int32_t* __r
     float x[DPL];
 #pragma unroll
     for (int j = 0; j < DPL; ++j) x[j] = xn[j];
-    const double y = (yc_n == pos) ? 1.0 : -1.0;
+    const double y01 = (yc_n == pos) ? 1.0 : 0.0;
     const double e = e_n;
     const float c = c_n;
     if (i + 1 < n) {
@@ -113,26 +103,19 @@ sgd_epoch_kernel(const float* __restrict__ X, int ldx, int d, const int32_t* __r
     for (int j = 0; j < DPL; ++j) acc += (double)__fmul_rn(w[j], x[j]);
     acc = warp_sum(acc);
     const double p = (double)(float)(acc * wscale) + intercept;
-    // loss / gradient
-    double cur_loss, dloss;
-    if (LOSS == SGD_HINGE) {       // Hinge on y in {-1,+1} (SK/linear_model/_sgd_fast.pyx.tp:131-146)
-      const double z = p * y;
-      if (z <= 1.0) { cur_loss = 1.0 - z; dloss = -y; } else { cur_loss = 0.0; dloss = 0.0; }
-    } else {                       // CyHalfBinomialLoss on y in {0,1} (SK/_loss/_loss.pyx.tp:256-266,686-725)
-      const double y01 = y > 0.0 ? 1.0 : 0.0;
-      double l1p;
-      if (p <= -37.0) l1p = exp(p);
-      else if (p <= -2.0) l1p = log1p(exp(p));
-      else if (p <= 18.0) l1p = log(__dadd_rn(1.0, exp(p)));
-      else if (p <= 33.3) l1p = __dadd_rn(p, exp(-p));
-      else l1p = p;
-      cur_loss = __dsub_rn(l1p, __dmul_rn(y01, p));
-      if (p > -37.0) {
-        const double et = exp(-p);
-        dloss = __ddiv_rn(__dsub_rn(1.0 - y01, __dmul_rn(y01, et)), __dadd_rn(1.0, et));
-      } else {
-        dloss = __dsub_rn(exp(p), y01);
-      }
+    // CyHalfBinomialLoss on y in {0,1} (SK/_loss/_loss.pyx.tp:256-266,686-725)
+    double l1p, dloss;
+    if (p <= -37.0) l1p = exp(p);
+    else if (p <= -2.0) l1p = log1p(exp(p));
+    else if (p <= 18.0) l1p = log(__dadd_rn(1.0, exp(p)));
+    else if (p <= 33.3) l1p = __dadd_rn(p, exp(-p));
+    else l1p = p;
+    const double cur_loss = __dsub_rn(l1p, __dmul_rn(y01, p));
+    if (p > -37.0) {
+      const double et = exp(-p);
+      dloss = __ddiv_rn(__dsub_rn(1.0 - y01, __dmul_rn(y01, et)), __dadd_rn(1.0, et));
+    } else {
+      dloss = __dsub_rn(exp(p), y01);
     }
     const float normf = (float)sqrt(sq_norm);
     objective_sum = __dadd_rn(objective_sum,
@@ -142,49 +125,23 @@ sgd_epoch_kernel(const float* __restrict__ X, int ldx, int d, const int32_t* __r
     // w.scale(c)
     wscale *= (double)c;
     sq_norm *= (double)__fmul_rn(c, c);
-    if (wscale < 1e-6) {          // reset_wscale(): sscal by float(wscale)
-      const float wf = (float)wscale;
-#pragma unroll
-      for (int j = 0; j < DPL; ++j) w[j] = __fmul_rn(w[j], wf);
+    if (wscale < 1e-6) {
+      sgd_reset_wscale<DPL>(w, wscale);
       wscale = 1.0;
     }
-    if (update != 0.0) {           // w.add(x, update)
-      const float cf = (float)update, wsf = (float)wscale;
-      const double q = (double)__fdiv_rn(cf, wsf);
-      double acc2 = 0.0;
-#pragma unroll
-      for (int j = 0; j < DPL; ++j) {
-        w[j] = (float)fma((double)x[j], q, (double)w[j]);
-        acc2 += (double)__fmul_rn(w[j], w[j]);
-      }
-      acc2 = warp_sum(acc2);
-      sq_norm = acc2 * (double)__fmul_rn(wsf, wsf);
-      if (fit_intercept) intercept += update;
+    if (update != 0.0) {
+      double q;
+      sq_norm = sgd_add<DPL>(w, x, update, wscale, fit_intercept, intercept, q);
     }
   }
-  // end of epoch (SK/linear_model/_sgd_fast.pyx.tp:570-628)
-  bool finite = isfinite(intercept);
-#pragma unroll
-  for (int j = 0; j < DPL; ++j) finite = finite && isfinite(w[j]);
-  finite = __all_sync(0xffffffffu, finite);
 #pragma unroll
   for (int j = 0; j < DPL; ++j) {
     const int k = lane + 32 * j;
     if (k < d) W[(size_t)col * ldw + k] = w[j];
   }
-  if (lane == 0) {
-    st.wscale = wscale; st.sq_norm = sq_norm; st.intercept = intercept;
-    st.t += (double)n;
-    st.n_iter += 1;
-    if (!finite) { st.done = 1; st.status = 5; }
-    else {
-      const double obj = objective_sum / (double)n;
-      if (tol > -INFINITY && obj > st.best_objective - tol) st.no_improve += 1; else st.no_improve = 0;
-      if (obj < st.best_objective) st.best_objective = obj;
-      if (st.no_improve >= n_iter_no_change) { st.done = 1; st.status = 1; }
-    }
-    state[col] = st;
-  }
+  st.wscale = wscale; st.sq_norm = sq_norm; st.intercept = intercept;
+  sgd_end_epoch<DPL>(st, w, intercept, objective_sum, n, tol, n_iter_no_change);
+  if (lane == 0) state[col] = st;
 }
 
 // Hinge loss, speculative blocks.  With hinge loss a sample whose margin y*p exceeds 1 changes
@@ -192,9 +149,9 @@ sgd_epoch_kernel(const float* __restrict__ X, int ldx, int d, const int32_t* __r
 // computes the dot products of the next T = 16 samples against the CURRENT weights at once
 // (independent FMAs, all loads in flight together), reduces them with a butterfly, and then walks
 // the 16 samples in order doing only the scalar recurrence; the first margin violator (or a
-// reset_wscale) applies its weight update exactly as the sequential kernel does and the block
-// restarts behind it.  Every value is computed by the same operations in the same order as in
-// sgd_epoch_kernel, so the result stays bit-identical to scikit-learn; only the waiting changes.
+// reset_wscale) applies its weight update exactly as _plain_sgd32 does and the block restarts
+// behind it.  Every value is computed by the same operations in the same order as one sample at a
+// time, so the result stays bit-identical to scikit-learn; only the waiting changes.
 template <int DPL>
 __global__ void __launch_bounds__(128)
 sgd_epoch_spec_kernel(const float* __restrict__ X, int ldx, int d, const int32_t* __restrict__ ycls,
@@ -285,7 +242,7 @@ sgd_epoch_spec_kernel(const float* __restrict__ X, int ldx, int d, const int32_t
     //  B. lane t evaluates sample t: prediction, margin, loss and objective term;
     //  C. the first event (margin violator or reset_wscale) is found with one ballot;
     //  D. the objective terms of samples 0..event are added in order;
-    //  E. the event's weight update is applied exactly as in the sequential kernel.
+    //  E. the event's weight update is applied exactly as one sample at a time.
     float c_all[T];
 #pragma unroll
     for (int q = 0; q < T; ++q) c_all[q] = __shfl_sync(FULL, c_l, q);
@@ -325,60 +282,38 @@ sgd_epoch_spec_kernel(const float* __restrict__ X, int ldx, int d, const int32_t
     if (ev >= 0) {
       const bool is_reset = (evmask >> ev) & 1u ? __shfl_sync(FULL, (int)reset_l, ev) != 0 : false;
       const bool is_viol = __shfl_sync(FULL, (int)viol_l, ev) != 0;
-      if (is_reset) {                 // reset_wscale(): sscal by float(wscale)
-        const float wf = (float)wscale;
-#pragma unroll
-        for (int j2 = 0; j2 < DPL; ++j2) w[j2] = __fmul_rn(w[j2], wf);
+      if (is_reset) {
+        sgd_reset_wscale<DPL>(w, wscale);
         wscale = 1.0;
       }
       if (is_viol) {
         const double y = __shfl_sync(FULL, y_l, ev);
         const double e = __shfl_sync(FULL, e_l, ev);
         const double update = -e * (-y);
-        if (update != 0.0) {           // w.add(x, update)
+        if (update != 0.0) {
           const int r = __shfl_sync(FULL, row_l, ev);
-          const float cf = (float)update, wsf = (float)wscale;
-          const double qd = (double)__fdiv_rn(cf, wsf);
-          double acc2 = 0.0;
+          float x[DPL];
 #pragma unroll
           for (int j2 = 0; j2 < DPL; ++j2) {
             const int k = lane + 32 * j2;
-            const float xv = k < ldx ? __ldg(X + (size_t)r * ldx + k) : 0.f;
-            w[j2] = (float)fma((double)xv, qd, (double)w[j2]);
-            acc2 += (double)__fmul_rn(w[j2], w[j2]);
+            x[j2] = k < ldx ? __ldg(X + (size_t)r * ldx + k) : 0.f;
           }
-          acc2 = warp_sum(acc2);
-          sq_norm = acc2 * (double)__fmul_rn(wsf, wsf);
-          if (fit_intercept) intercept += update;
+          double q;
+          sq_norm = sgd_add<DPL>(w, x, update, wscale, fit_intercept, intercept, q);
         }
       }
     }
     const int t = last + 1;
     i0 += t;
   }
-  // end of epoch (SK/linear_model/_sgd_fast.pyx.tp:570-628)
-  bool finite = isfinite(intercept);
-#pragma unroll
-  for (int j = 0; j < DPL; ++j) finite = finite && isfinite(w[j]);
-  finite = __all_sync(FULL, finite);
 #pragma unroll
   for (int j = 0; j < DPL; ++j) {
     const int k = lane + 32 * j;
     if (k < d) W[(size_t)col * ldw + k] = w[j];
   }
-  if (lane == 0) {
-    st.wscale = wscale; st.sq_norm = sq_norm; st.intercept = intercept;
-    st.t += (double)n;
-    st.n_iter += 1;
-    if (!finite) { st.done = 1; st.status = 5; }
-    else {
-      const double obj = objective_sum / (double)n;
-      if (tol > -INFINITY && obj > st.best_objective - tol) st.no_improve += 1; else st.no_improve = 0;
-      if (obj < st.best_objective) st.best_objective = obj;
-      if (st.no_improve >= n_iter_no_change) { st.done = 1; st.status = 1; }
-    }
-    state[col] = st;
-  }
+  st.wscale = wscale; st.sq_norm = sq_norm; st.intercept = intercept;
+  sgd_end_epoch<DPL>(st, w, intercept, objective_sum, n, tol, n_iter_no_change);
+  if (lane == 0) state[col] = st;
 }
 
 // w.reset_wscale() at the end of _plain_sgd, then export
@@ -406,28 +341,32 @@ static inline uint32_t xorshift_rand_r(uint32_t* seed) {   // SK/utils/_random.p
   return *seed % ((uint32_t)2147483647 + 1);
 }
 
-template <int LOSS>
-static cudaError_t launch_epoch(int dpl, int grid, cudaStream_t st, const float* X, int ldx, int d,
-                                const int32_t* ycls, const int32_t* order, const double* eta,
-                                const float* cfac, int64_t n, const int32_t* active, int n_active,
-                                const int32_t* col_pos, float* W, int ldw, SgdState* state, double alpha,
-                                int fit_intercept, double tol, int nnc) {
-  // SKDIST_B200_SGD_SPEC=0 falls back to the one-sample-at-a-time kernel (A/B timing)
-  static const bool spec = !(getenv("SKDIST_B200_SGD_SPEC") && getenv("SKDIST_B200_SGD_SPEC")[0] == '0');
+// Fisher-Yates with the SAME seed every epoch, applied to the evolving order (SK/utils/_seq_dataset.pyx.tp:137-145)
+static void sgd_shuffle(std::vector<int32_t>& order, uint32_t seed) {
+  const int64_t n = (int64_t)order.size();
+  for (int64_t i = 0; i < n - 1; ++i) {
+    int64_t j = i + xorshift_rand_r(&seed) % (uint32_t)(n - i);
+    std::swap(order[i], order[j]);
+  }
+}
+
+// one epoch on the warp-per-column kernels: speculative blocks for hinge, one sample at a time for log_loss
+static cudaError_t launch_epoch(Ctx* c, const SgdFit& f, int loss, int n_active) {
+  const int grid = (n_active + 3) / 4;
+#define SGD_ARGS                                                                                          \
+  c->X, (int)c->ldx, (int)c->d, c->ycls, f.order, f.eta, f.cfac, c->n, f.active, n_active, f.col_pos, f.W, f.ldw, \
+      f.state, f.alpha, f.fit_intercept, f.tol, f.n_iter_no_change
 #define SGD_CASE(D)                                                                                       \
   case D:                                                                                                 \
-    if (LOSS == SGD_HINGE && spec)                                                                        \
-      sgd_epoch_spec_kernel<D><<<grid, 128, 0, st>>>(X, ldx, d, ycls, order, eta, cfac, n, active, n_active, \
-                                                     col_pos, W, ldw, state, alpha, fit_intercept, tol, nnc); \
-    else                                                                                                  \
-      sgd_epoch_kernel<D, LOSS><<<grid, 128, 0, st>>>(X, ldx, d, ycls, order, eta, cfac, n, active, n_active, \
-                                                      col_pos, W, ldw, state, alpha, fit_intercept, tol, nnc); \
+    if (loss == SGD_HINGE) sgd_epoch_spec_kernel<D><<<grid, 128, 0, c->stream>>>(SGD_ARGS);              \
+    else sgd_epoch_kernel<D><<<grid, 128, 0, c->stream>>>(SGD_ARGS);                                     \
     break;
-  switch (dpl) {
+  switch (f.dpl) {
     SGD_CASE(1) SGD_CASE(2) SGD_CASE(4) SGD_CASE(8) SGD_CASE(16) SGD_CASE(32)
     default: return cudaErrorInvalidValue;
   }
 #undef SGD_CASE
+#undef SGD_ARGS
   return cudaGetLastError();
 }
 
@@ -436,18 +375,18 @@ int sgd_fit_batch(Ctx* c, int B, const int32_t* col_pos, int loss, double alpha,
                   double power_t, double optimal_init, int n_iter_no_change, float* coef_out,
                   double* intercept_out, int32_t* n_iter_out, double* t_out, int32_t* status_out) {
   const int64_t n = c->n;
-  const int d = (int)c->d, ldx = (int)c->ldx;
+  const int d = (int)c->d;
   if (d > 1024) return fail(c, "sgd: device path supports d <= 1024");
-  if (sgd_tc_supported(c, loss, shuffle))     // hinge: blocked-exact on the tensor cores (sgd_tc.cu), same results
-    return sgd_fit_batch_tc(c, B, col_pos, alpha, fit_intercept, max_iter, tol, shuffle, seed, lr_type, eta0, power_t,
-                            optimal_init, n_iter_no_change, coef_out, intercept_out, n_iter_out, t_out, status_out);
-  int dpl = 1;
-  while (dpl * 32 < d) dpl *= 2;
-  const int ldw = dpl * 32;
+  SgdFit f;
+  f.B = B;
+  f.dpl = 1;
+  while (f.dpl * 32 < d) f.dpl *= 2;
+  f.ldw = f.dpl * 32;
+  f.alpha = alpha; f.tol = tol; f.fit_intercept = fit_intercept; f.n_iter_no_change = n_iter_no_change;
   Scratch sx(c);
   float* W; SgdState* state; int32_t *order, *active, *dpos; double* eta; float* cfac;
   float* dcoef; double *dint, *dt; int32_t *dniter, *dstatus;
-  SKD_CUDA(c, sx.alloc(&W, (size_t)B * ldw));
+  SKD_CUDA(c, sx.alloc(&W, (size_t)B * f.ldw));
   SKD_CUDA(c, sx.alloc(&state, (size_t)B));
   SKD_CUDA(c, sx.alloc(&order, (size_t)n));
   SKD_CUDA(c, sx.alloc(&active, (size_t)B));
@@ -459,12 +398,18 @@ int sgd_fit_batch(Ctx* c, int B, const int32_t* col_pos, int loss, double alpha,
   SKD_CUDA(c, sx.alloc(&dt, (size_t)B));
   SKD_CUDA(c, sx.alloc(&dniter, (size_t)B));
   SKD_CUDA(c, sx.alloc(&dstatus, (size_t)B));
-  SKD_CUDA(c, cudaMemsetAsync(W, 0, (size_t)B * ldw * sizeof(float), c->stream));
+  f.W = W; f.state = state; f.col_pos = dpos; f.order = order; f.active = active; f.eta = eta; f.cfac = cfac;
+  SKD_CUDA(c, cudaMemsetAsync(W, 0, (size_t)B * f.ldw * sizeof(float), c->stream));
   std::vector<SgdState> hs(B);
   for (auto& s : hs) { s.wscale = 1.0; s.sq_norm = 0.0; s.intercept = 0.0; s.best_objective = INFINITY; s.t = 1.0;
-                       s.no_improve = 0; s.done = 0; s.n_iter = 0; s.status = 3; }
+                       s.no_improve = 0; s.done = 0; s.n_iter = 0; s.status = 3; s.objective_sum = 0.0; }
   SKD_CUDA(c, cudaMemcpyAsync(state, hs.data(), (size_t)B * sizeof(SgdState), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(dpos, col_pos, (size_t)B * 4, cudaMemcpyHostToDevice, c->stream));
+  std::unique_ptr<SgdTc> tc;
+  if (sgd_tc_supported(c, loss, shuffle)) {   // hinge: blocked-exact on the tensor cores, same results
+    tc.reset(new SgdTc(c));
+    if (tc->init(c, f)) return 1;
+  }
   std::vector<int32_t> hact(B), hord(n);
   for (int j = 0; j < B; ++j) hact[j] = j;
   for (int64_t i = 0; i < n; ++i) hord[i] = (int32_t)i;
@@ -473,41 +418,38 @@ int sgd_fit_batch(Ctx* c, int B, const int32_t* col_pos, int loss, double alpha,
   const bool trace = trace_env && trace_env[0] == '2';
   for (int epoch = 0; epoch < max_iter && n_active > 0; ++epoch) {
     auto tw0 = std::chrono::steady_clock::now();
-    if (shuffle) {   // Fisher-Yates with the SAME seed every epoch, applied to the evolving order
-      uint32_t s = seed;
-      for (int64_t i = 0; i < n - 1; ++i) {
-        int64_t j = i + xorshift_rand_r(&s) % (uint32_t)(n - i);
-        std::swap(hord[i], hord[j]);
-      }
-    }
-    if (shuffle || epoch == 0)
+    if (shuffle) sgd_shuffle(hord, seed);
+    const bool new_order = shuffle || epoch == 0;
+    if (new_order)
       SKD_CUDA(c, cudaMemcpyAsync(order, hord.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaMemcpyAsync(active, hact.data(), (size_t)n_active * 4, cudaMemcpyHostToDevice, c->stream));
     auto tw1 = std::chrono::steady_clock::now();
     const double t0 = 1.0 + (double)epoch * (double)n;
     sgd_schedule_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(n, t0, alpha, optimal_init, lr_type, eta0,
                                                                            power_t, eta, cfac);
-    cudaError_t e = loss == SGD_HINGE
-        ? launch_epoch<SGD_HINGE>(dpl, (n_active + 3) / 4, c->stream, c->X, ldx, d, c->ycls, order, eta, cfac, n, active,
-                                  n_active, dpos, W, ldw, state, alpha, fit_intercept, tol, n_iter_no_change)
-        : launch_epoch<SGD_LOG>(dpl, (n_active + 3) / 4, c->stream, c->X, ldx, d, c->ycls, order, eta, cfac, n, active,
-                                n_active, dpos, W, ldw, state, alpha, fit_intercept, tol, n_iter_no_change);
-    c->launches += 2;
-    if (e != cudaSuccess) return fail(c, std::string("sgd epoch launch: ") + cudaGetErrorString(e));
+    c->launches += 1;
+    if (tc) {
+      if (tc->epoch(c, f, epoch, n_active, new_order, trace)) return 1;
+    } else {
+      cudaError_t e = launch_epoch(c, f, loss, n_active);
+      c->launches += 1;
+      if (e != cudaSuccess) return fail(c, std::string("sgd epoch launch: ") + cudaGetErrorString(e));
+    }
     SKD_CUDA(c, cudaMemcpyAsync(hs.data(), state, (size_t)B * sizeof(SgdState), cudaMemcpyDeviceToHost, c->stream));
     SKD_CUDA(c, cudaStreamSynchronize(c->stream));
     c->h2d += n * 4; c->d2h += (int64_t)B * sizeof(SgdState);
     if (trace) {
       auto tw2 = std::chrono::steady_clock::now();
-      fprintf(stderr, "[skd trace] sgd epoch %3d active %5d host shuffle %7.2f ms device %8.2f ms\n", epoch, n_active,
-              std::chrono::duration<double, std::milli>(tw1 - tw0).count(),
+      fprintf(stderr, "[skd trace] %s epoch %3d active %5d host shuffle %7.2f ms device %8.2f ms\n", tc ? "sgd-tc" : "sgd",
+              epoch, n_active, std::chrono::duration<double, std::milli>(tw1 - tw0).count(),
               std::chrono::duration<double, std::milli>(tw2 - tw1).count());
     }
     n_active = 0;
     for (int j = 0; j < B; ++j)
       if (!hs[j].done) hact[n_active++] = j;
   }
-  sgd_finish_kernel<<<B, 128, 0, c->stream>>>(W, ldw, d, state, B, dcoef, dint, dniter, dt, dstatus);
+  if (tc && trace) tc->print_counters();
+  sgd_finish_kernel<<<B, 128, 0, c->stream>>>(W, f.ldw, d, state, B, dcoef, dint, dniter, dt, dstatus);
   c->launches += 1;
   SKD_CUDA(c, cudaGetLastError());
   SKD_CUDA(c, cudaMemcpyAsync(coef_out, dcoef, (size_t)B * d * 4, cudaMemcpyDeviceToHost, c->stream));

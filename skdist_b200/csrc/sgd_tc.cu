@@ -21,25 +21,19 @@
 // other sample gets the exact float32-product / float64-sum dot product of sgd.cu, and every
 // update is applied exactly as `_plain_sgd32` does.  Scalar recurrences (float64 norm and objective
 // in sample order) are kept operation for operation.  Hence identical coefficients, intercepts and
-// n_iter_, at tensor-core cost for 99 % of the samples.
+// n_iter_, at tensor-core cost for 99 % of the samples.  sgd_fit_batch (sgd.cu) runs the fit and
+// hands each epoch to SgdTc::epoch.
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
-#include <chrono>
 
-#include "skd_internal.h"
+#include "sgd_replay.h"
 #include "tc_ptx.h"
 
 namespace skd {
-
-struct SgdStateTc {            // sgd.cu's SgdState + the running objective of the current epoch
-  double wscale, sq_norm, intercept, best_objective, t;
-  int32_t no_improve, done, n_iter, status;
-  double objective_sum;
-};
 
 constexpr int ST_T = 2048;           // samples per block
 constexpr int ST_TILE = 128;
@@ -223,12 +217,6 @@ sgd_export_kernel(const float* __restrict__ W, int ldw, int d, int dpad, const i
   sgd_export_row<DPL>(w, lane, d, dpad, inv_sx, Wp + (size_t)a * dpad, wmeta + a);
 }
 
-__device__ __forceinline__ double sgd_warp_sum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // ------------------------------------------------------------------------------------------
 // ordered walk over one block of T samples, one warp per label column
 // ------------------------------------------------------------------------------------------
@@ -241,7 +229,7 @@ struct SgdScanParams {
   int64_t n; int row0, t_len;
   const int32_t* active; int n_active; const int32_t* col_pos;
   float* W; int ldw;
-  SgdStateTc* state;
+  SgdState* state;
   const float* S; const float* G; const float2* wmeta;
   __half* Wp; float2* wmeta_out;
   float inv_sx, inv_sx2;
@@ -262,7 +250,7 @@ sgd_scan_kernel(const SgdScanParams P) {
   if (a >= P.n_active) return;
   const int col = P.active[a];
   const int pos = P.col_pos[col];
-  SgdStateTc st = P.state[col];
+  SgdState st = P.state[col];
   float w[DPL];
 #pragma unroll
   for (int j = 0; j < DPL; ++j) {
@@ -365,7 +353,6 @@ sgd_scan_kernel(const SgdScanParams P) {
       const double y = __shfl_sync(FULL, y_l, ev);
       const double e = __shfl_sync(FULL, e_l, ev);
       const double wsb = __shfl_sync(FULL, ws_l, ev);
-      const double sqb = __shfl_sync(FULL, my_sq, ev);
       const double l2t = __shfl_sync(FULL, l2_l, ev);
       const float nxe = __shfl_sync(FULL, nx_l, ev);
       const bool is_cand = __shfl_sync(FULL, (int)cand_l, ev) != 0;
@@ -380,37 +367,25 @@ sgd_scan_kernel(const SgdScanParams P) {
       double acc = 0.0;
 #pragma unroll
       for (int j = 0; j < DPL; ++j) acc += (double)__fmul_rn(w[j], x[j]);
-      acc = sgd_warp_sum(acc);
+      acc = warp_sum(acc);
       const double p = (double)(float)(acc * wsb) + intercept;
       const double z = p * y;
       // (a sample that is only a reset event cleared the margin test: its exact margin is above 1 as well)
       const bool viol = is_cand && z <= 1.0;
       const double cur_loss = viol ? 1.0 - z : 0.0;
       objective_sum = __dadd_rn(objective_sum, __dadd_rn(cur_loss, l2t));
-      (void)sqb;
       sq_norm = __shfl_sync(FULL, my_sq_after, ev);          // w.scale(c): sq_norm *= c^2
       n_exact += 1;
-      if (is_reset) {                                          // w.reset_wscale(): sscal by float(wscale), wscale = 1
-        const float wf = (float)ws_reset;
-#pragma unroll
-        for (int j = 0; j < DPL; ++j) w[j] = __fmul_rn(w[j], wf);
+      if (is_reset) {
+        sgd_reset_wscale<DPL>(w, ws_reset);                   // the host's chain continues from wscale = 1
         exact_all = true;                                      // the block's products were taken with the old weights
       }
       if (viol) {
         const double update = -e * (-y);
-        if (update != 0.0) {                                   // w.add(x, update)
+        if (update != 0.0) {
           const double wsa = P.ws[(int64_t)P.row0 + i0 + ev + 1];   // wscale after this sample's scale step
-          const float cf = (float)update, wsf = (float)wsa;
-          const double qd = (double)__fdiv_rn(cf, wsf);
-          double acc2 = 0.0;
-#pragma unroll
-          for (int j = 0; j < DPL; ++j) {
-            w[j] = (float)fma((double)x[j], qd, (double)w[j]);
-            acc2 += (double)__fmul_rn(w[j], w[j]);
-          }
-          acc2 = sgd_warp_sum(acc2);
-          sq_norm = acc2 * (double)__fmul_rn(wsf, wsf);
-          if (P.fit_intercept) intercept += update;
+          double qd;
+          sq_norm = sgd_add<DPL>(w, x, update, wsa, P.fit_intercept, intercept, qd);
           n_viol += 1;
           // log the update for the margins of the samples still to come in this block
           if (nviol < ST_VMAX) {
@@ -432,30 +407,14 @@ sgd_scan_kernel(const SgdScanParams P) {
     const int k = lane + 32 * j;
     if (k < P.d) P.W[(size_t)col * P.ldw + k] = w[j];
   }
-  bool finite = true;
+  st.sq_norm = sq_norm; st.intercept = intercept; st.objective_sum = objective_sum;
   if (P.last_block) {
-    finite = isfinite(intercept);
-#pragma unroll
-    for (int j = 0; j < DPL; ++j) finite = finite && isfinite(w[j]);
-    finite = __all_sync(FULL, finite);
+    st.wscale = P.ws[P.n];
+    sgd_end_epoch<DPL>(st, w, intercept, objective_sum, P.n, P.tol, P.n_iter_no_change);
   } else {
     sgd_export_row<DPL>(w, lane, P.d, P.dpad, P.inv_sx, P.Wp + (size_t)a * P.dpad, P.wmeta_out + a);
   }
   if (lane == 0) {
-    st.sq_norm = sq_norm; st.intercept = intercept; st.objective_sum = objective_sum;
-    if (P.last_block) {      // end of epoch (SK/linear_model/_sgd_fast.pyx.tp:570-628)
-      st.wscale = P.ws[P.n];
-      st.t += (double)P.n;
-      st.n_iter += 1;
-      if (!finite) { st.done = 1; st.status = 5; }
-      else {
-        const double obj = objective_sum / (double)P.n;
-        if (P.tol > -INFINITY && obj > st.best_objective - P.tol) st.no_improve += 1; else st.no_improve = 0;
-        if (obj < st.best_objective) st.best_objective = obj;
-        if (st.no_improve >= P.n_iter_no_change) { st.done = 1; st.status = 1; }
-      }
-      st.objective_sum = 0.0;
-    }
     P.state[col] = st;
     if (P.counters) {
       atomicAdd(&P.counters[0], n_screen);
@@ -463,44 +422,6 @@ sgd_scan_kernel(const SgdScanParams P) {
       atomicAdd(&P.counters[2], n_viol);
     }
   }
-}
-
-__global__ void sgd_tc_finish_kernel(const float* __restrict__ W, int ldw, int d, const SgdStateTc* __restrict__ state,
-                                     int B, float* __restrict__ coef, double* __restrict__ intercept,
-                                     int32_t* __restrict__ n_iter, double* __restrict__ t_out,
-                                     int32_t* __restrict__ status) {
-  const int col = blockIdx.x;
-  if (col >= B) return;
-  const float wf = (float)state[col].wscale;      // w.reset_wscale() at the end of _plain_sgd
-  for (int k = threadIdx.x; k < d; k += blockDim.x) coef[(size_t)col * d + k] = __fmul_rn(W[(size_t)col * ldw + k], wf);
-  if (threadIdx.x == 0) {
-    intercept[col] = state[col].intercept;
-    n_iter[col] = state[col].n_iter;
-    t_out[col] = state[col].t;
-    status[col] = state[col].status;
-  }
-}
-
-// per-sample learning rate and weight-decay factor of one epoch (class independent; as in sgd.cu)
-__global__ void sgd_tc_schedule_kernel(int64_t n, double t0, double alpha, double optimal_init, int lr_type, double eta0,
-                                       double power_t, double* __restrict__ eta, float* __restrict__ cfac) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const double t = t0 + (double)i;
-  double e;
-  if (lr_type == 0) e = 1.0 / (alpha * (optimal_init + t - 1.0));   // "optimal"
-  else if (lr_type == 1) e = eta0;                                   // "constant"
-  else e = eta0 / pow(t, power_t);                                   // "invscaling"
-  eta[i] = e;
-  cfac[i] = (float)fmax(0.0, __dsub_rn(1.0, __dmul_rn(e, alpha)));  // w.scale(max(0, 1 - eta*alpha)) arg as float
-}
-
-static inline uint32_t tc_xorshift_rand_r(uint32_t* seed) {   // SK/utils/_random.pxd:20-34
-  if (*seed == 0) *seed = 1;
-  *seed ^= (uint32_t)(*seed << 13);
-  *seed ^= (uint32_t)(*seed >> 17);
-  *seed ^= (uint32_t)(*seed << 5);
-  return *seed % ((uint32_t)2147483647 + 1);
 }
 
 bool sgd_tc_supported(const Ctx* c, int loss, int shuffle) {
@@ -514,38 +435,17 @@ bool sgd_tc_supported(const Ctx* c, int loss, int shuffle) {
   return c->n >= 2 * ST_T;                              // small problems stay on the warp-per-column kernel
 }
 
-int sgd_fit_batch_tc(Ctx* c, int B, const int32_t* col_pos, double alpha, int fit_intercept, int max_iter, double tol,
-                     int shuffle, uint32_t seed, int lr_type, double eta0, double power_t, double optimal_init,
-                     int n_iter_no_change, float* coef_out, double* intercept_out, int32_t* n_iter_out, double* t_out,
-                     int32_t* status_out) {
+int SgdTc::init(Ctx* c, const SgdFit& f) {
   const int64_t n = c->n;
   const int d = (int)c->d, ldx = (int)c->ldx;
-  int dpl = 1;
-  while (dpl * 32 < d) dpl *= 2;
-  const int ldw = dpl * 32;
-  const int dpad = (d + 63) / 64 * 64;
-  const int64_t npad = (n + ST_T - 1) / ST_T * ST_T;
-  const int kpad = (B + ST_TILE - 1) / ST_TILE * ST_TILE;
-  Scratch sx(c);
-  float* W; SgdStateTc* state; int32_t *order, *active, *dpos, *ycls_p; double *eta, *dws; float *cfac, *xnorm, *xnorm_p;
-  float* dcoef; double *dint, *dt; int32_t *dniter, *dstatus;
-  __half *Xp, *Wp; float2* wmeta[2]; float *S, *G[2]; unsigned int* absmax; int2* gtiles; unsigned long long* counters;
-  SKD_CUDA(c, sx.alloc(&W, (size_t)B * ldw));
-  SKD_CUDA(c, sx.alloc(&state, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&order, (size_t)n));
-  SKD_CUDA(c, sx.alloc(&active, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&dpos, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&eta, (size_t)n));
+  dpad = (d + 63) / 64 * 64;
+  npad = (n + ST_T - 1) / ST_T * ST_T;
+  kpad = (f.B + ST_TILE - 1) / ST_TILE * ST_TILE;
+  unsigned int* absmax;
   SKD_CUDA(c, sx.alloc(&dws, (size_t)n + 1));
-  SKD_CUDA(c, sx.alloc(&cfac, (size_t)n));
   SKD_CUDA(c, sx.alloc(&xnorm, (size_t)n));
   SKD_CUDA(c, sx.alloc(&xnorm_p, (size_t)n));
   SKD_CUDA(c, sx.alloc(&ycls_p, (size_t)n));
-  SKD_CUDA(c, sx.alloc(&dcoef, (size_t)B * d));
-  SKD_CUDA(c, sx.alloc(&dint, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&dt, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&dniter, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&dstatus, (size_t)B));
   SKD_CUDA(c, sx.alloc(&Xp, (size_t)npad * dpad));
   SKD_CUDA(c, sx.alloc(&Wp, (size_t)kpad * dpad));
   SKD_CUDA(c, sx.alloc(&wmeta[0], (size_t)kpad));
@@ -558,35 +458,25 @@ int sgd_fit_batch_tc(Ctx* c, int B, const int32_t* col_pos, double alpha, int fi
   const int tiles_t = ST_T / ST_TILE;
   std::vector<int2> hg;
   for (int mi = 0; mi < tiles_t; ++mi) for (int ni = mi; ni < tiles_t; ++ni) hg.push_back(make_int2(mi, ni));
+  n_g = (int)hg.size();
   SKD_CUDA(c, sx.alloc(&gtiles, hg.size()));
   SKD_CUDA(c, cudaMemcpyAsync(gtiles, hg.data(), hg.size() * sizeof(int2), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemsetAsync(W, 0, (size_t)B * ldw * sizeof(float), c->stream));
   SKD_CUDA(c, cudaMemsetAsync(absmax, 0, 4, c->stream));
   SKD_CUDA(c, cudaMemsetAsync(counters, 0, 32, c->stream));
-  std::vector<SgdStateTc> hs(B);
-  for (auto& s : hs) { s.wscale = 1.0; s.sq_norm = 0.0; s.intercept = 0.0; s.best_objective = INFINITY; s.t = 1.0;
-                       s.no_improve = 0; s.done = 0; s.n_iter = 0; s.status = 3; s.objective_sum = 0.0; }
-  SKD_CUDA(c, cudaMemcpyAsync(state, hs.data(), (size_t)B * sizeof(SgdStateTc), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(dpos, col_pos, (size_t)B * 4, cudaMemcpyHostToDevice, c->stream));
   sgd_rownorm_kernel<<<(unsigned)((n + 7) / 8), 256, 0, c->stream>>>(c->X, n, ldx, d, xnorm, absmax);
   c->launches += 1;
   unsigned int hmax_bits = 0;
   SKD_CUDA(c, cudaMemcpyAsync(&hmax_bits, absmax, 4, cudaMemcpyDeviceToHost, c->stream));
   SKD_CUDA(c, cudaStreamSynchronize(c->stream));
   float hmax; memcpy(&hmax, &hmax_bits, 4);
-  float sxs = 1.f;
   if (hmax > 0.f && std::isfinite(hmax)) { int e; frexpf(hmax, &e); sxs = ldexpf(1.f, 13 - (e - 1)); }
-  const float inv_sx = 1.f / sxs, inv_sx2 = inv_sx * inv_sx;
+  inv_sx = 1.f / sxs;
+  inv_sx2 = inv_sx * inv_sx;
 
-  CUtensorMap map_x, map_w;
   if (tc_make_map_2d(c, &map_x, Xp, (uint64_t)npad, (uint64_t)dpad, ST_TILE)) return 1;
   if (tc_make_map_2d(c, &map_w, Wp, (uint64_t)kpad, (uint64_t)dpad, ST_TILE)) return 1;
-  const size_t gemm_smem = 1024 + (size_t)ST_STAGES * 2 * ST_TILE * 128 + sizeof(SgdGemmBars) + 64;
+  gemm_smem = 1024 + (size_t)ST_STAGES * 2 * ST_TILE * 128 + sizeof(SgdGemmBars) + 64;
   SKD_CUDA(c, cudaFuncSetAttribute(sgd_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem));
-
-  cudaStream_t sB;
-  cudaEvent_t ev_perm, ev_g[2], ev_scan[2], ev_t[3];
-  double t_gemm = 0.0, t_scan = 0.0; int t_cnt = 0;
   for (int i = 0; i < 3; ++i) SKD_CUDA(c, cudaEventCreate(&ev_t[i]));
   SKD_CUDA(c, cudaStreamCreateWithFlags(&sB, cudaStreamNonBlocking));
   SKD_CUDA(c, cudaEventCreateWithFlags(&ev_perm, cudaEventDisableTiming));
@@ -594,145 +484,115 @@ int sgd_fit_batch_tc(Ctx* c, int B, const int32_t* col_pos, double alpha, int fi
     SKD_CUDA(c, cudaEventCreateWithFlags(&ev_g[i], cudaEventDisableTiming));
     SKD_CUDA(c, cudaEventCreateWithFlags(&ev_scan[i], cudaEventDisableTiming));
   }
-  struct StreamGuard {
-    cudaStream_t s; cudaEvent_t* e[5];
-    ~StreamGuard() { cudaStreamSynchronize(s); for (auto p : e) cudaEventDestroy(*p); cudaStreamDestroy(s); }
-  } guard{sB, {&ev_perm, &ev_g[0], &ev_g[1], &ev_scan[0], &ev_scan[1]}};
-  std::vector<int32_t> hact(B), hord(n);
-  std::vector<float> hcfac(n);
-  std::vector<double> hws(n + 1);
-  for (int j = 0; j < B; ++j) hact[j] = j;
-  for (int64_t i = 0; i < n; ++i) hord[i] = (int32_t)i;
-  int n_active = B;
-  double wscale_epoch = 1.0;            // lazy scale at the start of the epoch (identical for all running columns)
-  const char* trace_env = getenv("SKDIST_B200_TRACE");
-  const bool trace = trace_env && trace_env[0] == '2';
-  for (int epoch = 0; epoch < max_iter && n_active > 0; ++epoch) {
-    auto tw0 = std::chrono::steady_clock::now();
-    if (shuffle) {   // Fisher-Yates with the SAME seed every epoch, applied to the evolving order
-      uint32_t s = seed;
-      for (int64_t i = 0; i < n - 1; ++i) {
-        int64_t j = i + tc_xorshift_rand_r(&s) % (uint32_t)(n - i);
-        std::swap(hord[i], hord[j]);
-      }
-    }
-    if (shuffle || epoch == 0)
-      SKD_CUDA(c, cudaMemcpyAsync(order, hord.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(active, hact.data(), (size_t)n_active * 4, cudaMemcpyHostToDevice, c->stream));
-    const double t0 = 1.0 + (double)epoch * (double)n;
-    sgd_tc_schedule_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(n, t0, alpha, optimal_init, lr_type, eta0,
-                                                                           power_t, eta, cfac);
-    // the lazy-scale chain wscale *= c_t of the epoch (one float64 multiply per sample, identical for every
-    // running column): evaluated once on the host from the device's own c_t
-    SKD_CUDA(c, cudaMemcpyAsync(hcfac.data(), cfac, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
-    if (shuffle || epoch == 0) {
-      const int64_t total = npad * (dpad / 8);
-      sgd_permute_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c->stream>>>(c->X, ldx, d, order, n, npad, dpad, sxs, Xp, c->ycls, xnorm,
-                                                                               ycls_p, xnorm_p);
-      c->launches += 1;
-    }
-    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-    {
-      double wsc = wscale_epoch;
-      for (int64_t i = 0; i < n; ++i) {
-        hws[i] = wsc;
-        wsc *= (double)hcfac[i];
-        if (wsc < 1e-6) wsc = 1.0;          // reset_wscale() (the scan kernel rescales the weights at this sample)
-      }
-      hws[n] = wsc;
-    }
-    SKD_CUDA(c, cudaMemcpyAsync(dws, hws.data(), (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-    const int kgroups = (n_active + ST_TILE - 1) / ST_TILE;
-    SKD_CUDA(c, cudaMemsetAsync(Wp, 0, (size_t)kpad * dpad * sizeof(__half), c->stream));
-#define SGD_TC_CASE(D, CALL) case D: CALL(D); break;
-#define SGD_EXPORT(D) sgd_export_kernel<D><<<(n_active + 3) / 4, 128, 0, c->stream>>>(W, ldw, d, dpad, active, n_active, inv_sx, Wp, wmeta[0])
-    switch (dpl) { SGD_TC_CASE(1, SGD_EXPORT) SGD_TC_CASE(2, SGD_EXPORT) SGD_TC_CASE(4, SGD_EXPORT) SGD_TC_CASE(8, SGD_EXPORT)
-                   SGD_TC_CASE(16, SGD_EXPORT) SGD_TC_CASE(32, SGD_EXPORT) default: return fail(c, "sgd: bad dpl"); }
-    c->launches += 2;
-    const int n_blocks = (int)((n + ST_T - 1) / ST_T);
-    // The Gram product of a block does not depend on the weights: it runs one block ahead on a second
-    // stream (two G buffers), so only S = X_T W^T sits between two scans.
-    SKD_CUDA(c, cudaEventRecord(ev_perm, c->stream));          // Xp of this epoch is complete
-    SKD_CUDA(c, cudaStreamWaitEvent(sB, ev_perm, 0));
-    auto launch_g = [&](int b) {
-      SgdGemmParams gg;
-      gg.S = S; gg.G = G[b & 1]; gg.row0 = b * ST_T; gg.n_colgroups = 1; gg.n_s = 0;
-      gg.n_g = (int)hg.size(); gg.gtiles = gtiles; gg.kchunks = dpad / 64;
-      sgd_gemm_kernel<<<gg.n_g, ST_THREADS, gemm_smem, sB>>>(map_x, map_w, gg);
-      cudaEventRecord(ev_g[b & 1], sB);
-    };
-    launch_g(0);
-    for (int b = 0; b < n_blocks; ++b) {
-      if (b + 1 < n_blocks) {
-        if (b >= 1) SKD_CUDA(c, cudaStreamWaitEvent(sB, ev_scan[(b + 1) & 1], 0));   // scan(b - 1) is done with that buffer
-        launch_g(b + 1);
-      }
-      SgdGemmParams gp;
-      gp.S = S; gp.G = G[b & 1]; gp.row0 = b * ST_T; gp.n_colgroups = kgroups; gp.n_s = tiles_t * kgroups;
-      gp.n_g = 0; gp.gtiles = gtiles; gp.kchunks = dpad / 64;
-      const bool tb = trace && (epoch == 1 || epoch == 20) && b >= 8 && b < 24;    // kernel split of 16 blocks
-      if (tb) cudaEventRecord(ev_t[0], c->stream);
-      sgd_gemm_kernel<<<gp.n_s, ST_THREADS, gemm_smem, c->stream>>>(map_x, map_w, gp);
-      if (tb) cudaEventRecord(ev_t[1], c->stream);
-      SKD_CUDA(c, cudaStreamWaitEvent(c->stream, ev_g[b & 1], 0));
-      SgdScanParams sp;
-      sp.X = c->X; sp.ldx = ldx; sp.d = d; sp.dpad = dpad; sp.ycls = c->ycls; sp.order = order; sp.eta = eta; sp.cfac = cfac;
-      sp.ws = dws; sp.ycls_p = ycls_p; sp.xnorm_p = xnorm_p; sp.n = n; sp.row0 = b * ST_T;
-      sp.t_len = (int)std::min<int64_t>(ST_T, n - (int64_t)b * ST_T);
-      sp.active = active; sp.n_active = n_active; sp.col_pos = dpos; sp.W = W; sp.ldw = ldw; sp.state = state;
-      sp.S = S; sp.G = G[b & 1]; sp.wmeta = wmeta[b & 1]; sp.Wp = Wp; sp.wmeta_out = wmeta[(b + 1) & 1];
-      sp.inv_sx = inv_sx; sp.inv_sx2 = inv_sx2; sp.alpha = alpha; sp.fit_intercept = fit_intercept;
-      sp.last_block = b == n_blocks - 1; sp.tol = tol; sp.n_iter_no_change = n_iter_no_change; sp.counters = counters;
-#define SGD_SCAN(D) sgd_scan_kernel<D><<<(n_active + 3) / 4, 128, 0, c->stream>>>(sp)
-      switch (dpl) { SGD_TC_CASE(1, SGD_SCAN) SGD_TC_CASE(2, SGD_SCAN) SGD_TC_CASE(4, SGD_SCAN) SGD_TC_CASE(8, SGD_SCAN)
-                     SGD_TC_CASE(16, SGD_SCAN) SGD_TC_CASE(32, SGD_SCAN) default: return fail(c, "sgd: bad dpl"); }
-      SKD_CUDA(c, cudaEventRecord(ev_scan[b & 1], c->stream));
-      if (tb) {
-        cudaEventRecord(ev_t[2], c->stream);
-        cudaEventSynchronize(ev_t[2]);
-        float m1 = 0.f, m2 = 0.f;
-        cudaEventElapsedTime(&m1, ev_t[0], ev_t[1]);
-        cudaEventElapsedTime(&m2, ev_t[1], ev_t[2]);
-        t_gemm += m1; t_scan += m2; t_cnt += 1;
-      }
-      c->launches += 3;
-    }
-    SKD_CUDA(c, cudaGetLastError());
-    SKD_CUDA(c, cudaMemcpyAsync(hs.data(), state, (size_t)B * sizeof(SgdStateTc), cudaMemcpyDeviceToHost, c->stream));
-    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-    c->h2d += n * 12; c->d2h += (int64_t)B * sizeof(SgdStateTc) + n * 4;
-    wscale_epoch = hws[n];
-    if (trace) {
-      auto tw2 = std::chrono::steady_clock::now();
-      fprintf(stderr, "[skd trace] sgd-tc epoch %3d active %5d  %8.2f ms\n", epoch, n_active,
-              std::chrono::duration<double, std::milli>(tw2 - tw0).count());
-      if (t_cnt > 0) {
-        fprintf(stderr, "[skd trace] sgd-tc epoch %3d per block (16 blocks, synchronised): S product %.1f us, wait for G + scan %.1f us\n",
-                epoch, 1e3 * t_gemm / t_cnt, 1e3 * t_scan / t_cnt);
-        t_gemm = t_scan = 0.0; t_cnt = 0;
-      }
-    }
-    n_active = 0;
-    for (int j = 0; j < B; ++j)
-      if (!hs[j].done) hact[n_active++] = j;
-  }
-  if (trace) {
-    unsigned long long hc[4];
-    cudaMemcpy(hc, counters, 32, cudaMemcpyDeviceToHost);
-    fprintf(stderr, "[skd trace] sgd-tc samples screened by the tensor-core margins %llu, exact dot products %llu, violators %llu\n",
-            hc[0], hc[1], hc[2]);
-  }
-  sgd_tc_finish_kernel<<<B, 128, 0, c->stream>>>(W, ldw, d, state, B, dcoef, dint, dniter, dt, dstatus);
-  c->launches += 1;
-  SKD_CUDA(c, cudaGetLastError());
-  SKD_CUDA(c, cudaMemcpyAsync(coef_out, dcoef, (size_t)B * d * 4, cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(intercept_out, dint, (size_t)B * 8, cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(n_iter_out, dniter, (size_t)B * 4, cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(t_out, dt, (size_t)B * 8, cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(status_out, dstatus, (size_t)B * 4, cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->d2h += (int64_t)B * (d * 4 + 24);
+  hcfac.resize(n);
+  hws.resize(n + 1);
   return 0;
+}
+
+SgdTc::~SgdTc() {
+  if (sB) cudaStreamSynchronize(sB);
+  for (cudaEvent_t e : {ev_perm, ev_g[0], ev_g[1], ev_scan[0], ev_scan[1], ev_t[0], ev_t[1], ev_t[2]})
+    if (e) cudaEventDestroy(e);
+  if (sB) cudaStreamDestroy(sB);
+}
+
+int SgdTc::epoch(Ctx* c, const SgdFit& f, int epoch, int n_active, bool new_order, bool trace) {
+  const int64_t n = c->n;
+  const int d = (int)c->d, ldx = (int)c->ldx;
+  // the lazy-scale chain wscale *= c_t of the epoch (one float64 multiply per sample, identical for every
+  // running column): evaluated once on the host from the device's own c_t
+  SKD_CUDA(c, cudaMemcpyAsync(hcfac.data(), f.cfac, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
+  if (new_order) {
+    const int64_t total = npad * (dpad / 8);
+    sgd_permute_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c->stream>>>(c->X, ldx, d, f.order, n, npad, dpad, sxs, Xp,
+                                                                             c->ycls, xnorm, ycls_p, xnorm_p);
+    c->launches += 1;
+  }
+  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  {
+    double wsc = wscale_epoch;
+    for (int64_t i = 0; i < n; ++i) {
+      hws[i] = wsc;
+      wsc *= (double)hcfac[i];
+      if (wsc < 1e-6) wsc = 1.0;          // reset_wscale() (the scan kernel rescales the weights at this sample)
+    }
+    hws[n] = wsc;
+    wscale_epoch = wsc;
+  }
+  SKD_CUDA(c, cudaMemcpyAsync(dws, hws.data(), (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+  c->h2d += n * 8; c->d2h += n * 4;
+  const int tiles_t = ST_T / ST_TILE;
+  const int kgroups = (n_active + ST_TILE - 1) / ST_TILE;
+  SKD_CUDA(c, cudaMemsetAsync(Wp, 0, (size_t)kpad * dpad * sizeof(__half), c->stream));
+#define SGD_TC_CASE(D, CALL) case D: CALL(D); break;
+#define SGD_EXPORT(D) sgd_export_kernel<D><<<(n_active + 3) / 4, 128, 0, c->stream>>>(f.W, f.ldw, d, dpad, f.active, n_active, inv_sx, Wp, wmeta[0])
+  switch (f.dpl) { SGD_TC_CASE(1, SGD_EXPORT) SGD_TC_CASE(2, SGD_EXPORT) SGD_TC_CASE(4, SGD_EXPORT) SGD_TC_CASE(8, SGD_EXPORT)
+                   SGD_TC_CASE(16, SGD_EXPORT) SGD_TC_CASE(32, SGD_EXPORT) default: return fail(c, "sgd: bad dpl"); }
+  c->launches += 1;
+  const int n_blocks = (int)((n + ST_T - 1) / ST_T);
+  double t_gemm = 0.0, t_scan = 0.0; int t_cnt = 0;
+  // The Gram product of a block does not depend on the weights: it runs one block ahead on a second
+  // stream (two G buffers), so only S = X_T W^T sits between two scans.
+  SKD_CUDA(c, cudaEventRecord(ev_perm, c->stream));          // Xp of this epoch is complete
+  SKD_CUDA(c, cudaStreamWaitEvent(sB, ev_perm, 0));
+  auto launch_g = [&](int b) {
+    SgdGemmParams gg;
+    gg.S = S; gg.G = G[b & 1]; gg.row0 = b * ST_T; gg.n_colgroups = 1; gg.n_s = 0;
+    gg.n_g = n_g; gg.gtiles = gtiles; gg.kchunks = dpad / 64;
+    sgd_gemm_kernel<<<gg.n_g, ST_THREADS, gemm_smem, sB>>>(map_x, map_w, gg);
+    cudaEventRecord(ev_g[b & 1], sB);
+  };
+  launch_g(0);
+  for (int b = 0; b < n_blocks; ++b) {
+    if (b + 1 < n_blocks) {
+      if (b >= 1) SKD_CUDA(c, cudaStreamWaitEvent(sB, ev_scan[(b + 1) & 1], 0));   // scan(b - 1) is done with that buffer
+      launch_g(b + 1);
+    }
+    SgdGemmParams gp;
+    gp.S = S; gp.G = G[b & 1]; gp.row0 = b * ST_T; gp.n_colgroups = kgroups; gp.n_s = tiles_t * kgroups;
+    gp.n_g = 0; gp.gtiles = gtiles; gp.kchunks = dpad / 64;
+    const bool tb = trace && (epoch == 1 || epoch == 20) && b >= 8 && b < 24;    // kernel split of 16 blocks
+    if (tb) cudaEventRecord(ev_t[0], c->stream);
+    sgd_gemm_kernel<<<gp.n_s, ST_THREADS, gemm_smem, c->stream>>>(map_x, map_w, gp);
+    if (tb) cudaEventRecord(ev_t[1], c->stream);
+    SKD_CUDA(c, cudaStreamWaitEvent(c->stream, ev_g[b & 1], 0));
+    SgdScanParams sp;
+    sp.X = c->X; sp.ldx = ldx; sp.d = d; sp.dpad = dpad; sp.ycls = c->ycls; sp.order = f.order; sp.eta = f.eta;
+    sp.cfac = f.cfac; sp.ws = dws; sp.ycls_p = ycls_p; sp.xnorm_p = xnorm_p; sp.n = n; sp.row0 = b * ST_T;
+    sp.t_len = (int)std::min<int64_t>(ST_T, n - (int64_t)b * ST_T);
+    sp.active = f.active; sp.n_active = n_active; sp.col_pos = f.col_pos; sp.W = f.W; sp.ldw = f.ldw; sp.state = f.state;
+    sp.S = S; sp.G = G[b & 1]; sp.wmeta = wmeta[b & 1]; sp.Wp = Wp; sp.wmeta_out = wmeta[(b + 1) & 1];
+    sp.inv_sx = inv_sx; sp.inv_sx2 = inv_sx2; sp.alpha = f.alpha; sp.fit_intercept = f.fit_intercept;
+    sp.last_block = b == n_blocks - 1; sp.tol = f.tol; sp.n_iter_no_change = f.n_iter_no_change; sp.counters = counters;
+#define SGD_SCAN(D) sgd_scan_kernel<D><<<(n_active + 3) / 4, 128, 0, c->stream>>>(sp)
+    switch (f.dpl) { SGD_TC_CASE(1, SGD_SCAN) SGD_TC_CASE(2, SGD_SCAN) SGD_TC_CASE(4, SGD_SCAN) SGD_TC_CASE(8, SGD_SCAN)
+                     SGD_TC_CASE(16, SGD_SCAN) SGD_TC_CASE(32, SGD_SCAN) default: return fail(c, "sgd: bad dpl"); }
+    SKD_CUDA(c, cudaEventRecord(ev_scan[b & 1], c->stream));
+    if (tb) {
+      cudaEventRecord(ev_t[2], c->stream);
+      cudaEventSynchronize(ev_t[2]);
+      float m1 = 0.f, m2 = 0.f;
+      cudaEventElapsedTime(&m1, ev_t[0], ev_t[1]);
+      cudaEventElapsedTime(&m2, ev_t[1], ev_t[2]);
+      t_gemm += m1; t_scan += m2; t_cnt += 1;
+    }
+    c->launches += 3;
+  }
+#undef SGD_SCAN
+#undef SGD_EXPORT
+#undef SGD_TC_CASE
+  SKD_CUDA(c, cudaGetLastError());
+  if (t_cnt > 0)
+    fprintf(stderr, "[skd trace] sgd-tc epoch %3d per block (16 blocks, synchronised): S product %.1f us, wait for G + scan %.1f us\n",
+            epoch, 1e3 * t_gemm / t_cnt, 1e3 * t_scan / t_cnt);
+  return 0;
+}
+
+void SgdTc::print_counters() {
+  unsigned long long hc[4];
+  cudaMemcpy(hc, counters, 32, cudaMemcpyDeviceToHost);
+  fprintf(stderr, "[skd trace] sgd-tc samples screened by the tensor-core margins %llu, exact dot products %llu, violators %llu\n",
+          hc[0], hc[1], hc[2]);
 }
 
 }  // namespace skd

@@ -255,11 +255,6 @@ int sgd_fit_batch(Ctx* c, int B, const int32_t* col_pos, int loss, double alpha,
                   double* intercept_out, int32_t* n_iter_out, double* t_out, int32_t* status_out);
 // 2-D fp16 row-major [rows x cols] TMA descriptor, box = [box_rows x 64 cols], 128B swizzle (logreg_tc.cu)
 int tc_make_map_2d(Ctx* c, CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows);
-bool sgd_tc_supported(const Ctx* c, int loss, int shuffle);
-int sgd_fit_batch_tc(Ctx* c, int B, const int32_t* col_pos, double alpha, int fit_intercept, int max_iter, double tol,
-                     int shuffle, uint32_t seed, int lr_type, double eta0, double power_t, double optimal_init,
-                     int n_iter_no_change, float* coef_out, double* intercept_out, int32_t* n_iter_out, double* t_out,
-                     int32_t* status_out);
 void forest_free(Ctx* c);
 int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_states, int n_classes,
                int max_features, int max_depth, int min_samples_split, int min_samples_leaf,
