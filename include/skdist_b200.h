@@ -110,7 +110,10 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
 /* Objective and gradient of B columns at caller-supplied points w_in[j*(d+1)+k] (float64;
  * cast to fp32 for the products as sklearn does).  loss_out[j], grad_out[j*(d+1)+k] follow
  * SK/linear_model/_linear_loss.py:291-379 exactly (mean loss + 0.5*l2*|w|^2, intercept last).
- * Diagnostic / test entry: it runs the same evaluation kernels as skd_logreg_fit_batch. */
+ * Diagnostic / test entry: it runs the evaluation kernel skd_logreg_fit_batch would run on the same
+ * columns, in the same slot layout (on the tensor cores: sorted by held-out fold into groups of 128
+ * slots, with the per-fold tile lists; TC_FIT_UNI when every column has the same col_pos and at most
+ * 32 folds are staged, TC_FIT otherwise).  Outputs are in column order. */
 int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const double* C,
                          const int32_t* col_fold, const int32_t* col_pos, int32_t fit_intercept,
                          double* loss_out, double* grad_out);

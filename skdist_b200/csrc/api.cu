@@ -95,6 +95,44 @@ static int alloc_eval_buffers(Ctx* c, Scratch& sx, LogregWork& w, int B, int slo
   return 0;
 }
 
+// Slot layout of a logistic batch, then its evaluation buffers (alloc_eval_buffers).  The tensor-core
+// path runs the fold-grouped layout: columns stable-sorted by held-out fold, every fold segment padded
+// with col = -1 slots to a multiple of 128 (one MMA group = one fold -> tile skipping), and w.uni_pos
+// set when every column is one-vs-rest with the same positive class.  hslots receives that layout;
+// it stays empty for the SIMT path, whose slot s is column s.
+static int alloc_logreg_slots(Ctx* c, Scratch& sx, LogregWork& w, int B, const int32_t* col_fold,
+                              const int32_t* col_pos, const int32_t* col_neg, std::vector<SlotMeta>& hslots) {
+  hslots.clear();
+  if (want_tc(c) && tc_supported(c)) {
+    std::vector<int> order(B);
+    for (int j = 0; j < B; ++j) order[j] = j;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return col_fold[a] < col_fold[b]; });
+    for (int i = 0; i < B;) {
+      const int f = col_fold[order[i]];
+      if (f > 127) return fail(c, "fold id above 127");
+      for (; i < B && col_fold[order[i]] == f; ++i) {
+        SlotMeta sm; sm.col = order[i]; sm.fold = f < 0 ? -1 : f; sm.pos = col_pos[order[i]];
+        sm.pad = (col_neg && col_neg[order[i]] >= 0) ? col_neg[order[i]] + 1 : 0;
+        hslots.push_back(sm);
+      }
+      while (hslots.size() % 128) { SlotMeta sm; sm.col = -1; sm.fold = f < 0 ? -1 : f; sm.pos = -1; sm.pad = 0; hslots.push_back(sm); }
+    }
+  }
+  if (alloc_eval_buffers(c, sx, w, B, hslots.empty() ? B : (int)hslots.size())) return 1;
+  w.grouped = !hslots.empty() && w.use_tc;
+  if (!w.grouped) {
+    hslots.clear();
+    return 0;
+  }
+  w.uni_pos = col_pos[0];
+  for (int j = 1; j < B; ++j)
+    if (col_pos[j] != col_pos[0]) { w.uni_pos = -1; break; }
+  if (col_neg)
+    for (int j = 0; j < B; ++j)
+      if (col_neg[j] >= 0) { w.uni_pos = -1; break; }   // pair masks are per column: general epilogue
+  return 0;
+}
+
 // Non-finite scan of the staged matrix: scikit-learn's estimators reject NaN / infinity in X
 // (check_array -> "Input X contains NaN."), so the staging call does too -- at HBM speed, on the
 // copy that is already on the device.
@@ -643,36 +681,8 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   LogregWork w;
   w.B = B; w.dp = dp;
   w.vec_stride = (size_t)(5 + 2 * m) * dp + 2 * m;
-  // Fold-grouped slot layout for the tensor-core path: columns sorted by held-out fold, every fold
-  // segment padded to a multiple of 128 slots (one MMA group = one fold -> tile skipping).
   std::vector<SlotMeta> hslots;
-  const bool grouped = want_tc(c) && tc_supported(c);
-  if (grouped) {
-    std::vector<int> order(B);
-    for (int j = 0; j < B; ++j) order[j] = j;
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return col_fold[a] < col_fold[b]; });
-    for (int i = 0; i < B;) {
-      int f = col_fold[order[i]], i0 = i;
-      if (f > 127) return fail(c, "skd_logreg_fit_batch: fold id above 127");
-      for (; i < B && col_fold[order[i]] == f; ++i) {
-        SlotMeta sm; sm.col = order[i]; sm.fold = f < 0 ? -1 : f; sm.pos = col_pos[order[i]];
-        sm.pad = (col_neg && col_neg[order[i]] >= 0) ? col_neg[order[i]] + 1 : 0;
-        hslots.push_back(sm);
-      }
-      (void)i0;
-      while (hslots.size() % 128) { SlotMeta sm; sm.col = -1; sm.fold = f < 0 ? -1 : f; sm.pos = -1; sm.pad = 0; hslots.push_back(sm); }
-    }
-  }
-  if (alloc_eval_buffers(c, sx, w, B, grouped ? (int)hslots.size() : B)) return 1;
-  w.grouped = grouped && w.use_tc;
-  if (w.grouped) {
-    w.uni_pos = col_pos[0];
-    for (int j = 1; j < B; ++j)
-      if (col_pos[j] != col_pos[0]) { w.uni_pos = -1; break; }
-    if (col_neg)
-      for (int j = 0; j < B; ++j)
-        if (col_neg[j] >= 0) { w.uni_pos = -1; break; }   // pair masks are per column: general epilogue
-  }
+  if (alloc_logreg_slots(c, sx, w, B, col_fold, col_pos, col_neg, hslots)) return 1;
   SKD_CUDA(c, sx.alloc(&w.sc, (size_t)B));
   SKD_CUDA(c, sx.alloc(&w.vec, (size_t)B * w.vec_stride));
   SKD_CUDA(c, sx.alloc(&w.l2, (size_t)B));
@@ -856,7 +866,6 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
   const int64_t n = c->n, d = c->d, ldx = c->ldx;
   const int dp = (int)d + 1;
   std::vector<double> l2(B), inv_n(B);
-  std::vector<SlotMeta> hs(B);
   std::vector<float> hw((size_t)B * ldx + B, 0.f);
   for (int j = 0; j < B; ++j) {
     int f = col_fold[j];
@@ -867,17 +876,23 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
     }
     l2[j] = 1.0 / (C[j] * (double)ntrain);
     inv_n[j] = 1.0 / (double)ntrain;
-    hs[j].col = j; hs[j].fold = f; hs[j].pos = col_pos[j]; hs[j].pad = 0;
     for (int k = 0; k < d; ++k) hw[(size_t)j * ldx + k] = (float)w_in[(size_t)j * dp + k];
     hw[(size_t)B * ldx + j] = fit_intercept ? (float)w_in[(size_t)j * dp + d] : 0.f;
   }
   Scratch sx(c);
   LogregWork w;
   w.B = B; w.dp = dp;
-  if (alloc_eval_buffers(c, sx, w, B)) return 1;
+  // the slot layout of skd_logreg_fit_batch: fold-grouped on the tensor cores, slot s = column s on SIMT
+  std::vector<SlotMeta> hs;
+  if (alloc_logreg_slots(c, sx, w, B, col_fold, col_pos, nullptr, hs)) return 1;
+  if (!w.grouped) {
+    hs.resize(B);
+    for (int j = 0; j < B; ++j) { hs[j].col = j; hs[j].fold = col_fold[j] < 0 ? -1 : col_fold[j]; hs[j].pos = col_pos[j]; hs[j].pad = 0; }
+  }
+  const int n_slots = (int)hs.size();
   SKD_CUDA(c, sx.alloc(&w.l2, (size_t)B));
   SKD_CUDA(c, sx.alloc(&w.inv_n, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&w.slot, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&w.slot, (size_t)n_slots));
   SKD_CUDA(c, sx.alloc(&w.n_act, 1));
   double *dx, *df, *dg;
   SKD_CUDA(c, sx.alloc(&dx, (size_t)B * dp));
@@ -885,18 +900,17 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
   SKD_CUDA(c, sx.alloc(&dg, (size_t)B * dp));
   SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(w.slot, hs.data(), B * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(w.slot, hs.data(), n_slots * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(dx, w_in, (size_t)B * dp * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   if (w.use_tc) {
-    int32_t nb = B;
-    SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &nb, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    if (tc_export(c, w, B, dx, fit_intercept)) return 1;
+    SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &n_slots, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    if (tc_export(c, w, n_slots, dx, fit_intercept)) return 1;
   } else {
     SKD_CUDA(c, cudaMemcpyAsync(w.Wact, hw.data(), hw.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
   }
   int nz_used = 0;
-  if (eval_dispatch(c, w, B, &nz_used)) return 1;
-  if (lbfgs_dev_gather(c, w, B, nz_used, fit_intercept, dx, df, dg)) return 1;
+  if (eval_dispatch(c, w, n_slots, &nz_used)) return 1;
+  if (lbfgs_dev_gather(c, w, n_slots, nz_used, fit_intercept, dx, df, dg)) return 1;
   SKD_CUDA(c, cudaMemcpyAsync(loss_out, df, B * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(grad_out, dg, (size_t)B * dp * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   SKD_CUDA(c, cudaStreamSynchronize(c->stream));

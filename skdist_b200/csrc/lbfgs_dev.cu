@@ -153,9 +153,10 @@ lb_reduce_kernel(const float* __restrict__ gradp, int nz, int n_act, int ldx, co
   gradr[e] = acc;
 }
 
-// Diagnostic / test entry: objective and gradient of every slot at caller-supplied points.
+// Diagnostic / test entry: objective and gradient of every column at caller-supplied points.  The
+// partials are indexed by slot, the column's constants, point and outputs by slot[s].col.
 __global__ void __launch_bounds__(LB_THREADS)
-lb_gather_kernel(int n_act, int nz_used, int d, int ldx, int fit_intercept,
+lb_gather_kernel(int n_act, int nz_used, int d, int ldx, int fit_intercept, const SlotMeta* __restrict__ slot,
                  const double* __restrict__ lossp, const double* __restrict__ gsump,
                  const float* __restrict__ gradp, const double* __restrict__ gscale,
                  const double* __restrict__ l2v,
@@ -164,10 +165,12 @@ lb_gather_kernel(int n_act, int nz_used, int d, int ldx, int fit_intercept,
   __shared__ double red[8];
   const int s = blockIdx.x;
   if (s >= n_act) return;
+  const int col = slot[s].col;
+  if (col < 0) return;   // padding slot of the fold-grouped layout
   CtaPar P{red};
   double f = gather_fg(P, s, n_act, nz_used, d, ldx, fit_intercept, lossp, gsump, gradp, gscale,
-                       l2v[s], inv_nv[s], xin + (size_t)s * (d + 1), gout + (size_t)s * (d + 1));
-  if (threadIdx.x == 0) fout[s] = f;
+                       l2v[col], inv_nv[col], xin + (size_t)col * (d + 1), gout + (size_t)col * (d + 1));
+  if (threadIdx.x == 0) fout[col] = f;
 }
 
 __global__ void lb_init_kernel(LbfgsScalars* sc, double* vec, size_t vec_stride, int B, int n,
@@ -425,7 +428,7 @@ int lbfgs_dev_readback(Ctx* c, LogregWork& w, int* n_act_out, int* n_run_out) {
 int lbfgs_dev_gather(Ctx* c, LogregWork& w, int n_act, int nz_used, int fit_intercept,
                      const double* dx, double* df, double* dg) {
   lb_gather_kernel<<<n_act, LB_THREADS, 0, c->stream>>>(n_act, nz_used, (int)c->d, w.ldw,
-                                                        fit_intercept, w.lossp, w.gsump, w.gradp,
+                                                        fit_intercept, w.slot, w.lossp, w.gsump, w.gradp,
                                                         w.gscale, w.l2, w.inv_n, dx, df, dg);
   c->launches += 1;
   SKD_CUDA(c, cudaGetLastError());

@@ -64,6 +64,11 @@ __global__ void tc_colmax_kernel(const float* __restrict__ X, int64_t n, int ldx
   atomicMax(&colmax_bits[k], __float_as_uint(m));  // non-negative floats order as uints
 }
 
+// Exponent of the power-of-two scale that brings a maximum m = f * 2^e (frexpf) into [2^13, 2^14):
+// 13 - floor(log2 m).  Capped at 127 so that the scale stays a finite float: a maximum below 2^-114
+// then lands below 2^13, and only loses fp16 relative precision on contributions that small.
+__device__ __forceinline__ int pow2_scale_exp(int e) { return min((int)XSCALE_TARGET_EXP - (e - 1), 127); }
+
 // scale[k] = 2^(13 - floor(log2(colmax))) ; gscale[k] = 1 / (scale[k] * 2^14)
 __global__ void tc_scale_kernel(const unsigned int* __restrict__ colmax_bits, int d, int dpad,
                                 float* __restrict__ xscale, double* __restrict__ gscale) {
@@ -75,7 +80,7 @@ __global__ void tc_scale_kernel(const unsigned int* __restrict__ colmax_bits, in
     if (m > 0.f && isfinite(m)) {
       int e;
       frexpf(m, &e);  // m = f * 2^e, f in [0.5, 1)  -> floor(log2 m) = e - 1
-      s = ldexpf(1.f, (int)XSCALE_TARGET_EXP - (e - 1));
+      s = ldexpf(1.f, pow2_scale_exp(e));
     }
   }
   xscale[k] = s;
@@ -154,7 +159,7 @@ tc_export_kernel(const double* __restrict__ vec, size_t vec_stride, const SlotMe
     if (threadIdx.x == 0) { TcSlotParam p; p.inv_t = 1.f; p.bias = 0.f; p.fold = sm.fold; p.pos = -1; p.neg1 = 0; p.col = -1; sp[s] = p; }
     return;
   }
-  const double* x = xin ? xin + (size_t)s * (d + 1) : vec + (size_t)sm.col * vec_stride;
+  const double* x = xin ? xin + (size_t)sm.col * (d + 1) : vec + (size_t)sm.col * vec_stride;
   float m = 0.f;
   for (int k = threadIdx.x; k < d; k += 128) m = fmaxf(m, fabsf((float)x[k] / xscale[k]));
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -165,7 +170,7 @@ tc_export_kernel(const double* __restrict__ vec, size_t vec_stride, const SlotMe
   if (m > 0.f && isfinite(m)) {
     int e;
     frexpf(m, &e);
-    t = ldexpf(1.f, (int)XSCALE_TARGET_EXP - (e - 1));
+    t = ldexpf(1.f, pow2_scale_exp(e));
   }
   for (int k = threadIdx.x; k < dpad; k += 128) {
     float v = 0.f;
@@ -878,7 +883,10 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
   prm.ybits = mode == TC_FIT ? w.ybits : nullptr;
   prm.mbits = mode == TC_FIT ? w.mbits : nullptr;
   prm.rb_words = w.rb_words;
-  const bool uni = mode == TC_FIT && w.grouped && w.uni_pos >= 0 && c->ycls && !w.ybits && !w.mbits;
+  // TC_FIT_UNI reads a row's sign from the list of the group's fold, so it needs one list per staged
+  // fold (tc_prepare builds them for at most 32 folds); otherwise TC_FIT decodes the fold per element
+  const bool uni = mode == TC_FIT && w.grouped && w.uni_pos >= 0 && c->ycls && !w.ybits && !w.mbits &&
+                   t.n_lists == c->n_folds + 1;
   if (uni && (!t.rowsg_valid || t.rowsg_pos != w.uni_pos)) {
     if (!t.rowsg) SKD_CUDA(c, cudaMalloc((void**)&t.rowsg, (size_t)t.n_lists * t.npad * sizeof(float)));
     tc_rowsg_kernel<<<(unsigned)((t.npad + 255) / 256), 256, 0, c->stream>>>(c->ycls, c->fold, c->n, t.npad,

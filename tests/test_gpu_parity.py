@@ -62,26 +62,6 @@ def _fold_ids(y, cv):
     return fold
 
 
-def test_loss_grad_matches_oracle(eng):
-    X, y = make_g1_classification(6000, 40, seed=21)
-    fold = _fold_ids(y, 4)
-    eng.stage_x(X); eng.stage_labels(y); eng.stage_folds(fold, 4)
-    rng = np.random.default_rng(0)
-    B = 9
-    W = rng.standard_normal((B, 41)) * 0.3
-    C = np.logspace(-3, 3, B)
-    cf = np.array([-1, 0, 1, 2, 3, 0, 1, 2, 3], np.int32)
-    f, g = eng.logreg_loss_grad(W, C, cf, np.ones(B, np.int32))
-    for j in range(B):
-        m = np.ones(len(y), bool) if cf[j] < 0 else fold != cf[j]
-        fo, go = lo.loss_gradient(W[j], X[m], y[m].astype(np.float32), 1.0 / (C[j] * m.sum()))
-        assert abs(f[j] - fo) <= 2e-6 * abs(fo)
-        # tensor cores: fp32 accumulation in the tensor core rounds toward zero -> ~1e-5 relative bias
-        # on large same-sign sums (random W); vanishes near an optimum
-        tol = 3e-6 if eng.kernel == 1 else 5e-5
-        np.testing.assert_allclose(g[j], go, rtol=0, atol=tol * np.abs(go).max())
-
-
 def test_scores_are_exact_for_given_coefficients(eng):
     X, y = make_g1_classification(5000, 24, seed=22)
     fold = _fold_ids(y, 5)
