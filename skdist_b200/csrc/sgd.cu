@@ -26,19 +26,30 @@ namespace skd {
 
 enum { SGD_HINGE = 0 };
 
-// per-sample learning rate and weight-decay factor of one epoch (class independent)
+enum { SGD_LR_OPTIMAL = 0, SGD_LR_CONSTANT = 1, SGD_LR_INVSCALING = 2 };
+
+// per-sample learning rate and weight-decay factor of one epoch (class independent): "optimal" and "constant"
+// (invscaling is evaluated on the host, see sgd_fit_batch)
 __global__ void sgd_schedule_kernel(int64_t n, double t0, double alpha, double optimal_init,
-                                    int lr_type, double eta0, double power_t, double* __restrict__ eta,
+                                    int lr_type, double eta0, double* __restrict__ eta,
                                     float* __restrict__ cfac) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const double t = t0 + (double)i;
-  double e;
-  if (lr_type == 0) e = 1.0 / (alpha * (optimal_init + t - 1.0));   // "optimal"
-  else if (lr_type == 1) e = eta0;                                   // "constant"
-  else e = eta0 / pow(t, power_t);                                   // "invscaling"
+  const double e = lr_type == SGD_LR_OPTIMAL ? 1.0 / (alpha * (optimal_init + t - 1.0)) : eta0;
   eta[i] = e;
   cfac[i] = (float)fmax(0.0, __dsub_rn(1.0, __dmul_rn(e, alpha)));  // w.scale(max(0, 1 - eta*alpha)) arg as float
+}
+
+// "invscaling": eta0 / pow(t, power_t) with the C library's pow, the one scikit-learn's Cython loop calls.  CUDA's
+// double pow is only accurate to 2 ulp, and a different eta moves the float64 intercept.
+static void sgd_invscaling_schedule(int64_t n, double t0, double alpha, double eta0, double power_t,
+                                    std::vector<double>& eta, std::vector<float>& cfac) {
+  for (int64_t i = 0; i < n; ++i) {
+    const double e = eta0 / pow(t0 + (double)i, power_t);
+    eta[i] = e;
+    cfac[i] = (float)fmax(0.0, 1.0 - e * alpha);
+  }
 }
 
 // log_loss, one sample at a time
@@ -411,6 +422,8 @@ int sgd_fit_batch(Ctx* c, int B, const int32_t* col_pos, int loss, double alpha,
     if (tc->init(c, f)) return 1;
   }
   std::vector<int32_t> hact(B), hord(n);
+  std::vector<double> heta(lr_type == SGD_LR_INVSCALING ? n : 0);
+  std::vector<float> hcfac(heta.size());
   for (int j = 0; j < B; ++j) hact[j] = j;
   for (int64_t i = 0; i < n; ++i) hord[i] = (int32_t)i;
   int n_active = B;
@@ -425,9 +438,16 @@ int sgd_fit_batch(Ctx* c, int B, const int32_t* col_pos, int loss, double alpha,
     SKD_CUDA(c, cudaMemcpyAsync(active, hact.data(), (size_t)n_active * 4, cudaMemcpyHostToDevice, c->stream));
     auto tw1 = std::chrono::steady_clock::now();
     const double t0 = 1.0 + (double)epoch * (double)n;
-    sgd_schedule_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(n, t0, alpha, optimal_init, lr_type, eta0,
-                                                                           power_t, eta, cfac);
-    c->launches += 1;
+    if (lr_type == SGD_LR_INVSCALING) {
+      sgd_invscaling_schedule(n, t0, alpha, eta0, power_t, heta, hcfac);
+      SKD_CUDA(c, cudaMemcpyAsync(eta, heta.data(), (size_t)n * 8, cudaMemcpyHostToDevice, c->stream));
+      SKD_CUDA(c, cudaMemcpyAsync(cfac, hcfac.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
+      c->h2d += n * 12;
+    } else {
+      sgd_schedule_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(n, t0, alpha, optimal_init, lr_type, eta0,
+                                                                             eta, cfac);
+      c->launches += 1;
+    }
     if (tc) {
       if (tc->epoch(c, f, epoch, n_active, new_order, trace)) return 1;
     } else {

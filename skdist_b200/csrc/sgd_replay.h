@@ -104,7 +104,8 @@ struct SgdTc {
   // one epoch after the schedule kernel has filled eta / cfac: permute X when `new_order`, replay the
   // lazy-scale chain on the host, export W, then per block of samples the S / G products and the scan
   int epoch(Ctx* c, const SgdFit& f, int epoch, int n_active, bool new_order, bool trace);
-  void print_counters();   // screened / exact / violating sample visits of the whole fit (SKDIST_B200_TRACE=2)
+  void print_counters();   // screened / exact / violating sample visits of the whole fit and the scans whose
+                           // violator log filled up (SKDIST_B200_TRACE=2)
 
   Scratch sx;
   int dpad = 0, kpad = 0, n_g = 0;

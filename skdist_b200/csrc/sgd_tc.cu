@@ -235,7 +235,8 @@ struct SgdScanParams {
   float inv_sx, inv_sx2;
   double alpha; int fit_intercept; int last_block;
   double tol; int n_iter_no_change;
-  unsigned long long* counters;   // [0] samples screened out, [1] exact evaluations, [2] violators
+  unsigned long long* counters;   // [0] samples screened out, [1] exact evaluations, [2] violators,
+                                  // [3] (column, block) scans whose violator log filled up (exact from there on)
 };
 
 template <int DPL>
@@ -267,6 +268,7 @@ sgd_scan_kernel(const SgdScanParams P) {
   int* vj = s_vj[wib];
   const float* Srow = P.S + (size_t)a * ST_T;
   unsigned long long n_screen = 0, n_exact = 0, n_viol = 0;
+  bool vlog_full = false;
 
   // per-sample inputs of the window [i0, i0 + 32): coalesced loads in walk order, requested one
   // window ahead (the window normally advances by 32; after an event it is re-read)
@@ -395,6 +397,7 @@ sgd_scan_kernel(const SgdScanParams P) {
             __syncwarp();
           } else {
             exact_all = true;
+            vlog_full = true;
           }
         }
       }
@@ -420,6 +423,7 @@ sgd_scan_kernel(const SgdScanParams P) {
       atomicAdd(&P.counters[0], n_screen);
       atomicAdd(&P.counters[1], n_exact);
       atomicAdd(&P.counters[2], n_viol);
+      if (vlog_full) atomicAdd(&P.counters[3], 1ull);
     }
   }
 }
@@ -591,8 +595,8 @@ int SgdTc::epoch(Ctx* c, const SgdFit& f, int epoch, int n_active, bool new_orde
 void SgdTc::print_counters() {
   unsigned long long hc[4];
   cudaMemcpy(hc, counters, 32, cudaMemcpyDeviceToHost);
-  fprintf(stderr, "[skd trace] sgd-tc samples screened by the tensor-core margins %llu, exact dot products %llu, violators %llu\n",
-          hc[0], hc[1], hc[2]);
+  fprintf(stderr, "[skd trace] sgd-tc samples screened by the tensor-core margins %llu, exact dot products %llu, violators %llu, "
+          "violator-log overflows %llu\n", hc[0], hc[1], hc[2], hc[3]);
 }
 
 }  // namespace skd

@@ -73,6 +73,27 @@ def _binary_estimator(template, coef_row, n_features, X_dtype, **extra):
     return est
 
 
+SGD_DIVERGED = 5        # sgd_fit_batch status: a column's weights or intercept became non-finite
+
+
+def _check_sgd_status(template, status, n_iter):
+    """Report the SGD columns' outcomes as scikit-learn's per-column fits would, in column order: a column whose
+    weights or intercept became non-finite raises `_plain_sgd`'s ValueError with its epoch, and a column that ran
+    all max_iter epochs with a tolerance set emits `BaseSGDClassifier._fit`'s ConvergenceWarning (once)."""
+    from sklearn.exceptions import ConvergenceWarning
+    status = np.asarray(status).astype(np.int64)
+    n_iter = np.asarray(n_iter).astype(np.int64)
+    bad = np.flatnonzero(status == SGD_DIVERGED)
+    done = n_iter if bad.size == 0 else n_iter[:bad[0]]       # the columns scikit-learn fits before it raises
+    tol = template.tol
+    if tol is not None and tol > -np.inf and np.any(done == template.max_iter):
+        warnings.warn("Maximum number of iteration reached before convergence. Consider increasing max_iter to "
+                      "improve the fit.", ConvergenceWarning)
+    if bad.size:
+        raise ValueError("Floating-point under-/overflow occurred at epoch #%d. Scaling input data with "
+                         "StandardScaler or MinMaxScaler might help." % int(n_iter[bad[0]]))
+
+
 def _negatives_rows(pos_mask, max_negatives, random_state, method):
     """Training rows of one label column under the reference's negative down-sampling
     (`_negatives_mask`, ref multiclass.py:76-106): every positive row plus the negatives that
@@ -199,13 +220,15 @@ class DistOneVsRestClassifier(_ScParamMixin, OneVsRestClassifier):
         elif type(base) is SGDClassifier:
             res = eng.sgd_fit_batch(base, mine.astype(np.int32))
             packed = np.concatenate([res["coef"], res["n_iter"][:, None].astype(np.float64),
-                                     res["t"][:, None]], axis=1)
-            extra_of = lambda row: {"n_iter_": int(row[-2]), "t_": float(row[-1])}
+                                     res["t"][:, None], res["status"][:, None].astype(np.float64)], axis=1)
+            extra_of = lambda row: {"n_iter_": int(row[-3]), "t_": float(row[-2])}
         else:
             raise NotImplementedError(
                 "%s has no device path; supported base estimators: LogisticRegression(solver='lbfgs'), "
                 "SGDClassifier.  (No CPU fallback by design.)" % type(base).__name__)
         full = parallel.all_gather_columns(packed, len(col_ids), rank, world)
+        if type(base) is SGDClassifier:
+            _check_sgd_status(base, full[:, -1], full[:, -3])
         by_col = {int(c): full[i] for i, c in enumerate(col_ids)}
         ests = []
         cols = [1] if (K == 2 and not multilabel) else range(n_cols)
@@ -310,7 +333,7 @@ class DistOneVsOneClassifier(_ScParamMixin, OneVsOneClassifier):
         rank, world, _ = parallel.dist_info()
         eng = get_engine()
         mine = parallel.shard_indices(len(pairs), rank, world)
-        packed = np.zeros((len(mine), d + 3))
+        packed = np.zeros((len(mine), d + 4))
         for r, k in enumerate(mine):
             i, j = pairs[k]
             cond = (ycls == i) | (ycls == j)
@@ -321,7 +344,9 @@ class DistOneVsOneClassifier(_ScParamMixin, OneVsOneClassifier):
             packed[r, :d + 1] = res["coef"][0]
             packed[r, d + 1] = res["n_iter"][0]
             packed[r, d + 2] = res["t"][0]
+            packed[r, d + 3] = res["status"][0]
         full = parallel.all_gather_columns(packed, len(pairs), rank, world)
+        _check_sgd_status(base, full[:, d + 3], full[:, d + 1])
         make = _Cloner(base)
         self.estimators_ = tuple(
             _binary_estimator(make, full[k][:d + 1], d, X_arr.dtype, n_iter_=int(full[k][d + 1]), t_=float(full[k][d + 2]))
