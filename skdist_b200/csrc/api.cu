@@ -769,10 +769,18 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   int32_t* hist = nullptr;
   const long hist_cap = max_rounds + rounds_per_sync + 4;
   SKD_CUDA(c, sx.alloc(&hist, (size_t)2 * hist_cap));
+  // SKDIST_B200_TRACE=2 on the tensor-core path: every evaluation also records its work deal
+  const bool trace_rounds = tr.on && c->prof && getenv("SKDIST_B200_TRACE")[0] == '2';
+  int32_t* deal_hist = nullptr;
+  if (trace_rounds && w.use_tc) {
+    SKD_CUDA(c, sx.alloc(&deal_hist, (size_t)4 * hist_cap));
+    SKD_CUDA(c, cudaMemsetAsync(deal_hist, 0, (size_t)4 * hist_cap * sizeof(int32_t), c->stream));
+  }
   std::vector<int> ev_round;              // round index of every profiled evaluation
   while (n_run > 0) {
     for (int k = 0; k < rounds_per_sync; ++k) {
       int nz_used = 0;
+      if (deal_hist) w.deal_log = rounds < hist_cap ? deal_hist + 4 * rounds : nullptr;
       if (c->prof) {
         if (c->prof_events.size() < ev_used + 2) {
           cudaEvent_t a, b;
@@ -806,6 +814,12 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   std::vector<int32_t> hhist((size_t)2 * std::max<long>(rounds, 1), 0);
   if (force_rounds == 0 && rounds > 0)
     SKD_CUDA(c, cudaMemcpyAsync(hhist.data(), hist, (size_t)2 * rounds * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  std::vector<int32_t> hdeal;
+  if (deal_hist) {
+    hdeal.resize((size_t)4 * std::min<long>(std::max<long>(rounds, 1), hist_cap));
+    SKD_CUDA(c, cudaMemcpyAsync(hdeal.data(), deal_hist, hdeal.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+    w.deal_log = nullptr;
+  }
   SKD_CUDA(c, cudaStreamSynchronize(c->stream));
   long live_rounds = 0;
   for (size_t e = 0; e < ev_round.size(); ++e) {
@@ -824,9 +838,13 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
     for (size_t i = 0; i + 1 < ev_used; i += 2) {
       float ms = 0.f;
       SKD_CUDA(c, cudaEventElapsedTime(&ms, c->prof_events[i], c->prof_events[i + 1]));
-      if (tr.on && getenv("SKDIST_B200_TRACE")[0] == '2')
-        fprintf(stderr, "[skd trace] round %3d slots %5d running %5d eval %7.3f ms\n", (int)(i / 2), round_act[i / 2],
-                round_run[i / 2], ms);
+      const size_t r = i / 2;
+      if (trace_rounds && 4 * r + 3 < hdeal.size())   // tensor-core deal: live groups, half-padding groups, CTAs, CTAs over >1 group
+        fprintf(stderr, "[skd trace] round %3d slots %5d running %5d groups %4d half %3d ctas %3d cross %3d eval %7.3f ms\n",
+                (int)r, round_act[r], round_run[r], hdeal[4 * r], hdeal[4 * r + 1], hdeal[4 * r + 2], hdeal[4 * r + 3], ms);
+      else if (trace_rounds)
+        fprintf(stderr, "[skd trace] round %3d slots %5d running %5d eval %7.3f ms\n", (int)r, round_act[r],
+                round_run[r], ms);
       if (round_run[i / 2] <= 0) continue;      // enqueued past convergence: the kernels returned at once
       c->prof_eval_ms += ms;
       c->prof_eval_flops += round_flops[i / 2];
@@ -1193,6 +1211,9 @@ int skd_linear_r2_batch(skd_ctx* ctx, int32_t B, const float* coef, const int32_
     SKD_CUDA(c, sx.alloc(&w.n_act, 1));
     SKD_CUDA(c, cudaMemsetAsync(w.Wh, 0, wbytes, c->stream));
     SKD_CUDA(c, cudaMemsetAsync(w.Wl, 0, wbytes, c->stream));
+    const size_t n_part = (size_t)tc_partials_per_slot() * B;   // per-chunk squared-error sums
+    SKD_CUDA(c, sx.alloc(&w.lossp, n_part));
+    SKD_CUDA(c, cudaMemsetAsync(w.lossp, 0, n_part * sizeof(double), c->stream));
     std::vector<double> hx((size_t)B * w.dp);
     for (size_t i = 0; i < hx.size(); ++i) hx[i] = (double)coef[i];
     double* dx;

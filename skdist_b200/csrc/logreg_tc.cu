@@ -39,8 +39,8 @@ namespace skd {
 constexpr int TC_BC = 128;       // slots per group
 constexpr int TC_R = 64;         // rows per tile (the unit of the tile lists and row bit matrices)
 constexpr int TC_SUB = 32;       // rows per ring sub-tile (wgmma N of GEMM1, K of GEMM2)
-constexpr int TC_NCH = 132;      // fixed row chunks per group (one partial sum per (chunk, slot)); 132 = 4 * 3 * 11
-                                 // divides evenly over 132 / 66 / 44 / 33 / 22 CTAs per group (1, 2, 3, 4, 6 groups per GPU)
+constexpr int TC_NCH = 132;      // fixed row chunks per group (one partial sum per (chunk, slot)); fixing it fixes
+                                 // the summation order of every result
 constexpr int TC_THREADS = 384;  // producer warpgroup + two consumer warpgroups
 // register split of the warpgroups (setmaxnreg): 128 * 24 + 256 * 240 = 64 512 of the SM's 65 536
 constexpr uint32_t TC_PRODUCER_REGS = 24;
@@ -218,6 +218,8 @@ struct TcParams {
   const uint32_t* mbits;     // TC_FIT: per-column training-row bits (nullptr: every row of the training folds)
   long long rb_words;
   int g_passes;              // MMA passes of the gradient product: 3 = G_hi X_hi + G_lo X_hi + G_hi X_lo, 2 = without G_lo X_hi
+  int32_t* deal_log;         // nullptr, or {live groups, groups whose second half is padding, CTAs, CTAs whose
+                             // range spans two or more groups} of this launch (the last entry zeroed by the caller)
 };
 
 // TC_FIT_UNI: fit where every slot of a group shares (held-out fold, positive class): the row's
@@ -288,21 +290,61 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
   __syncthreads();   // the last block-wide barrier: the roles part here
 
   // Work split.  A group's tile list (all tiles, or the tiles with training rows of the group's
-  // fold) is cut into TC_NCH fixed chunks; a unit = (group, chunk); the groups * TC_NCH units are
-  // dealt to the CTAs in contiguous ranges.  A chunk is always accumulated by ONE CTA from a zeroed
-  // accumulator and written to partial slot `chunk`, so the partial sums -- and with them every
-  // fitted coefficient -- do not depend on the grid, on how many columns share the batch, or on how
-  // many GPUs the columns were dealt to.  (The host picks grid = groups * parts so that all groups
-  // stream the same rows at the same time and X comes from HBM about once.)
+  // fold) is cut into TC_NCH fixed chunks; a unit = (group, chunk).  A chunk is always accumulated by
+  // ONE CTA from a zeroed accumulator and written to partial slot `chunk`, so the partial sums -- and
+  // with them every fitted coefficient -- do not depend on the grid, on how many columns share the
+  // batch, or on how many GPUs the columns were dealt to.
+  // The deal is made here, from the live slot count (the host's count may be a few optimiser rounds
+  // old).  The units of the live groups are ordered band-major: bands of band_w consecutive chunks,
+  // within a band by group, then by chunk.  That order is cut into gridDim.x equal contiguous ranges,
+  // one per CTA.  band_w is one CTA's share, so the CTAs of a band run different groups over the same
+  // rows at the same time and X comes from HBM about once per launch.  Every unit weighs the same,
+  // also when the group's second consumer warpgroup holds only padding (it then computes nothing, see
+  // the consumers): weighing such a unit half made the launches with such groups slower, because the
+  // live consumer alone takes much more than half the time of a full group's chunk.
   const int n_live = prm.n_act_dev ? min(prm.n_act, (int)*prm.n_act_dev) : prm.n_act;
-  const long long units = (long long)prm.groups * TC_NCH;
-  const long long u_begin = (long long)blockIdx.x * units / gridDim.x;
-  const long long u_end = (long long)(blockIdx.x + 1) * units / gridDim.x;
-  struct TcItem { int g, z, t0, t1; const int32_t* tl; };
-  auto get_item = [&](long long u, TcItem& it) -> bool {
-    it.g = (int)(u / TC_NCH);
-    it.z = (int)(u % TC_NCH);
-    if (it.g * TC_BC >= n_live) return false;   // group emptied since the host last looked
+  const int n_groups = max(0, min(prm.groups, (n_live + TC_BC - 1) / TC_BC));
+  // a fold segment is padded at its end and 128-aligned: slots [64, 128) of a group are all padding
+  // exactly when slot 64 is
+  auto half_padding = [&](int g) -> bool {
+    const int s = g * TC_BC + 64;
+    return s >= n_live || prm.sp[s].col < 0;
+  };
+  struct TcWalk { int g, z, b0, b1, pos; };   // unit (g, chunk z) in band [b0, b1), its position in the order
+  const long long total = (long long)TC_NCH * n_groups;
+  const int pos_begin = (int)((long long)blockIdx.x * total / gridDim.x);
+  const int pos_end = (int)((long long)(blockIdx.x + 1) * total / gridDim.x);
+  const int band_w = (int)min((long long)TC_NCH, max(1LL, (total + gridDim.x - 1) / gridDim.x));
+  TcWalk start{0, TC_NCH, TC_NCH, TC_NCH, (int)total};
+  if (pos_begin < pos_end) {
+    start.b0 = pos_begin / (band_w * n_groups) * band_w;   // every earlier band is band_w chunks wide
+    start.b1 = min(start.b0 + band_w, TC_NCH);
+    const int off = pos_begin - start.b0 * n_groups, width = start.b1 - start.b0;
+    start.g = off / width;
+    start.z = start.b0 + off % width;
+    start.pos = pos_begin;
+  }
+  auto next_unit = [&](TcWalk& w) {
+    ++w.pos;
+    if (++w.z < w.b1) return;
+    if (++w.g == n_groups) { w.g = 0; w.b0 = w.b1; w.b1 = min(w.b1 + band_w, TC_NCH); }
+    w.z = w.b0;
+  };
+  if (prm.deal_log && threadIdx.x == 0) {
+    if (blockIdx.x == 0) {
+      int halves = 0;
+      for (int g = 0; g < n_groups; ++g) halves += half_padding(g) ? 1 : 0;
+      prm.deal_log[0] = n_groups;
+      prm.deal_log[1] = halves;
+      prm.deal_log[2] = gridDim.x;
+    }
+    if (pos_begin < pos_end && pos_end > start.pos + (start.b1 - start.z)) atomicAdd(prm.deal_log + 3, 1);
+  }
+  struct TcItem { int g, z, t0, t1; bool half; const int32_t* tl; };
+  auto get_item = [&](const TcWalk& w, TcItem& it) -> bool {
+    it.g = w.g;
+    it.z = w.z;
+    it.half = half_padding(w.g);
     int cnt = prm.n_tiles;
     it.tl = nullptr;
     if (prm.tilelist) {
@@ -329,7 +371,7 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
     if (threadIdx.x == 0) {
       uint32_t k = 0;
       int w_loads = 0, g_prev = -1;
-      for (long long u = u_begin; u < u_end; ++u) {
+      for (TcWalk u = start; u.pos < pos_end; next_unit(u)) {
         TcItem it;
         if (!get_item(u, it)) continue;
         if (it.g != g_prev) {
@@ -385,7 +427,7 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
 
   uint32_t h = 0;          // running sub-tile counter (ring position), identical in both consumers
   int w_loads = 0, g_prev = -1;
-  for (long long u = u_begin; u < u_end; ++u) {
+  for (TcWalk u = start; u.pos < pos_end; next_unit(u)) {
     TcItem it;
     if (!get_item(u, it)) continue;
     const int g = it.g, z_part = it.z;
@@ -396,6 +438,21 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
       if (g_prev >= 0 && wg_leader) mbar_arrive(&bars->w_free);
       mbar_wait(&bars->w_full, (w_loads++) & 1, 200);
       g_prev = g;
+    }
+    if (cw == 1 && it.half) {
+      // all 64 slots of this warpgroup are padding: no products, no epilogue, no partials.  It still
+      // takes its turns (so the other consumer's hand-overs complete) and releases every stage once
+      // the stage is loaded (the ring's phases then stay in step with the producer's).
+      for (int j = 0; j < nsub; ++j) {
+        const uint32_t hh = h + j, sl = hh % NS;
+        mbar_wait(&bars->full[sl], (hh / NS) & 1, 211);
+        turn_begin();
+        turn_end();
+        if (wg_leader) mbar_arrive(&bars->empty[sl]);
+      }
+      if (IS_FIT) { turn_begin(); turn_end(); }   // the turn of the item's last GEMM2
+      h += nsub;
+      continue;
     }
 
     // the two slots of this thread
@@ -631,8 +688,8 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
           if (IS_FIT) {   // partial (z_part, slot) has exactly one writer
             prm.lossp[(size_t)z_part * prm.n_act + slot[s]] = ls * (double)INV_G;
             prm.gsump[(size_t)z_part * prm.n_act + slot[s]] = gs * (double)INV_G;
-          } else {
-            atomicAdd(prm.lossp + slot[s], ls);   // sum of squared residuals (parts add up)
+          } else {        // sum of squared residuals of chunk z_part (added in chunk order by tc_r2)
+            prm.lossp[(size_t)z_part * prm.n_act + slot[s]] = ls;
           }
         }
       }
@@ -842,15 +899,11 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
   const int nchunk = t.dpad / 64;
   const int groups = (n_act + TC_BC - 1) / TC_BC;
   const int n_tiles = (int)(t.npad / TC_R);
-  // Grid: units = (group, chunk) pairs (see the kernel).  With few groups every group gets the same
-  // number of CTAs ("parts", at most one per chunk), so all groups stream the same rows at the same
-  // time and the other groups' reads hit L2; with many groups the units are simply dealt evenly.
+  // Grid: one CTA per SM (fewer if there are fewer (group, chunk) units); every CTA makes its share
+  // of the deal from the live slot count on the device (see the kernel), so the launch shape does not
+  // depend on how stale the host's count is.
   const long long units = (long long)groups * TC_NCH;
-  int grid = c->sm_count;
-  int parts = groups <= c->sm_count ? c->sm_count / groups : 0;
-  if (parts > TC_NCH) parts = TC_NCH;
-  if (parts > 0) grid = groups * parts;
-  if ((long long)grid > units) grid = (int)units;
+  const int grid = (int)std::min<long long>(c->sm_count, units);
   const int nz = TC_NCH;
   if (mode == TC_FIT) {
     if ((int64_t)nz * n_act > w.cap_sc) return fail(c, "tc_eval: partial buffer too small");
@@ -883,6 +936,7 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
   prm.ybits = mode == TC_FIT ? w.ybits : nullptr;
   prm.mbits = mode == TC_FIT ? w.mbits : nullptr;
   prm.rb_words = w.rb_words;
+  prm.deal_log = mode == TC_FIT ? w.deal_log : nullptr;
   // TC_FIT_UNI reads a row's sign from the list of the group's fold, so it needs one list per staged
   // fold (tc_prepare builds them for at most 32 folds); otherwise TC_FIT decodes the fold per element
   const bool uni = mode == TC_FIT && w.grouped && w.uni_pos >= 0 && c->ycls && !w.ybits && !w.mbits &&
@@ -923,13 +977,24 @@ int tc_score(Ctx* c, LogregWork& w, int n_act, int64_t* dcorrect, int64_t* dcoun
   return tc_run(c, w, n_act, TC_SCORE, nullptr, (unsigned long long*)dcorrect, (unsigned long long*)dcount);
 }
 
-// Sum of squared residuals / row counts of n_act regression slots (sp.fold = scoring code).
+__global__ void tc_chunk_sum_kernel(const double* __restrict__ part, int n_act, double* __restrict__ out) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n_act) return;
+  double acc = 0.0;
+  for (int z = 0; z < TC_NCH; ++z) acc += part[(size_t)z * n_act + s];
+  out[s] = acc;
+}
+
+// Sum of squared residuals / row counts of n_act regression slots (sp.fold = scoring code).  The kernel
+// writes one partial per (chunk, slot) into w.lossp ([TC_NCH x n_act], zeroed by the caller: chunks
+// without tiles are not written); they are added here in chunk order, so the sums do not depend on
+// which CTA ran which chunk.
 int tc_r2(Ctx* c, LogregWork& w, int n_act, double* dsse, int64_t* dcount) {
-  double* keep = w.lossp;
-  w.lossp = dsse;
-  int rc = tc_run(c, w, n_act, TC_R2, nullptr, nullptr, (unsigned long long*)dcount);
-  w.lossp = keep;
-  return rc;
+  if (tc_run(c, w, n_act, TC_R2, nullptr, nullptr, (unsigned long long*)dcount)) return 1;
+  tc_chunk_sum_kernel<<<(n_act + 255) / 256, 256, 0, c->stream>>>(w.lossp, n_act, dsse);
+  c->launches += 1;
+  SKD_CUDA(c, cudaGetLastError());
+  return 0;
 }
 
 }  // namespace skd

@@ -240,6 +240,7 @@ struct LogregWork {
   int32_t slot_cap = 0;        // slots incl. padding at the start of the solve
   int32_t* n_run = nullptr;    // device scalar: columns still running
   int32_t uni_pos = -1;        // >= 0: every column of the batch has this positive class (grouped layout only)
+  int32_t* deal_log = nullptr; // device [4] or nullptr: the next evaluation's work deal (TcParams::deal_log)
 };
 
 // forward (Z = X W^T, pointwise loss / gradient on training rows) + backward (G^T X)
