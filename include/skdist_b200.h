@@ -87,6 +87,15 @@ int skd_stage_column_masks(skd_ctx* ctx, int32_t B, const uint8_t* mask);
 int skd_stage_row_bits(skd_ctx* ctx, int32_t B, const uint8_t* label_bits, const uint8_t* train_bits,
                        int64_t bytes_per_col);
 
+/* Class weights for the NEXT skd_logreg_fit_batch, skd_logreg_loss_grad or skd_logreg_multinomial_fit_batch
+ * call (one-shot; w = NULL or B = 0 clears).  w [B x K] float32, finite and >= 0: weight of each class in
+ * column j (binary calls: K = 2, w[2j] for label 0 and w[2j + 1] for label 1; multinomial: K = n_classes,
+ * indexed by class id).  sw_sum [B] > 0: the sum of the per-row weights over the column's training rows.
+ * The call that reads them fails unless its B (and K) match.  Each training row's loss and gradient entry
+ * is multiplied by its weight, and sw_sum takes the place of n_train in the mean and in the l2 strength
+ * 1 / (C sw_sum).  ref: `class_weight` of LogisticRegression (SK/linear_model/_logistic.py:429-474). */
+int skd_stage_class_weights(skd_ctx* ctx, int32_t B, int32_t K, const float* w, const double* sw_sum);
+
 /* Batched binary L2 logistic regression (lbfgs), B independent columns sharing X.
  * Column j: positives = rows with y_class == col_pos[j]; training rows = rows whose fold id
  * != col_fold[j] (col_fold[j] < 0: all rows); l2 strength = 1 / (C[j] * n_train_j).

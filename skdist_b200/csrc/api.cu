@@ -4,6 +4,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <mutex>
 #include <thread>
 #include <atomic>
@@ -549,6 +550,54 @@ int skd_stage_row_bits(skd_ctx* ctx, int32_t B, const uint8_t* label_bits, const
   return 0;
 }
 
+int skd_stage_class_weights(skd_ctx* ctx, int32_t B, int32_t K, const float* w, const double* sw_sum) {
+  if (!ctx) return fail(nullptr, "skd_stage_class_weights: ctx is NULL");
+  Ctx* c = &ctx->c;
+  c->cw_cols = 0; c->cw_k = 0;
+  c->h_cw.clear(); c->h_swsum.clear();
+  if (B <= 0 || !w) return 0;   // cleared
+  if (K < 2 || !sw_sum) return fail(c, "skd_stage_class_weights: bad arguments");
+  for (int64_t i = 0; i < (int64_t)B * K; ++i)
+    if (!(std::isfinite(w[i]) && w[i] >= 0.f)) return fail(c, "skd_stage_class_weights: weights must be finite and >= 0");
+  for (int j = 0; j < B; ++j)
+    if (!(std::isfinite(sw_sum[j]) && sw_sum[j] > 0.0))
+      return fail(c, "skd_stage_class_weights: the sum of a column's weights must be finite and positive");
+  c->h_cw.assign(w, w + (size_t)B * K);
+  c->h_swsum.assign(sw_sum, sw_sum + B);
+  c->cw_cols = B;
+  c->cw_k = K;
+  return 0;
+}
+
+namespace {
+// Staged class weights are one-shot: the guard takes them off the context for the call that reads them.
+struct ClassWeightGuard {
+  std::vector<float> w; std::vector<double> sw_sum; int32_t cols, k;
+  explicit ClassWeightGuard(Ctx* c) : cols(c->cw_cols), k(c->cw_k) {
+    w.swap(c->h_cw); sw_sum.swap(c->h_swsum); c->cw_cols = 0; c->cw_k = 0;
+  }
+  // Binary columns: weights scaled by the power of two 2^-e that brings the larger one into (1/2, 1], so
+  // that |G| <= 2^14 holds in the fp16 operand of the tensor-core gradient product; 2^e goes into inv_n.
+  // Both scalings are exact.  l2 = 1 / (C sw_sum), inv_n = 2^e / sw_sum (SK/linear_model/_logistic.py:474, 580).
+  int binary(Ctx* c, const char* who, int B, const double* C, std::vector<float2>& cw, std::vector<double>& l2,
+             std::vector<double>& inv_n) const {
+    if (cols != B || k != 2) return fail(c, std::string(who) + ": staged class weights do not match this batch (B x 2)");
+    cw.resize(B);
+    for (int j = 0; j < B; ++j) {
+      const float mx = std::max(w[2 * j], w[2 * j + 1]);
+      if (!(mx > 0.f)) return fail(c, std::string(who) + ": every class weight of a column is 0");
+      int e;
+      const float f = frexpf(mx, &e);   // mx = f 2^e, f in [1/2, 1)
+      if (f == 0.5f) e -= 1;             // a power of two becomes exactly 1
+      cw[j] = make_float2(ldexpf(w[2 * j], -e), ldexpf(w[2 * j + 1], -e));
+      l2[j] = 1.0 / (C[j] * sw_sum[j]);
+      inv_n[j] = ldexp(1.0 / sw_sum[j], e);
+    }
+    return 0;
+  }
+};
+}  // namespace
+
 int skd_set_kernel(skd_ctx* ctx, int32_t which) {
   if (!ctx) return -1;
   int prev = ctx->c.kernel_choice;
@@ -611,6 +660,7 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
                          double* gpu_seconds_out) {
   if (!ctx) return fail(nullptr, "skd_logreg_fit_batch: ctx is NULL");
   Ctx* c = &ctx->c;
+  const ClassWeightGuard staged_cw(c);   // one-shot: staged class weights do not outlive this call
   if (!c->X || !c->ycls) return fail(c, "skd_logreg_fit_batch: stage X and labels first");
   if (B <= 0 || !C || !col_fold || !col_pos || !coef_out || !n_iter_out || !status_out)
     return fail(c, "skd_logreg_fit_batch: bad arguments");
@@ -675,6 +725,8 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
     inv_n[j] = 1.0 / (double)ntrain;
     mean_ntrain += (double)ntrain / B;
   }
+  std::vector<float2> hcw;
+  if (staged_cw.cols > 0 && staged_cw.binary(c, "skd_logreg_fit_batch", B, C, hcw, l2, inv_n)) return 1;
 
   Trace tr(c, "logreg_fit");
   Scratch sx(c);
@@ -696,6 +748,13 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
     SKD_CUDA(c, sx.alloc(&w.col_neg1, (size_t)B));
   }
   SKD_CUDA(c, sx.alloc(&w.n_evals, (size_t)B));
+  if (!hcw.empty()) {
+    float2* dcw;
+    SKD_CUDA(c, sx.alloc(&dcw, (size_t)B));
+    SKD_CUDA(c, cudaMemcpyAsync(dcw, hcw.data(), B * sizeof(float2), cudaMemcpyHostToDevice, c->stream));
+    c->h2d += (int64_t)B * 8;
+    w.cw = dcw;
+  }
   const bool use_fmask = staged_masks.cols > 0;
   if (use_fmask) {
     if (staged_masks.cols != B || (int64_t)staged_masks.mask.size() != (int64_t)B * d)
@@ -877,6 +936,7 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
                          double* loss_out, double* grad_out) {
   if (!ctx) return fail(nullptr, "skd_logreg_loss_grad: ctx is NULL");
   Ctx* c = &ctx->c;
+  const ClassWeightGuard staged_cw(c);   // one-shot: staged class weights do not outlive this call
   if (!c->X || !c->ycls) return fail(c, "skd_logreg_loss_grad: stage X and labels first");
   if (B <= 0 || !w_in || !C || !col_fold || !col_pos || !loss_out || !grad_out)
     return fail(c, "skd_logreg_loss_grad: bad arguments");
@@ -897,9 +957,17 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
     for (int k = 0; k < d; ++k) hw[(size_t)j * ldx + k] = (float)w_in[(size_t)j * dp + k];
     hw[(size_t)B * ldx + j] = fit_intercept ? (float)w_in[(size_t)j * dp + d] : 0.f;
   }
+  std::vector<float2> hcw;
+  if (staged_cw.cols > 0 && staged_cw.binary(c, "skd_logreg_loss_grad", B, C, hcw, l2, inv_n)) return 1;
   Scratch sx(c);
   LogregWork w;
   w.B = B; w.dp = dp;
+  if (!hcw.empty()) {
+    float2* dcw;
+    SKD_CUDA(c, sx.alloc(&dcw, (size_t)B));
+    SKD_CUDA(c, cudaMemcpyAsync(dcw, hcw.data(), B * sizeof(float2), cudaMemcpyHostToDevice, c->stream));
+    w.cw = dcw;
+  }
   // the slot layout of skd_logreg_fit_batch: fold-grouped on the tensor cores, slot s = column s on SIMT
   std::vector<SlotMeta> hs;
   if (alloc_logreg_slots(c, sx, w, B, col_fold, col_pos, nullptr, hs)) return 1;
@@ -1022,6 +1090,7 @@ int skd_logreg_multinomial_fit_batch(skd_ctx* ctx, int32_t B, int32_t n_classes,
                                      int32_t* n_evals_out, double* gpu_seconds_out) {
   if (!ctx) return fail(nullptr, "skd_logreg_multinomial_fit_batch: ctx is NULL");
   Ctx* c = &ctx->c;
+  const ClassWeightGuard staged_cw(c);   // one-shot: staged class weights do not outlive this call
   if (!c->X || !c->ycls) return fail(c, "skd_logreg_multinomial_fit_batch: stage X and labels first");
   if (B <= 0 || n_classes < 2 || !C || !col_fold || !coef_out || !n_iter_out || !status_out)
     return fail(c, "skd_logreg_multinomial_fit_batch: bad arguments");
@@ -1038,6 +1107,8 @@ int skd_logreg_multinomial_fit_batch(skd_ctx* ctx, int32_t B, int32_t n_classes,
   c->fmask_cols = 0;
   if (mask_cols > 0 && (mask_cols != B || (int64_t)masks.size() != (int64_t)B * c->d))
     return fail(c, "skd_logreg_multinomial_fit_batch: staged column masks do not match the batch");
+  if (staged_cw.cols > 0 && (staged_cw.cols != B || staged_cw.k != n_classes))
+    return fail(c, "skd_logreg_multinomial_fit_batch: staged class weights do not match this batch (B x n_classes)");
   SKD_CUDA(c, cudaSetDevice(c->device));
   Trace tr(c, "multinomial_fit");
   cudaEvent_t e0, e1;
@@ -1045,7 +1116,8 @@ int skd_logreg_multinomial_fit_batch(skd_ctx* ctx, int32_t B, int32_t n_classes,
   SKD_CUDA(c, cudaEventCreate(&e1));
   SKD_CUDA(c, cudaEventRecord(e0, c->stream));
   const int rc = multi_fit(c, B, n_classes, C, col_fold, fit_intercept, tol, max_iter, mask_cols > 0 ? masks.data() : nullptr,
-                           coef_out, n_iter_out, status_out, loss_out, n_evals_out);
+                           staged_cw.cols > 0 ? staged_cw.w.data() : nullptr,
+                           staged_cw.cols > 0 ? staged_cw.sw_sum.data() : nullptr, coef_out, n_iter_out, status_out, loss_out, n_evals_out);
   float ms = 0.f;
   if (!rc) {
     cudaEventRecord(e1, c->stream);

@@ -32,11 +32,12 @@ __global__ void __launch_bounds__(256)
 mn_pointwise_kernel(float* __restrict__ G, int ldg, int64_t n, int64_t rpc, int K,
                     const SlotMeta* __restrict__ cand, const int32_t* __restrict__ n_act_dev, int n_act_in,
                     const int32_t* __restrict__ ycls, const int8_t* __restrict__ fold,
-                    double* __restrict__ lossp) {
+                    double* __restrict__ lossp, const float* __restrict__ cw) {
   __shared__ double red[8];
   const int a = blockIdx.x, z = blockIdx.y;
   if (a >= *n_act_dev) return;
   const int f = cand[a].fold;
+  const float* wk = cw ? cw + (size_t)cand[a].col * K : nullptr;   // class weights of the candidate
   const int64_t row_begin = (int64_t)z * rpc;
   int64_t row_end = row_begin + rpc;
   if (row_end > n) row_end = n;
@@ -56,10 +57,20 @@ mn_pointwise_kernel(float* __restrict__ G, int ldg, int64_t n, int64_t rpc, int 
     const float sum_f = (float)sum;
     float loss = (float)(log((double)sum_f) + (double)mx);
     loss -= zr[y];
-    for (int k = 0; k < K; ++k) {
-      float p = (float)exp((double)zr[k] - (double)mx);
-      p /= sum_f;
-      zr[k] = p - (k == y ? 1.f : 0.f);
+    if (wk) {   // sample weight of the row: float32 products, as SK/_loss/_loss.pyx.tp:1348-1350
+      const float sw = wk[y];
+      for (int k = 0; k < K; ++k) {
+        float p = (float)exp((double)zr[k] - (double)mx);
+        p /= sum_f;
+        zr[k] = (p - (k == y ? 1.f : 0.f)) * sw;
+      }
+      loss *= sw;
+    } else {
+      for (int k = 0; k < K; ++k) {
+        float p = (float)exp((double)zr[k] - (double)mx);
+        p /= sum_f;
+        zr[k] = p - (k == y ? 1.f : 0.f);
+      }
     }
     acc += (double)loss;
   }
@@ -150,8 +161,8 @@ static int64_t candidates_per_pass(const Ctx* c, int K, int nz) {
 }
 
 int multi_fit(Ctx* c, int B, int K, const double* C, const int32_t* col_fold, int fit_intercept, double tol,
-              int max_iter, const uint8_t* fmask, float* coef_out, int32_t* n_iter_out, int32_t* status_out,
-              double* loss_out, int32_t* n_evals_out) {
+              int max_iter, const uint8_t* fmask, const float* cw, const double* sw_sum, float* coef_out,
+              int32_t* n_iter_out, int32_t* status_out, double* loss_out, int32_t* n_evals_out) {
   const int64_t n = c->n, ldx = c->ldx;
   const int dp = (int)c->d + 1, m = 10;
   int nz;
@@ -165,8 +176,10 @@ int multi_fit(Ctx* c, int B, int K, const double* C, const int32_t* col_fold, in
       const int f = col_fold[b0 + j];
       const int64_t ntrain = f >= 0 ? n - c->fold_count[f] : n;
       if (ntrain <= 0) return fail(c, "skd_logreg_multinomial_fit_batch: empty training set");
-      l2[j] = 1.0 / (C[b0 + j] * (double)ntrain);   // SK/linear_model/_logistic.py:580
-      inv_n[j] = 1.0 / (double)ntrain;
+      // weighted: the sum of the per-row weights takes the place of n_train (SK/linear_model/_logistic.py:474)
+      const double sw = sw_sum ? sw_sum[b0 + j] : (double)ntrain;
+      l2[j] = 1.0 / (C[b0 + j] * sw);   // SK/linear_model/_logistic.py:580
+      inv_n[j] = 1.0 / sw;
     }
     Scratch sx(c);
     MultiWork w;
@@ -197,6 +210,13 @@ int multi_fit(Ctx* c, int B, int K, const double* C, const int32_t* col_fold, in
       SKD_CUDA(c, cudaMemcpyAsync(w.fmask, fmask + (size_t)b0 * c->d, (size_t)Bb * c->d, cudaMemcpyHostToDevice, c->stream));
       c->h2d += (int64_t)Bb * c->d;
     }
+    if (cw) {
+      float* dcw;
+      SKD_CUDA(c, sx.alloc(&dcw, (size_t)Bb * K));
+      SKD_CUDA(c, cudaMemcpyAsync(dcw, cw + (size_t)b0 * K, (size_t)Bb * K * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+      c->h2d += (int64_t)Bb * K * 4;
+      w.cw = dcw;
+    }
     if (multi_lbfgs_init(c, w, d_fold, tol, max_iter)) return 1;
 
     // several optimiser rounds per host round trip; the kernels read the live candidate count from
@@ -210,7 +230,7 @@ int multi_fit(Ctx* c, int B, int K, const double* C, const int32_t* col_fold, in
         const int ns = n_act * K;
         if (simt_raw_prediction(c, ns, w.W, w.W + slots * ldx, w.G, w.ldg)) return 1;
         mn_pointwise_kernel<<<dim3(n_act, nz), 256, 0, c->stream>>>(w.G, w.ldg, n, rpc, K, w.cand, w.n_act, n_act,
-                                                                   c->ycls, c->fold, w.lossp);
+                                                                   c->ycls, c->fold, w.lossp, w.cw);
         mn_colsum_kernel<<<dim3((ns + 63) / 64, nz), 256, 0, c->stream>>>(w.G, w.ldg, n, rpc, ns, w.gsump);
         c->launches += 2;
         if (simt_backward(c, w.G, w.ldg, ns, nz, rpc, w.gradp)) return 1;

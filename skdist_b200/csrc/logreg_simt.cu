@@ -54,7 +54,7 @@ fwd_kernel(const float* __restrict__ X, int64_t n, int ldx, const float* __restr
            double* __restrict__ gsump, int64_t* __restrict__ correct, int64_t* __restrict__ count,
            float* __restrict__ dec, int ldd, const float* __restrict__ yreal,
            const uint32_t* __restrict__ ybits = nullptr, const uint32_t* __restrict__ mbits = nullptr,
-           long long rb_words = 0) {
+           long long rb_words = 0, const float2* __restrict__ cw = nullptr) {
   __shared__ float As[TK][TM + 4];
   __shared__ float Bs[TK][TN + 4];
   __shared__ double red[16][TN + 1];
@@ -147,6 +147,12 @@ fwd_kernel(const float* __restrict__ X, int64_t n, int ldx, const float* __restr
             double y = ypos ? 1.0 : 0.0;
             double l, g;
             loss_grad_half_binomial(y, (double)raw, l, g);
+            if (cw) {   // the row's class weight times the double results (SK/_loss/_loss.pyx.tp:1083-1084)
+              const float2 wc = cw[scol[j]];
+              const double sw = (double)(ypos ? wc.y : wc.x);
+              l *= sw;
+              g *= sw;
+            }
             float lf = (float)l, gf = (float)g;   // sklearn stores both as float32
             acc_loss[j] += (double)lf;
             acc_g[j] += (double)gf;
@@ -306,7 +312,7 @@ int simt_eval(Ctx* c, LogregWork& w, int n_act, int* nz_used) {
   fwd_kernel<MODE_FIT><<<gf, 256, 0, c->stream>>>(
       c->X, c->n, ldx, w.Wact, w.Wact + (size_t)w.B * ldx /*bias block*/, w.slot, n_act, c->ycls,
       c->fold, rpc, w.G, w.ldg, w.lossp, w.gsump, nullptr, nullptr, nullptr, 0, nullptr, w.ybits, w.mbits,
-      (long long)w.rb_words);
+      (long long)w.rb_words, w.cw);
   dim3 gb((ldx + 63) / 64, (n_act + TN - 1) / TN, nz);
   bwd_kernel<<<gb, 256, 0, c->stream>>>(c->X, c->n, ldx, w.G, w.ldg, n_act, rpc, w.gradp);
   c->launches += 2;

@@ -220,11 +220,15 @@ struct TcParams {
   int g_passes;              // MMA passes of the gradient product: 3 = G_hi X_hi + G_lo X_hi + G_hi X_lo, 2 = without G_lo X_hi
   int32_t* deal_log;         // nullptr, or {live groups, groups whose second half is padding, CTAs, CTAs whose
                              // range spans two or more groups} of this launch (the last entry zeroed by the caller)
+  const float2* cw;          // TC_FIT_W / TC_FIT_UNI_W: per-column {label-0, label-1} class weights, largest <= 1
 };
 
 // TC_FIT_UNI: fit where every slot of a group shares (held-out fold, positive class): the row's
-// sign/mask comes from a precomputed per-fold array instead of being decoded per element
-enum { TC_FIT = 0, TC_SCORE = 1, TC_R2 = 2, TC_FIT_UNI = 3 };
+// sign/mask comes from a precomputed per-fold array instead of being decoded per element.
+// TC_FIT_W / TC_FIT_UNI_W: the same two fits with class weights (each row's loss and gradient entry
+// times its column's weight for the row's label), separate instantiations so that the unweighted
+// ones stay as they are.
+enum { TC_FIT = 0, TC_SCORE = 1, TC_R2 = 2, TC_FIT_UNI = 3, TC_FIT_W = 4, TC_FIT_UNI_W = 5 };
 
 // shared memory of one CTA: W_hi, W_lo [NCHUNK][128 slots x 64 fp16] + the ring of sub-tiles
 template <int NCHUNK>
@@ -265,7 +269,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant__ CUtensorMap map_xl,
                const __grid_constant__ CUtensorMap map_wh, const __grid_constant__ CUtensorMap map_wl,
                const TcParams prm) {
-  constexpr bool IS_FIT = MODE == TC_FIT || MODE == TC_FIT_UNI;
+  constexpr bool UNI = MODE == TC_FIT_UNI || MODE == TC_FIT_UNI_W;   // row sign from the per-fold arrays
+  constexpr bool DECODE = MODE == TC_FIT || MODE == TC_FIT_W;        // row sign decoded per element
+  constexpr bool WEIGHTED = MODE == TC_FIT_W || MODE == TC_FIT_UNI_W;
+  constexpr bool IS_FIT = UNI || DECODE;
   using SM = TcSmem<NCHUNK>;
   constexpr int NS = SM::NS;
   extern __shared__ uint8_t smem_raw[];
@@ -474,8 +481,14 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
       zi[s] = IS_FIT ? sp[s].inv_t * INV_G : sp[s].inv_t;
       zb0[s] = IS_FIT ? sp[s].bias * INV_G : sp[s].bias;
     }
+    float2 cwt[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};   // class weights of the two slots
+    if constexpr (WEIGHTED) {
+#pragma unroll
+      for (int s = 0; s < 2; ++s)
+        if (sp[s].col >= 0) cwt[s] = __ldg(prm.cw + sp[s].col);
+    }
     const float* rsg = nullptr;
-    if (MODE == TC_FIT_UNI) {
+    if (UNI) {
       const int f = prm.sp[g * TC_BC].fold;
       const int li = (f >= 0 && f < prm.n_lists - 1) ? f : prm.n_lists - 1;
       rsg = prm.rowsg + (size_t)li * prm.rowsg_ld;
@@ -547,7 +560,7 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         const int r = r0 + 8 * q + cq;
-        if (MODE == TC_FIT_UNI) {
+        if (UNI) {
           const float2 v = __ldg(reinterpret_cast<const float2*>(rsg + r));
           rm[2 * q] = __float_as_uint(v.x); rm[2 * q + 1] = __float_as_uint(v.y);
         } else {
@@ -560,7 +573,7 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
         }
       }
       uint32_t ybw[2] = {0u, 0u}, mbw[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
-      if (MODE == TC_FIT && (prm.ybits || prm.mbits)) {
+      if (DECODE && (prm.ybits || prm.mbits)) {
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
           if (sp[s].col < 0) continue;
@@ -581,7 +594,7 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
           const int s = (i >> 1) & 1;
           const int rr = 2 * (i >> 2) + (i & 1);        // index into rm: row r0 + 8 (i >> 2) + cq + (i & 1)
           float sg;                       // -y * 2^14 for a training row, 0 otherwise
-          if (MODE == TC_FIT_UNI) {
+          if (UNI) {
             sg = __uint_as_float(rm[rr]);
           } else {
             const uint32_t m = rm[rr];
@@ -589,13 +602,16 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
             const int cls = (int)(m & 0x00FFFFFFu);
             bool yb = cls == sp[s].pos;
             bool train = (fr != 0xFF) && (fr != sp[s].fold) && (sp[s].neg1 == 0 || yb || cls == sp[s].neg1 - 1);
-            if (MODE == TC_FIT) {             // staged row bit matrices (multilabel targets, sampled negatives)
+            {                                 // staged row bit matrices (multilabel targets, sampled negatives)
               const int bit = 8 * (i >> 2) + cq + (i & 1);
               if (prm.ybits) yb = (ybw[s] >> bit) & 1u;
               if (prm.mbits) train = train && ((mbw[s] >> bit) & 1u);
             }
             sg = train ? (yb ? -GSCALE : GSCALE) : 0.f;
           }
+          // factor of the row's loss and gradient entry: sg times the class weight of the row's label
+          // (label 1 exactly when sg < 0); the margin below keeps the unweighted sg
+          const float sgw = WEIGHTED ? sg * (sg < 0.f ? cwt[s].y : cwt[s].x) : sg;
           const float zp = fmaf(zf[i], zi[s], zb0[s]);
           const float uu = sg * zp;       // = -y * z
           const float e = ex2_approx(-fabsf(uu) * 1.4426950408889634f);
@@ -603,8 +619,8 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
           const float loss = fmaf(lg2_approx(s1), 0.6931471805599453f, fmaxf(uu, 0.f));
           const float r = rcp_approx(s1);
           const float sig = (uu >= 0.f) ? r : e * r;
-          gv[i] = sg * sig;               // 2^14 * dloss/dz
-          lt[s] = fmaf(fabsf(sg), loss, lt[s]);   // 2^14 * loss
+          gv[i] = sgw * sig;              // 2^14 * weight * dloss/dz
+          lt[s] = fmaf(fabsf(sgw), loss, lt[s]);   // 2^14 * weight * loss
           gt[s] += gv[i];
         }
 #pragma unroll
@@ -958,7 +974,11 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
   prm.n_lists = t.n_lists;
   prm.n_tiles_ld = n_tiles;
   if (mode == TC_R2 && !t.yreal_pad) return fail(c, "tc_r2: targets not staged");
-  cudaError_t e = uni ? tc_launch<TC_FIT_UNI>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)
+  prm.cw = mode == TC_FIT ? w.cw : nullptr;
+  const bool weighted = prm.cw != nullptr;
+  cudaError_t e = (uni && weighted) ? tc_launch<TC_FIT_UNI_W>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)
+                  : uni ? tc_launch<TC_FIT_UNI>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)
+                  : (mode == TC_FIT && weighted) ? tc_launch<TC_FIT_W>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)
                   : mode == TC_FIT ? tc_launch<TC_FIT>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)
                   : mode == TC_SCORE ? tc_launch<TC_SCORE>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)
                                      : tc_launch<TC_R2>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm);

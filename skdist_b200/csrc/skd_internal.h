@@ -93,6 +93,12 @@ struct Ctx {
   std::vector<uint32_t> h_ybits, h_mbits;
   int32_t rb_cols = 0;
   int64_t rb_words = 0;
+  // per-column class weights staged for the next fit / loss-gradient call (skd_stage_class_weights):
+  // h_cw [cw_cols x cw_k] weight of each class (binary calls: label 0, label 1), h_swsum [cw_cols] the
+  // sum of the column's per-row weights over its training rows
+  std::vector<float> h_cw;
+  std::vector<double> h_swsum;
+  int32_t cw_cols = 0, cw_k = 0;
   // scratch pool: device blocks released by finished calls, reused by the next ones (Scratch below)
   std::vector<std::pair<void*, size_t>> pool_free;
   size_t pool_bytes = 0;
@@ -216,6 +222,8 @@ struct LogregWork {
   const uint32_t* ybits = nullptr;  // [B x rb_words] or nullptr: bit r of column j = its label of row r (instead of class id == pos)
   const uint32_t* mbits = nullptr;  // [B x rb_words] or nullptr: bit r of column j = row r trains the column
   int64_t rb_words = 0;
+  const float2* cw = nullptr;  // [B] or nullptr: {label-0, label-1} weights of column j, largest <= 1
+                               // (the power of two that normalised them is folded into inv_n)
   int32_t* n_evals = nullptr;  // [B]
   // per slot (active batch)
   SlotMeta* slot = nullptr;    // [B]
@@ -289,12 +297,14 @@ struct MultiWork {
   float* gradp = nullptr;        // [nz x B*K x ldx]
   int32_t* n_act = nullptr;      // device scalar: active candidates
   uint8_t* fmask = nullptr;      // [B x d] or nullptr: 1 = feature takes part in the candidate's fit
+  const float* cw = nullptr;     // [B x K] or nullptr: weight of each class in the candidate's fit
 };
 int multi_lbfgs_init(Ctx* c, MultiWork& w, const int32_t* d_col_fold, double tol, int max_iter);
 int multi_lbfgs_enqueue(Ctx* c, MultiWork& w, int n_act_in, int fit_intercept, int32_t* hist);
 int multi_lbfgs_finish(Ctx* c, MultiWork& w, float* dcoef, int32_t* dniter, int32_t* dstatus, double* dloss);
 int multi_fit(Ctx* c, int B, int K, const double* C, const int32_t* col_fold, int fit_intercept, double tol,
-              int max_iter, const uint8_t* fmask /*[B x d] or nullptr*/, float* coef_out, int32_t* n_iter_out,
+              int max_iter, const uint8_t* fmask /*[B x d] or nullptr*/,
+              const float* cw /*[B x K] or nullptr*/, const double* sw_sum /*[B] or nullptr*/, float* coef_out, int32_t* n_iter_out,
               int32_t* status_out, double* loss_out, int32_t* n_evals_out);
 int multi_score(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold, int64_t* conf_out);
 int logloss_batch(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold, const int32_t* col_pos,

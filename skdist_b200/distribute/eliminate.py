@@ -27,7 +27,7 @@ from .. import parallel
 from ..engine import get_engine
 from .base import _clone, _parse_partitions, _ScParamMixin
 from .folds import _fold_ids
-from .logreg_family import _check_logreg, _count_metric
+from .logreg_family import _check_logreg, _ClassWeights, _count_metric
 from .utils import _check_multimetric_scoring
 
 __all__ = ["DistFeatureEliminator"]
@@ -62,7 +62,7 @@ class DistFeatureEliminator(_ScParamMixin, ClassifierMixin, BaseEstimator):
             raise NotImplementedError(
                 "%s has no device path in DistFeatureEliminator; supported: LogisticRegression(solver='lbfgs')."
                 "  (No CPU fallback by design.)" % type(self.estimator).__name__)
-        p = _check_logreg(_clone(self.estimator))
+        p = _check_logreg(_clone(self.estimator), class_weight=True)
         scorers, _ = _check_multimetric_scoring(self.estimator, scoring=self.scoring)
         metric = _count_metric(scorers["score"])
         if metric is None or metric[0] not in ("accuracy", "roc_auc"):
@@ -93,8 +93,11 @@ class DistFeatureEliminator(_ScParamMixin, ClassifierMixin, BaseEstimator):
         eng.stage_folds(fold, n_splits)
         kw = dict(fit_intercept=p["fit_intercept"], tol=p["tol"], max_iter=p["max_iter"])
         one = np.ones(1, np.int32)
+        weights = _ClassWeights(classes, ycls)
+        weights.set_folds(fold, [np.asarray(train) for train, _ in cv_splits])
 
         def fit(C, folds):
+            weights.stage(eng, [p["class_weight"]] * len(C), folds)
             if multi:
                 return eng.logreg_multinomial_fit_batch(C, folds, n_classes, **kw)
             return eng.logreg_fit_batch(C, folds, np.ones(len(C), np.int32), **kw)

@@ -63,13 +63,15 @@ def _classes_and_ids(y, enc=None):
     return classes, np.searchsorted(classes, y).astype(np.int32)
 
 
-def _cv_fold_ids(cv, X, y, groups, n_samples, enc=None):
+def _cv_fold_ids(cv, X, y, groups, n_samples, enc=None, train_orders=None):
     """(fold id per row, n_splits) of a cross-validator.  The generic route materialises every
     (train, test) index pair like the reference does (search.py:379) and converts them; the two
     splitters `check_cv` produces for an integer `cv` -- unshuffled `StratifiedKFold` / `KFold` -- are
     restated directly (no per-split index arrays, no sorts over the rows), fold for fold what
     SK/model_selection/_split.py:774-841 (`_make_test_folds`) and :531-547 (`_iter_test_indices`) give.
-    `enc` (a _TargetCodes of y) saves the hash pass when the caller already has it."""
+    `enc` (a _TargetCodes of y) saves the hash pass when the caller already has it.  A list passed as
+    `train_orders` receives the train index arrays of the splits when the splits were materialised (else
+    every split's train rows are its complement in ascending order, as the two restated splitters give)."""
     from sklearn.model_selection import KFold, StratifiedKFold
     if type(cv) is KFold and not cv.shuffle and groups is None:
         k = cv.n_splits
@@ -98,10 +100,12 @@ def _cv_fold_ids(cv, X, y, groups, n_samples, enc=None):
                     fold[np.flatnonzero(y_encoded == c)] = np.repeat(np.arange(k, dtype=np.int8), alloc)
                 return fold, k
     cv_splitted = list(cv.split(X, y, groups))
+    if train_orders is not None:
+        train_orders[:] = [np.asarray(train) for train, _ in cv_splitted]
     return _fold_ids(cv_splitted, n_samples), len(cv_splitted)
 
 
-def _cv_fold_groups(cv, X, y, groups, n_samples, enc=None):
+def _cv_fold_groups(cv, X, y, groups, n_samples, enc=None, train_orders=None):
     """Fold-id layouts for ANY cross-validator whose train sets are the complements of its test sets
     (ShuffleSplit, StratifiedShuffleSplit, RepeatedKFold, RepeatedStratifiedKFold, LeavePOut,
     PredefinedSplit, Group* ... as well as the partitions `_cv_fold_ids` handles directly).
@@ -111,13 +115,16 @@ def _cv_fold_groups(cv, X, y, groups, n_samples, enc=None):
     fold id k, rows in none of the layout's test sets carry the extra id `n_folds - 1` that no column
     holds out.  A partition is one layout (no extra id); ShuffleSplit(n) is n layouts of one split.
     The search re-stages the fold ids (n bytes) per layout; X stays staged.  Splitters whose train set
-    is not the complement of the test set (TimeSeriesSplit) have no device path."""
+    is not the complement of the test set (TimeSeriesSplit) have no device path.  `train_orders`: as in
+    `_cv_fold_ids`."""
     try:
-        fold, n_splits = _cv_fold_ids(cv, X, y, groups, n_samples, enc)
+        fold, n_splits = _cv_fold_ids(cv, X, y, groups, n_samples, enc, train_orders)
         return [(fold, n_splits, list(range(n_splits)))], n_splits
     except NotImplementedError:
         pass
     cv_splitted = list(cv.split(X, y, groups))
+    if train_orders is not None:
+        train_orders[:] = [np.asarray(train) for train, _ in cv_splitted]
     n_splits = len(cv_splitted)
     layouts = []       # [used mask, fold ids, split indices]
     for s, (train, test) in enumerate(cv_splitted):

@@ -17,7 +17,7 @@ from .. import parallel
 from .base import _clone, _merged_params
 from .folds import _classes_and_ids
 
-_LOGREG_SEARCHABLE = {"C", "tol", "max_iter", "fit_intercept"}
+_LOGREG_SEARCHABLE = {"C", "tol", "max_iter", "fit_intercept", "class_weight"}
 
 
 def _resolve(estimator, params):
@@ -27,9 +27,10 @@ def _resolve(estimator, params):
     return est
 
 
-def _check_logreg(est):
+def _check_logreg(est, class_weight=False):
     """Raise unless `est` is a configuration the batched lbfgs kernel path reproduces
-    (SK/linear_model/_logistic.py:1355-1593)."""
+    (SK/linear_model/_logistic.py:1355-1593).  class_weight=True: the caller passes the class weights
+    to the engine."""
     p = est if isinstance(est, dict) else est.get_params(deep=False)
     bad = []
     if p.get("solver", "lbfgs") != "lbfgs":
@@ -39,7 +40,7 @@ def _check_logreg(est):
         bad.append("penalty=%r (only 'l2')" % (pen,))
     if p.get("l1_ratio", 0.0) not in (None, 0, 0.0):
         bad.append("l1_ratio=%r" % (p["l1_ratio"],))
-    if p.get("class_weight", None) is not None:
+    if not class_weight and p.get("class_weight", None) is not None:
         bad.append("class_weight")
     if p.get("dual", False):
         bad.append("dual=True")
@@ -143,6 +144,63 @@ def _metric_from_counts(kind, correct, count, pred_pos, actual_pos):
     raise ValueError(kind)
 
 
+class _ClassWeights:
+    """Per-column class weights of LogisticRegression(class_weight=...) fits, as
+    SK/linear_model/_logistic.py:409-474 forms them: compute_class_weight on the labels of the fit's own
+    training rows (classes = the labels present there), cast to float32, and sw_sum = the float32 sum of
+    the per-row weights in the order of those rows.  Weights depend on (class_weight, held-out fold) only."""
+
+    def __init__(self, classes, y_class):
+        self.classes, self.y_class = classes, y_class
+        self.fold, self.train_rows, self.cache = None, None, {}
+
+    def set_folds(self, fold, train_rows=None):
+        """fold ids of the staged layout; train_rows[f] = training rows of local fold f in the splitter's
+        order (None: the rows outside fold f in ascending order, as every partition splitter gives them)."""
+        self.fold, self.train_rows, self.cache = np.asarray(fold), train_rows, {}
+
+    def _train(self, f):
+        if f < 0:
+            return np.arange(len(self.y_class))
+        if self.train_rows is not None and self.train_rows[f] is not None:
+            return self.train_rows[f]
+        return np.flatnonzero(self.fold != f)
+
+    def column(self, class_weight, f):
+        """(float32 weight of every class id, sw_sum) of a fit on the training rows of fold f (-1: all rows)."""
+        key = (repr(class_weight), int(f))
+        if key not in self.cache:
+            self.cache[key] = _fit_class_weights(class_weight, self.y_class[self._train(f)], self.classes)
+        return self.cache[key]
+
+    def stage(self, eng, class_weights, folds):
+        """Stage the weights of columns (class_weight, held-out fold) for the next fit; nothing when no
+        column is weighted (the unweighted kernels then run)."""
+        if all(cw is None for cw in class_weights):
+            return
+        _stage_columns(eng, [self.column(cw, f) for cw, f in zip(class_weights, folds)])
+
+
+def _fit_class_weights(class_weight, ids, classes):
+    """(float32 weight of every class id, sw_sum) of ONE fit whose training rows, in the fit's order, carry
+    the class ids `ids` (labels classes[ids]): what SK/linear_model/_logistic.py:409-474 forms from
+    class_weight (classes = the labels present in the fit, weights cast to float32, sw_sum = the float32
+    sum of the per-row weights).  Errors of compute_class_weight propagate."""
+    from sklearn.utils.class_weight import compute_class_weight
+    w = np.ones(len(classes), dtype=np.float32)
+    if class_weight is None:
+        return w, float(len(ids))
+    present = np.unique(ids)
+    w[:] = 0.0      # a class without training rows carries no weight
+    w[present] = compute_class_weight(class_weight, classes=classes[present], y=classes[ids]).astype(np.float32)
+    return w, float(np.sum(w[ids]))
+
+
+def _stage_columns(eng, cols):
+    """Stage [(weights, sw_sum)] of the columns of the next fit."""
+    eng.stage_class_weights(np.stack([c[0] for c in cols]), np.array([c[1] for c in cols]))
+
+
 class _LogRegFamily:
     """(candidate x fold) columns of binary L2 logistic regression."""
 
@@ -150,7 +208,7 @@ class _LogRegFamily:
 
     def __init__(self, estimator, candidate_params, X, y, scorers, enc=None):
         self.estimator = estimator
-        self.cands = [_check_logreg(q) for q in _merged_params(estimator, candidate_params)]
+        self.cands = [_check_logreg(q, class_weight=True) for q in _merged_params(estimator, candidate_params)]
         for p in candidate_params:
             extra = set(p) - _LOGREG_SEARCHABLE
             if extra:
@@ -161,6 +219,7 @@ class _LogRegFamily:
         if len(self.classes_) != 2:
             raise NotImplementedError(
                 "this family is binary (got %d classes)" % len(self.classes_))
+        self.weights = _ClassWeights(self.classes_, self.y_class)
         # every scorer must be a count-based metric (accuracy / precision / recall / f1 / balanced
         # accuracy on predict); scoring=None -> _PassthroughScorer -> estimator.score == accuracy
         self.metrics = {}
@@ -180,12 +239,18 @@ class _LogRegFamily:
             parallel.stage_x_replicated(eng, X)
         eng.stage_labels(self.y_class)
         eng.stage_folds(fold, n_splits)
+        self.weights.set_folds(fold)
         if self.needs_pred_pos:     # positives per fold: only the precision / recall / f1 formulas use them
             self.pos_in_fold = np.bincount(np.asarray(fold)[self.y_class == 1], minlength=n_splits).astype(np.int64)
             self.total_pos = int(self.pos_in_fold.sum())
         else:
             self.pos_in_fold = np.zeros(n_splits, dtype=np.int64)
             self.total_pos = 0
+
+    def set_train_rows(self, train_rows):
+        """Training rows of every fold of the staged layout in the splitter's order (None entries: the
+        rows outside the fold, ascending): the order sw_sum of a weighted column is summed in."""
+        self.weights.set_folds(self.weights.fold, train_rows)
 
     def _scores(self, eng, coef, codes, pos, actual_pos):
         """{scorer name: per-column value} on the rows selected by the scoring codes."""
@@ -239,6 +304,7 @@ class _LogRegFamily:
             C = np.array([self.cands[c]["C"] for c in cand[idx]], dtype=np.float64)
             pos = np.ones(len(idx), dtype=np.int32)
             t0 = time.time()
+            self.weights.stage(eng, [self.cands[c]["class_weight"] for c in cand[idx]], fold[idx])
             res = eng.logreg_fit_batch(C, fold[idx], pos, fit_intercept=fi, tol=tol, max_iter=mi)
             t1 = time.time()
             vals, count = self._scores(eng, res["coef"], fold[idx], pos, self.pos_in_fold[fold[idx]])
@@ -273,7 +339,8 @@ class _LogRegFamily:
         return out
 
     def refit(self, eng, params, X_dtype, n_features):
-        p = _check_logreg(_resolve(self.estimator, params))
+        p = _check_logreg(_resolve(self.estimator, params), class_weight=True)
+        self.weights.stage(eng, [p["class_weight"]], [-1])
         res = eng.logreg_fit_batch(np.array([p["C"]]), np.array([-1], dtype=np.int32),
                                    np.array([1], dtype=np.int32), fit_intercept=p["fit_intercept"],
                                    tol=p["tol"], max_iter=p["max_iter"])
@@ -297,8 +364,9 @@ class _LogRegFamily:
     def fold_proba(self, eng, params, fold, n_splits):
         """preds_ support (ref search.py:551-560): per-fold refit of the best params,
         predict_proba on the held-out rows, stacked in fold order."""
-        p = _check_logreg(_resolve(self.estimator, params))
+        p = _check_logreg(_resolve(self.estimator, params), class_weight=True)
         f = np.arange(n_splits, dtype=np.int32)
+        self.weights.stage(eng, [p["class_weight"]] * n_splits, f)
         res = eng.logreg_fit_batch(np.full(n_splits, p["C"]), f, np.ones(n_splits, dtype=np.int32),
                                    fit_intercept=p["fit_intercept"], tol=p["tol"], max_iter=p["max_iter"])
         dec = eng.linear_decision(res["coef"])
@@ -319,7 +387,7 @@ class _MultinomialFamily(_LogRegFamily):
 
     def __init__(self, estimator, candidate_params, X, y, scorers, enc=None):
         self.estimator = estimator
-        self.cands = [_check_logreg(q) for q in _merged_params(estimator, candidate_params)]
+        self.cands = [_check_logreg(q, class_weight=True) for q in _merged_params(estimator, candidate_params)]
         for p in candidate_params:
             extra = set(p) - _LOGREG_SEARCHABLE
             if extra:
@@ -328,6 +396,7 @@ class _MultinomialFamily(_LogRegFamily):
                     % (sorted(extra), sorted(_LOGREG_SEARCHABLE)))
         self.classes_, self.y_class = _classes_and_ids(y, enc)
         self.n_classes = len(self.classes_)
+        self.weights = _ClassWeights(self.classes_, self.y_class)
         self.metrics = {}
         for name, scorer in scorers.items():
             m = _count_metric(scorer)
@@ -343,6 +412,7 @@ class _MultinomialFamily(_LogRegFamily):
             parallel.stage_x_replicated(eng, X)
         eng.stage_labels(self.y_class)
         eng.stage_folds(fold, n_splits)
+        self.weights.set_folds(fold)
 
     def run_columns(self, eng, cols, n_splits, return_train_score):
         cols = np.asarray(cols, dtype=np.int64)
@@ -365,6 +435,7 @@ class _MultinomialFamily(_LogRegFamily):
             idx = np.asarray(idx)
             C = np.array([self.cands[c]["C"] for c in cand[idx]], dtype=np.float64)
             t0 = time.time()
+            self.weights.stage(eng, [self.cands[c]["class_weight"] for c in cand[idx]], fold[idx])
             res = eng.logreg_multinomial_fit_batch(C, fold[idx], self.n_classes, fit_intercept=fi, tol=tol,
                                                    max_iter=mi)
             t1 = time.time()
@@ -391,7 +462,8 @@ class _MultinomialFamily(_LogRegFamily):
         return _metric_from_confusion(kind, average, conf)
 
     def refit(self, eng, params, X_dtype, n_features):
-        p = _check_logreg(_resolve(self.estimator, params))
+        p = _check_logreg(_resolve(self.estimator, params), class_weight=True)
+        self.weights.stage(eng, [p["class_weight"]], [-1])
         res = eng.logreg_multinomial_fit_batch(np.array([p["C"]]), np.array([-1], dtype=np.int32), self.n_classes,
                                                fit_intercept=p["fit_intercept"], tol=p["tol"],
                                                max_iter=p["max_iter"])
@@ -414,8 +486,9 @@ class _MultinomialFamily(_LogRegFamily):
 
     def fold_proba(self, eng, params, fold, n_splits):
         from sklearn.utils.extmath import softmax
-        p = _check_logreg(_resolve(self.estimator, params))
+        p = _check_logreg(_resolve(self.estimator, params), class_weight=True)
         f = np.arange(n_splits, dtype=np.int32)
+        self.weights.stage(eng, [p["class_weight"]] * n_splits, f)
         res = eng.logreg_multinomial_fit_batch(np.full(n_splits, p["C"]), f, self.n_classes,
                                                fit_intercept=p["fit_intercept"], tol=p["tol"],
                                                max_iter=p["max_iter"])

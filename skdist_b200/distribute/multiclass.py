@@ -200,18 +200,27 @@ class DistOneVsRestClassifier(_ScParamMixin, OneVsRestClassifier):
             col_ids = np.flatnonzero(~const)
         mine = col_ids[parallel.shard_indices(len(col_ids), rank, world)]
         if type(base) is LogisticRegression:
-            from .logreg_family import _check_logreg
-            p = _check_logreg(_clone(base))
+            from .logreg_family import _check_logreg, _fit_class_weights, _stage_columns
+            p = _check_logreg(_clone(base), class_weight=True)
+            labels = train = None
             if use_bits and len(mine):
                 if multilabel:
                     labels = np.ascontiguousarray(Y[:, mine].toarray().T.astype(bool))
                 else:
                     labels = ycls[None, :] == mine[:, None].astype(np.int32)
-                train = None
                 if self.max_negatives is not None:
                     train = np.stack([_negatives_rows(labels[i], self.max_negatives, self.random_state, self.method)
                                       for i in range(len(mine))])
                 eng.stage_row_bits(labels if multilabel else None, train)
+            if p["class_weight"] is not None and len(mine):
+                # every column's binary fit: its 0/1 labels on its training rows (ascending), as _fit_binary
+                # hands them to the estimator (ref multiclass.py:141-151)
+                cols = []
+                for i, k in enumerate(mine):
+                    y01 = labels[i] if labels is not None else ycls == k
+                    rows = np.flatnonzero(train[i]) if train is not None else slice(None)
+                    cols.append(_fit_class_weights(p["class_weight"], y01[rows].astype(np.intp), np.array([0, 1])))
+                _stage_columns(eng, cols)
             res = eng.logreg_fit_batch(np.full(len(mine), p["C"]), np.full(len(mine), -1, np.int32),
                                        mine.astype(np.int32), fit_intercept=p["fit_intercept"],
                                        tol=p["tol"], max_iter=p["max_iter"])
@@ -290,8 +299,8 @@ class DistOneVsOneClassifier(_ScParamMixin, OneVsOneClassifier):
             raise NotImplementedError(
                 "%s has no one-vs-one device path; supported base estimators: LogisticRegression(solver='lbfgs'), "
                 "SGDClassifier.  (No CPU fallback by design.)" % type(base).__name__)
-        from .logreg_family import _check_logreg
-        p = _check_logreg(_clone(base))
+        from .logreg_family import _check_logreg, _fit_class_weights, _stage_columns
+        p = _check_logreg(_clone(base), class_weight=True)
         ycls = np.searchsorted(self.classes_, y_arr).astype(np.int32)
         rank, world, _ = parallel.dist_info()
         eng = get_engine()
@@ -301,6 +310,13 @@ class DistOneVsOneClassifier(_ScParamMixin, OneVsOneClassifier):
         mine = parallel.shard_indices(len(pairs), rank, world)
         neg = np.array([pairs[k][0] for k in mine], dtype=np.int32)      # y_binary: class i -> 0, class j -> 1 (ref :159-161)
         pos = np.array([pairs[k][1] for k in mine], dtype=np.int32)
+        if p["class_weight"] is not None and len(mine):
+            # the pair's rows (ascending, X[cond] of ref :157-158) labelled 0 / 1
+            cols = []
+            for i, j in zip(neg, pos):
+                yp = ycls[(ycls == i) | (ycls == j)]
+                cols.append(_fit_class_weights(p["class_weight"], (yp == j).astype(np.intp), np.array([0, 1])))
+            _stage_columns(eng, cols)
         res = eng.logreg_fit_batch(np.full(len(mine), p["C"]), np.full(len(mine), -1, np.int32), pos,
                                    fit_intercept=p["fit_intercept"], tol=p["tol"], max_iter=p["max_iter"],
                                    col_neg=neg)

@@ -114,7 +114,8 @@ class DistBaseSearchCV(_ScParamMixin):
                         n_splits, n_candidates, n_candidates * n_splits))
                 _parse_partitions(self.partitions, n_candidates * n_splits)
                 enc = _encode_target(y_arr) if is_classifier(estimator) else None   # one hash pass over y for both
-                layouts, n_splits = _cv_fold_groups(cv, X, y_arr, groups, n_samples, enc)
+                train_orders = []       # train index arrays of the splits, when the splitter gave them
+                layouts, n_splits = _cv_fold_groups(cv, X, y_arr, groups, n_samples, enc, train_orders)
                 fold = layouts[0][0]
                 family = _pick_family(estimator, candidate_params, X_arr, y_arr, scorers, enc)
                 if hasattr(family, "prepare"):      # host-only statistics of the folds (no engine calls)
@@ -136,6 +137,8 @@ class DistBaseSearchCV(_ScParamMixin):
             if li > 0 and hasattr(family, "prepare"):
                 family.prepare(fold_l, nf_l)
             family.stage(eng, X_arr, fold_l, nf_l, x_staged=True)
+            if hasattr(family, "set_train_rows"):    # training rows of every local fold, in the splitter's order
+                family.set_train_rows([train_orders[s] if train_orders else None for s in idx_l])
             k_l = len(idx_l)
             # local columns cand * nf_l + f, f < k_l (the extra fold id of a layout is never held out).
             # Ranks are dealt blocks of 128 consecutive candidates of ONE fold (fold-major order).

@@ -159,6 +159,18 @@ class Engine:
         check(self._lib.skd_stage_row_bits(self._h, B, ptr(packed[0]) if packed[0] is not None else None,
                                            ptr(packed[1]) if packed[1] is not None else None, bpc), self._h)
 
+    def stage_class_weights(self, w, sw_sum):
+        """[B, K] class weights and [B] sums of the per-row weights consumed by the next logreg_fit_batch /
+        logreg_loss_grad (K = 2: label 0, label 1) or logreg_multinomial_fit_batch (K = n_classes).
+        None clears."""
+        if w is None:
+            check(self._lib.skd_stage_class_weights(self._h, 0, 0, None, None), self._h)
+            return
+        w = np.ascontiguousarray(w, dtype=np.float32)
+        sw_sum = np.ascontiguousarray(sw_sum, dtype=np.float64)
+        assert w.ndim == 2 and sw_sum.shape == (w.shape[0],)
+        check(self._lib.skd_stage_class_weights(self._h, w.shape[0], w.shape[1], ptr(w), ptr(sw_sum)), self._h)
+
     def logreg_fit_batch(self, C, col_fold, col_pos, fit_intercept=True, tol=1e-4, max_iter=100, col_neg=None):
         """B binary lbfgs fits sharing the staged X.  col_neg[j] >= 0 restricts column j to the rows
         of class col_pos[j] / col_neg[j] (one-vs-one pair); None or < 0 = one-vs-rest."""
