@@ -96,6 +96,17 @@ int skd_stage_row_bits(skd_ctx* ctx, int32_t B, const uint8_t* label_bits, const
  * 1 / (C sw_sum).  ref: `class_weight` of LogisticRegression (SK/linear_model/_logistic.py:429-474). */
 int skd_stage_class_weights(skd_ctx* ctx, int32_t B, int32_t K, const float* w, const double* sw_sum);
 
+/* Class weights for the NEXT skd_forest_fit (classification; one-shot, cleared by that call even when it
+ * fails; n_classes <= 0, or w = NULL without balanced_subsample, clears).  Tree t is fitted with
+ * sample_weight count_i * cw[y_i]: w [n_classes] float64, finite and >= 0, the same for every tree, or
+ * balanced_subsample != 0 (w unused): per tree cw_k = n / (K_present * N_k) from the tree's bootstrap class
+ * counts N_k (compute_class_weight("balanced") of the bootstrap sample; absent classes 0).  Rows of weight 0
+ * leave the tree.  min_weight_fraction_leaf replaces the fit's min_weight_leaf: per tree, fraction * (sum of
+ * the tree's weights).  The fit fails if its n_classes differs or it is a regression fit.
+ * ref: `class_weight` of the forest classifiers (ensemble.py:68-109, 229-238). */
+int skd_stage_forest_class_weights(skd_ctx* ctx, int32_t n_classes, const double* w, int32_t balanced_subsample,
+                                   double min_weight_fraction_leaf);
+
 /* Batched binary L2 logistic regression (lbfgs), B independent columns sharing X.
  * Column j: positives = rows with y_class == col_pos[j]; training rows = rows whose fold id
  * != col_fold[j] (col_fold[j] < 0: all rows); l2 strength = 1 / (C[j] * n_train_j).

@@ -569,6 +569,27 @@ int skd_stage_class_weights(skd_ctx* ctx, int32_t B, int32_t K, const float* w, 
   return 0;
 }
 
+int skd_stage_forest_class_weights(skd_ctx* ctx, int32_t n_classes, const double* w, int32_t balanced_subsample,
+                                   double min_weight_fraction_leaf) {
+  if (!ctx) return fail(nullptr, "skd_stage_forest_class_weights: ctx is NULL");
+  Ctx* c = &ctx->c;
+  c->forest_cw = ForestClassWeights();
+  if (n_classes <= 0 || (!w && !balanced_subsample)) return 0;   // cleared
+  if (!(std::isfinite(min_weight_fraction_leaf) && min_weight_fraction_leaf >= 0.0 && min_weight_fraction_leaf <= 0.5))
+    return fail(c, "skd_stage_forest_class_weights: min_weight_fraction_leaf must be in [0, 0.5]");
+  ForestClassWeights cw;
+  cw.n_classes = n_classes;
+  cw.balanced_subsample = balanced_subsample != 0;
+  cw.min_weight_fraction = min_weight_fraction_leaf;
+  if (!cw.balanced_subsample) {
+    for (int k = 0; k < n_classes; ++k)
+      if (!(std::isfinite(w[k]) && w[k] >= 0.0)) return fail(c, "skd_stage_forest_class_weights: weights must be finite and >= 0");
+    cw.w.assign(w, w + n_classes);
+  }
+  c->forest_cw = std::move(cw);
+  return 0;
+}
+
 namespace {
 // Staged class weights are one-shot: the guard takes them off the context for the call that reads them.
 struct ClassWeightGuard {
@@ -1348,8 +1369,10 @@ struct skd_forest {
     std::vector<uint8_t> mgl;
     std::vector<double> thr, imp, wn, val;
     std::vector<uint32_t> compact;     // 8 words per node (throughput builder); expanded by skd_forest_tree_copy
+    std::vector<double> cw;            // class weights the tree was built with (compact records of a weighted fit)
   };
   std::vector<Tree> trees;
+  ForestClassWeights cw;               // staged for the fit (n_classes == 0: unweighted)
   std::vector<float> binval;           // [d][256] distinct feature values (thresholds of compact records)
 };
 
@@ -1360,6 +1383,13 @@ static void forest_sink(void* arg, int t, const SkdTreeView* v) {
   tr.max_depth = v->max_depth; tr.n_classes = v->n_classes; tr.node_count = m;
   if (v->compact) {
     tr.compact.assign(v->compact, v->compact + (size_t)m * 8);
+    if (f->cw.n_classes) {
+      tr.cw = f->cw.w;
+      if (f->cw.balanced_subsample) {   // the root record's class sums are the bootstrap class counts
+        tr.cw.resize(v->n_classes);
+        forest_subsample_weights(v->compact + 4, v->n_classes, tr.cw.data());
+      }
+    }
     return;
   }
   tr.left.assign(v->left, v->left + m); tr.right.assign(v->right, v->right + m);
@@ -1376,6 +1406,8 @@ int skd_forest_fit(skd_ctx* ctx, int32_t n_trees, const uint8_t* sample_counts, 
                    int32_t splitter, const double* y_regression, skd_forest** out, double* gpu_seconds_out) {
   if (!ctx) return fail(nullptr, "skd_forest_fit: ctx is NULL");
   Ctx* c = &ctx->c;
+  ForestClassWeights cw;               // staged class weights are one-shot: taken off the context whatever happens
+  std::swap(cw, c->forest_cw);
   if (!out) return fail(c, "skd_forest_fit: out is NULL");
   *out = nullptr;
   if (!c->X || (!y_regression && !c->ycls)) return fail(c, "skd_forest_fit: stage X and labels first");
@@ -1385,12 +1417,14 @@ int skd_forest_fit(skd_ctx* ctx, int32_t n_trees, const uint8_t* sample_counts, 
   SKD_CUDA(c, cudaSetDevice(c->device));
   skd_forest* f = new skd_forest();
   f->trees.resize(n_trees);
+  f->cw = cw;
   cudaEvent_t e0, e1;
   SKD_CUDA(c, cudaEventCreate(&e0));
   SKD_CUDA(c, cudaEventCreate(&e1));
   SKD_CUDA(c, cudaEventRecord(e0, c->stream));
   int rc = forest_fit(c, n_trees, sample_counts, rand_states, n_classes, max_features, max_depth, min_samples_split,
-                      min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter, y_regression, forest_sink, f);
+                      min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter, y_regression,
+                      cw.n_classes ? &cw : nullptr, forest_sink, f);
   if (!rc) f->binval = c->forest.h_binval;
   float ms = 0.f;
   if (!rc) {
@@ -1432,10 +1466,16 @@ int skd_forest_tree_copy(skd_forest* f, int32_t tree, int32_t* left, int32_t* ri
     //   impurity   = 1 - (sum_c s_c^2) / (weighted_n * weighted_n)             (Gini, :650-680; what the parent's
     //                children_impurity computed from the same integers)
     //   threshold  = v[a] / 2 + v[b] / 2                                        (SK/tree/_splitter.pyx:459-461)
+    // With class weights every s_c above is the weighted sum cw_c * s_c (one rounding), as in the builder,
+    // except the impurity of a right child: the builder (like scikit-learn) forms it at the parent from
+    // sum_right = cw_c * t_c - cw_c * l_c and w_right = w_node - w_left (ff_proxy4w), which with non-dyadic
+    // weights can differ in the last bits from the child's own sums; it is recomputed that way below, so the
+    // tree reports the impurity the builder compared with EPSILON and used in the improvement.
     const size_t m = (size_t)t.node_count;
     const int C = t.n_classes;
     const uint32_t* r = t.compact.data();
     const float* bv = f->binval.data();
+    const double* cw = t.cw.empty() ? nullptr : t.cw.data();
     for (size_t i = 0; i < m; ++i, r += 8) {
       const int32_t rc = (int32_t)r[0];
       const uint32_t code = r[1];
@@ -1453,8 +1493,10 @@ int skd_forest_tree_copy(skd_forest* f, int32_t tree, int32_t* left, int32_t* ri
         }
       }
       volatile double w = 0.0, sq = 0.0;
+      double s[4];
       for (int c = 0; c < C; ++c) {
-        const double a = (double)r[4 + c];
+        const volatile double a = cw ? cw[c] * (double)r[4 + c] : (double)r[4 + c];
+        s[c] = a;
         w = w + a;
         const volatile double aa = a * a;      // volatile: no contraction of the product into the sum
         sq = sq + aa;
@@ -1462,8 +1504,27 @@ int skd_forest_tree_copy(skd_forest* f, int32_t tree, int32_t* left, int32_t* ri
       if (n_node_samples) n_node_samples[i] = (int32_t)r[2];
       if (weighted_n_node_samples) weighted_n_node_samples[i] = w;
       if (impurity) { const volatile double ww = w * w; const volatile double q = sq / ww; impurity[i] = 1.0 - q; }
-      if (value) for (int c = 0; c < C; ++c) value[i * C + c] = (double)r[4 + c] / w;
+      if (value) for (int c = 0; c < C; ++c) value[i * C + c] = s[c] / w;
       if (missing_go_to_left) missing_go_to_left[i] = 0;
+    }
+    if (impurity && cw) {
+      r = t.compact.data();
+      for (size_t i = 0; i < m; ++i) {
+        const int32_t rc = (int32_t)r[i * 8];
+        if ((r[i * 8 + 1] & 0xFFFFu) == 0xFFFFu || rc <= 0) continue;
+        const uint32_t* tp = r + i * 8 + 4;           // the parent's class sums
+        const uint32_t* lp = r + (i + 1) * 8 + 4;     // the left child's
+        volatile double wn = 0.0, wl = 0.0, sqr = 0.0;
+        for (int c = 0; c < C; ++c) { const volatile double st = cw[c] * (double)tp[c]; wn = wn + st; }
+        for (int c = 0; c < C; ++c) {
+          const volatile double st = cw[c] * (double)tp[c], a = cw[c] * (double)lp[c];
+          const volatile double b = st - a, bb = b * b;
+          wl = wl + a;
+          sqr = sqr + bb;
+        }
+        const volatile double wr = wn - wl, ww = wr * wr, q = sqr / ww;
+        impurity[rc] = 1.0 - q;
+      }
     }
     if (missing_go_to_left) {      // n_left > n_right (SK/tree/_splitter.pyx: best_split.missing_go_to_left with no missing values)
       r = t.compact.data();

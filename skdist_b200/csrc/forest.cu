@@ -83,6 +83,10 @@ struct FoParams {
   int32_t* o_maxdepth;        // [slots]
   int32_t* o_status;          // [slots] 0 ok, 1 node capacity, 2 stack capacity
   long long* o_prof;          // [slots][16] cycles per builder phase (SKDIST_B200_FOREST_PROF=1), else nullptr
+  // class weights, read only by the weighted instantiation (W): as FfParams
+  int cw_bs;
+  const double* cw;
+  double min_weight_fraction;
 };
 
 __device__ __forceinline__ uint32_t fo_rand_r(uint32_t* seed) {   // SK/utils/_random.pxd:20-34
@@ -105,6 +109,24 @@ __device__ __forceinline__ void fo_children_impurity(const unsigned long long* s
   for (int c = 0; c < CM; ++c) {
     if (c < C) {
       const double a = (double)sl[c], b = (double)(st[c] - sl[c]);
+      sql = __dadd_rn(sql, __dmul_rn(a, a));
+      sqr = __dadd_rn(sqr, __dmul_rn(b, b));
+    }
+  }
+  *il = __dsub_rn(1.0, __ddiv_rn(sql, __dmul_rn(wl, wl)));
+  *ir = __dsub_rn(1.0, __ddiv_rn(sqr, __dmul_rn(wr, wr)));
+}
+// ... with class weights: sum_left[c] = w_c * count, sum_right[c] = sum_total[c] - sum_left[c]
+// (ClassificationCriterion.update, SK/tree/_criterion.pyx)
+template <int CM>
+__device__ __forceinline__ void fo_children_impurity_w(const unsigned long long* sl, const unsigned long long* st,
+                                                       const double* cw, int C, double wl, double wr, double* il,
+                                                       double* ir) {
+  double sql = 0.0, sqr = 0.0;
+#pragma unroll
+  for (int c = 0; c < CM; ++c) {
+    if (c < C) {
+      const double a = __dmul_rn(cw[c], (double)sl[c]), b = __dsub_rn(__dmul_rn(cw[c], (double)st[c]), a);
       sql = __dadd_rn(sql, __dmul_rn(a, a));
       sqr = __dadd_rn(sqr, __dmul_rn(b, b));
     }
@@ -139,12 +161,15 @@ __device__ __forceinline__ void fo_children_mse(const unsigned long long* sl, co
   *ir = __dsub_rn(__ddiv_rn(sq_r, wr), __dmul_rn(mr, mr));
 }
 
-// CM: compile-time bound on the class count (3 statistics when REG), so the per-class arrays of a thread live in registers
+// CM: compile-time bound on the class count (3 statistics when REG), so the per-class arrays of a thread live in registers.
+// W: class weights (classification only).  Histograms, records and the partition keep the integer
+// counts; the float64 statistics are w_c * count (one rounding), in scikit-learn's operation order.
 #define FO_TICK(ph) do { if (P.o_prof && tid == 0) { const long long _t = clock64(); prof[ph] += _t - tlast; tlast = _t; } } while (0)
 #define FOR_C(c) _Pragma("unroll") for (int c = 0; c < CM; ++c) if (c < C)
-template <int CM, bool REG>
+template <int CM, bool REG, bool W>
 __global__ void __launch_bounds__(FO_THREADS)
 forest_build_kernel(const FoParams P) {
+  static_assert(!(REG && W), "class weights are a classification feature");
   const int slot = blockIdx.x;
   if (slot >= P.n_trees) return;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -169,6 +194,7 @@ forest_build_kernel(const FoParams P) {
   __shared__ double s_dbl[4];
   __shared__ FoRecord rec_spill;
   __shared__ unsigned long long best_sl[FO_MAXC];
+  __shared__ double s_cw[W ? FO_MAXC : 1];   // W: this tree's class weights
   int2* undo = reinterpret_cast<int2*>(fo_sm + 2 * d);      // [d + 16] swap log of the speculative draws
   float* sbv = reinterpret_cast<float*>(undo + (d + 16));   // [FO_KB_MAX][256] distinct values of the batch features
   FoRecord* sstack = reinterpret_cast<FoRecord*>(sbv + FO_KB_MAX * FO_BINS);   // [FO_SSTK] top of the DFS stack
@@ -181,6 +207,8 @@ forest_build_kernel(const FoParams P) {
   __shared__ int base_s;
   if (tid == 0) base_s = 0;
   for (int i = tid; i < d; i += FO_THREADS) features[i] = i;
+  // balanced_subsample: 1 until the root's class sums give the weights (only absent classes get 0)
+  if constexpr (W) if (tid < FO_MAXC) s_cw[tid] = P.cw_bs || tid >= C ? 1.0 : P.cw[tid];
   __syncthreads();
   unsigned long long my_sums[CM];
 #pragma unroll
@@ -189,7 +217,8 @@ forest_build_kernel(const FoParams P) {
     const int64_t i = i0 + tid;
     unsigned int w = 0, yc = 0;
     if (i < n) { w = cnt[i]; if (!REG) yc = (unsigned)P.ycls[i]; }
-    const int keep = w != 0;
+    int keep = w != 0;
+    if constexpr (W) keep = keep && s_cw[yc] != 0.0;   // rows of weight 0 leave the tree (Splitter.init)
     const unsigned bal = __ballot_sync(0xffffffffu, keep);
     if (lane == 0) wsum[wid][0] = __popc(bal);
     __syncthreads();
@@ -227,7 +256,21 @@ forest_build_kernel(const FoParams P) {
   __syncthreads();
   double w_samples = 0.0;
   if constexpr (REG) w_samples = st_d(red[0]);
+  else if constexpr (W) {
+    if (P.cw_bs) {   // compute_class_weight("balanced") of the bootstrap sample: n / (K_present * N_c)
+      if (tid < C) {
+        unsigned long long nt = 0; int kp = 0;
+        for (int c = 0; c < C; ++c) { nt += red[c]; kp += red[c] != 0; }
+        s_cw[tid] = red[tid] ? __ddiv_rn((double)nt, __dmul_rn((double)kp, (double)red[tid])) : 0.0;
+      }
+      __syncthreads();
+    }
+    FOR_C(c) w_samples = __dadd_rn(w_samples, __dmul_rn(s_cw[c], (double)red[c]));
+  }
   else { FOR_C(c) w_samples += (double)red[c]; }    // weighted_n_samples (integer valued)
+  // BaseDecisionTree._fit: min_weight_leaf = min_weight_fraction_leaf * sum(sample_weight)
+  const double mwl_w = W ? __dmul_rn(P.min_weight_fraction, w_samples) : 0.0;
+#define MIN_WEIGHT_LEAF (W ? mwl_w : P.min_weight_leaf)
 
   long long prof[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   long long tlast = clock64();
@@ -260,14 +303,19 @@ forest_build_kernel(const FoParams P) {
     const int n_node = end - start;
     double w_node = 0.0;
     if constexpr (REG) w_node = st_d(rec.sums[0]);
+    else if constexpr (W) { FOR_C(c) w_node = __dadd_rn(w_node, __dmul_rn(s_cw[c], (double)rec.sums[c])); }
     else { FOR_C(c) w_node += (double)rec.sums[c]; }
     double impurity = rec.impurity;
     bool is_leaf = depth >= P.max_depth || n_node < P.min_samples_split || n_node < 2 * P.min_samples_leaf ||
-                   w_node < 2.0 * P.min_weight_leaf;
+                   w_node < 2.0 * MIN_WEIGHT_LEAF;
     if (first) {   // root: node_impurity()  (SK/tree/_criterion.pyx:620-640)
       if constexpr (REG) {   // MSE.node_impurity
         const double mean = __ddiv_rn(st_d(rec.sums[1]), w_node);
         impurity = __dsub_rn(__ddiv_rn(st_d(rec.sums[2]), w_node), __dmul_rn(mean, mean));
+      } else if constexpr (W) {
+        double sq = 0.0;
+        FOR_C(c) { const double a = __dmul_rn(s_cw[c], (double)rec.sums[c]); sq = __dadd_rn(sq, __dmul_rn(a, a)); }
+        impurity = __dsub_rn(1.0, __ddiv_rn(sq, __dmul_rn(w_node, w_node)));
       } else {
         double sq = 0.0;
         FOR_C(c) { const double a = (double)rec.sums[c]; sq = __dadd_rn(sq, __dmul_rn(a, a)); }
@@ -467,14 +515,18 @@ forest_build_kernel(const FoParams P) {
                 if (n_left >= P.min_samples_leaf && n_right >= P.min_samples_leaf) {
                   double wl = 0.0;
                   if constexpr (REG) wl = st_d(sl[0]);
+                  else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(s_cw[c], (double)sl[c])); }
                   else { FOR_C(c) wl += (double)sl[c]; }
                   const double wr = w_node - wl;
-                  if (!(wl < P.min_weight_leaf || wr < P.min_weight_leaf)) {
+                  if (!(wl < MIN_WEIGHT_LEAF || wr < MIN_WEIGHT_LEAF)) {
                     double il, ir;
                     if constexpr (REG) {
                       fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
                       const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
                       R->proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
+                    } else if constexpr (W) {
+                      fo_children_impurity_w<CM>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
+                      R->proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
                     } else {
                       fo_children_impurity<CM>(sl, rec.sums, C, wl, wr, &il, &ir);
                       R->proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
@@ -510,14 +562,18 @@ forest_build_kernel(const FoParams P) {
               if (n_left < P.min_samples_leaf || n_right < P.min_samples_leaf) continue;
               double wl = 0.0;
               if constexpr (REG) wl = st_d(sl[0]);
+              else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(s_cw[c], (double)sl[c])); }
               else { FOR_C(c) wl += (double)sl[c]; }
               const double wr = w_node - wl;
-              if (wl < P.min_weight_leaf || wr < P.min_weight_leaf) continue;
+              if (wl < MIN_WEIGHT_LEAF || wr < MIN_WEIGHT_LEAF) continue;
               double il, ir, proxy;
               if constexpr (REG) {     // MSE.proxy_impurity_improvement: sum_l^2 / w_l + sum_r^2 / w_r
                 fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
                 const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
                 proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
+              } else if constexpr (W) {
+                fo_children_impurity_w<CM>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
+                proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
               } else {
                 fo_children_impurity<CM>(sl, rec.sums, C, wl, wr, &il, &ir);
                 proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
@@ -586,6 +642,7 @@ forest_build_kernel(const FoParams P) {
         if (best_pos < end) {
           double wl = 0.0;
           if constexpr (REG) wl = st_d(best_sl[0]);
+          else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(s_cw[c], (double)best_sl[c])); }
           else { FOR_C(c) wl += (double)best_sl[c]; }
           const double wr = w_node - wl;
           // impurity_improvement (SK/tree/_criterion.pyx:163-190)
@@ -658,6 +715,9 @@ forest_build_kernel(const FoParams P) {
       }
       if constexpr (REG) {
         P.o_val[nb + node_id] = __ddiv_rn(st_d(rec.sums[1]), w_node);               // node mean (MSE.node_value)
+      } else if constexpr (W) {
+        FOR_C(c)
+          P.o_val[(nb + node_id) * C + c] = __ddiv_rn(__dmul_rn(s_cw[c], (double)rec.sums[c]), w_node);
       } else {
         FOR_C(c)
           P.o_val[(nb + node_id) * C + c] = __ddiv_rn((double)rec.sums[c], w_node);   // class fractions
@@ -693,6 +753,7 @@ forest_build_kernel(const FoParams P) {
 
 #undef FOR_C
 #undef FO_TICK
+#undef MIN_WEIGHT_LEAF
 
 // ------------------------------------ binning ---------------------------------------------
 // column f of X -> contiguous buffer
@@ -823,16 +884,26 @@ int forest_prepare(Ctx* c) {
 int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_states, int n_classes,
                int max_features, int max_depth, int min_samples_split, int min_samples_leaf,
                double min_weight_leaf, double min_impurity_decrease, int random_split, const double* h_yreal,
-               ForestSink sink, void* sink_arg) {
+               const ForestClassWeights* cw, ForestSink sink, void* sink_arg) {
   if (forest_prepare(c)) return 1;
   const bool reg = h_yreal != nullptr;       // regression trees (MSE) on float64 targets
   if (reg) n_classes = 1;
   if (n_classes < 1 || n_classes > FO_MAXC) return fail(c, "forest: device path supports up to 16 classes");
   if (!reg && !c->ycls) return fail(c, "forest: stage labels first");
+  const bool weighted = cw != nullptr;
+  if (weighted && reg) return fail(c, "forest: class weights are staged but this is a regression fit");
+  if (weighted && cw->n_classes != n_classes) return fail(c, "forest: staged class weights do not match n_classes");
   const int64_t n = c->n;
   const int d = (int)c->d;
   if ((size_t)4 * d * sizeof(int) > 6 * 1024) return fail(c, "forest: device path supports up to 384 features (shared-memory feature permutation)");
-  const bool fast = forest_fast_supported(c, n_classes, reg, random_split);
+  bool fast = forest_fast_supported(c, n_classes, reg, random_split);
+  if (fast && weighted && !cw->balanced_subsample) {
+    // the float32 rank value of the fast builder needs the positive weights within 2^40 of each other
+    // (balanced_subsample weights are within n of each other)
+    double lo = INFINITY, hi = 0.0;
+    for (double w : cw->w) if (w > 0.0) { lo = std::min(lo, w); hi = std::max(hi, w); }
+    if (!(hi > 0.0) || hi > 1099511627776.0 * lo) fast = false;
+  }
   const int stack_cap = 4096;
   const size_t rec_bytes = fast ? forest_fast_record_bytes(n_classes) : sizeof(FoRecord);
   const size_t node_bytes = fast ? 32 : (size_t)(4 * 4 + 1 + 8 * 3 + 8 * n_classes);   // fast builder: compact records
@@ -851,15 +922,25 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
     SKD_CUDA(c, cudaMemcpyAsync(dy, h_yreal, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c->stream));
     c->h2d += n * 8;
   }
+  double* dcw = nullptr;
+  Scratch sw(c);
+  if (weighted) {
+    std::vector<double> hw(FO_MAXC, 1.0);
+    if (!cw->balanced_subsample) std::copy(cw->w.begin(), cw->w.end(), hw.begin());
+    SKD_CUDA(c, sw.alloc(&dcw, (size_t)FO_MAXC));
+    SKD_CUDA(c, cudaMemcpyAsync(dcw, hw.data(), FO_MAXC * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    c->h2d += FO_MAXC * 8;
+  }
   const size_t smem_general = (size_t)2 * d * sizeof(int) + (size_t)(d + 16) * sizeof(int2) +
                               (size_t)FO_KB_MAX * FO_BINS * sizeof(float) + (size_t)FO_SSTK * sizeof(FoRecord);
-  if (!fast) {
-    SKD_CUDA(c, cudaFuncSetAttribute(forest_build_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_general));
-    SKD_CUDA(c, cudaFuncSetAttribute(forest_build_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_general));
-    SKD_CUDA(c, cudaFuncSetAttribute(forest_build_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_general));
-    SKD_CUDA(c, cudaFuncSetAttribute(forest_build_kernel<FO_MAXC, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_general));
-    SKD_CUDA(c, cudaFuncSetAttribute(forest_build_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_general));
-  }
+  // the general builder for this fit (CM: class-count bound; W: class weights)
+  void (*general)(const FoParams) = nullptr;
+  if (reg) general = forest_build_kernel<4, true, false>;
+  else if (n_classes <= 2) general = weighted ? forest_build_kernel<2, false, true> : forest_build_kernel<2, false, false>;
+  else if (n_classes <= 4) general = weighted ? forest_build_kernel<4, false, true> : forest_build_kernel<4, false, false>;
+  else if (n_classes <= 8) general = weighted ? forest_build_kernel<8, false, true> : forest_build_kernel<8, false, false>;
+  else general = weighted ? forest_build_kernel<FO_MAXC, false, true> : forest_build_kernel<FO_MAXC, false, false>;
+  if (!fast) SKD_CUDA(c, cudaFuncSetAttribute(general, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_general));
   std::vector<int> pending(n_trees);
   for (int t = 0; t < n_trees; ++t) pending[t] = t;
   c->forest_kernel_ms = 0.0;
@@ -919,6 +1000,9 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
     P.random_split = random_split ? 1 : 0;
     P.counts = dcounts; P.rand_state = drs; P.stack_cap = stack_cap; P.node_cap = node_cap;
     P.o_prof = d_prof;
+    if (weighted) {
+      P.cw_bs = cw->balanced_subsample ? 1 : 0; P.cw = dcw; P.min_weight_fraction = cw->min_weight_fraction;
+    }
     FfParams F;
     memset(&F, 0, sizeof(F));
     F.xrow = c->forest.xrow; F.ycls = c->ycls; F.n = n; F.d = d; F.dp = c->forest.dp; F.n_classes = n_classes;
@@ -929,6 +1013,7 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
     F.stack_cap = stack_cap; F.node_cap = node_cap;
     F.o_nodes = d_nodes;
     F.o_count = P.o_count; F.o_maxdepth = P.o_maxdepth; F.o_status = P.o_status; F.o_prof = d_prof;
+    F.weighted = weighted ? 1 : 0; F.cw_bs = P.cw_bs; F.cw = P.cw; F.min_weight_fraction = P.min_weight_fraction;
     std::vector<int32_t> hcount(slots), hdepth(slots), hstatus(slots);
     std::vector<uint32_t> hrs(slots);
     std::vector<int> failed;
@@ -955,11 +1040,7 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
       if (fast) {
         if (forest_fast_launch(c, F, nt)) return 1;
       } else {
-        if (reg) forest_build_kernel<4, true><<<nt, FO_THREADS, smem_general, c->stream>>>(P);
-        else if (n_classes <= 2) forest_build_kernel<2, false><<<nt, FO_THREADS, smem_general, c->stream>>>(P);
-        else if (n_classes <= 4) forest_build_kernel<4, false><<<nt, FO_THREADS, smem_general, c->stream>>>(P);
-        else if (n_classes <= 8) forest_build_kernel<8, false><<<nt, FO_THREADS, smem_general, c->stream>>>(P);
-        else forest_build_kernel<FO_MAXC, false><<<nt, FO_THREADS, smem_general, c->stream>>>(P);
+        general<<<nt, FO_THREADS, smem_general, c->stream>>>(P);
         c->launches += 1;
       }
       SKD_CUDA(c, cudaGetLastError());

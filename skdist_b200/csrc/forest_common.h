@@ -4,6 +4,8 @@
 #include <stdint.h>
 #include <cuda_runtime.h>
 
+#include <vector>
+
 namespace skd {
 
 struct Ctx;
@@ -31,7 +33,32 @@ struct FfParams {
   uint32_t* o_nodes;          // [trees][node_cap][8] compact node records (see forest_fast.cu: _add_node)
   int32_t* o_count; int32_t* o_maxdepth; int32_t* o_status;    // [trees]; status 0 ok, 1 node capacity, 2 stack capacity
   long long* o_prof;          // [trees][16] cycles per builder phase / node counts (SKDIST_B200_FOREST_PROF=1), else nullptr
+  // class weights (see ForestClassWeights); read only by the weighted instantiation
+  int weighted, cw_bs;        // weighted fit; balanced_subsample (weights formed per tree from its root class sums)
+  const double* cw;           // [n_classes] weights shared by every tree (cw_bs == 0)
+  double min_weight_fraction; // min_weight_leaf of a tree = fraction * its weighted_n_samples
 };
+
+// Class weights of a forest classifier fit.  Tree t is fitted with sample_weight count_i * w[y_i]: every
+// node statistic is w_c * (integer class count), formed in float64 with one rounding.
+struct ForestClassWeights {
+  int n_classes = 0;                 // 0: none staged
+  std::vector<double> w;             // [n_classes], unused with balanced_subsample
+  bool balanced_subsample = false;   // per tree: w_c = n / (K_present * N_c) from the bootstrap class counts N_c
+  double min_weight_fraction = 0.0;
+};
+
+// balanced_subsample weights from a tree's integer root class sums (compute_class_weight("balanced") of
+// the bootstrap sample: n_samples / (n_present_classes * bincount); absent classes 0).  The builders form
+// the same two float64 operations on the device.
+inline void forest_subsample_weights(const uint32_t* sums, int C, double* w) {
+  uint64_t n = 0; int kp = 0;
+  for (int c = 0; c < C; ++c) { n += sums[c]; kp += sums[c] != 0; }
+  for (int c = 0; c < C; ++c) {
+    const volatile double den = (double)kp * (double)sums[c];
+    w[c] = sums[c] ? (double)n / den : 0.0;
+  }
+}
 
 bool forest_fast_supported(const Ctx* c, int n_classes, bool reg, int random_split);
 int forest_fast_slots_per_sm();

@@ -122,8 +122,42 @@ __device__ __noinline__ FfProxy ff_proxy4(uint32_t l0, uint32_t l1, uint32_t l2,
   r.proxy = __dsub_rn(__dmul_rn(-wr, r.ir), __dmul_rn(wl, r.il));
   return r;
 }
-template <int CM>
+// Weighted builds (W): the class weights of the CTA's tree, set before the tree's first node.  Every weighted
+// statistic is cw_c * (integer count) in float64.  The float32 rank value works on the weights scaled by the
+// power of two ff_cwscale that brings the largest into [1/2, 1) (ranks, bars and w_node all carry the same
+// exact factor; the host keeps the fast builder to weights within 2^40 of each other, so no float32
+// product or square under- or overflows).
+__shared__ double ff_cw[4];
+__shared__ float ff_cwf[4];
+__shared__ double ff_cwscale;
+
+// ... the same proxy with class weights: sum_left[c] = cw_c * l_c, sum_right[c] = cw_c * t_c - sum_left[c]
+// (ClassificationCriterion.update), w_l = sum_c sum_left[c], w_r = w_node - w_l
+__device__ __noinline__ FfProxy ff_proxy4w(uint32_t l0, uint32_t l1, uint32_t l2, uint32_t l3,
+                                           uint32_t t0, uint32_t t1, uint32_t t2, uint32_t t3, int C, double w_node) {
+  const uint32_t l[4] = {l0, l1, l2, l3}, t[4] = {t0, t1, t2, t3};
+  double sql = 0.0, sqr = 0.0, wl = 0.0;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    if (c < C) {
+      const double a = __dmul_rn(ff_cw[c], (double)l[c]), b = __dsub_rn(__dmul_rn(ff_cw[c], (double)t[c]), a);
+      wl = __dadd_rn(wl, a);
+      sql = __dadd_rn(sql, __dmul_rn(a, a));
+      sqr = __dadd_rn(sqr, __dmul_rn(b, b));
+    }
+  }
+  const double wr = w_node - wl;
+  FfProxy r;
+  r.il = __dsub_rn(1.0, __ddiv_rn(sql, __dmul_rn(wl, wl)));
+  r.ir = __dsub_rn(1.0, __ddiv_rn(sqr, __dmul_rn(wr, wr)));
+  r.proxy = __dsub_rn(__dmul_rn(-wr, r.ir), __dmul_rn(wl, r.il));
+  return r;
+}
+template <int CM, bool W>
 __device__ __forceinline__ FfProxy ff_proxy(const uint32_t (&sl)[CM], const uint32_t* st, int C, double w_node) {
+  if constexpr (W)
+    return ff_proxy4w(sl[0], CM > 1 ? sl[1] : 0u, CM > 2 ? sl[2] : 0u, CM > 3 ? sl[3] : 0u,
+                      st[0], CM > 1 ? st[1] : 0u, CM > 2 ? st[2] : 0u, CM > 3 ? st[3] : 0u, C, w_node);
   return ff_proxy4(sl[0], CM > 1 ? sl[1] : 0u, CM > 2 ? sl[2] : 0u, CM > 3 ? sl[3] : 0u,
                    st[0], CM > 1 ? st[1] : 0u, CM > 2 ? st[2] : 0u, CM > 3 ? st[3] : 0u, C, w_node);
 }
@@ -131,20 +165,35 @@ __device__ __forceinline__ FfProxy ff_proxy(const uint32_t (&sl)[CM], const uint
 // float32 rank value of a split: sq_l / w_l + sq_r / w_r (= proxy + w_node in exact arithmetic; the
 // float32 value is within 2^-20 * w_node of it).  Candidates, features and batches are compared on it;
 // scikit-learn's float64 expression is evaluated only for values within FF_BAR * w_node of each other.
+// Weighted: a_c = cw_c l_c and b_c = cw_c r_c in float32 (scaled cw_c), w_l = sum a_c, w_r = sum b_c (no
+// cancellation against w_node): within 2^-18 * w_node, bar FF_BAR_W (DESIGN.md §4).
 constexpr float FF_BAR = 1.9073486328125e-6f;      // 2^-19
-template <int CM>
+constexpr float FF_BAR_W = 7.62939453125e-6f;      // 2^-17
+template <int CM, bool W>
 __device__ __forceinline__ float ff_rank(const uint32_t* sl, const uint32_t* st, int C, float w_node) {
   float wl = 0.f, sql = 0.f, sqr = 0.f;
+  if constexpr (W) {
+    float wr = 0.f;
+#pragma unroll
+    for (int c = 0; c < CM; ++c) if (c < C) {
+      const float a = __fmul_rn(ff_cwf[c], (float)sl[c]), b = __fmul_rn(ff_cwf[c], (float)(st[c] - sl[c]));
+      wl += a; wr += b; sql = fmaf(a, a, sql); sqr = fmaf(b, b, sqr);
+    }
+    return __fdividef(sql, wl) + __fdividef(sqr, wr);
+  }
 #pragma unroll
   for (int c = 0; c < CM; ++c) if (c < C) { const float a = (float)sl[c], b = (float)(st[c] - sl[c]); wl += a; sql = fmaf(a, a, sql); sqr = fmaf(b, b, sqr); }
   return __fdividef(sql, wl) + __fdividef(sqr, w_node - wl);
 }
-template <int CM>
+template <int CM, bool W>
 __device__ __forceinline__ bool ff_weights_ok(const uint32_t* sl, int C, double w_node, double min_weight_leaf) {
   if (!(min_weight_leaf > 0.0)) return true;
   double wl = 0.0;
 #pragma unroll
-  for (int c = 0; c < CM; ++c) if (c < C) wl += (double)sl[c];
+  for (int c = 0; c < CM; ++c) if (c < C) {
+    if constexpr (W) wl = __dadd_rn(wl, __dmul_rn(ff_cw[c], (double)sl[c]));
+    else wl += (double)sl[c];
+  }
   return !(wl < min_weight_leaf || w_node - wl < min_weight_leaf);
 }
 
@@ -152,7 +201,7 @@ __device__ __forceinline__ bool ff_weights_ok(const uint32_t* sl, int C, double 
 // feature's best split in *R.  Two histogram layouts: packed = 0: H[c][256] class weights (32-bit) then
 // [256] sample counts; packed = 1: class pairs in 16-bit halves H[c / 2][256], then sample counts, two
 // bins per word, from word `hcw`.  st = the node's class sums (shared memory).
-template <int CM>
+template <int CM, bool W>
 __device__ __noinline__ void ff_scan(const unsigned int* H, int packed, int hcw, int lane, int C, int n_node,
                                      const uint32_t* st, double w_node, int min_samples_leaf,
                                      double min_weight_leaf, FfResult<CM>* R) {
@@ -203,7 +252,7 @@ __device__ __noinline__ void ff_scan(const unsigned int* H, int packed, int hcw,
   const int mylast = pmask ? lane * 8 + 31 - __clz(pmask) : -1;
   const int glast = __reduce_max_sync(0xffffffffu, mylast);
   const bool is_const = glast <= gfirst;      // distinct values are > 1e-7 apart (host check): one bin == constant
-  const float wnf = (float)w_node;
+  const float wnf = W ? (float)(w_node * ff_cwscale) : (float)w_node;
   // pass 1: float32 rank value of every candidate of this lane: its best and second best
   float pbest = -INFINITY, psecond = -INFINITY;
   if (!is_const) {
@@ -221,8 +270,8 @@ __device__ __noinline__ void ff_scan(const unsigned int* H, int packed, int hcw,
       if (!pm && nxt >= (1 << 20)) break;       // last present bin of the node: no boundary above it
       const int n_left = (int)run_cnt;
       if (n_left < min_samples_leaf || n_node - n_left < min_samples_leaf) continue;
-      if (!ff_weights_ok<CM>(s2, C, w_node, min_weight_leaf)) continue;   // exact test: an invalid candidate must not set the bar
-      const float pt = ff_rank<CM>(s2, st, C, wnf);
+      if (!ff_weights_ok<CM, W>(s2, C, w_node, min_weight_leaf)) continue;   // exact test: an invalid candidate must not set the bar
+      const float pt = ff_rank<CM, W>(s2, st, C, wnf);
       if (pt > pbest) { psecond = pbest; pbest = pt; }
       else if (pt > psecond) psecond = pt;
     }
@@ -234,7 +283,7 @@ __device__ __noinline__ void ff_scan(const unsigned int* H, int packed, int hcw,
     if (lane == 0) { R->proxy = -INFINITY; R->ptil = -INFINITY; R->exact = 1; R->n_left = 1 << 30; R->code = is_const ? (1 << 16) : 0; }
     return;
   }
-  const float pthr = pmax - wnf * FF_BAR;
+  const float pthr = pmax - wnf * (W ? FF_BAR_W : FF_BAR);
   // Is the best candidate alone within the bar?  (a lane's best and second best tell "none", "one" or
   // "several" of its candidates are near)
   const int nnear = (pbest >= pthr ? 1 : 0) + (psecond >= pthr ? 1 : 0);
@@ -260,10 +309,10 @@ __device__ __noinline__ void ff_scan(const unsigned int* H, int packed, int hcw,
       if (!pm && nxt >= (1 << 20)) break;
       const int n_left = (int)run_cnt;
       if (n_left < min_samples_leaf || n_node - n_left < min_samples_leaf) continue;
-      if (!ff_weights_ok<CM>(sl, C, w_node, min_weight_leaf)) continue;
-      const float pt = ff_rank<CM>(sl, st, C, wnf);
+      if (!ff_weights_ok<CM, W>(sl, C, w_node, min_weight_leaf)) continue;
+      const float pt = ff_rank<CM, W>(sl, st, C, wnf);
       if (!(pt >= pthr)) continue;
-      const double proxy = single ? 0.0 : ff_proxy<CM>(sl, st, C, w_node).proxy;
+      const double proxy = single ? 0.0 : ff_proxy<CM, W>(sl, st, C, w_node).proxy;
       if (single || proxy > bproxy) {
         const int nb2 = pm ? lane * 8 + __ffs(pm) - 1 : nxt;
         bproxy = proxy; bpt = pt; bnl = n_left; bcode = (lane * 8 + j) | (nb2 << 8);
@@ -292,7 +341,9 @@ __device__ __noinline__ void ff_scan(const unsigned int* H, int packed, int hcw,
 
 #define FF_TICK(ph) do { if (P.o_prof && tid == 0) { const long long _t = clock64(); s_prof[ph] += _t - tlast; tlast = _t; } } while (0)
 
-template <int CM>
+// W: class weights.  The counts, histograms, records and the partition are those of the unweighted build;
+// the float64 statistics are cw_c * count (ff_proxy4w) and the float32 rank takes the weighted bar.
+template <int CM, bool W>
 __global__ void __launch_bounds__(FF_THREADS, 7)
 forest_fast_kernel(const FfParams P) {
   typedef typename FfAcc<CM>::T acc_t;
@@ -335,6 +386,8 @@ forest_fast_kernel(const FfParams P) {
   // ---- initialise the tree: samples with non-zero weight in ascending order (Splitter.init) ----
   for (int i = tid; i < d; i += FF_THREADS) features[i] = (uint8_t)i;
   if (tid < 4) best_sl[tid] = 0;
+  // balanced_subsample: 1 until the root's class sums give the weights (only absent classes get 0)
+  if constexpr (W) if (tid < 4) ff_cw[tid] = P.cw_bs || tid >= C ? 1.0 : P.cw[tid];
   __syncthreads();
   int n_nz = 0;
   {
@@ -350,6 +403,7 @@ forest_fast_kernel(const FfParams P) {
         const int64_t i = i0 + q * FF_THREADS + tid;
         w4[q] = 0; y4[q] = 0;
         if (i < n) { w4[q] = cnt[i]; y4[q] = (unsigned)P.ycls[i]; }
+        if constexpr (W) if (ff_cw[y4[q]] == 0.0) w4[q] = 0;     // rows of weight 0 leave the tree (Splitter.init)
         const unsigned bal = __ballot_sync(0xffffffffu, w4[q] != 0);
         if (lane == 0) wsum[q * FF_WARPS + wid] = __popc(bal);
         rk4[q] = __popc(bal & ((1u << lane) - 1));
@@ -388,8 +442,33 @@ forest_fast_kernel(const FfParams P) {
   }
   __syncthreads();
   double w_samples = 0.0;          // weighted_n_samples (integer valued)
+  if constexpr (W) {
+    if (P.cw_bs) {   // compute_class_weight("balanced") of the bootstrap sample: n / (K_present * N_c)
+      if (tid < C) {
+        uint32_t nt = 0; int kp = 0;
+        for (int c = 0; c < C; ++c) { nt += best_sl[c]; kp += best_sl[c] != 0; }
+        ff_cw[tid] = best_sl[tid] ? __ddiv_rn((double)nt, __dmul_rn((double)kp, (double)best_sl[tid])) : 0.0;
+      }
+      __syncthreads();
+    }
+    if (tid == 0) {
+      double mx = 0.0;
+      for (int c = 0; c < C; ++c) mx = fmax(mx, ff_cw[c]);
+      int e = 0;
+      frexp(mx, &e);
+      ff_cwscale = ldexp(1.0, -e);
+    }
+    __syncthreads();
+    if (tid < 4) ff_cwf[tid] = (float)(ff_cw[tid] * ff_cwscale);
 #pragma unroll
-  for (int c = 0; c < CM; ++c) if (c < C) w_samples += (double)best_sl[c];
+    for (int c = 0; c < CM; ++c) if (c < C) w_samples = __dadd_rn(w_samples, __dmul_rn(ff_cw[c], (double)best_sl[c]));
+  } else {
+#pragma unroll
+    for (int c = 0; c < CM; ++c) if (c < C) w_samples += (double)best_sl[c];
+  }
+  // BaseDecisionTree._fit: min_weight_leaf = min_weight_fraction_leaf * sum(sample_weight)
+  const double mwl_w = W ? __dmul_rn(P.min_weight_fraction, w_samples) : 0.0;
+#define MIN_WEIGHT_LEAF (W ? mwl_w : P.min_weight_leaf)
 
   uint32_t rstate = P.rand_state[slot];
   int sp = 0, node_count = 0, max_depth_seen = -1, status = 0;
@@ -421,14 +500,20 @@ forest_fast_kernel(const FfParams P) {
     const int n_known = rec->flags & 0xFFFF;
     double w_node = 0.0;
 #pragma unroll
-    for (int c = 0; c < CM; ++c) if (c < C) w_node += (double)rec->sums[c];
+    for (int c = 0; c < CM; ++c) if (c < C) {
+      if constexpr (W) w_node = __dadd_rn(w_node, __dmul_rn(ff_cw[c], (double)rec->sums[c]));
+      else w_node += (double)rec->sums[c];
+    }
     double impurity = rec->impurity;
     bool is_leaf = depth >= P.max_depth || n_node < P.min_samples_split || n_node < 2 * P.min_samples_leaf ||
-                   w_node < 2.0 * P.min_weight_leaf;
+                   w_node < 2.0 * MIN_WEIGHT_LEAF;
     if (first) {   // root: node_impurity()  (SK/tree/_criterion.pyx:620-640)
       double sq = 0.0;
 #pragma unroll
-      for (int c = 0; c < CM; ++c) if (c < C) { const double a = (double)rec->sums[c]; sq = __dadd_rn(sq, __dmul_rn(a, a)); }
+      for (int c = 0; c < CM; ++c) if (c < C) {
+        const double a = W ? __dmul_rn(ff_cw[c], (double)rec->sums[c]) : (double)rec->sums[c];
+        sq = __dadd_rn(sq, __dmul_rn(a, a));
+      }
       impurity = __dsub_rn(1.0, __ddiv_rn(sq, __dmul_rn(w_node, w_node)));
       first = false;
     }
@@ -552,7 +637,7 @@ forest_fast_kernel(const FfParams P) {
           FF_TICK(3);
           for (int k = wid; k < nbatch; k += FF_WARPS) {
             const unsigned int* H = U + k * hstrideA;
-            ff_scan<CM>(H, 0, 0, lane, C, n_node, rec->sums, w_node, P.min_samples_leaf, P.min_weight_leaf, &results[k]);
+            ff_scan<CM, W>(H, 0, 0, lane, C, n_node, rec->sums, w_node, P.min_samples_leaf, MIN_WEIGHT_LEAF, &results[k]);
           }
         } else if (!small) {
           // ---- staged histogram node: warp k builds and scans the packed histogram of item k ----
@@ -580,7 +665,7 @@ forest_fast_kernel(const FfParams P) {
               }
             }
             __syncwarp();
-            ff_scan<CM>(H, 1, hcw, lane, C, n_node, rec->sums, w_node, P.min_samples_leaf, P.min_weight_leaf, &results[k]);
+            ff_scan<CM, W>(H, 1, hcw, lane, C, n_node, rec->sums, w_node, P.min_samples_leaf, MIN_WEIGHT_LEAF, &results[k]);
           }
         } else {
           // ---- staged node of <= 32 samples: lane j holds sample j; every lane counts the samples
@@ -612,12 +697,12 @@ forest_fast_kernel(const FfParams P) {
             float pt = -INFINITY;
             const int n_left = (int)(acc >> CNT);
             if (cand && n_left >= P.min_samples_leaf && n_node - n_left >= P.min_samples_leaf &&
-                ff_weights_ok<CM>(sl, C, w_node, P.min_weight_leaf))
-              pt = ff_rank<CM>(sl, rec->sums, C, (float)w_node);
+                ff_weights_ok<CM, W>(sl, C, w_node, MIN_WEIGHT_LEAF))
+              pt = ff_rank<CM, W>(sl, rec->sums, C, W ? (float)(w_node * ff_cwscale) : (float)w_node);
             float pm = pt;
 #pragma unroll 1
             for (int o = 16; o > 0; o >>= 1) pm = fmaxf(pm, __shfl_xor_sync(0xffffffffu, pm, o));
-            const bool near = pt > -INFINITY && pt >= pm - (float)w_node * FF_BAR;
+            const bool near = pt > -INFINITY && pt >= pm - (W ? (float)(w_node * ff_cwscale) * FF_BAR_W : (float)w_node * FF_BAR);
             const unsigned nm = __ballot_sync(0xffffffffu, near);
             FfResult<CM>* R = &results[k];
             if (nm == 0u) {
@@ -631,7 +716,7 @@ forest_fast_kernel(const FfParams P) {
             double proxy = 0.0;
             if (kmin != kmax) {          // different candidates within the bar: scikit-learn's float64 expression decides
               proxy = -INFINITY;
-              if (near) proxy = ff_proxy<CM>(sl, rec->sums, C, w_node).proxy;
+              if (near) proxy = ff_proxy<CM, W>(sl, rec->sums, C, w_node).proxy;
               double wp = proxy; int wnl = near ? n_left : (1 << 30);
 #pragma unroll 1
               for (int o = 16; o > 0; o >>= 1) {
@@ -661,7 +746,7 @@ forest_fast_kernel(const FfParams P) {
               // `proxy > best_proxy` of the reference, decided on the float32 rank values whenever they are
               // more than the bar apart and on scikit-learn's float64 expression otherwise
               if (R.ptil > -INFINITY) {
-                const float bar = (float)w_node * FF_BAR;
+                const float bar = W ? (float)(w_node * ff_cwscale) * FF_BAR_W : (float)w_node * FF_BAR;
                 bool take;
                 if (best_nl <= 0 || R.ptil > best_ptil + bar) {          // first valid split / surely larger
                   take = true; best_exact = R.exact != 0; best_proxy = R.proxy;
@@ -672,7 +757,7 @@ forest_fast_kernel(const FfParams P) {
                     uint32_t bs[CM];
 #pragma unroll
                     for (int c = 0; c < CM; ++c) bs[c] = best_sl[c];
-                    best_proxy = ff_proxy<CM>(bs, rec->sums, C, w_node).proxy;
+                    best_proxy = ff_proxy<CM, W>(bs, rec->sums, C, w_node).proxy;
                     best_exact = true;
                   }
                   double rp = R.proxy;
@@ -680,7 +765,7 @@ forest_fast_kernel(const FfParams P) {
                     uint32_t rs2[CM];
 #pragma unroll
                     for (int c = 0; c < CM; ++c) rs2[c] = R.sl[c];
-                    rp = ff_proxy<CM>(rs2, rec->sums, C, w_node).proxy;
+                    rp = ff_proxy<CM, W>(rs2, rec->sums, C, w_node).proxy;
                   }
                   take = rp > best_proxy;
                   if (take) best_proxy = rp;
@@ -718,12 +803,15 @@ forest_fast_kernel(const FfParams P) {
         if (best_nl > 0) {
           double wl = 0.0;
 #pragma unroll
-          for (int c = 0; c < CM; ++c) if (c < C) wl += (double)best_sl[c];
+          for (int c = 0; c < CM; ++c) if (c < C) {
+            if constexpr (W) wl = __dadd_rn(wl, __dmul_rn(ff_cw[c], (double)best_sl[c]));
+            else wl += (double)best_sl[c];
+          }
           const double wr = w_node - wl;
           uint32_t bs[CM];
 #pragma unroll
           for (int c = 0; c < CM; ++c) bs[c] = best_sl[c];
-          const FfProxy pr = ff_proxy<CM>(bs, rec->sums, C, w_node);
+          const FfProxy pr = ff_proxy<CM, W>(bs, rec->sums, C, w_node);
           const double il = pr.il, ir = pr.ir;
           // impurity_improvement (SK/tree/_criterion.pyx:163-190)
           const double a = __dmul_rn(__ddiv_rn(wr, w_node), ir);
@@ -890,6 +978,7 @@ forest_fast_kernel(const FfParams P) {
   }
 }
 #undef FF_TICK
+#undef MIN_WEIGHT_LEAF
 
 // ---- host side -----------------------------------------------------------------------------
 static size_t ff_smem_bytes(int CM, int d) {
@@ -927,15 +1016,11 @@ int forest_fast_launch(Ctx* c, FfParams& P, int nt) {
   const int CM = P.n_classes <= 2 ? 2 : 4;
   const size_t smem = ff_smem_bytes(CM, P.d);
   P.n_trees = nt;
-  if (CM == 2) {
-    SKD_CUDA(c, cudaFuncSetAttribute(forest_fast_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    SKD_CUDA(c, cudaFuncSetAttribute(forest_fast_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    forest_fast_kernel<2><<<nt, FF_THREADS, smem, c->stream>>>(P);
-  } else {
-    SKD_CUDA(c, cudaFuncSetAttribute(forest_fast_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    SKD_CUDA(c, cudaFuncSetAttribute(forest_fast_kernel<4>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    forest_fast_kernel<4><<<nt, FF_THREADS, smem, c->stream>>>(P);
-  }
+  void (*kern)(const FfParams) = CM == 2 ? (P.weighted ? forest_fast_kernel<2, true> : forest_fast_kernel<2, false>)
+                                        : (P.weighted ? forest_fast_kernel<4, true> : forest_fast_kernel<4, false>);
+  SKD_CUDA(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  SKD_CUDA(c, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  kern<<<nt, FF_THREADS, smem, c->stream>>>(P);
   SKD_CUDA(c, cudaGetLastError());
   c->launches += 1;
   return 0;

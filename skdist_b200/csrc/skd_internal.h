@@ -8,6 +8,7 @@
 #include <utility>
 #include <vector>
 
+#include "forest_common.h"
 #include "lbfgs_core.h"
 
 namespace skd {
@@ -99,6 +100,8 @@ struct Ctx {
   std::vector<float> h_cw;
   std::vector<double> h_swsum;
   int32_t cw_cols = 0, cw_k = 0;
+  // class weights for the next forest fit (skd_stage_forest_class_weights; n_classes == 0: none)
+  ForestClassWeights forest_cw;
   // scratch pool: device blocks released by finished calls, reused by the next ones (Scratch below)
   std::vector<std::pair<void*, size_t>> pool_free;
   size_t pool_bytes = 0;
@@ -268,7 +271,7 @@ void forest_free(Ctx* c);
 int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_states, int n_classes,
                int max_features, int max_depth, int min_samples_split, int min_samples_leaf,
                double min_weight_leaf, double min_impurity_decrease, int random_split, const double* h_yreal,
-               ForestSink sink, void* sink_arg);
+               const ForestClassWeights* cw, ForestSink sink, void* sink_arg);
 int predict_device(Ctx* c, const float* dX, int64_t m, int ldx, int d, int B, const float* dW, float* dout);
 int forest_predict_device(Ctx* c, const float* dX, int64_t m, int ldx, int n_trees, const int64_t* d_off,
                           const void* d_node, const double* d_thr, const double* d_val, int C, double* d_out);

@@ -174,7 +174,21 @@ _LIMITS = """
     thresholds back to raw units -- the trees scikit-learn builds on the coded matrix, not bit-identical to the
     reference on the raw one), at most 16 classes, at most
     384 features, bootstrap multiplicities up to 255, no missing values, `criterion` gini / squared
-    error, no `class_weight`, `max_leaf_nodes`, `sample_weight` or multi-output targets."""
+    error, no `max_leaf_nodes`, `sample_weight` or multi-output targets; `class_weight` (classifiers) may
+    be a dict, "balanced" or "balanced_subsample", not "subsample" or a list of dicts."""
+
+_CLASS_WEIGHT = """
+
+    `class_weight` follows the reference's per-tree task (ref ensemble.py:68-109): tree t is fitted with
+    sample_weight = (bootstrap multiplicity) * cw[y], cw from scikit-learn's `compute_class_weight` on all of
+    y ("balanced", dict: absent classes 1.0) or, for "balanced_subsample" with bootstrap, on the tree's
+    bootstrap sample (absent classes 0).  Rows of weight 0 leave the tree.  scikit-learn 1.9's own
+    RandomForestClassifier differs for a dict or "balanced" with bootstrap=True: it draws the bootstrap
+    with the class weights as sampling probabilities and fits on plain multiplicities; with
+    "balanced_subsample", or bootstrap=False, the two agree.  The trees equal the reference's bit for bit
+    when the weighted sums are exact (integer or dyadic weights); otherwise node statistics agree to
+    rounding and a split can differ only between candidates whose Gini proxies lie within rounding of
+    each other (DESIGN.md §4)."""
 
 
 class _DistForestClassifier(_ScParamMixin):
@@ -233,8 +247,10 @@ class _DistForestClassifier(_ScParamMixin):
             bad.append("criterion=%r (only 'gini')" % self.criterion)
         if self.max_leaf_nodes is not None:
             bad.append("max_leaf_nodes (best-first builder)")
-        if self.class_weight is not None:
-            bad.append("class_weight")
+        cw = self.class_weight
+        if cw is not None and not (isinstance(cw, dict) or cw in ("balanced", "balanced_subsample")):
+            bad.append("class_weight=%r (dict, 'balanced' or 'balanced_subsample'; 'subsample' is a removed "
+                       "scikit-learn mode, a list of dicts is multi-output)" % (cw,))
         if self.min_impurity_split is not None:
             bad.append("min_impurity_split")
         if bad:
@@ -256,6 +272,24 @@ class _DistForestClassifier(_ScParamMixin):
         mss = self.min_samples_split
         msl = self.min_samples_leaf
         return mf_i, max_depth, mss, msl
+
+    def _class_weights(self, y):
+        """(per-class weights or None, balanced_subsample) of the reference's per-tree sample_weight
+        (ref ensemble.py:68-109, 229-238)."""
+        cw = self.class_weight
+        if cw is None:
+            return None, False
+        if isinstance(cw, str) and cw == "balanced_subsample":
+            if self.bootstrap:
+                return None, True                     # per tree, on the device, from its bootstrap class counts
+            cw = "balanced"                           # no bootstrap: the sample is all of y
+        from sklearn.utils.class_weight import compute_class_weight
+        w = np.asarray(compute_class_weight(cw, classes=self.classes_, y=y), dtype=np.float64)
+        if not (np.all(np.isfinite(w)) and np.all(w >= 0)):
+            raise ValueError("class_weight must be finite and >= 0")
+        if not np.any(w > 0):
+            raise ValueError("class_weight gives every class weight 0")
+        return w, False
 
     def fit(self, X, y, sample_weight=None):
         """Build the forest (ref ensemble.py:177-336)."""
@@ -279,6 +313,8 @@ class _DistForestClassifier(_ScParamMixin):
             self.classes_, y_enc = np.unique(y, return_inverse=True)   # ref :229 (_validate_y_class_weight)
             self.n_classes_ = len(self.classes_)
         mf_i, max_depth, mss, msl = self._resolved(d)
+        cw, cw_subsample = (None, False) if self._regression else self._class_weights(y)
+        weighted = cw is not None or cw_subsample
         if not isinstance(mss, (int, np.integer)):
             mss = max(2, int(np.ceil(mss * n)))
         if not isinstance(msl, (int, np.integer)):
@@ -329,6 +365,9 @@ class _DistForestClassifier(_ScParamMixin):
         # (the throughput builder of csrc/forest_fast.cu keeps seven trees per SM resident, the general
         # one two: a chunk is one full wave of the builder that will run)
         fast = not self._regression and self._splitter == 0 and self.n_classes_ <= 4 and d <= 255
+        if cw is not None and fast:       # the library keeps positive dict weights within 2^40 on the throughput builder
+            pos = cw[cw > 0]
+            fast = bool(pos.max() <= 2.0 ** 40 * pos.min())
         chunk = int(os.environ.get("SKDIST_B200_FOREST_CHUNK", "1036" if fast else "296"))
         chunks = [my_states[i:i + chunk] for i in range(0, len(my_states), chunk)]
 
@@ -341,6 +380,8 @@ class _DistForestClassifier(_ScParamMixin):
 
         def build(counts, rs):
             try:
+                if weighted:      # one-shot: staged for each chunk's fit (min_weight_leaf per tree: fraction * sum w)
+                    eng.stage_forest_class_weights(self.n_classes_, cw, cw_subsample, self.min_weight_fraction_leaf)
                 return eng.forest_fit(counts, rs, self.n_classes_, mf_i, max_depth, int(mss), int(msl),
                                       float(min_weight_leaf), float(self.min_impurity_decrease),
                                       splitter=self._splitter, y_regression=y_reg)
@@ -400,7 +441,7 @@ class _DistForestClassifier(_ScParamMixin):
 
 class DistRandomForestClassifier(_DistForestClassifier, RandomForestClassifier):
     __doc__ = """Same as sklearn `RandomForestClassifier` with every tree built on an H100.
-    Constructor mirrors ref ensemble.py:378-422 (``sc`` is the FIRST positional argument).""" + _LIMITS
+    Constructor mirrors ref ensemble.py:378-422 (``sc`` is the FIRST positional argument).""" + _LIMITS + _CLASS_WEIGHT
 
     _splitter = 0
     _tree_cls = DecisionTreeClassifier
@@ -419,7 +460,7 @@ class DistRandomForestClassifier(_DistForestClassifier, RandomForestClassifier):
 class DistExtraTreesClassifier(_DistForestClassifier, ExtraTreesClassifier):
     __doc__ = """Same as sklearn `ExtraTreesClassifier` with every tree built on an H100 (random splitter:
     one uniformly drawn threshold per drawn feature, no bootstrap by default).
-    Constructor mirrors ref ensemble.py:437-478 (``sc`` is the FIRST positional argument).""" + _LIMITS
+    Constructor mirrors ref ensemble.py:437-478 (``sc`` is the FIRST positional argument).""" + _LIMITS + _CLASS_WEIGHT
 
     _splitter = 1
     _tree_cls = ExtraTreeClassifier

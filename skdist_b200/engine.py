@@ -344,6 +344,19 @@ class Engine:
                 "coef32": coef, "intercept": intercept, "n_iter": n_iter, "t": t, "status": status,
                 "gpu_seconds": secs.value}
 
+    def stage_forest_class_weights(self, n_classes, w=None, balanced_subsample=False, min_weight_fraction_leaf=0.0):
+        """Class weights of the next forest_fit: w [n_classes] float64 (the same for every tree), or
+        balanced_subsample=True (per tree from its bootstrap class counts; w unused).  min_weight_fraction_leaf
+        replaces that fit's min_weight_leaf (per tree: fraction * its sum of weights).  n_classes = 0 clears."""
+        if balanced_subsample or not n_classes:
+            check(self._lib.skd_stage_forest_class_weights(self._h, int(n_classes), None, int(bool(balanced_subsample)),
+                                                           float(min_weight_fraction_leaf)), self._h)
+            return
+        w = np.ascontiguousarray(w, dtype=np.float64)
+        assert w.shape == (n_classes,)
+        check(self._lib.skd_stage_forest_class_weights(self._h, int(n_classes), ptr(w), 0,
+                                                       float(min_weight_fraction_leaf)), self._h)
+
     def forest_fit(self, sample_counts, rand_states, n_classes, max_features, max_depth, min_samples_split,
                    min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter=0, y_regression=None):
         """Build len(rand_states) classifier trees.  sample_counts [n_trees, n] uint8 (bootstrap
