@@ -14,6 +14,9 @@
 // ascending order ARE the sorted distinct values, so every candidate split, its class counts and
 // the threshold (v[p-1]/2 + v[p]/2) equal what the sort-based scan sees.  The tree topology, the
 // RNG consumption and therefore every later draw are bit-identical to scikit-learn's.
+// The random splitter (node_split_random, ExtraTrees) uses the same histograms when every feature has
+// codes, and otherwise reads the raw float32 values (min / max pass, drawn threshold, left-side pass),
+// so it takes continuous features.
 // No tensor cores: the work is integer histogramming, bound by gather bandwidth / latency.
 #include <math.h>
 #include <stdlib.h>
@@ -58,8 +61,9 @@ constexpr int FO_SSTK = 128;     // builder-stack entries kept in shared memory 
 constexpr int FO_HIST_WORDS = 40 * FO_BINS;   // KB * (C + 1) * 256 <= this
 
 struct FoParams {
-  const uint8_t* xbin;        // [d][n] bin codes, feature-major
+  const uint8_t* xbin;        // [d][n] bin codes, feature-major (best splitter)
   const float* binval;        // [d][256] distinct values ascending
+  const float* xval;          // [d][n] raw values, feature-major: random splitter on features without codes, else nullptr
   const int32_t* ycls;        // [n] class ids (classification)
   const double* yreal;        // [n] float64 targets (regression: MSE criterion), else nullptr
   int64_t n;
@@ -166,7 +170,9 @@ __device__ __forceinline__ void fo_children_mse(const unsigned long long* sl, co
 // counts; the float64 statistics are w_c * count (one rounding), in scikit-learn's operation order.
 #define FO_TICK(ph) do { if (P.o_prof && tid == 0) { const long long _t = clock64(); prof[ph] += _t - tlast; tlast = _t; } } while (0)
 #define FOR_C(c) _Pragma("unroll") for (int c = 0; c < CM; ++c) if (c < C)
-template <int CM, bool REG, bool W>
+// RAW: random splitter over the raw values (P.xval), a separate instantiation so that the histogram
+// instantiations keep their register allocation.
+template <int CM, bool REG, bool W, bool RAW>
 __global__ void __launch_bounds__(FO_THREADS)
 forest_build_kernel(const FoParams P) {
   static_assert(!(REG && W), "class weights are a classification feature");
@@ -184,7 +190,11 @@ forest_build_kernel(const FoParams P) {
   extern __shared__ int fo_sm[];
   int* features = fo_sm;                     // [d]
   int* constant_features = fo_sm + d;        // [d]
-  __shared__ unsigned int hist[FO_HIST_WORDS];   // per batch item: [c][bin] class weights (c < C), then [bin] sample counts
+  // best splitter, per batch item: [c][bin] class weights (c < C), then [bin] sample counts;
+  // random splitter: [item][c][thread] left-side statistics of each thread's samples
+  __shared__ __align__(16) unsigned int hist[FO_HIST_WORDS];
+  __shared__ float s_mm[2][FO_THREADS / 32][FO_KB_MAX];   // random splitter: per-warp min / max of the batch features
+  __shared__ int s_nl[FO_THREADS / 32][FO_KB_MAX];        // random splitter: per-warp left counts
   __shared__ FoItem items[FO_KB_MAX];
   __shared__ FoResult results[FO_KB_MAX];
   __shared__ int s_sim_nd, s_sim_ulen;
@@ -241,17 +251,20 @@ forest_build_kernel(const FoParams P) {
     __syncthreads();
   }
   const int n_nz = base_s;
-  // reduce the class sums over the block (integers: exact)
+  // reduce the class sums over the block in a fixed order (warps, then the warp totals in warp order):
+  // integers are exact anyway, the float64 regression sums are then the same from run to run
   __shared__ unsigned long long red[FO_MAXC];
-  if (tid < FO_MAXC) red[tid] = 0;
-  __syncthreads();
+  unsigned long long* wred = reinterpret_cast<unsigned long long*>(hist);   // [warp][FO_MAXC]
   FOR_C(c) {
     unsigned long long v = my_sums[c];
     for (int o = 16; o > 0; o >>= 1) v = st_add<REG>(v, __shfl_xor_sync(0xffffffffu, v, o));
-    if (lane == 0) {
-      if constexpr (REG) atomicAdd(reinterpret_cast<double*>(&red[c]), st_d(v));   // 0 bit pattern == 0.0
-      else atomicAdd(&red[c], v);
-    }
+    if (lane == 0) wred[wid * FO_MAXC + c] = v;
+  }
+  __syncthreads();
+  if (tid < C) {
+    unsigned long long v = 0;   // 0 bit pattern == 0.0
+    for (int w = 0; w < FO_THREADS / 32; ++w) v = st_add<REG>(v, wred[w * FO_MAXC + tid]);
+    red[tid] = v;
   }
   __syncthreads();
   double w_samples = 0.0;
@@ -374,144 +387,118 @@ forest_build_kernel(const FoParams P) {
           s_ctrl[1] = s_fi; s_ctrl[7] = s_nv; s_sim_nd = s_nd; s_sim_rs = s_rs; s_sim_ulen = ulen;
           if (nbatch == 0) { f_i = s_fi; n_visited = s_nv; n_drawn = s_nd; rstate = s_rs; }
         } else if (tid >= 32) {
-          // meanwhile the other warps clear the histograms of a full batch
+          // meanwhile the other warps clear the histograms (random splitter: the per-thread left
+          // statistics, KB * C * FO_THREADS words, 64-bit when REG, which this covers) of a full batch
           for (int i = tid - 32; i < KB * hstride; i += FO_THREADS - 32) hist[i] = 0;
         }
         __syncthreads();
         FO_TICK(1);
         const int nbatch = s_ctrl[0];
         if (nbatch == 0) break;
-        // --- histograms of all batch features in one pass over the node's samples ---
-        // the distinct values of the batch features are staged in the same phase (their loads overlap
-        // the gathers below); the scan reads them inside dependent per-candidate loops
-        float stage[FO_KB_MAX];   // FO_KB_MAX * 256 values / 256 threads
+        if constexpr (RAW) {
+          // ------------------- node_split_random over the raw float32 values -------------------
+          // (SK/tree/_splitter.pyx node_split_random, DensePartitioner find_min_max / partition_samples)
+          int fk[FO_KB_MAX];   // batch item k reads the column P.xval + fk[k] * n
 #pragma unroll
-        for (int q = 0; q < FO_KB_MAX; ++q)
-          stage[q] = q < nbatch ? __ldg(P.binval + (size_t)items[q].f * FO_BINS + tid) : 0.f;
-        FO_TICK(2);
-        {
-          // all gathers of a sample are issued before the first atomic: one memory round trip per
-          // sample instead of one per feature (the dependent load -> atomic chain serialised them)
-          const uint8_t* col[FO_KB_MAX];
+          for (int k = 0; k < FO_KB_MAX; ++k) fk[k] = items[k < nbatch ? k : 0].f;
+          // pass A: min and max of every batch feature over the node's samples (exact in any order);
+          // all gathers of a sample are issued before the first use
+          float mn[FO_KB_MAX], mx[FO_KB_MAX];
 #pragma unroll
-          for (int k = 0; k < FO_KB_MAX; ++k) col[k] = P.xbin + (size_t)items[k < nbatch ? k : 0].f * n;
+          for (int k = 0; k < FO_KB_MAX; ++k) { mn[k] = INFINITY; mx[k] = -INFINITY; }
+          for (int i = start + tid; i < end; i += FO_THREADS) {
+            const unsigned s = samp[i].x;
+            float v[FO_KB_MAX];
+#pragma unroll
+            for (int k = 0; k < FO_KB_MAX; ++k) v[k] = k < nbatch ? __ldg(P.xval + (size_t)fk[k] * n + s) : 0.f;
+#pragma unroll
+            for (int k = 0; k < FO_KB_MAX; ++k) { mn[k] = fminf(mn[k], v[k]); mx[k] = fmaxf(mx[k], v[k]); }
+          }
+#pragma unroll
+          for (int k = 0; k < FO_KB_MAX; ++k) {
+            for (int o = 16; o > 0; o >>= 1) {
+              mn[k] = fminf(mn[k], __shfl_xor_sync(0xffffffffu, mn[k], o));
+              mx[k] = fmaxf(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o));
+            }
+            if (lane == 0) { s_mm[0][wid][k] = mn[k]; s_mm[1][wid][k] = mx[k]; }
+          }
+          __syncthreads();
+          FO_TICK(3);
+          // every thread forms the same decisions: constant test in float32, threshold
+          // rand_uniform(min, max) in float64 (SK/tree/_utils.pyx), and min if it lands on max
+          double thr[FO_KB_MAX];
+#pragma unroll
+          for (int k = 0; k < FO_KB_MAX; ++k) {
+            float lo = s_mm[0][0][k], hi = s_mm[1][0][k];
+            for (int w = 1; w < FO_THREADS / 32; ++w) { lo = fminf(lo, s_mm[0][w][k]); hi = fmaxf(hi, s_mm[1][w][k]); }
+            thr[k] = -INFINITY;    // constant (or not in the batch): no sample goes left
+            if (k < nbatch && !(hi <= lo + FEATURE_THRESHOLD)) {
+              const double dlo = (double)lo, dhi = (double)hi;
+              double t = __dadd_rn(__ddiv_rn(__dmul_rn(__dsub_rn(dhi, dlo), (double)items[k].rnd), 2147483647.0), dlo);
+              if (t == dhi) t = dlo;
+              thr[k] = t;
+            }
+            if (tid == 0 && k < nbatch) { results[k].is_const = thr[k] == -INFINITY; results[k].thr = thr[k]; }
+          }
+          // pass B: (double)x <= threshold goes left (DensePartitioner.partition_samples); every thread
+          // sums its own samples in order into its own column of `hist`, so that the reduction below
+          // has a fixed order and the float64 regression sums are the same from run to run
+          unsigned nl[FO_KB_MAX];
+#pragma unroll
+          for (int k = 0; k < FO_KB_MAX; ++k) nl[k] = 0;
           for (int i = start + tid; i < end; i += FO_THREADS) {
             const uint2 sv = samp[i];
             const unsigned cls = sv.y & 0xFF, wgt = sv.y >> 8;
             double yv = 0.0;
             if constexpr (REG) yv = __ldg(P.yreal + sv.x);
-            unsigned bbs[FO_KB_MAX];
+            float v[FO_KB_MAX];
 #pragma unroll
-            for (int k = 0; k < FO_KB_MAX; ++k) bbs[k] = k < nbatch ? (unsigned)__ldg(col[k] + sv.x) : 0u;
+            for (int k = 0; k < FO_KB_MAX; ++k) v[k] = k < nbatch ? __ldg(P.xval + (size_t)fk[k] * n + sv.x) : 0.f;
             const double wy = __dmul_rn((double)wgt, yv), wyy = __dmul_rn(wy, yv);
 #pragma unroll
             for (int k = 0; k < FO_KB_MAX; ++k) {
-              if (k < nbatch) {
-                unsigned int* H = hist + k * hstride;
+              if ((double)v[k] <= thr[k]) {
+                nl[k] += 1;
                 if constexpr (REG) {
-                  double* Hd = reinterpret_cast<double*>(H);
-                  atomicAdd(&Hd[0 * FO_BINS + bbs[k]], (double)wgt);
-                  atomicAdd(&Hd[1 * FO_BINS + bbs[k]], wy);
-                  atomicAdd(&Hd[2 * FO_BINS + bbs[k]], wyy);
-                  atomicAdd(&H[6 * FO_BINS + bbs[k]], 1u);
+                  double* A = reinterpret_cast<double*>(hist) + k * 3 * FO_THREADS + tid;
+                  A[0] += (double)wgt;
+                  A[FO_THREADS] += wy;
+                  A[2 * FO_THREADS] += wyy;
                 } else {
-                  atomicAdd(&H[cls * FO_BINS + bbs[k]], wgt);
-                  atomicAdd(&H[C * FO_BINS + bbs[k]], 1u);
+                  hist[(k * C + cls) * FO_THREADS + tid] += wgt;
                 }
               }
             }
           }
 #pragma unroll
-          for (int q = 0; q < FO_KB_MAX; ++q)
-            if (q < nbatch) sbv[q * FO_BINS + tid] = stage[q];
-        }
-        __syncthreads();
-        FO_TICK(3);
-        // --- one warp per feature: scan the 256 bins (8 per lane) in ascending order ---
-        for (int k = wid; k < nbatch; k += FO_THREADS / 32) {
-          const unsigned int* H = hist + k * hstride;
-          const float* bv = sbv + k * FO_BINS;
-          const int cnt_off = REG ? 6 * FO_BINS : C * FO_BINS;
-          // statistic c of bin bb as a 64-bit pattern (class weight, or float64 sum for regression)
-          auto hbin = [&](int c, int bb) -> unsigned long long {
-            if constexpr (REG) return d_st(reinterpret_cast<const double*>(H)[c * FO_BINS + bb]);
-            else return (unsigned long long)H[c * FO_BINS + bb];
-          };
-          unsigned cntb[8];
-          unsigned ltot = 0, pmask = 0;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { cntb[j] = H[cnt_off + lane * 8 + j]; ltot += cntb[j]; if (cntb[j]) pmask |= 1u << j; }
-          // exclusive prefix of sample counts over lanes
-          unsigned pre = ltot;
-          for (int o = 1; o < 32; o <<= 1) { unsigned v = __shfl_up_sync(0xffffffffu, pre, o); if (lane >= o) pre += v; }
-          pre -= ltot;
-          // class-weight prefixes
-          unsigned long long clspre[CM];
-          FOR_C(c) {
-            unsigned long long t = 0;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) t = st_add<REG>(t, hbin(c, lane * 8 + j));
-            unsigned long long incl = t;
-            for (int o = 1; o < 32; o <<= 1) {
-              unsigned long long v = __shfl_up_sync(0xffffffffu, incl, o);
-              if (lane >= o) incl = st_add<REG>(v, incl);
-            }
-            const unsigned long long up = __shfl_up_sync(0xffffffffu, incl, 1);   // exclusive prefix
-            clspre[c] = lane > 0 ? up : 0ull;
+          for (int k = 0; k < FO_KB_MAX; ++k) {
+            const unsigned t = __reduce_add_sync(0xffffffffu, nl[k]);
+            if (lane == 0) s_nl[wid][k] = (int)t;
           }
-          // first present bin of this lane, then "first present bin in any later lane"
-          const int myfirst = pmask ? lane * 8 + __ffs(pmask) - 1 : 1 << 20;
-          int nxt = 1 << 20;   // first present bin among lanes > lane
-          {
-            int v = myfirst;
-            // suffix minimum (exclusive)
-            int run = v;
-            for (int o = 1; o < 32; o <<= 1) { int u = __shfl_down_sync(0xffffffffu, run, o); if (lane + o < 32) run = min(run, u); }
-            int nx = __shfl_down_sync(0xffffffffu, run, 1);
-            nxt = lane < 31 ? nx : (1 << 20);
-          }
-          const int gfirst = __reduce_min_sync(0xffffffffu, myfirst);
-          const int mylast = pmask ? lane * 8 + 31 - __clz(pmask) : -1;
-          const int glast = __reduce_max_sync(0xffffffffu, mylast);
-          const bool is_const = bv[glast] <= bv[gfirst] + FEATURE_THRESHOLD;
-          if (P.random_split) {
-            // one candidate per feature: threshold = rand_uniform(min, max) (SK/tree/_utils.pyx:57-61),
-            // samples with (double)value <= threshold go left (DensePartitioner.partition_samples)
-            FoResult* R = &results[k];
-            double thr = 0.0;
-            unsigned nl_lane = 0;
+          __syncthreads();
+          FO_TICK(4);
+          // one warp per feature: left statistics over the threads (each lane 8 threads in order,
+          // then a fixed butterfly), then the split's proxy as node_split_random evaluates it
+          for (int k = wid; k < nbatch; k += FO_THREADS / 32) {
             unsigned long long sl[CM];
-            FOR_C(c) sl[c] = 0;
-            int nin = 0;
-            if (!is_const) {
-              const double lo = (double)bv[gfirst], hi = (double)bv[glast];
-              thr = __dadd_rn(__ddiv_rn(__dmul_rn(__dsub_rn(hi, lo), (double)items[k].rnd), 2147483647.0), lo);
-              if (thr == hi) thr = lo;
+            FOR_C(c) {
+              unsigned long long v = 0;
 #pragma unroll
               for (int j = 0; j < 8; ++j) {
-                const int bb = lane * 8 + j;
-                if ((double)bv[bb] <= thr) {
-                  nin += 1;
-                  nl_lane += cntb[j];
-                  FOR_C(c) sl[c] = st_add<REG>(sl[c], hbin(c, bb));
-                }
+                const int t = lane * 8 + j;
+                if constexpr (REG) v = st_add<REG>(v, d_st(reinterpret_cast<const double*>(hist)[(k * 3 + c) * FO_THREADS + t]));
+                else v += hist[(k * C + c) * FO_THREADS + t];
               }
-            }
-            const unsigned n_left_u = __reduce_add_sync(0xffffffffu, nl_lane);
-            const int cutbin = (int)__reduce_add_sync(0xffffffffu, (unsigned)nin) - 1;
-            FOR_C(c) {
-              // lanes hold consecutive bin ranges: an ordered inclusive scan, read from the last lane
-              unsigned long long v = sl[c];
-              for (int o = 1; o < 32; o <<= 1) {
-                unsigned long long u = __shfl_up_sync(0xffffffffu, v, o);
-                if (lane >= o) v = st_add<REG>(u, v);
-              }
-              sl[c] = __shfl_sync(0xffffffffu, v, 31);
+              for (int o = 16; o > 0; o >>= 1) v = st_add<REG>(v, __shfl_xor_sync(0xffffffffu, v, o));
+              sl[c] = v;
             }
             if (lane == 0) {
-              R->is_const = is_const; R->proxy = -INFINITY; R->pos = end; R->bin = cutbin; R->thr = thr;
-              if (!is_const) {
-                const int n_left = (int)n_left_u, n_right = n_node - n_left;
+              FoResult* R = &results[k];
+              R->proxy = -INFINITY; R->pos = end; R->bin = -1;
+              if (!R->is_const) {
+                int n_left = 0;
+                for (int w = 0; w < FO_THREADS / 32; ++w) n_left += s_nl[w][k];
+                const int n_right = n_node - n_left;
                 if (n_left >= P.min_samples_leaf && n_right >= P.min_samples_leaf) {
                   double wl = 0.0;
                   if constexpr (REG) wl = st_d(sl[0]);
@@ -537,66 +524,225 @@ forest_build_kernel(const FoParams P) {
                 }
               }
             }
-            continue;
           }
-          // candidates of this lane in ascending bin order
-          double bproxy = -INFINITY, bil = 0.0, bir = 0.0;
-          int bpos = 1 << 30, bbin = -1, bnext = -1;
-          unsigned long long bsl[CM];
-          FOR_C(c) bsl[c] = 0;
-          if (!is_const) {
-            unsigned run_cnt = pre;
-            unsigned long long sl[CM];
-            FOR_C(c) sl[c] = clspre[c];
-            for (int j = 0; j < 8; ++j) {
-              if (!cntb[j]) continue;
-              const int bb = lane * 8 + j;
-              run_cnt += cntb[j];
-              FOR_C(c) sl[c] = st_add<REG>(sl[c], hbin(c, bb));
-              // next present bin
-              const unsigned higher = pmask & ~((2u << j) - 1u);
-              const int nb2 = higher ? lane * 8 + __ffs(higher) - 1 : nxt;
-              if (nb2 >= (1 << 20)) continue;                              // last present bin
-              if (!(bv[nb2] > bv[bb] + FEATURE_THRESHOLD)) continue;       // values within 1e-7: same run
-              const int n_left = (int)run_cnt, n_right = n_node - n_left;
-              if (n_left < P.min_samples_leaf || n_right < P.min_samples_leaf) continue;
-              double wl = 0.0;
-              if constexpr (REG) wl = st_d(sl[0]);
-              else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(s_cw[c], (double)sl[c])); }
-              else { FOR_C(c) wl += (double)sl[c]; }
-              const double wr = w_node - wl;
-              if (wl < MIN_WEIGHT_LEAF || wr < MIN_WEIGHT_LEAF) continue;
-              double il, ir, proxy;
-              if constexpr (REG) {     // MSE.proxy_impurity_improvement: sum_l^2 / w_l + sum_r^2 / w_r
-                fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
-                const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
-                proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
-              } else if constexpr (W) {
-                fo_children_impurity_w<CM>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
-                proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
-              } else {
-                fo_children_impurity<CM>(sl, rec.sums, C, wl, wr, &il, &ir);
-                proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
-              }
-              if (proxy > bproxy) {
-                bproxy = proxy; bil = il; bir = ir; bpos = start + n_left; bbin = bb; bnext = nb2;
-                FOR_C(c) bsl[c] = sl[c];
+        } else {
+          // --- histograms of all batch features in one pass over the node's samples ---
+          // the distinct values of the batch features are staged in the same phase (their loads overlap
+          // the gathers below); the scan reads them inside dependent per-candidate loops
+          float stage[FO_KB_MAX];   // FO_KB_MAX * 256 values / 256 threads
+#pragma unroll
+          for (int q = 0; q < FO_KB_MAX; ++q)
+            stage[q] = q < nbatch ? __ldg(P.binval + (size_t)items[q].f * FO_BINS + tid) : 0.f;
+          FO_TICK(2);
+          {
+            // all gathers of a sample are issued before the first atomic: one memory round trip per
+            // sample instead of one per feature (the dependent load -> atomic chain serialised them)
+            const uint8_t* col[FO_KB_MAX];
+#pragma unroll
+            for (int k = 0; k < FO_KB_MAX; ++k) col[k] = P.xbin + (size_t)items[k < nbatch ? k : 0].f * n;
+            for (int i = start + tid; i < end; i += FO_THREADS) {
+              const uint2 sv = samp[i];
+              const unsigned cls = sv.y & 0xFF, wgt = sv.y >> 8;
+              double yv = 0.0;
+              if constexpr (REG) yv = __ldg(P.yreal + sv.x);
+              unsigned bbs[FO_KB_MAX];
+#pragma unroll
+              for (int k = 0; k < FO_KB_MAX; ++k) bbs[k] = k < nbatch ? (unsigned)__ldg(col[k] + sv.x) : 0u;
+              const double wy = __dmul_rn((double)wgt, yv), wyy = __dmul_rn(wy, yv);
+#pragma unroll
+              for (int k = 0; k < FO_KB_MAX; ++k) {
+                if (k < nbatch) {
+                  unsigned int* H = hist + k * hstride;
+                  if constexpr (REG) {
+                    double* Hd = reinterpret_cast<double*>(H);
+                    atomicAdd(&Hd[0 * FO_BINS + bbs[k]], (double)wgt);
+                    atomicAdd(&Hd[1 * FO_BINS + bbs[k]], wy);
+                    atomicAdd(&Hd[2 * FO_BINS + bbs[k]], wyy);
+                    atomicAdd(&H[6 * FO_BINS + bbs[k]], 1u);
+                  } else {
+                    atomicAdd(&H[cls * FO_BINS + bbs[k]], wgt);
+                    atomicAdd(&H[C * FO_BINS + bbs[k]], 1u);
+                  }
+                }
               }
             }
+#pragma unroll
+            for (int q = 0; q < FO_KB_MAX; ++q)
+              if (q < nbatch) sbv[q * FO_BINS + tid] = stage[q];
           }
-          // warp arg-max; ties keep the smallest position (the sequential scan's strict '>')
-          double wp = bproxy; int wpos = bpos;
-          for (int o = 16; o > 0; o >>= 1) {
-            const double op = __shfl_xor_sync(0xffffffffu, wp, o);
-            const int opos = __shfl_xor_sync(0xffffffffu, wpos, o);
-            if (op > wp || (op == wp && opos < wpos)) { wp = op; wpos = opos; }
-          }
-          FoResult* R = &results[k];
-          if (lane == 0) { R->is_const = is_const; R->proxy = wp; R->pos = wpos; }
-          if (bpos == wpos && bproxy == wp && wp > -INFINITY) {   // unique lane: positions are unique per bin
-            R->bin = bbin; R->il = bil; R->ir = bir;
-            R->thr = (double)bv[bbin] / 2.0 + (double)bv[bnext] / 2.0;
-            FOR_C(c) R->sl[c] = bsl[c];
+          __syncthreads();
+          FO_TICK(3);
+          // --- one warp per feature: scan the 256 bins (8 per lane) in ascending order ---
+          for (int k = wid; k < nbatch; k += FO_THREADS / 32) {
+            const unsigned int* H = hist + k * hstride;
+            const float* bv = sbv + k * FO_BINS;
+            const int cnt_off = REG ? 6 * FO_BINS : C * FO_BINS;
+            // statistic c of bin bb as a 64-bit pattern (class weight, or float64 sum for regression)
+            auto hbin = [&](int c, int bb) -> unsigned long long {
+              if constexpr (REG) return d_st(reinterpret_cast<const double*>(H)[c * FO_BINS + bb]);
+              else return (unsigned long long)H[c * FO_BINS + bb];
+            };
+            unsigned cntb[8];
+            unsigned ltot = 0, pmask = 0;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { cntb[j] = H[cnt_off + lane * 8 + j]; ltot += cntb[j]; if (cntb[j]) pmask |= 1u << j; }
+            // exclusive prefix of sample counts over lanes
+            unsigned pre = ltot;
+            for (int o = 1; o < 32; o <<= 1) { unsigned v = __shfl_up_sync(0xffffffffu, pre, o); if (lane >= o) pre += v; }
+            pre -= ltot;
+            // class-weight prefixes
+            unsigned long long clspre[CM];
+            FOR_C(c) {
+              unsigned long long t = 0;
+#pragma unroll
+              for (int j = 0; j < 8; ++j) t = st_add<REG>(t, hbin(c, lane * 8 + j));
+              unsigned long long incl = t;
+              for (int o = 1; o < 32; o <<= 1) {
+                unsigned long long v = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl = st_add<REG>(v, incl);
+              }
+              const unsigned long long up = __shfl_up_sync(0xffffffffu, incl, 1);   // exclusive prefix
+              clspre[c] = lane > 0 ? up : 0ull;
+            }
+            // first present bin of this lane, then "first present bin in any later lane"
+            const int myfirst = pmask ? lane * 8 + __ffs(pmask) - 1 : 1 << 20;
+            int nxt = 1 << 20;   // first present bin among lanes > lane
+            {
+              int v = myfirst;
+              // suffix minimum (exclusive)
+              int run = v;
+              for (int o = 1; o < 32; o <<= 1) { int u = __shfl_down_sync(0xffffffffu, run, o); if (lane + o < 32) run = min(run, u); }
+              int nx = __shfl_down_sync(0xffffffffu, run, 1);
+              nxt = lane < 31 ? nx : (1 << 20);
+            }
+            const int gfirst = __reduce_min_sync(0xffffffffu, myfirst);
+            const int mylast = pmask ? lane * 8 + 31 - __clz(pmask) : -1;
+            const int glast = __reduce_max_sync(0xffffffffu, mylast);
+            const bool is_const = bv[glast] <= bv[gfirst] + FEATURE_THRESHOLD;
+            if (P.random_split) {   // features on bin codes only
+              // one candidate per feature: threshold = rand_uniform(min, max) (SK/tree/_utils.pyx:57-61),
+              // samples with (double)value <= threshold go left (DensePartitioner.partition_samples)
+              FoResult* R = &results[k];
+              double thr = 0.0;
+              unsigned nl_lane = 0;
+              unsigned long long sl[CM];
+              FOR_C(c) sl[c] = 0;
+              int nin = 0;
+              if (!is_const) {
+                const double lo = (double)bv[gfirst], hi = (double)bv[glast];
+                thr = __dadd_rn(__ddiv_rn(__dmul_rn(__dsub_rn(hi, lo), (double)items[k].rnd), 2147483647.0), lo);
+                if (thr == hi) thr = lo;
+  #pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                  const int bb = lane * 8 + j;
+                  if ((double)bv[bb] <= thr) {
+                    nin += 1;
+                    nl_lane += cntb[j];
+                    FOR_C(c) sl[c] = st_add<REG>(sl[c], hbin(c, bb));
+                  }
+                }
+              }
+              const unsigned n_left_u = __reduce_add_sync(0xffffffffu, nl_lane);
+              const int cutbin = (int)__reduce_add_sync(0xffffffffu, (unsigned)nin) - 1;
+              FOR_C(c) {
+                // lanes hold consecutive bin ranges: an ordered inclusive scan, read from the last lane
+                unsigned long long v = sl[c];
+                for (int o = 1; o < 32; o <<= 1) {
+                  unsigned long long u = __shfl_up_sync(0xffffffffu, v, o);
+                  if (lane >= o) v = st_add<REG>(u, v);
+                }
+                sl[c] = __shfl_sync(0xffffffffu, v, 31);
+              }
+              if (lane == 0) {
+                R->is_const = is_const; R->proxy = -INFINITY; R->pos = end; R->bin = cutbin; R->thr = thr;
+                if (!is_const) {
+                  const int n_left = (int)n_left_u, n_right = n_node - n_left;
+                  if (n_left >= P.min_samples_leaf && n_right >= P.min_samples_leaf) {
+                    double wl = 0.0;
+                    if constexpr (REG) wl = st_d(sl[0]);
+                    else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(s_cw[c], (double)sl[c])); }
+                    else { FOR_C(c) wl += (double)sl[c]; }
+                    const double wr = w_node - wl;
+                    if (!(wl < MIN_WEIGHT_LEAF || wr < MIN_WEIGHT_LEAF)) {
+                      double il, ir;
+                      if constexpr (REG) {
+                        fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
+                        const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
+                        R->proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
+                      } else if constexpr (W) {
+                        fo_children_impurity_w<CM>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
+                        R->proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
+                      } else {
+                        fo_children_impurity<CM>(sl, rec.sums, C, wl, wr, &il, &ir);
+                        R->proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
+                      }
+                      R->pos = start + n_left; R->il = il; R->ir = ir;
+                      FOR_C(c) R->sl[c] = sl[c];
+                    }
+                  }
+                }
+              }
+              continue;
+            }
+            // candidates of this lane in ascending bin order
+            double bproxy = -INFINITY, bil = 0.0, bir = 0.0;
+            int bpos = 1 << 30, bbin = -1, bnext = -1;
+            unsigned long long bsl[CM];
+            FOR_C(c) bsl[c] = 0;
+            if (!is_const) {
+              unsigned run_cnt = pre;
+              unsigned long long sl[CM];
+              FOR_C(c) sl[c] = clspre[c];
+              for (int j = 0; j < 8; ++j) {
+                if (!cntb[j]) continue;
+                const int bb = lane * 8 + j;
+                run_cnt += cntb[j];
+                FOR_C(c) sl[c] = st_add<REG>(sl[c], hbin(c, bb));
+                // next present bin
+                const unsigned higher = pmask & ~((2u << j) - 1u);
+                const int nb2 = higher ? lane * 8 + __ffs(higher) - 1 : nxt;
+                if (nb2 >= (1 << 20)) continue;                              // last present bin
+                if (!(bv[nb2] > bv[bb] + FEATURE_THRESHOLD)) continue;       // values within 1e-7: same run
+                const int n_left = (int)run_cnt, n_right = n_node - n_left;
+                if (n_left < P.min_samples_leaf || n_right < P.min_samples_leaf) continue;
+                double wl = 0.0;
+                if constexpr (REG) wl = st_d(sl[0]);
+                else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(s_cw[c], (double)sl[c])); }
+                else { FOR_C(c) wl += (double)sl[c]; }
+                const double wr = w_node - wl;
+                if (wl < MIN_WEIGHT_LEAF || wr < MIN_WEIGHT_LEAF) continue;
+                double il, ir, proxy;
+                if constexpr (REG) {     // MSE.proxy_impurity_improvement: sum_l^2 / w_l + sum_r^2 / w_r
+                  fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
+                  const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
+                  proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
+                } else if constexpr (W) {
+                  fo_children_impurity_w<CM>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
+                  proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
+                } else {
+                  fo_children_impurity<CM>(sl, rec.sums, C, wl, wr, &il, &ir);
+                  proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
+                }
+                if (proxy > bproxy) {
+                  bproxy = proxy; bil = il; bir = ir; bpos = start + n_left; bbin = bb; bnext = nb2;
+                  FOR_C(c) bsl[c] = sl[c];
+                }
+              }
+            }
+            // warp arg-max; ties keep the smallest position (the sequential scan's strict '>')
+            double wp = bproxy; int wpos = bpos;
+            for (int o = 16; o > 0; o >>= 1) {
+              const double op = __shfl_xor_sync(0xffffffffu, wp, o);
+              const int opos = __shfl_xor_sync(0xffffffffu, wpos, o);
+              if (op > wp || (op == wp && opos < wpos)) { wp = op; wpos = opos; }
+            }
+            FoResult* R = &results[k];
+            if (lane == 0) { R->is_const = is_const; R->proxy = wp; R->pos = wpos; }
+            if (bpos == wpos && bproxy == wp && wp > -INFINITY) {   // unique lane: positions are unique per bin
+              R->bin = bbin; R->il = bil; R->ir = bir;
+              R->thr = (double)bv[bbin] / 2.0 + (double)bv[bnext] / 2.0;
+              FOR_C(c) R->sl[c] = bsl[c];
+            }
           }
         }
         __syncthreads();
@@ -666,7 +812,10 @@ forest_build_kernel(const FoParams P) {
 
       if (best_pos < end) {
         // --- partition_samples_final: stable partition (keeps sample indices ascending) ---
-        const uint8_t* xb = P.xbin + (size_t)best_feature * n;
+        // (random splitter over raw values: the value against the drawn threshold, as partition_samples)
+        constexpr bool raw = RAW;
+        const uint8_t* xb = raw ? nullptr : P.xbin + (size_t)best_feature * n;
+        const float* xv = raw ? P.xval + (size_t)best_feature * n : nullptr;
         __shared__ int loff, roff;
         if (tid == 0) { loff = start; roff = best_pos; }
         __syncthreads();
@@ -674,7 +823,11 @@ forest_build_kernel(const FoParams P) {
           const int i = i0 + tid;
           uint2 sv = make_uint2(0, 0);
           int isl = 0, isr = 0;
-          if (i < end) { sv = samp[i]; isl = xb[sv.x] <= (unsigned)best_bin; isr = !isl; }
+          if (i < end) {
+            sv = samp[i];
+            isl = raw ? (double)__ldg(xv + sv.x) <= best_thr : xb[sv.x] <= (unsigned)best_bin;
+            isr = !isl;
+          }
           const unsigned bl = __ballot_sync(0xffffffffu, isl), br = __ballot_sync(0xffffffffu, isr);
           if (lane == 0) { wsum[wid][0] = __popc(bl); wsum[wid][1] = __popc(br); }
           __syncthreads();
@@ -811,30 +964,44 @@ void forest_free(Ctx* c) {
   if (f.xbin) cudaFree(f.xbin);
   if (f.binval) cudaFree(f.binval);
   if (f.xrow) cudaFree(f.xrow);
+  if (f.xval) cudaFree(f.xval);
   f = ForestData();
 }
 
-// Bin codes of the staged X (feature-major uint8) + the distinct values per feature.
-int forest_prepare(Ctx* c) {
+// Bin codes of the staged X (feature-major uint8) + the distinct values per feature, for the best
+// splitter.  A feature with more than 256 distinct values gets no codes: only the random splitter,
+// which reads raw values, can split it.  values: also keep the raw values feature-major (xval, 4 n d
+// bytes) for the random splitter; a later random-splitter fit on the same X adds them to the codes.
+int forest_prepare(Ctx* c, bool values) {
   ForestData& fd = c->forest;
-  if (fd.valid) return 0;
-  forest_free(c);
+  if (fd.valid && (fd.xval || !values)) return 0;
   const int64_t n = c->n;
   const int d = (int)c->d, ldx = (int)c->ldx;
+  const unsigned g = (unsigned)((n + 255) / 256);
+  if (fd.valid) {
+    SKD_CUDA(c, cudaMalloc((void**)&fd.xval, (size_t)d * n * sizeof(float)));
+    for (int f = 0; f < d; ++f) fo_extract_col<<<g, 256, 0, c->stream>>>(c->X, n, ldx, f, fd.xval + (size_t)f * n);
+    c->launches += d;
+    SKD_CUDA(c, cudaGetLastError());
+    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+    return 0;
+  }
+  forest_free(c);
   SKD_CUDA(c, cudaMalloc((void**)&fd.xbin, (size_t)d * n));
   SKD_CUDA(c, cudaMalloc((void**)&fd.binval, (size_t)d * FO_BINS * sizeof(float)));
+  if (values) SKD_CUDA(c, cudaMalloc((void**)&fd.xval, (size_t)d * n * sizeof(float)));
   float *col, *srt, *dvals; int* dn;
   Scratch sx(c);
   SKD_CUDA(c, sx.alloc(&col, (size_t)n));
   SKD_CUDA(c, sx.alloc(&srt, (size_t)n));
   SKD_CUDA(c, sx.alloc(&dvals, (size_t)FO_BINS));
   SKD_CUDA(c, sx.alloc(&dn, 1));
-  const unsigned g = (unsigned)((n + 255) / 256);
   std::vector<float> hv(FO_BINS);
-  bool well_separated = true;
+  bool well_separated = true, all_coded = true;
   for (int f = 0; f < d; ++f) {
-    fo_extract_col<<<g, 256, 0, c->stream>>>(c->X, n, ldx, f, col);
-    SKD_CUDA(c, cudaMemcpyAsync(srt, col, (size_t)n * 4, cudaMemcpyDeviceToDevice, c->stream));
+    float* cf = values ? fd.xval + (size_t)f * n : col;   // the column is the raw-value copy when one is kept
+    fo_extract_col<<<g, 256, 0, c->stream>>>(c->X, n, ldx, f, cf);
+    SKD_CUDA(c, cudaMemcpyAsync(srt, cf, (size_t)n * 4, cudaMemcpyDeviceToDevice, c->stream));
     thrust::sort(thrust::cuda::par.on(c->stream), thrust::device_pointer_cast(srt), thrust::device_pointer_cast(srt + n));
     SKD_CUDA(c, cudaMemsetAsync(dn, 0, 4, c->stream));
     fo_mark_unique<<<g, 256, 0, c->stream>>>(srt, n, dn, dvals);
@@ -842,11 +1009,15 @@ int forest_prepare(Ctx* c) {
     SKD_CUDA(c, cudaMemcpyAsync(&nu, dn, 4, cudaMemcpyDeviceToHost, c->stream));
     SKD_CUDA(c, cudaMemcpyAsync(hv.data(), dvals, FO_BINS * 4, cudaMemcpyDeviceToHost, c->stream));
     SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-    if (nu > FO_BINS) {
-      char b[200];
-      snprintf(b, sizeof(b), "forest: feature %d has %d distinct values; the histogram splitter needs <= %d "
-               "(continuous features need the sort-based splitter, not built yet)", f, nu, FO_BINS);
-      return fail(c, b);
+    c->launches += 2;
+    if (nu > FO_BINS) {   // no codes; the distinct values stay +inf
+      if (all_coded) { fd.uncoded_feature = f; fd.uncoded_distinct = nu; }
+      all_coded = false;
+      std::fill(hv.begin(), hv.end(), INFINITY);
+      fd.h_binval.insert(fd.h_binval.end(), hv.begin(), hv.end());
+      SKD_CUDA(c, cudaMemcpyAsync(fd.binval + (size_t)f * FO_BINS, hv.data(), FO_BINS * 4, cudaMemcpyHostToDevice, c->stream));
+      SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+      continue;
     }
     for (int i = 0; i < nu; ++i)
       if (hv[i] != hv[i]) return fail(c, "forest: NaN feature values are not supported on the device path");
@@ -857,18 +1028,19 @@ int forest_prepare(Ctx* c) {
     fd.h_binval.insert(fd.h_binval.end(), hv.begin(), hv.end());
     SKD_CUDA(c, cudaMemcpyAsync(dvals, hv.data(), FO_BINS * 4, cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaMemcpyAsync(fd.binval + (size_t)f * FO_BINS, hv.data(), FO_BINS * 4, cudaMemcpyHostToDevice, c->stream));
-    fo_bin_col<<<g, 256, 0, c->stream>>>(col, n, dvals, nu, fd.xbin + (size_t)f * n);
+    fo_bin_col<<<g, 256, 0, c->stream>>>(cf, n, dvals, nu, fd.xbin + (size_t)f * n);
     SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-    c->launches += 3;
+    c->launches += 1;
   }
   fd.dp = (d + 15) / 16 * 16;
-  SKD_CUDA(c, cudaMalloc((void**)&fd.xrow, (size_t)n * fd.dp));
-  {
+  if (all_coded) {   // the throughput builder's row-major codes
+    SKD_CUDA(c, cudaMalloc((void**)&fd.xrow, (size_t)n * fd.dp));
     const int64_t total = n * (fd.dp / 4);
     fo_rowmajor_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c->stream>>>(fd.xbin, n, d, fd.dp, fd.xrow);
     c->launches += 1;
   }
-  fd.well_separated = well_separated;
+  fd.all_coded = all_coded;
+  fd.well_separated = well_separated && all_coded;
   SKD_CUDA(c, cudaGetLastError());
   SKD_CUDA(c, cudaStreamSynchronize(c->stream));
   fd.valid = true;
@@ -885,7 +1057,18 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
                int max_features, int max_depth, int min_samples_split, int min_samples_leaf,
                double min_weight_leaf, double min_impurity_decrease, int random_split, const double* h_yreal,
                const ForestClassWeights* cw, ForestSink sink, void* sink_arg) {
-  if (forest_prepare(c)) return 1;
+  if (forest_prepare(c, false)) return 1;
+  // the random splitter reads raw values when a feature has no bin codes; on codes alone its histogram
+  // form is faster (config-4 lattice, H100: profiles/README.md)
+  const bool raw_values = random_split && !c->forest.all_coded;
+  if (raw_values && forest_prepare(c, true)) return 1;
+  if (!random_split && !c->forest.all_coded) {
+    char b[220];
+    snprintf(b, sizeof(b), "forest: feature %d has %d distinct values; the histogram splitter needs <= %d "
+             "(continuous features need the sort-based splitter, not built yet)", c->forest.uncoded_feature,
+             c->forest.uncoded_distinct, FO_BINS);
+    return fail(c, b);
+  }
   const bool reg = h_yreal != nullptr;       // regression trees (MSE) on float64 targets
   if (reg) n_classes = 1;
   if (n_classes < 1 || n_classes > FO_MAXC) return fail(c, "forest: device path supports up to 16 classes");
@@ -935,11 +1118,13 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
                               (size_t)FO_KB_MAX * FO_BINS * sizeof(float) + (size_t)FO_SSTK * sizeof(FoRecord);
   // the general builder for this fit (CM: class-count bound; W: class weights)
   void (*general)(const FoParams) = nullptr;
-  if (reg) general = forest_build_kernel<4, true, false>;
-  else if (n_classes <= 2) general = weighted ? forest_build_kernel<2, false, true> : forest_build_kernel<2, false, false>;
-  else if (n_classes <= 4) general = weighted ? forest_build_kernel<4, false, true> : forest_build_kernel<4, false, false>;
-  else if (n_classes <= 8) general = weighted ? forest_build_kernel<8, false, true> : forest_build_kernel<8, false, false>;
-  else general = weighted ? forest_build_kernel<FO_MAXC, false, true> : forest_build_kernel<FO_MAXC, false, false>;
+#define FO_PICK(CM, REG, W) (raw_values ? forest_build_kernel<CM, REG, W, true> : forest_build_kernel<CM, REG, W, false>)
+  if (reg) general = FO_PICK(4, true, false);
+  else if (n_classes <= 2) general = weighted ? FO_PICK(2, false, true) : FO_PICK(2, false, false);
+  else if (n_classes <= 4) general = weighted ? FO_PICK(4, false, true) : FO_PICK(4, false, false);
+  else if (n_classes <= 8) general = weighted ? FO_PICK(8, false, true) : FO_PICK(8, false, false);
+  else general = weighted ? FO_PICK(FO_MAXC, false, true) : FO_PICK(FO_MAXC, false, false);
+#undef FO_PICK
   if (!fast) SKD_CUDA(c, cudaFuncSetAttribute(general, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_general));
   std::vector<int> pending(n_trees);
   for (int t = 0; t < n_trees; ++t) pending[t] = t;
@@ -992,7 +1177,7 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
     long long* d_prof = nullptr;
     if (want_prof) SKD_CUDA(c, sx.alloc(&d_prof, (size_t)slots * 16));
     P.stack = (FoRecord*)dstack;
-    P.xbin = c->forest.xbin; P.binval = c->forest.binval; P.ycls = c->ycls; P.yreal = dy;
+    P.xbin = c->forest.xbin; P.binval = c->forest.binval; P.xval = raw_values ? c->forest.xval : nullptr; P.ycls = c->ycls; P.yreal = dy;
     P.n = n; P.d = d; P.n_classes = n_classes;
     P.max_features = max_features; P.max_depth = max_depth; P.min_samples_split = min_samples_split;
     P.min_samples_leaf = min_samples_leaf; P.min_weight_leaf = min_weight_leaf;

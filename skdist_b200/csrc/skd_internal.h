@@ -41,11 +41,14 @@ struct TcData {
 
 // binned copy of the staged X for the forest builder (forest.cu)
 struct ForestData {
-  uint8_t* xbin = nullptr;   // [d][n] bin code of every value, feature-major
+  uint8_t* xbin = nullptr;   // [d][n] bin code of every value, feature-major (features with codes only)
   float* binval = nullptr;   // [d][256] distinct values of each feature, ascending (+inf padded)
-  uint8_t* xrow = nullptr;   // [n][dp] the same codes row-major, dp = d rounded up to 16 (forest_fast.cu)
+  uint8_t* xrow = nullptr;   // [n][dp] the same codes row-major, dp = d rounded up to 16 (forest_fast.cu); only when all_coded
+  float* xval = nullptr;     // [d][n] raw values, feature-major: staged by the first random-splitter fit
   int dp = 0;
   bool well_separated = false;   // every feature's adjacent distinct values are more than 1e-7 apart
+  bool all_coded = false;        // every feature has <= 256 distinct values (bin codes): the best splitter can run
+  int uncoded_feature = -1, uncoded_distinct = 0;   // the first feature without codes and its distinct values
   std::vector<float> h_binval;   // host copy of binval (thresholds of compact node records are formed on the host)
   bool valid = false;
 };

@@ -167,12 +167,14 @@ def _finish_tree(t, template_params, state, n_features, n_classes, max_features_
 _LIMITS = """
 
     Limits of the device path (checked when the trees are built; `NotImplementedError` otherwise, there
-    is no CPU fallback): every feature may take at most 256 distinct values (the exact splitter works on
-    per-feature value histograms: data on a lattice, counts, categorical codes, quantised measurements --
-    continuous float features need a sort-based splitter that is not built; the opt-in histogram mode
-    `SKDIST_B200_FOREST_MAX_BINS=<2..256>` replaces such features by equal-count bin codes and maps the
-    thresholds back to raw units -- the trees scikit-learn builds on the coded matrix, not bit-identical to the
-    reference on the raw one), at most 16 classes, at most
+    is no CPU fallback): with the best splitter (RandomForest) every feature may take at most 256 distinct
+    values (it works on per-feature value histograms: data on a lattice, counts, categorical codes, quantised
+    measurements -- continuous float features need a sort-based splitter that is not built; the opt-in
+    histogram mode `SKDIST_B200_FOREST_MAX_BINS=<2..256>` replaces such features by equal-count bin codes and
+    maps the thresholds back to raw units -- the trees scikit-learn builds on the coded matrix, not
+    bit-identical to the reference on the raw one); the random splitter (ExtraTrees, RandomTreesEmbedding)
+    reads the raw float32 values and takes any finite X (with the switch set it, too, is fitted on the coded
+    matrix), at most 16 classes, at most
     384 features, bootstrap multiplicities up to 255, no missing values, `criterion` gini / squared
     error, no `max_leaf_nodes`, `sample_weight` or multi-output targets; `class_weight` (classifiers) may
     be a dict, "balanced" or "balanced_subsample", not "subsample" or a list of dicts."""
@@ -459,7 +461,8 @@ class DistRandomForestClassifier(_DistForestClassifier, RandomForestClassifier):
 
 class DistExtraTreesClassifier(_DistForestClassifier, ExtraTreesClassifier):
     __doc__ = """Same as sklearn `ExtraTreesClassifier` with every tree built on an H100 (random splitter:
-    one uniformly drawn threshold per drawn feature, no bootstrap by default).
+    one uniformly drawn threshold per drawn feature over the raw float32 values, no bootstrap by default;
+    continuous features are fitted exactly, scikit-learn's trees bit for bit).
     Constructor mirrors ref ensemble.py:437-478 (``sc`` is the FIRST positional argument).""" + _LIMITS + _CLASS_WEIGHT
 
     _splitter = 1
@@ -518,7 +521,8 @@ class DistRandomForestRegressor(_DistForestRegressor, RandomForestRegressor):
 
 
 class DistExtraTreesRegressor(_DistForestRegressor, ExtraTreesRegressor):
-    __doc__ = """Same as sklearn `ExtraTreesRegressor` with every tree built on an H100.
+    __doc__ = """Same as sklearn `ExtraTreesRegressor` with every tree built on an H100 (random splitter over
+    the raw float32 values: continuous features need no binning).
     Constructor mirrors ref ensemble.py:584-616.""" + _LIMITS
 
     _splitter = 1
