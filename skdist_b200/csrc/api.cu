@@ -5,6 +5,8 @@
 
 #include <algorithm>
 #include <cmath>
+#include <functional>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <atomic>
@@ -36,6 +38,32 @@ struct skd_lbfgs {
 
 static inline int64_t round_up(int64_t a, int64_t b) { return (a + b - 1) / b * b; }
 
+namespace skd {
+int pack_coef(Ctx* c, Scratch& sx, int rows, const float* coef, int64_t d, int64_t ldx, float** dW) {
+  std::vector<float> h((size_t)rows * ldx + rows, 0.f);
+  for (int j = 0; j < rows; ++j) {
+    memcpy(&h[(size_t)j * ldx], coef + (size_t)j * (d + 1), d * sizeof(float));
+    h[(size_t)rows * ldx + j] = coef[(size_t)j * (d + 1) + d];
+  }
+  SKD_CUDA(c, sx.alloc(dW, h.size()));
+  SKD_CUDA(c, cudaMemcpyAsync(*dW, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->h2d += (int64_t)h.size() * 4;
+  return 0;
+}
+}  // namespace skd
+
+// Copy of n host values into a per-row device vector of the context (buffer reused when it holds n)
+template <class T>
+static int stage_device_vector(Ctx* c, T*& dst, int64_t& cap, const T* src, int64_t n) {
+  if (dst && cap < n) { cudaFree(dst); dst = nullptr; }
+  if (!dst) { SKD_CUDA(c, cudaMalloc((void**)&dst, (size_t)n * sizeof(T))); cap = n; }
+  SKD_CUDA(c, cudaMemcpyAsync(dst, src, (size_t)n * sizeof(T), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->h2d += n * (int64_t)sizeof(T);
+  return 0;
+}
+
 // Which evaluation kernel serves this batch: the tensor-core kernel (logreg_tc.cu) or SIMT fp32.
 static int eval_dispatch(Ctx* c, LogregWork& w, int n_act, int* nz_used) {
   if (w.use_tc) return tc_eval(c, w, n_act, nz_used);
@@ -49,12 +77,50 @@ static bool want_tc(const Ctx* c) {
   return tc_supported(c) && !getenv("SKDIST_B200_FORCE_SIMT");
 }
 
+// want_tc, failing when tensor cores are forced (skd_set_kernel 2) on a shape they do not support
+static int use_tensor_cores(Ctx* c, bool* use_tc) {
+  if (c->kernel_choice == 2 && !tc_supported(c))
+    return fail(c, "tensor-core path requested but the staged shape is unsupported (needs d <= 256)");
+  *use_tc = want_tc(c);
+  return 0;
+}
+
+// Tensor-core weights of `slots` slots: fp16 hi / lo coefficients (zeroed padding) and slot parameters.
+static int alloc_tc_weights(Ctx* c, Scratch& sx, LogregWork& w, int slots) {
+  w.ldw = c->tc.dpad;
+  w.slots_pad_cap = (int)round_up(slots, 128);
+  const size_t wbytes = (size_t)w.slots_pad_cap * c->tc.dpad * 2;
+  SKD_CUDA(c, sx.alloc((uint8_t**)&w.Wh, wbytes));
+  SKD_CUDA(c, sx.alloc((uint8_t**)&w.Wl, wbytes));
+  SKD_CUDA(c, sx.alloc((uint8_t**)&w.sp, (size_t)w.slots_pad_cap * tc_slot_param_bytes()));
+  SKD_CUDA(c, cudaMemsetAsync(w.Wh, 0, wbytes, c->stream));
+  SKD_CUDA(c, cudaMemsetAsync(w.Wl, 0, wbytes, c->stream));
+  return 0;
+}
+
+// Tensor-core setup of a scoring pass: slot s = column s of coef [B x (d+1)], exported into the weights.
+static int tc_scoring_setup(Ctx* c, Scratch& sx, LogregWork& w, int B, const float* coef, SlotMeta* dslot) {
+  if (tc_prepare(c)) return 1;
+  w.B = B; w.dp = (int)c->d + 1; w.use_tc = true;
+  w.slot = dslot;
+  if (alloc_tc_weights(c, sx, w, B)) return 1;
+  SKD_CUDA(c, sx.alloc(&w.n_act, 1));
+  std::vector<double> hx((size_t)B * w.dp);
+  for (size_t i = 0; i < hx.size(); ++i) hx[i] = (double)coef[i];
+  double* dx;
+  SKD_CUDA(c, sx.alloc(&dx, hx.size()));
+  int32_t nb = B;
+  SKD_CUDA(c, cudaMemcpyAsync(dx, hx.data(), hx.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &nb, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->h2d += (int64_t)hx.size() * 8;
+  return tc_export(c, w, B, dx, 1);
+}
+
 // Decide the evaluation path for a batch and allocate its evaluation buffers.
 static int alloc_eval_buffers(Ctx* c, Scratch& sx, LogregWork& w, int B, int slot_cap = 0) {
   const int64_t n = c->n, ldx = c->ldx;
-  if (c->kernel_choice == 2 && !tc_supported(c))
-    return fail(c, "tensor-core path requested but the staged shape is unsupported (needs d <= 256)");
-  w.use_tc = want_tc(c);
+  if (use_tensor_cores(c, &w.use_tc)) return 1;
   if (slot_cap < B) slot_cap = B;
   w.slot_cap = slot_cap;
   // partial sums per slot: row chunks of the SIMT grid, or the fixed chunk count of the tensor-core kernel
@@ -65,15 +131,8 @@ static int alloc_eval_buffers(Ctx* c, Scratch& sx, LogregWork& w, int B, int slo
   SKD_CUDA(c, sx.alloc(&w.gsump, (size_t)w.cap_sc));
   if (w.use_tc) {
     if (tc_prepare(c)) return 1;
-    w.ldw = c->tc.dpad;
     w.gscale = c->tc.gscale;
-    w.slots_pad_cap = (int)round_up(slot_cap, 128);
-    size_t wbytes = (size_t)w.slots_pad_cap * c->tc.dpad * 2;
-    SKD_CUDA(c, sx.alloc((uint8_t**)&w.Wh, wbytes));
-    SKD_CUDA(c, sx.alloc((uint8_t**)&w.Wl, wbytes));
-    SKD_CUDA(c, sx.alloc((uint8_t**)&w.sp, (size_t)w.slots_pad_cap * tc_slot_param_bytes()));
-    SKD_CUDA(c, cudaMemsetAsync(w.Wh, 0, wbytes, c->stream));
-    SKD_CUDA(c, cudaMemsetAsync(w.Wl, 0, wbytes, c->stream));
+    if (alloc_tc_weights(c, sx, w, slot_cap)) return 1;
     SKD_CUDA(c, sx.alloc(&w.gradp, (size_t)w.cap_sc * w.ldw));
     SKD_CUDA(c, sx.alloc(&w.gradr, (size_t)w.slots_pad_cap * w.ldw));
   } else {
@@ -339,7 +398,7 @@ static void drop_stale_row_vectors(Ctx* c, int64_t n_new) {
   c->fold_count.clear();
   c->h_fold.clear();
   c->h_ycls.clear();
-  c->rb_cols = 0;
+  c->row_bits = {};
   c->tc.meta_valid = false;
   c->vec_n = n_new;
 }
@@ -458,12 +517,8 @@ int skd_stage_labels(skd_ctx* ctx, const int32_t* y, int64_t n) {
   Ctx* c = &ctx->c;
   if (!y || n != c->n) return fail(c, "skd_stage_labels: n does not match the staged X");
   SKD_CUDA(c, cudaSetDevice(c->device));
-  if (c->ycls && c->ycls_cap < n) { cudaFree(c->ycls); c->ycls = nullptr; }
-  if (!c->ycls) { SKD_CUDA(c, cudaMalloc((void**)&c->ycls, (size_t)n * sizeof(int32_t))); c->ycls_cap = n; }
-  SKD_CUDA(c, cudaMemcpyAsync(c->ycls, y, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  if (stage_device_vector(c, c->ycls, c->ycls_cap, y, n)) return 1;
   c->h_ycls.assign(y, y + n);
-  c->h2d += n * (int64_t)sizeof(int32_t);
   c->tc.meta_valid = false;
   return 0;
 }
@@ -473,11 +528,7 @@ int skd_stage_targets(skd_ctx* ctx, const float* y, int64_t n) {
   Ctx* c = &ctx->c;
   if (!y || n != c->n) return fail(c, "skd_stage_targets: n does not match the staged X");
   SKD_CUDA(c, cudaSetDevice(c->device));
-  if (c->yreal && c->yreal_cap < n) { cudaFree(c->yreal); c->yreal = nullptr; }
-  if (!c->yreal) { SKD_CUDA(c, cudaMalloc((void**)&c->yreal, (size_t)n * sizeof(float))); c->yreal_cap = n; }
-  SKD_CUDA(c, cudaMemcpyAsync(c->yreal, y, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->h2d += n * (int64_t)sizeof(float);
+  if (stage_device_vector(c, c->yreal, c->yreal_cap, y, n)) return 1;
   c->tc.meta_valid = false;
   return 0;
 }
@@ -500,25 +551,20 @@ int skd_stage_folds(skd_ctx* ctx, const int8_t* fold_id, int64_t n, int32_t n_fo
     if (f < 0 || f >= n_folds) return fail(c, "skd_stage_folds: fold id out of range");
     c->fold_count[f] += 1;
   }
-  if (c->fold_store && c->fold_cap < n) { cudaFree(c->fold_store); c->fold_store = nullptr; }
-  if (!c->fold_store) { SKD_CUDA(c, cudaMalloc((void**)&c->fold_store, (size_t)n)); c->fold_cap = n; }
+  if (stage_device_vector(c, c->fold_store, c->fold_cap, fold_id, n)) return 1;
   c->fold = c->fold_store;
-  SKD_CUDA(c, cudaMemcpyAsync(c->fold, fold_id, (size_t)n, cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
   c->n_folds = n_folds;
-  c->h2d += n;
   return 0;
 }
 
 int skd_stage_column_masks(skd_ctx* ctx, int32_t B, const uint8_t* mask) {
   if (!ctx) return fail(nullptr, "skd_stage_column_masks: ctx is NULL");
   Ctx* c = &ctx->c;
-  c->fmask_cols = 0;
-  c->h_fmask.clear();
+  c->fmask = {};
   if (!mask || B <= 0) return 0;   // cleared
   if (!c->X) return fail(c, "skd_stage_column_masks: stage X first");
-  c->h_fmask.assign(mask, mask + (size_t)B * c->d);
-  c->fmask_cols = B;
+  c->fmask.mask.assign(mask, mask + (size_t)B * c->d);
+  c->fmask.cols = B;
   return 0;
 }
 
@@ -526,8 +572,7 @@ int skd_stage_row_bits(skd_ctx* ctx, int32_t B, const uint8_t* label_bits, const
                        int64_t bytes_per_col) {
   if (!ctx) return fail(nullptr, "skd_stage_row_bits: ctx is NULL");
   Ctx* c = &ctx->c;
-  c->rb_cols = 0; c->rb_words = 0;
-  c->h_ybits.clear(); c->h_mbits.clear();
+  c->row_bits = {};
   if (B <= 0 || (!label_bits && !train_bits)) return 0;   // cleared
   if (!c->X) return fail(c, "skd_stage_row_bits: stage X first");
   if (bytes_per_col * 8 < c->n) return fail(c, "skd_stage_row_bits: fewer bits per column than staged rows");
@@ -543,18 +588,17 @@ int skd_stage_row_bits(skd_ctx* ctx, int32_t B, const uint8_t* label_bits, const
       }
     }
   };
-  if (label_bits) pack(label_bits, c->h_ybits);
-  if (train_bits) pack(train_bits, c->h_mbits);
-  c->rb_cols = B;
-  c->rb_words = words;
+  if (label_bits) pack(label_bits, c->row_bits.y);
+  if (train_bits) pack(train_bits, c->row_bits.m);
+  c->row_bits.cols = B;
+  c->row_bits.words = words;
   return 0;
 }
 
 int skd_stage_class_weights(skd_ctx* ctx, int32_t B, int32_t K, const float* w, const double* sw_sum) {
   if (!ctx) return fail(nullptr, "skd_stage_class_weights: ctx is NULL");
   Ctx* c = &ctx->c;
-  c->cw_cols = 0; c->cw_k = 0;
-  c->h_cw.clear(); c->h_swsum.clear();
+  c->cw = {};
   if (B <= 0 || !w) return 0;   // cleared
   if (K < 2 || !sw_sum) return fail(c, "skd_stage_class_weights: bad arguments");
   for (int64_t i = 0; i < (int64_t)B * K; ++i)
@@ -562,10 +606,10 @@ int skd_stage_class_weights(skd_ctx* ctx, int32_t B, int32_t K, const float* w, 
   for (int j = 0; j < B; ++j)
     if (!(std::isfinite(sw_sum[j]) && sw_sum[j] > 0.0))
       return fail(c, "skd_stage_class_weights: the sum of a column's weights must be finite and positive");
-  c->h_cw.assign(w, w + (size_t)B * K);
-  c->h_swsum.assign(sw_sum, sw_sum + B);
-  c->cw_cols = B;
-  c->cw_k = K;
+  c->cw.w.assign(w, w + (size_t)B * K);
+  c->cw.sw_sum.assign(sw_sum, sw_sum + B);
+  c->cw.cols = B;
+  c->cw.k = K;
   return 0;
 }
 
@@ -573,7 +617,7 @@ int skd_stage_forest_class_weights(skd_ctx* ctx, int32_t n_classes, const double
                                    double min_weight_fraction_leaf) {
   if (!ctx) return fail(nullptr, "skd_stage_forest_class_weights: ctx is NULL");
   Ctx* c = &ctx->c;
-  c->forest_cw = ForestClassWeights();
+  c->forest_cw = {};
   if (n_classes <= 0 || (!w && !balanced_subsample)) return 0;   // cleared
   if (!(std::isfinite(min_weight_fraction_leaf) && min_weight_fraction_leaf >= 0.0 && min_weight_fraction_leaf <= 0.5))
     return fail(c, "skd_stage_forest_class_weights: min_weight_fraction_leaf must be in [0, 0.5]");
@@ -590,34 +634,105 @@ int skd_stage_forest_class_weights(skd_ctx* ctx, int32_t n_classes, const double
   return 0;
 }
 
-namespace {
-// Staged class weights are one-shot: the guard takes them off the context for the call that reads them.
-struct ClassWeightGuard {
-  std::vector<float> w; std::vector<double> sw_sum; int32_t cols, k;
-  explicit ClassWeightGuard(Ctx* c) : cols(c->cw_cols), k(c->cw_k) {
-    w.swap(c->h_cw); sw_sum.swap(c->h_swsum); c->cw_cols = 0; c->cw_k = 0;
+// Staged class weights of binary columns: weights scaled by the power of two 2^-e that brings the larger one
+// into (1/2, 1], so that |G| <= 2^14 holds in the fp16 operand of the tensor-core gradient product; 2^e goes
+// into inv_n.  Both scalings are exact.  l2 = 1 / (C sw_sum), inv_n = 2^e / sw_sum
+// (SK/linear_model/_logistic.py:474, 580).
+static int binary_class_weights(Ctx* c, const char* who, const StagedClassWeights& cw, int B, const double* C,
+                                std::vector<float2>& hcw, std::vector<double>& l2, std::vector<double>& inv_n) {
+  if (cw.cols != B || cw.k != 2) return fail(c, std::string(who) + ": staged class weights do not match this batch (B x 2)");
+  hcw.resize(B);
+  for (int j = 0; j < B; ++j) {
+    const float mx = std::max(cw.w[2 * j], cw.w[2 * j + 1]);
+    if (!(mx > 0.f)) return fail(c, std::string(who) + ": every class weight of a column is 0");
+    int e;
+    const float f = frexpf(mx, &e);   // mx = f 2^e, f in [1/2, 1)
+    if (f == 0.5f) e -= 1;             // a power of two becomes exactly 1
+    hcw[j] = make_float2(ldexpf(cw.w[2 * j], -e), ldexpf(cw.w[2 * j + 1], -e));
+    l2[j] = 1.0 / (C[j] * cw.sw_sum[j]);
+    inv_n[j] = ldexp(1.0 / cw.sw_sum[j], e);
   }
-  // Binary columns: weights scaled by the power of two 2^-e that brings the larger one into (1/2, 1], so
-  // that |G| <= 2^14 holds in the fp16 operand of the tensor-core gradient product; 2^e goes into inv_n.
-  // Both scalings are exact.  l2 = 1 / (C sw_sum), inv_n = 2^e / sw_sum (SK/linear_model/_logistic.py:474, 580).
-  int binary(Ctx* c, const char* who, int B, const double* C, std::vector<float2>& cw, std::vector<double>& l2,
-             std::vector<double>& inv_n) const {
-    if (cols != B || k != 2) return fail(c, std::string(who) + ": staged class weights do not match this batch (B x 2)");
-    cw.resize(B);
-    for (int j = 0; j < B; ++j) {
-      const float mx = std::max(w[2 * j], w[2 * j + 1]);
-      if (!(mx > 0.f)) return fail(c, std::string(who) + ": every class weight of a column is 0");
-      int e;
-      const float f = frexpf(mx, &e);   // mx = f 2^e, f in [1/2, 1)
-      if (f == 0.5f) e -= 1;             // a power of two becomes exactly 1
-      cw[j] = make_float2(ldexpf(w[2 * j], -e), ldexpf(w[2 * j + 1], -e));
-      l2[j] = 1.0 / (C[j] * sw_sum[j]);
-      inv_n[j] = ldexp(1.0 / sw_sum[j], e);
+  return 0;
+}
+
+// Training-set size n_train of every logistic column, then l2 = 1 / (C n_train) (SK/linear_model/_logistic.py:580)
+// and inv_n = 1 / n_train.  The rows of the column's held-out fold col_fold[j] (< 0: none) do not train;
+// with col_neg (pair columns, col_neg[j] >= 0) only the rows of class col_pos[j] or col_neg[j] train; staged
+// train bits (bits->m) replace the count.  col_neg and bits may be null.
+static int column_train_sizes(Ctx* c, const char* who, int B, const double* C, const int32_t* col_fold,
+                              const int32_t* col_pos, const int32_t* col_neg, const StagedRowBits* bits,
+                              std::vector<double>& l2, std::vector<double>& inv_n, double* mean_ntrain = nullptr) {
+  const int64_t n = c->n;
+  l2.resize(B);
+  inv_n.resize(B);
+  std::vector<int64_t> pair_counts;
+  int max_cls = -1;
+  double mean = 0.0;
+  for (int j = 0; j < B; ++j) {
+    int f = col_fold[j];
+    int64_t ntrain = n;
+    if (f >= 0) {
+      if (!c->fold || f >= c->n_folds) return fail(c, std::string(who) + ": col_fold refers to an unstaged fold");
+      ntrain = n - c->fold_count[f];
     }
+    if (col_neg && col_neg[j] >= 0) {   // pair column: only rows of class col_pos[j] or col_neg[j] train
+      if ((int64_t)c->h_ycls.size() != n) return fail(c, std::string(who) + ": labels not staged");
+      if (col_neg[j] == col_pos[j]) return fail(c, std::string(who) + ": col_neg equals col_pos");
+      if (pair_counts.empty()) {         // rows per (class, fold) once per call
+        for (int64_t i = 0; i < n; ++i) if (c->h_ycls[i] > max_cls) max_cls = c->h_ycls[i];
+        pair_counts.assign((size_t)(max_cls + 1) * (c->n_folds + 1), 0);
+        for (int64_t i = 0; i < n; ++i) {
+          const int fi = c->h_fold.empty() ? 0 : (int)c->h_fold[i];
+          if (c->h_ycls[i] >= 0) pair_counts[(size_t)c->h_ycls[i] * (c->n_folds + 1) + (c->h_fold.empty() ? 0 : fi)] += 1;
+        }
+      }
+      ntrain = 0;
+      for (int cls : {col_pos[j], col_neg[j]}) {
+        if (cls < 0 || cls > max_cls) continue;
+        for (int ff = 0; ff < (c->h_fold.empty() ? 1 : c->n_folds); ++ff)
+          if (ff != f) ntrain += pair_counts[(size_t)cls * (c->n_folds + 1) + ff];
+      }
+    }
+    if (bits && bits->cols > 0 && !bits->m.empty()) {      // training rows of the column = set bits of its mask
+      ntrain = 0;
+      const uint32_t* mw = bits->m.data() + (size_t)j * bits->words;
+      for (int64_t q = 0; q < bits->words; ++q) ntrain += __builtin_popcount(mw[q]);
+    }
+    if (ntrain <= 0) return fail(c, std::string(who) + ": empty training set");
+    if (!(C[j] > 0.0)) return fail(c, std::string(who) + ": C must be positive");
+    l2[j] = 1.0 / (C[j] * (double)ntrain);
+    inv_n[j] = 1.0 / (double)ntrain;
+    mean += (double)ntrain / B;
+  }
+  if (mean_ntrain) *mean_ntrain = mean;
+  return 0;
+}
+
+// Device time of a span of one call on the context's stream; the events are freed on every path.
+struct DeviceTimer {
+  Ctx* c;
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  explicit DeviceTimer(Ctx* c_) : c(c_) {}
+  ~DeviceTimer() {
+    if (e0) cudaEventDestroy(e0);
+    if (e1) cudaEventDestroy(e1);
+  }
+  int start() {
+    SKD_CUDA(c, cudaEventCreate(&e0));
+    SKD_CUDA(c, cudaEventCreate(&e1));
+    SKD_CUDA(c, cudaEventRecord(e0, c->stream));
+    return 0;
+  }
+  // ends the span, waits for it and writes its length in seconds to *seconds (when not null)
+  int stop(double* seconds) {
+    SKD_CUDA(c, cudaEventRecord(e1, c->stream));
+    SKD_CUDA(c, cudaEventSynchronize(e1));
+    float ms = 0.f;
+    SKD_CUDA(c, cudaEventElapsedTime(&ms, e0, e1));
+    if (seconds) *seconds = ms * 1e-3;
     return 0;
   }
 };
-}  // namespace
 
 int skd_set_kernel(skd_ctx* ctx, int32_t which) {
   if (!ctx) return -1;
@@ -681,19 +796,12 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
                          double* gpu_seconds_out) {
   if (!ctx) return fail(nullptr, "skd_logreg_fit_batch: ctx is NULL");
   Ctx* c = &ctx->c;
-  const ClassWeightGuard staged_cw(c);   // one-shot: staged class weights do not outlive this call
+  const StagedClassWeights staged_cw = std::exchange(c->cw, {});
+  const StagedMasks staged_masks = std::exchange(c->fmask, {});
+  const StagedRowBits staged_bits = std::exchange(c->row_bits, {});
   if (!c->X || !c->ycls) return fail(c, "skd_logreg_fit_batch: stage X and labels first");
   if (B <= 0 || !C || !col_fold || !col_pos || !coef_out || !n_iter_out || !status_out)
     return fail(c, "skd_logreg_fit_batch: bad arguments");
-  // staged column masks are one-shot: whatever happens in this call, they do not outlive it
-  struct MaskGuard {
-    Ctx* c; std::vector<uint8_t> mask; int32_t cols;
-    explicit MaskGuard(Ctx* c_) : c(c_), cols(c_->fmask_cols) { mask.swap(c_->h_fmask); c_->fmask_cols = 0; }
-  } staged_masks(c);
-  struct BitsGuard {     // staged row bit matrices are one-shot as well
-    std::vector<uint32_t> y, m; int32_t cols; int64_t words;
-    explicit BitsGuard(Ctx* c_) : cols(c_->rb_cols), words(c_->rb_words) { y.swap(c_->h_ybits); m.swap(c_->h_mbits); c_->rb_cols = 0; c_->rb_words = 0; }
-  } staged_bits(c);
   if (staged_bits.cols > 0) {
     if (staged_bits.cols != B) return fail(c, "skd_logreg_fit_batch: staged row bit matrices do not match this batch");
     for (int j = 0; j < B; ++j)
@@ -702,52 +810,16 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   }
   if (max_iter < 1) return fail(c, "skd_logreg_fit_batch: max_iter must be >= 1");
   SKD_CUDA(c, cudaSetDevice(c->device));
-  const int64_t n = c->n, d = c->d, ldx = c->ldx;
+  const int64_t d = c->d;
   const int dp = (int)d + 1, m = 10;
 
-  // host-side per-column constants
-  std::vector<double> l2(B), inv_n(B);
-  std::vector<int64_t> pair_counts;
-  int max_cls = -1;
+  std::vector<double> l2, inv_n;
   double mean_ntrain = 0.0;
-  for (int j = 0; j < B; ++j) {
-    int f = col_fold[j];
-    int64_t ntrain = n;
-    if (f >= 0) {
-      if (!c->fold || f >= c->n_folds) return fail(c, "skd_logreg_fit_batch: col_fold refers to an unstaged fold");
-      ntrain = n - c->fold_count[f];
-    }
-    if (col_neg && col_neg[j] >= 0) {   // pair column: only rows of class col_pos[j] or col_neg[j] train
-      if ((int64_t)c->h_ycls.size() != n) return fail(c, "skd_logreg_fit_batch: labels not staged");
-      if (col_neg[j] == col_pos[j]) return fail(c, "skd_logreg_fit_batch: col_neg equals col_pos");
-      if (pair_counts.empty()) {         // rows per (class, fold) once per call
-        for (int64_t i = 0; i < n; ++i) if (c->h_ycls[i] > max_cls) max_cls = c->h_ycls[i];
-        pair_counts.assign((size_t)(max_cls + 1) * (c->n_folds + 1), 0);
-        for (int64_t i = 0; i < n; ++i) {
-          const int fi = c->h_fold.empty() ? 0 : (int)c->h_fold[i];
-          if (c->h_ycls[i] >= 0) pair_counts[(size_t)c->h_ycls[i] * (c->n_folds + 1) + (c->h_fold.empty() ? 0 : fi)] += 1;
-        }
-      }
-      ntrain = 0;
-      for (int cls : {col_pos[j], col_neg[j]}) {
-        if (cls < 0 || cls > max_cls) continue;
-        for (int ff = 0; ff < (c->h_fold.empty() ? 1 : c->n_folds); ++ff)
-          if (ff != f) ntrain += pair_counts[(size_t)cls * (c->n_folds + 1) + ff];
-      }
-    }
-    if (staged_bits.cols > 0 && !staged_bits.m.empty()) {      // training rows of the column = set bits of its mask
-      ntrain = 0;
-      const uint32_t* mw = staged_bits.m.data() + (size_t)j * staged_bits.words;
-      for (int64_t q = 0; q < staged_bits.words; ++q) ntrain += __builtin_popcount(mw[q]);
-    }
-    if (ntrain <= 0) return fail(c, "skd_logreg_fit_batch: empty training set");
-    if (!(C[j] > 0.0)) return fail(c, "skd_logreg_fit_batch: C must be positive");
-    l2[j] = 1.0 / (C[j] * (double)ntrain);  // SK/linear_model/_logistic.py:580
-    inv_n[j] = 1.0 / (double)ntrain;
-    mean_ntrain += (double)ntrain / B;
-  }
+  if (column_train_sizes(c, "skd_logreg_fit_batch", B, C, col_fold, col_pos, col_neg, &staged_bits, l2, inv_n,
+                         &mean_ntrain))
+    return 1;
   std::vector<float2> hcw;
-  if (staged_cw.cols > 0 && staged_cw.binary(c, "skd_logreg_fit_batch", B, C, hcw, l2, inv_n)) return 1;
+  if (staged_cw.cols > 0 && binary_class_weights(c, "skd_logreg_fit_batch", staged_cw, B, C, hcw, l2, inv_n)) return 1;
 
   Trace tr(c, "logreg_fit");
   Scratch sx(c);
@@ -811,10 +883,8 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   SKD_CUDA(c, sx.alloc(&dloss, (size_t)B));
 
   tr.mark("alloc");
-  cudaEvent_t e0, e1;
-  SKD_CUDA(c, cudaEventCreate(&e0));
-  SKD_CUDA(c, cudaEventCreate(&e1));
-  SKD_CUDA(c, cudaEventRecord(e0, c->stream));
+  DeviceTimer timer(c);
+  if (timer.start()) return 1;
   SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(w.col_fold, col_fold, B * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
@@ -838,7 +908,6 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   int n_run = B;
   const long max_rounds = (long)max_iter * 52 + 16;
   long rounds = 0;
-  const long force_rounds = getenv("SKDIST_B200_FORCE_ROUNDS") ? atol(getenv("SKDIST_B200_FORCE_ROUNDS")) : 0;
   std::vector<double> round_flops;
   std::vector<int> round_act, round_run;
   size_t ev_used = 0;
@@ -877,14 +946,9 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
         ev_used += 2;
         ev_round.push_back((int)rounds);
       }
-      if (force_rounds > 0) {   // timing experiments: repeat the evaluation of the initial point
-        if (++rounds >= force_rounds) break;
-        continue;
-      }
       if (lbfgs_dev_enqueue(c, w, n_act, nz_used, fit_intercept, hist + 2 * rounds)) return 1;
       if (++rounds > max_rounds) return fail(c, "skd_logreg_fit_batch: round limit exceeded (internal error)");
     }
-    if (force_rounds > 0) { if (rounds >= force_rounds) break; continue; }
     int n_next = 0, r_next = 0;
     if (lbfgs_dev_readback(c, w, &n_next, &r_next)) return 1;
     n_act = n_next;
@@ -892,7 +956,7 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   }
   // true per-round counts (columns evaluated in round r = running after round r - 1)
   std::vector<int32_t> hhist((size_t)2 * std::max<long>(rounds, 1), 0);
-  if (force_rounds == 0 && rounds > 0)
+  if (rounds > 0)
     SKD_CUDA(c, cudaMemcpyAsync(hhist.data(), hist, (size_t)2 * rounds * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
   std::vector<int32_t> hdeal;
   if (deal_hist) {
@@ -904,14 +968,14 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   long live_rounds = 0;
   for (size_t e = 0; e < ev_round.size(); ++e) {
     const int r = ev_round[e];
-    const int running = (force_rounds > 0 || r == 0) ? B : hhist[2 * (r - 1) + 1];
-    const int slots = (force_rounds > 0 || r == 0) ? (w.grouped ? (int)hslots.size() : B) : hhist[2 * (r - 1)];
+    const int running = r == 0 ? B : hhist[2 * (r - 1) + 1];
+    const int slots = r == 0 ? (w.grouped ? (int)hslots.size() : B) : hhist[2 * (r - 1)];
     round_flops.push_back(4.0 * (double)d * (double)running * mean_ntrain);
     round_act.push_back(slots);
     round_run.push_back(running);
   }
   for (long r = 0; r < rounds; ++r)
-    if (force_rounds > 0 || r == 0 || hhist[2 * (r - 1) + 1] > 0) ++live_rounds;
+    if (r == 0 || hhist[2 * (r - 1) + 1] > 0) ++live_rounds;
   tr.mark("rounds");
   if (c->prof) {
     SKD_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -940,14 +1004,8 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
     SKD_CUDA(c, cudaMemcpyAsync(loss_out, dloss, (size_t)B * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   if (n_evals_out)
     SKD_CUDA(c, cudaMemcpyAsync(n_evals_out, w.n_evals, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaEventRecord(e1, c->stream));
-  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  if (timer.stop(gpu_seconds_out)) return 1;
   c->d2h += (int64_t)B * (dp * 4 + 20);
-  float ms = 0.f;
-  SKD_CUDA(c, cudaEventElapsedTime(&ms, e0, e1));
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  if (gpu_seconds_out) *gpu_seconds_out = ms * 1e-3;
   tr.mark("finish");
   return 0;
 }
@@ -957,29 +1015,22 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
                          double* loss_out, double* grad_out) {
   if (!ctx) return fail(nullptr, "skd_logreg_loss_grad: ctx is NULL");
   Ctx* c = &ctx->c;
-  const ClassWeightGuard staged_cw(c);   // one-shot: staged class weights do not outlive this call
+  const StagedClassWeights staged_cw = std::exchange(c->cw, {});
   if (!c->X || !c->ycls) return fail(c, "skd_logreg_loss_grad: stage X and labels first");
   if (B <= 0 || !w_in || !C || !col_fold || !col_pos || !loss_out || !grad_out)
     return fail(c, "skd_logreg_loss_grad: bad arguments");
   SKD_CUDA(c, cudaSetDevice(c->device));
-  const int64_t n = c->n, d = c->d, ldx = c->ldx;
+  const int64_t d = c->d, ldx = c->ldx;
   const int dp = (int)d + 1;
-  std::vector<double> l2(B), inv_n(B);
+  std::vector<double> l2, inv_n;
+  if (column_train_sizes(c, "skd_logreg_loss_grad", B, C, col_fold, col_pos, nullptr, nullptr, l2, inv_n)) return 1;
   std::vector<float> hw((size_t)B * ldx + B, 0.f);
   for (int j = 0; j < B; ++j) {
-    int f = col_fold[j];
-    int64_t ntrain = n;
-    if (f >= 0) {
-      if (!c->fold || f >= c->n_folds) return fail(c, "skd_logreg_loss_grad: unstaged fold");
-      ntrain = n - c->fold_count[f];
-    }
-    l2[j] = 1.0 / (C[j] * (double)ntrain);
-    inv_n[j] = 1.0 / (double)ntrain;
     for (int k = 0; k < d; ++k) hw[(size_t)j * ldx + k] = (float)w_in[(size_t)j * dp + k];
     hw[(size_t)B * ldx + j] = fit_intercept ? (float)w_in[(size_t)j * dp + d] : 0.f;
   }
   std::vector<float2> hcw;
-  if (staged_cw.cols > 0 && staged_cw.binary(c, "skd_logreg_loss_grad", B, C, hcw, l2, inv_n)) return 1;
+  if (staged_cw.cols > 0 && binary_class_weights(c, "skd_logreg_loss_grad", staged_cw, B, C, hcw, l2, inv_n)) return 1;
   Scratch sx(c);
   LogregWork w;
   w.B = B; w.dp = dp;
@@ -1024,18 +1075,14 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
   return 0;
 }
 
-// Pack caller coefficients [B x (d+1)] into the kernel layout: weights [B x ldx] + bias [B].
-static int pack_coef(Ctx* c, Scratch& sx, int B, const float* coef, float** dW) {
-  const int64_t d = c->d, ldx = c->ldx;
-  std::vector<float> h((size_t)B * ldx + B, 0.f);
+// Scoring codes (score_code_selects) of a scoring entry: -1 is not a code, and a code names a staged fold.
+static int check_score_codes(Ctx* c, const char* who, int B, const int32_t* col_fold) {
   for (int j = 0; j < B; ++j) {
-    memcpy(&h[(size_t)j * ldx], coef + (size_t)j * (d + 1), d * sizeof(float));
-    h[(size_t)B * ldx + j] = coef[(size_t)j * (d + 1) + d];
+    if (col_fold[j] == -1) return fail(c, std::string(who) + ": col_fold -1 is not a scoring code");
+    const int f = score_code_fold(col_fold[j]);
+    if (f >= 0 && (!c->fold || f >= c->n_folds))
+      return fail(c, std::string(who) + ": col_fold refers to an unstaged fold");
   }
-  SKD_CUDA(c, sx.alloc(dW, h.size()));
-  SKD_CUDA(c, cudaMemcpyAsync(*dW, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->h2d += (int64_t)h.size() * 4;
   return 0;
 }
 
@@ -1046,17 +1093,12 @@ int skd_linear_score_batch(skd_ctx* ctx, int32_t B, const float* coef, const int
   if (!c->X || !c->ycls) return fail(c, "skd_linear_score_batch: stage X and labels first");
   if (B <= 0 || !coef || !col_fold || !col_pos || !correct_out || !count_out)
     return fail(c, "skd_linear_score_batch: bad arguments");
+  if (check_score_codes(c, "skd_linear_score_batch", B, col_fold)) return 1;
   SKD_CUDA(c, cudaSetDevice(c->device));
   Trace tr(c, "score");
   Scratch sx(c);
   std::vector<SlotMeta> hs(B);
-  for (int j = 0; j < B; ++j) {
-    int f = col_fold[j] >= 0 ? col_fold[j] : (col_fold[j] <= -3 ? -3 - col_fold[j] : -1);
-    if (col_fold[j] == -1) return fail(c, "skd_linear_score_batch: col_fold -1 is not a scoring code");
-    if (f >= 0 && (!c->fold || f >= c->n_folds))
-      return fail(c, "skd_linear_score_batch: col_fold refers to an unstaged fold");
-    hs[j].col = j; hs[j].fold = col_fold[j]; hs[j].pos = col_pos[j]; hs[j].pad = 0;
-  }
+  for (int j = 0; j < B; ++j) { hs[j].col = j; hs[j].fold = col_fold[j]; hs[j].pos = col_pos[j]; hs[j].pad = 0; }
   SlotMeta* dslot; int64_t *dcorrect, *dcount;
   SKD_CUDA(c, sx.alloc(&dslot, (size_t)B));
   SKD_CUDA(c, sx.alloc(&dcorrect, (size_t)B));
@@ -1064,38 +1106,18 @@ int skd_linear_score_batch(skd_ctx* ctx, int32_t B, const float* coef, const int
   SKD_CUDA(c, cudaMemcpyAsync(dslot, hs.data(), B * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemsetAsync(dcorrect, 0, B * sizeof(int64_t), c->stream));
   SKD_CUDA(c, cudaMemsetAsync(dcount, 0, B * sizeof(int64_t), c->stream));
-  if (c->kernel_choice == 2 && !tc_supported(c))
-    return fail(c, "tensor-core path requested but the staged shape is unsupported (needs d <= 256)");
-  if (want_tc(c)) {
+  bool use_tc;
+  if (use_tensor_cores(c, &use_tc)) return 1;
+  if (use_tc) {
     // tensor-core GEMM1-only pass with a counting epilogue (logreg_tc.cu, TC_SCORE)
-    if (tc_prepare(c)) return 1;
     LogregWork w;
-    w.B = B; w.dp = (int)c->d + 1; w.use_tc = true; w.ldw = c->tc.dpad;
-    w.slot = dslot;
-    w.slots_pad_cap = (int)round_up(B, 128);
-    size_t wbytes = (size_t)w.slots_pad_cap * c->tc.dpad * 2;
-    SKD_CUDA(c, sx.alloc((uint8_t**)&w.Wh, wbytes));
-    SKD_CUDA(c, sx.alloc((uint8_t**)&w.Wl, wbytes));
-    SKD_CUDA(c, sx.alloc((uint8_t**)&w.sp, (size_t)w.slots_pad_cap * tc_slot_param_bytes()));
-    SKD_CUDA(c, sx.alloc(&w.n_act, 1));
-    SKD_CUDA(c, cudaMemsetAsync(w.Wh, 0, wbytes, c->stream));
-    SKD_CUDA(c, cudaMemsetAsync(w.Wl, 0, wbytes, c->stream));
-    std::vector<double> hx((size_t)B * w.dp);
-    for (size_t i = 0; i < hx.size(); ++i) hx[i] = (double)coef[i];
-    double* dx;
-    SKD_CUDA(c, sx.alloc(&dx, hx.size()));
-    int32_t nb = B;
-    SKD_CUDA(c, cudaMemcpyAsync(dx, hx.data(), hx.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &nb, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-    c->h2d += (int64_t)hx.size() * 8;
+    if (tc_scoring_setup(c, sx, w, B, coef, dslot)) return 1;
     tr.mark("setup");
-    if (tc_export(c, w, B, dx, 1)) return 1;
     if (tc_score(c, w, B, dcorrect, dcount)) return 1;
     tr.mark("kernel");
   } else {
     float* dW;
-    if (pack_coef(c, sx, B, coef, &dW)) return 1;
+    if (pack_coef(c, sx, B, coef, c->d, c->ldx, &dW)) return 1;
     if (simt_score(c, B, dW, dslot, dcorrect, dcount)) return 1;
   }
   SKD_CUDA(c, cudaMemcpyAsync(correct_out, dcorrect, B * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
@@ -1111,57 +1133,42 @@ int skd_logreg_multinomial_fit_batch(skd_ctx* ctx, int32_t B, int32_t n_classes,
                                      int32_t* n_evals_out, double* gpu_seconds_out) {
   if (!ctx) return fail(nullptr, "skd_logreg_multinomial_fit_batch: ctx is NULL");
   Ctx* c = &ctx->c;
-  const ClassWeightGuard staged_cw(c);   // one-shot: staged class weights do not outlive this call
+  const StagedClassWeights staged_cw = std::exchange(c->cw, {});
+  const StagedMasks staged_masks = std::exchange(c->fmask, {});
   if (!c->X || !c->ycls) return fail(c, "skd_logreg_multinomial_fit_batch: stage X and labels first");
   if (B <= 0 || n_classes < 2 || !C || !col_fold || !coef_out || !n_iter_out || !status_out)
     return fail(c, "skd_logreg_multinomial_fit_batch: bad arguments");
   if (max_iter < 1) return fail(c, "skd_logreg_multinomial_fit_batch: max_iter must be >= 1");
-  for (int j = 0; j < B; ++j) {
-    if (col_fold[j] >= 0 && (!c->fold || col_fold[j] >= c->n_folds))
-      return fail(c, "skd_logreg_multinomial_fit_batch: col_fold refers to an unstaged fold");
-    if (!(C[j] > 0.0)) return fail(c, "skd_logreg_multinomial_fit_batch: C must be positive");
-  }
-  // staged column masks are one-shot: whatever happens in this call, they do not outlive it
-  std::vector<uint8_t> masks;
-  masks.swap(c->h_fmask);
-  const int32_t mask_cols = c->fmask_cols;
-  c->fmask_cols = 0;
-  if (mask_cols > 0 && (mask_cols != B || (int64_t)masks.size() != (int64_t)B * c->d))
+  std::vector<double> l2, inv_n;
+  if (column_train_sizes(c, "skd_logreg_multinomial_fit_batch", B, C, col_fold, nullptr, nullptr, nullptr, l2, inv_n))
+    return 1;
+  if (staged_masks.cols > 0 && (staged_masks.cols != B || (int64_t)staged_masks.mask.size() != (int64_t)B * c->d))
     return fail(c, "skd_logreg_multinomial_fit_batch: staged column masks do not match the batch");
-  if (staged_cw.cols > 0 && (staged_cw.cols != B || staged_cw.k != n_classes))
-    return fail(c, "skd_logreg_multinomial_fit_batch: staged class weights do not match this batch (B x n_classes)");
+  if (staged_cw.cols > 0) {
+    if (staged_cw.cols != B || staged_cw.k != n_classes)
+      return fail(c, "skd_logreg_multinomial_fit_batch: staged class weights do not match this batch (B x n_classes)");
+    // the sum of the per-row weights takes the place of n_train (SK/linear_model/_logistic.py:474)
+    for (int j = 0; j < B; ++j) {
+      l2[j] = 1.0 / (C[j] * staged_cw.sw_sum[j]);
+      inv_n[j] = 1.0 / staged_cw.sw_sum[j];
+    }
+  }
   SKD_CUDA(c, cudaSetDevice(c->device));
   Trace tr(c, "multinomial_fit");
-  cudaEvent_t e0, e1;
-  SKD_CUDA(c, cudaEventCreate(&e0));
-  SKD_CUDA(c, cudaEventCreate(&e1));
-  SKD_CUDA(c, cudaEventRecord(e0, c->stream));
-  const int rc = multi_fit(c, B, n_classes, C, col_fold, fit_intercept, tol, max_iter, mask_cols > 0 ? masks.data() : nullptr,
-                           staged_cw.cols > 0 ? staged_cw.w.data() : nullptr,
-                           staged_cw.cols > 0 ? staged_cw.sw_sum.data() : nullptr, coef_out, n_iter_out, status_out, loss_out, n_evals_out);
-  float ms = 0.f;
-  if (!rc) {
-    cudaEventRecord(e1, c->stream);
-    cudaEventSynchronize(e1);
-    cudaEventElapsedTime(&ms, e0, e1);
-  }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  if (gpu_seconds_out) *gpu_seconds_out = ms * 1e-3;
-  return rc;
+  DeviceTimer timer(c);
+  if (timer.start()) return 1;
+  if (multi_fit(c, B, n_classes, l2.data(), inv_n.data(), col_fold, fit_intercept, tol, max_iter,
+                staged_masks.cols > 0 ? staged_masks.mask.data() : nullptr,
+                staged_cw.cols > 0 ? staged_cw.w.data() : nullptr, coef_out, n_iter_out, status_out, loss_out, n_evals_out))
+    return 1;
+  return timer.stop(gpu_seconds_out);
 }
 
 static int multinomial_check(Ctx* c, const char* who, int32_t B, int32_t n_classes, const float* coef,
                              const int32_t* col_fold) {
   if (!c->X || !c->ycls) return fail(c, std::string(who) + ": stage X and labels first");
   if (B <= 0 || n_classes < 2 || !coef || !col_fold) return fail(c, std::string(who) + ": bad arguments");
-  for (int j = 0; j < B; ++j) {
-    const int f = col_fold[j] >= 0 ? col_fold[j] : (col_fold[j] <= -3 ? -3 - col_fold[j] : -1);
-    if (col_fold[j] == -1) return fail(c, std::string(who) + ": col_fold -1 is not a scoring code");
-    if (f >= 0 && (!c->fold || f >= c->n_folds))
-      return fail(c, std::string(who) + ": col_fold refers to an unstaged fold");
-  }
-  return 0;
+  return check_score_codes(c, who, B, col_fold);
 }
 
 int skd_multinomial_confusion_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, const float* coef,
@@ -1207,12 +1214,7 @@ int skd_linear_auc_batch(skd_ctx* ctx, int32_t B, const float* coef, const int32
   if (!c->X || !c->ycls) return fail(c, "skd_linear_auc_batch: stage X and labels first");
   if (B <= 0 || !coef || !col_fold || !col_pos || !u2_out || !n_pos_out || !n_neg_out)
     return fail(c, "skd_linear_auc_batch: bad arguments");
-  for (int j = 0; j < B; ++j) {
-    const int f = col_fold[j] >= 0 ? col_fold[j] : (col_fold[j] <= -3 ? -3 - col_fold[j] : -1);
-    if (col_fold[j] == -1) return fail(c, "skd_linear_auc_batch: col_fold -1 is not a scoring code");
-    if (f >= 0 && (!c->fold || f >= c->n_folds))
-      return fail(c, "skd_linear_auc_batch: col_fold refers to an unstaged fold");
-  }
+  if (check_score_codes(c, "skd_linear_auc_batch", B, col_fold)) return 1;
   SKD_CUDA(c, cudaSetDevice(c->device));
   Trace tr(c, "auc");
   return auc_batch(c, B, coef, col_fold, col_pos, u2_out, n_pos_out, n_neg_out);
@@ -1250,21 +1252,10 @@ int skd_ridge_fit_batch(skd_ctx* ctx, int32_t B, const double* alpha, const int3
       hold[j] = n_folds;   // hold out nothing
     }
   }
-  cudaEvent_t e0, e1;
-  SKD_CUDA(c, cudaEventCreate(&e0));
-  SKD_CUDA(c, cudaEventCreate(&e1));
-  SKD_CUDA(c, cudaEventRecord(e0, c->stream));
-  int rc = ridge_fit_batch(c, B, alpha, hold.data(), fit_intercept, coef_out, status_out);
-  float ms = 0.f;
-  if (!rc) {
-    cudaEventRecord(e1, c->stream);
-    cudaEventSynchronize(e1);
-    cudaEventElapsedTime(&ms, e0, e1);
-  }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  if (gpu_seconds_out) *gpu_seconds_out = ms * 1e-3;
-  return rc;
+  DeviceTimer timer(c);
+  if (timer.start()) return 1;
+  if (ridge_fit_batch(c, B, alpha, hold.data(), fit_intercept, coef_out, status_out)) return 1;
+  return timer.stop(gpu_seconds_out);
 }
 
 int skd_linear_r2_batch(skd_ctx* ctx, int32_t B, const float* coef, const int32_t* col_fold,
@@ -1273,15 +1264,11 @@ int skd_linear_r2_batch(skd_ctx* ctx, int32_t B, const float* coef, const int32_
   Ctx* c = &ctx->c;
   if (!c->X || !c->yreal) return fail(c, "skd_linear_r2_batch: stage X and targets first");
   if (B <= 0 || !coef || !col_fold || !sse_out || !count_out) return fail(c, "skd_linear_r2_batch: bad arguments");
+  if (check_score_codes(c, "skd_linear_r2_batch", B, col_fold)) return 1;
   SKD_CUDA(c, cudaSetDevice(c->device));
   Scratch sx(c);
   std::vector<SlotMeta> hs(B);
-  for (int j = 0; j < B; ++j) {
-    int f = col_fold[j] >= 0 ? col_fold[j] : (col_fold[j] <= -3 ? -3 - col_fold[j] : -1);
-    if (col_fold[j] == -1) return fail(c, "skd_linear_r2_batch: col_fold -1 is not a scoring code");
-    if (f >= 0 && (!c->fold || f >= c->n_folds)) return fail(c, "skd_linear_r2_batch: col_fold refers to an unstaged fold");
-    hs[j].col = j; hs[j].fold = col_fold[j]; hs[j].pos = 0; hs[j].pad = 0;
-  }
+  for (int j = 0; j < B; ++j) { hs[j].col = j; hs[j].fold = col_fold[j]; hs[j].pos = 0; hs[j].pad = 0; }
   SlotMeta* dslot; double* dsse; int64_t* dcount;
   SKD_CUDA(c, sx.alloc(&dslot, (size_t)B));
   SKD_CUDA(c, sx.alloc(&dsse, (size_t)B));
@@ -1289,38 +1276,18 @@ int skd_linear_r2_batch(skd_ctx* ctx, int32_t B, const float* coef, const int32_
   SKD_CUDA(c, cudaMemcpyAsync(dslot, hs.data(), B * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemsetAsync(dsse, 0, B * sizeof(double), c->stream));
   SKD_CUDA(c, cudaMemsetAsync(dcount, 0, B * sizeof(int64_t), c->stream));
-  if (c->kernel_choice == 2 && !tc_supported(c))
-    return fail(c, "tensor-core path requested but the staged shape is unsupported (needs d <= 256)");
-  if (want_tc(c)) {
-    if (tc_prepare(c)) return 1;
+  bool use_tc;
+  if (use_tensor_cores(c, &use_tc)) return 1;
+  if (use_tc) {
     LogregWork w;
-    w.B = B; w.dp = (int)c->d + 1; w.use_tc = true; w.ldw = c->tc.dpad;
-    w.slot = dslot;
-    w.slots_pad_cap = (int)round_up(B, 128);
-    size_t wbytes = (size_t)w.slots_pad_cap * c->tc.dpad * 2;
-    SKD_CUDA(c, sx.alloc((uint8_t**)&w.Wh, wbytes));
-    SKD_CUDA(c, sx.alloc((uint8_t**)&w.Wl, wbytes));
-    SKD_CUDA(c, sx.alloc((uint8_t**)&w.sp, (size_t)w.slots_pad_cap * tc_slot_param_bytes()));
-    SKD_CUDA(c, sx.alloc(&w.n_act, 1));
-    SKD_CUDA(c, cudaMemsetAsync(w.Wh, 0, wbytes, c->stream));
-    SKD_CUDA(c, cudaMemsetAsync(w.Wl, 0, wbytes, c->stream));
+    if (tc_scoring_setup(c, sx, w, B, coef, dslot)) return 1;
     const size_t n_part = (size_t)tc_partials_per_slot() * B;   // per-chunk squared-error sums
     SKD_CUDA(c, sx.alloc(&w.lossp, n_part));
     SKD_CUDA(c, cudaMemsetAsync(w.lossp, 0, n_part * sizeof(double), c->stream));
-    std::vector<double> hx((size_t)B * w.dp);
-    for (size_t i = 0; i < hx.size(); ++i) hx[i] = (double)coef[i];
-    double* dx;
-    SKD_CUDA(c, sx.alloc(&dx, hx.size()));
-    int32_t nb = B;
-    SKD_CUDA(c, cudaMemcpyAsync(dx, hx.data(), hx.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &nb, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-    c->h2d += (int64_t)hx.size() * 8;
-    if (tc_export(c, w, B, dx, 1)) return 1;
     if (tc_r2(c, w, B, dsse, dcount)) return 1;
   } else {
     float* dW;
-    if (pack_coef(c, sx, B, coef, &dW)) return 1;
+    if (pack_coef(c, sx, B, coef, c->d, c->ldx, &dW)) return 1;
     if (simt_r2(c, B, dW, dslot, dsse, dcount)) return 1;
   }
   SKD_CUDA(c, cudaMemcpyAsync(sse_out, dsse, B * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
@@ -1343,23 +1310,12 @@ int skd_sgd_fit_batch(skd_ctx* ctx, int32_t B, const int32_t* col_pos, int32_t l
   if (loss < 0 || loss > 1 || lr_type < 0 || lr_type > 2 || !(alpha > 0.0) || max_iter < 1)
     return fail(c, "skd_sgd_fit_batch: unsupported loss / learning rate / alpha / max_iter");
   SKD_CUDA(c, cudaSetDevice(c->device));
-  cudaEvent_t e0, e1;
-  SKD_CUDA(c, cudaEventCreate(&e0));
-  SKD_CUDA(c, cudaEventCreate(&e1));
-  SKD_CUDA(c, cudaEventRecord(e0, c->stream));
-  int rc = sgd_fit_batch(c, B, col_pos, loss, alpha, fit_intercept, max_iter, tol, shuffle, seed, lr_type, eta0,
-                         power_t, optimal_init, n_iter_no_change, coef_out, intercept_out, n_iter_out, t_out,
-                         status_out);
-  float ms = 0.f;
-  if (!rc) {
-    cudaEventRecord(e1, c->stream);
-    cudaEventSynchronize(e1);
-    cudaEventElapsedTime(&ms, e0, e1);
-  }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  if (gpu_seconds_out) *gpu_seconds_out = ms * 1e-3;
-  return rc;
+  DeviceTimer timer(c);
+  if (timer.start()) return 1;
+  if (sgd_fit_batch(c, B, col_pos, loss, alpha, fit_intercept, max_iter, tol, shuffle, seed, lr_type, eta0, power_t,
+                    optimal_init, n_iter_no_change, coef_out, intercept_out, n_iter_out, t_out, status_out))
+    return 1;
+  return timer.stop(gpu_seconds_out);
 }
 
 struct skd_forest {
@@ -1406,8 +1362,7 @@ int skd_forest_fit(skd_ctx* ctx, int32_t n_trees, const uint8_t* sample_counts, 
                    int32_t splitter, const double* y_regression, skd_forest** out, double* gpu_seconds_out) {
   if (!ctx) return fail(nullptr, "skd_forest_fit: ctx is NULL");
   Ctx* c = &ctx->c;
-  ForestClassWeights cw;               // staged class weights are one-shot: taken off the context whatever happens
-  std::swap(cw, c->forest_cw);
+  const ForestClassWeights cw = std::exchange(c->forest_cw, {});
   if (!out) return fail(c, "skd_forest_fit: out is NULL");
   *out = nullptr;
   if (!c->X || (!y_regression && !c->ycls)) return fail(c, "skd_forest_fit: stage X and labels first");
@@ -1415,28 +1370,18 @@ int skd_forest_fit(skd_ctx* ctx, int32_t n_trees, const uint8_t* sample_counts, 
       splitter < 0 || splitter > 1)
     return fail(c, "skd_forest_fit: bad arguments");
   SKD_CUDA(c, cudaSetDevice(c->device));
-  skd_forest* f = new skd_forest();
+  std::unique_ptr<skd_forest> f(new skd_forest());
   f->trees.resize(n_trees);
   f->cw = cw;
-  cudaEvent_t e0, e1;
-  SKD_CUDA(c, cudaEventCreate(&e0));
-  SKD_CUDA(c, cudaEventCreate(&e1));
-  SKD_CUDA(c, cudaEventRecord(e0, c->stream));
-  int rc = forest_fit(c, n_trees, sample_counts, rand_states, n_classes, max_features, max_depth, min_samples_split,
-                      min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter, y_regression,
-                      cw.n_classes ? &cw : nullptr, forest_sink, f);
-  if (!rc) f->binval = c->forest.h_binval;
-  float ms = 0.f;
-  if (!rc) {
-    cudaEventRecord(e1, c->stream);
-    cudaEventSynchronize(e1);
-    cudaEventElapsedTime(&ms, e0, e1);
-  }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  if (gpu_seconds_out) *gpu_seconds_out = ms * 1e-3;
-  if (rc) { delete f; return rc; }
-  *out = f;
+  DeviceTimer timer(c);
+  if (timer.start()) return 1;
+  if (forest_fit(c, n_trees, sample_counts, rand_states, n_classes, max_features, max_depth, min_samples_split,
+                 min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter, y_regression,
+                 cw.n_classes ? &cw : nullptr, forest_sink, f.get()))
+    return 1;
+  f->binval = c->forest.h_binval;
+  if (timer.stop(gpu_seconds_out)) return 1;
+  *out = f.release();
   return 0;
 }
 
@@ -1577,45 +1522,48 @@ int skd_forest_tree_nodes(skd_forest* f, int32_t tree, void* nodes64, double* va
 
 void skd_forest_free(skd_forest* f) { delete f; }
 
+// Streams m new rows [m x d] (row pitch ld) through `kernel(dX, rows, ldx, dO)` in row chunks of <= 256 MiB:
+// threaded pinned-bounce H2D (stage_rows_h2d), one pass of the kernel, D2H of the (small) result of
+// out_row_bytes per row into out.  The copy engine is the bottleneck.  *seconds: wall time of the chunks.
+static int stream_rows(Ctx* c, Scratch& sx, const float* Xnew, int64_t m, int64_t d, int64_t ld, size_t out_row_bytes,
+                       void* out, double* seconds,
+                       const std::function<int(const float* dX, int64_t rows, int ldx, void* dO)>& kernel) {
+  const int64_t ldx = round_up(d, 4);
+  int64_t rows_per_chunk = std::max<int64_t>(1, ((int64_t)256 << 20) / (ldx * 4));
+  if (rows_per_chunk > m) rows_per_chunk = m;
+  float* dX; uint8_t* dO;
+  SKD_CUDA(c, sx.alloc(&dX, (size_t)rows_per_chunk * ldx));
+  SKD_CUDA(c, sx.alloc(&dO, (size_t)rows_per_chunk * out_row_bytes));
+  if (ldx != d) SKD_CUDA(c, cudaMemsetAsync(dX, 0, (size_t)rows_per_chunk * ldx * 4, c->stream));
+  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  auto w0 = std::chrono::steady_clock::now();
+  for (int64_t r0 = 0; r0 < m; r0 += rows_per_chunk) {
+    const int64_t mr = std::min(rows_per_chunk, m - r0);
+    if (stage_rows_h2d(c, dX, ldx, Xnew + r0 * ld, mr, d, ld)) return 1;
+    if (kernel(dX, mr, (int)ldx, dO)) return 1;
+    SKD_CUDA(c, cudaMemcpyAsync((uint8_t*)out + r0 * out_row_bytes, dO, (size_t)mr * out_row_bytes,
+                                cudaMemcpyDeviceToHost, c->stream));
+    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+    c->h2d += mr * d * 4;
+    c->d2h += mr * (int64_t)out_row_bytes;
+  }
+  if (seconds) *seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - w0).count();
+  return 0;
+}
+
 int skd_predict_linear(skd_ctx* ctx, const float* Xnew, int64_t m, int64_t d, int64_t ld, int32_t B,
                        const float* coef, float* out, double* gpu_seconds_out) {
   if (!ctx) return fail(nullptr, "skd_predict_linear: ctx is NULL");
   Ctx* c = &ctx->c;
   if (!Xnew || m <= 0 || d <= 0 || ld < d || B <= 0 || !coef || !out) return fail(c, "skd_predict_linear: bad arguments");
   SKD_CUDA(c, cudaSetDevice(c->device));
-  const int64_t ldx = round_up(d, 4);
   Scratch sx(c);
-  // weights [B x ldx] + bias[B]
-  std::vector<float> hw((size_t)B * ldx + B, 0.f);
-  for (int j = 0; j < B; ++j) {
-    memcpy(&hw[(size_t)j * ldx], coef + (size_t)j * (d + 1), d * sizeof(float));
-    hw[(size_t)B * ldx + j] = coef[(size_t)j * (d + 1) + d];
-  }
   float* dW;
-  SKD_CUDA(c, sx.alloc(&dW, hw.size()));
-  SKD_CUDA(c, cudaMemcpyAsync(dW, hw.data(), hw.size() * 4, cudaMemcpyHostToDevice, c->stream));
-  // row chunks of <= 256 MiB: threaded pinned-bounce H2D (stage_rows_h2d), one pass of the kernel,
-  // D2H of the (small) result.  The copy engine is the bottleneck (4*d bytes in per row, 4*B out).
-  int64_t rows_per_chunk = std::max<int64_t>(1, ((int64_t)256 << 20) / (ldx * 4));
-  if (rows_per_chunk > m) rows_per_chunk = m;
-  float *dX, *dO;
-  SKD_CUDA(c, sx.alloc(&dX, (size_t)rows_per_chunk * ldx));
-  SKD_CUDA(c, sx.alloc(&dO, (size_t)rows_per_chunk * B));
-  if (ldx != d) SKD_CUDA(c, cudaMemsetAsync(dX, 0, (size_t)rows_per_chunk * ldx * 4, c->stream));
-  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-  auto w0 = std::chrono::steady_clock::now();
-  for (int64_t r0 = 0; r0 < m; r0 += rows_per_chunk) {
-    int64_t mr = std::min(rows_per_chunk, m - r0);
-    if (stage_rows_h2d(c, dX, ldx, Xnew + r0 * ld, mr, d, ld)) return 1;
-    if (predict_device(c, dX, mr, (int)ldx, (int)d, B, dW, dO)) return 1;
-    SKD_CUDA(c, cudaMemcpyAsync(out + r0 * B, dO, (size_t)mr * B * 4, cudaMemcpyDeviceToHost, c->stream));
-    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-    c->h2d += mr * d * 4;
-    c->d2h += mr * (int64_t)B * 4;
-  }
-  if (gpu_seconds_out)
-    *gpu_seconds_out = std::chrono::duration<double>(std::chrono::steady_clock::now() - w0).count();
-  return 0;
+  if (pack_coef(c, sx, B, coef, d, round_up(d, 4), &dW)) return 1;
+  return stream_rows(c, sx, Xnew, m, d, ld, (size_t)B * 4, out, gpu_seconds_out,
+                     [&](const float* dX, int64_t rows, int ldx, void* dO) {
+                       return predict_device(c, dX, rows, ldx, (int)d, B, dW, (float*)dO);
+                     });
 }
 
 int skd_forest_predict(skd_ctx* ctx, const float* Xnew, int64_t m, int64_t d, int64_t ld,
@@ -1656,28 +1604,11 @@ int skd_forest_predict(skd_ctx* ctx, const float* Xnew, int64_t m, int64_t d, in
   SKD_CUDA(c, cudaMemcpyAsync(d_thr, threshold, (size_t)total * 8, cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(d_val, value, (size_t)total * n_classes * 8, cudaMemcpyHostToDevice, c->stream));
   c->h2d += total * (int64_t)(16 + 8 + 8 * n_classes);
-  const int64_t ldx = round_up(d, 4);
-  int64_t rows_per_chunk = std::max<int64_t>(1, ((int64_t)256 << 20) / (ldx * 4));
-  if (rows_per_chunk > m) rows_per_chunk = m;
-  float* dX; double* dO;
-  SKD_CUDA(c, sx.alloc(&dX, (size_t)rows_per_chunk * ldx));
-  SKD_CUDA(c, sx.alloc(&dO, (size_t)rows_per_chunk * n_classes));
-  if (ldx != d) SKD_CUDA(c, cudaMemsetAsync(dX, 0, (size_t)rows_per_chunk * ldx * 4, c->stream));
-  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-  auto w0 = std::chrono::steady_clock::now();
-  for (int64_t r0 = 0; r0 < m; r0 += rows_per_chunk) {
-    const int64_t mr = std::min(rows_per_chunk, m - r0);
-    if (stage_rows_h2d(c, dX, ldx, Xnew + r0 * ld, mr, d, ld)) return 1;
-    if (forest_predict_device(c, dX, mr, (int)ldx, n_trees, d_off, d_node, d_thr, d_val, n_classes, dO)) return 1;
-    SKD_CUDA(c, cudaMemcpyAsync(proba_out + r0 * n_classes, dO, (size_t)mr * n_classes * 8, cudaMemcpyDeviceToHost,
-                                c->stream));
-    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-    c->h2d += mr * d * 4;
-    c->d2h += mr * (int64_t)n_classes * 8;
-  }
-  if (gpu_seconds_out)
-    *gpu_seconds_out = std::chrono::duration<double>(std::chrono::steady_clock::now() - w0).count();
-  return 0;
+  return stream_rows(c, sx, Xnew, m, d, ld, (size_t)n_classes * 8, proba_out, gpu_seconds_out,
+                     [&](const float* dX, int64_t rows, int ldx, void* dO) {
+                       return forest_predict_device(c, dX, rows, ldx, n_trees, d_off, d_node, d_thr, d_val, n_classes,
+                                                    (double*)dO);
+                     });
 }
 
 int skd_linear_decision(skd_ctx* ctx, int32_t B, const float* coef, float* out) {
@@ -1688,7 +1619,7 @@ int skd_linear_decision(skd_ctx* ctx, int32_t B, const float* coef, float* out) 
   SKD_CUDA(c, cudaSetDevice(c->device));
   Scratch sx(c);
   float *dW, *dout;
-  if (pack_coef(c, sx, B, coef, &dW)) return 1;
+  if (pack_coef(c, sx, B, coef, c->d, c->ldx, &dW)) return 1;
   SKD_CUDA(c, sx.alloc(&dout, (size_t)c->n * B));
   if (B <= 16 && c->ldx * 4 * 8 <= 48 * 1024) {
     if (predict_device(c, c->X, c->n, (int)c->ldx, (int)c->d, B, dW, dout)) return 1;

@@ -17,8 +17,6 @@
 // decision_function computes them in fp32.
 #include <cub/device/device_radix_sort.cuh>
 
-#include <string.h>
-
 #include <algorithm>
 
 #include "skd_internal.h"
@@ -122,7 +120,7 @@ auc_count_kernel(const unsigned long long* __restrict__ keys, const int64_t* __r
 }
 
 // col_fold: scoring codes of skd_linear_score_batch.  u2_out / n_pos_out / n_neg_out: [B].
-int auc_batch(Ctx* c, int B, const float* dW_host_packed, const int32_t* col_fold, const int32_t* col_pos,
+int auc_batch(Ctx* c, int B, const float* coef, const int32_t* col_fold, const int32_t* col_pos,
               int64_t* u2_out, int64_t* n_pos_out, int64_t* n_neg_out) {
   const int64_t n = c->n, ldx = c->ldx;
   // row selection lists, one per distinct code
@@ -135,7 +133,7 @@ int auc_batch(Ctx* c, int B, const float* dW_host_packed, const int32_t* col_fol
     const int cd = codes[q];
     for (int64_t r = 0; r < n; ++r) {
       const int fd = c->h_fold.empty() ? -1 : (int)c->h_fold[r];
-      if (cd == -2 || (cd >= 0 && fd == cd) || (cd <= -3 && fd != (-3 - cd))) lists[q].push_back(r);
+      if (score_code_selects(cd, fd)) lists[q].push_back(r);
     }
   }
   auto list_of = [&](int cd) { return (size_t)(std::lower_bound(codes.begin(), codes.end(), cd) - codes.begin()); };
@@ -147,12 +145,6 @@ int auc_batch(Ctx* c, int B, const float* dW_host_packed, const int32_t* col_fol
   for (int b0 = 0; b0 < B; b0 += per) {
     const int Bb = std::min(per, B - b0);
     Scratch sx(c);
-    // weights of this block: [Bb x ldx] then bias [Bb]
-    std::vector<float> h((size_t)Bb * ldx + Bb, 0.f);
-    for (int j = 0; j < Bb; ++j) {
-      memcpy(&h[(size_t)j * ldx], dW_host_packed + (size_t)(b0 + j) * (c->d + 1), c->d * sizeof(float));
-      h[(size_t)Bb * ldx + j] = dW_host_packed[(size_t)(b0 + j) * (c->d + 1) + c->d];
-    }
     std::vector<int64_t> off(Bb + 1, 0);
     for (int j = 0; j < Bb; ++j) off[j + 1] = off[j] + (int64_t)lists[list_of(col_fold[b0 + j])].size();
     const int64_t total = off[Bb];
@@ -161,17 +153,15 @@ int auc_batch(Ctx* c, int B, const float* dW_host_packed, const int32_t* col_fol
     int32_t* dpos;
     unsigned long long *k0, *k1;
     long long* dout;
-    SKD_CUDA(c, sx.alloc(&dW, h.size()));
+    if (pack_coef(c, sx, Bb, coef + (size_t)b0 * (c->d + 1), c->d, ldx, &dW)) return 1;
     SKD_CUDA(c, sx.alloc(&dec, (size_t)n * Bb));
     SKD_CUDA(c, sx.alloc(&doff, (size_t)Bb + 1));
     SKD_CUDA(c, sx.alloc(&dpos, (size_t)Bb));
     SKD_CUDA(c, sx.alloc(&k0, (size_t)std::max<int64_t>(total, 1)));
     SKD_CUDA(c, sx.alloc(&k1, (size_t)std::max<int64_t>(total, 1)));
     SKD_CUDA(c, sx.alloc(&dout, (size_t)3 * Bb));
-    SKD_CUDA(c, cudaMemcpyAsync(dW, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaMemcpyAsync(doff, off.data(), off.size() * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaMemcpyAsync(dpos, col_pos + b0, Bb * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    c->h2d += (int64_t)h.size() * 4;
     if (simt_decision(c, Bb, dW, dec)) return 1;
     // keys, one launch per selection list (the columns that use it)
     std::vector<int64_t*> drows(codes.size(), nullptr);

@@ -19,8 +19,6 @@
 //
 // First CUDA path of this objective: fp32 CUDA cores (the binary objective's tensor-core kernel does
 // not cover it yet, DESIGN.md "multinomial").
-#include <string.h>
-
 #include <algorithm>
 
 #include "skd_internal.h"
@@ -103,7 +101,7 @@ mn_colsum_kernel(const float* __restrict__ G, int ldg, int64_t n, int64_t rpc, i
 
 // confusion counts conf[b][true class][predicted class] of argmax_k z (first maximum, like
 // numpy.argmax in LinearClassifierMixin.predict, SK/linear_model/_base.py:351-374) on the rows
-// selected by the candidate's fold code: f >= 0 rows of fold f; -2 every row; -3-f rows NOT in fold f.
+// selected by the candidate's scoring code (score_code_selects).
 // Every count-based multiclass metric (accuracy, precision / recall / f1 with any averaging,
 // balanced accuracy) is a function of this matrix.  SMEM = 1: the CTA counts in shared memory first.
 template <int SMEM>
@@ -125,7 +123,7 @@ mn_confusion_kernel(const float* __restrict__ Z, int ldz, int64_t n, int64_t rpc
   if (row_end > n) row_end = n;
   for (int64_t r = row_begin + threadIdx.x; r < row_end; r += 256) {
     const int fd = fold ? (int)fold[r] : -1;
-    const bool test = cd == -2 || (cd >= 0 && fd == cd) || (cd <= -3 && fd != (-3 - cd));
+    const bool test = score_code_selects(cd, fd);
     const int y = ycls[r];
     if (!test || y < 0 || y >= K) continue;
     const float* zr = Z + r * ldz + (size_t)b * K;
@@ -160,8 +158,8 @@ static int64_t candidates_per_pass(const Ctx* c, int K, int nz) {
   return b < 1 ? 1 : b;
 }
 
-int multi_fit(Ctx* c, int B, int K, const double* C, const int32_t* col_fold, int fit_intercept, double tol,
-              int max_iter, const uint8_t* fmask, const float* cw, const double* sw_sum, float* coef_out,
+int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold, int fit_intercept,
+              double tol, int max_iter, const uint8_t* fmask, const float* cw, float* coef_out,
               int32_t* n_iter_out, int32_t* status_out, double* loss_out, int32_t* n_evals_out) {
   const int64_t n = c->n, ldx = c->ldx;
   const int dp = (int)c->d + 1, m = 10;
@@ -171,16 +169,6 @@ int multi_fit(Ctx* c, int B, int K, const double* C, const int32_t* col_fold, in
   const int64_t per_pass = candidates_per_pass(c, K, nz);
   for (int64_t b0 = 0; b0 < B; b0 += per_pass) {
     const int Bb = (int)std::min<int64_t>(per_pass, B - b0);
-    std::vector<double> l2(Bb), inv_n(Bb);
-    for (int j = 0; j < Bb; ++j) {
-      const int f = col_fold[b0 + j];
-      const int64_t ntrain = f >= 0 ? n - c->fold_count[f] : n;
-      if (ntrain <= 0) return fail(c, "skd_logreg_multinomial_fit_batch: empty training set");
-      // weighted: the sum of the per-row weights takes the place of n_train (SK/linear_model/_logistic.py:474)
-      const double sw = sw_sum ? sw_sum[b0 + j] : (double)ntrain;
-      l2[j] = 1.0 / (C[b0 + j] * sw);   // SK/linear_model/_logistic.py:580
-      inv_n[j] = 1.0 / sw;
-    }
     Scratch sx(c);
     MultiWork w;
     w.B = Bb; w.K = K; w.dp = dp; w.nz = nz; w.rpc = rpc;
@@ -201,8 +189,8 @@ int multi_fit(Ctx* c, int B, int K, const double* C, const int32_t* col_fold, in
     SKD_CUDA(c, sx.alloc(&w.gsump, (size_t)nz * slots));
     SKD_CUDA(c, sx.alloc(&w.gradp, (size_t)nz * slots * ldx));
     SKD_CUDA(c, sx.alloc(&w.n_act, 1));
-    SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2.data(), Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n.data(), Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2 + b0, Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n + b0, Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaMemcpyAsync(d_fold, col_fold + b0, Bb * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     c->h2d += (int64_t)Bb * 20;
     if (fmask) {     // per-candidate feature masks (DistFeatureEliminator): masked weights stay exactly 0
@@ -274,24 +262,16 @@ int multi_score(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold
     const int Bb = (int)std::min<int64_t>(per_pass, B - b0);
     const size_t slots = (size_t)Bb * K;
     Scratch sx(c);
-    std::vector<float> h(slots * ldx + slots, 0.f);
-    for (size_t s = 0; s < slots; ++s) {
-      const float* src = coef + ((size_t)b0 * K + s) * dp;
-      memcpy(&h[s * ldx], src, d * sizeof(float));
-      h[slots * ldx + s] = src[d];
-    }
     float *dW, *Z;
     int32_t* dcode;
     unsigned long long* dconf;
     const int ldz = (int)slots;
-    SKD_CUDA(c, sx.alloc(&dW, h.size()));
+    if (pack_coef(c, sx, (int)slots, coef + (size_t)b0 * K * dp, d, ldx, &dW)) return 1;
     SKD_CUDA(c, sx.alloc(&Z, (size_t)n * ldz));
     SKD_CUDA(c, sx.alloc(&dcode, (size_t)Bb));
     SKD_CUDA(c, sx.alloc(&dconf, (size_t)Bb * KK));
-    SKD_CUDA(c, cudaMemcpyAsync(dW, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaMemcpyAsync(dcode, col_fold + b0, Bb * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaMemsetAsync(dconf, 0, (size_t)Bb * KK * sizeof(unsigned long long), c->stream));
-    c->h2d += (int64_t)h.size() * 4;
     if (simt_raw_prediction(c, (int)slots, dW, dW + slots * ldx, Z, ldz)) return 1;
     const size_t smem = KK * sizeof(unsigned int);
     if (smem <= 48 * 1024)
@@ -302,7 +282,7 @@ int multi_score(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold
     SKD_CUDA(c, cudaGetLastError());
     SKD_CUDA(c, cudaMemcpyAsync(conf_out + (size_t)b0 * KK, dconf, (size_t)Bb * KK * sizeof(int64_t),
                                 cudaMemcpyDeviceToHost, c->stream));
-    SKD_CUDA(c, cudaStreamSynchronize(c->stream));   // h is read by the async copy until here
+    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
     c->d2h += (int64_t)Bb * KK * 8;
   }
   return 0;
@@ -331,8 +311,7 @@ mn_logloss_kernel(const float* __restrict__ Z, int ldz, int64_t n, int64_t rpc, 
   unsigned long long nn = 0;
   for (int64_t r = row_begin + threadIdx.x; r < row_end; r += 256) {
     const int fd = fold ? (int)fold[r] : -1;
-    const bool test = cd == -2 || (cd >= 0 && fd == cd) || (cd <= -3 && fd != (-3 - cd));
-    if (!test) continue;
+    if (!score_code_selects(cd, fd)) continue;
     const int y = ycls[r];
     double p;
     if (K == 1) {
@@ -383,28 +362,20 @@ int logloss_batch(Ctx* c, int B, int K, const float* coef, const int32_t* col_fo
     const int Bb = (int)std::min<int64_t>(per_pass, B - b0);
     const size_t slots = (size_t)Bb * K;
     Scratch sx(c);
-    std::vector<float> h(slots * ldx + slots, 0.f);
-    for (size_t s = 0; s < slots; ++s) {
-      const float* src = coef + ((size_t)b0 * K + s) * dp;
-      memcpy(&h[s * ldx], src, d * sizeof(float));
-      h[slots * ldx + s] = src[d];
-    }
     float *dW, *Z;
     int32_t *dcode, *dpos = nullptr;
     double* dloss;
     unsigned long long* dcount;
     const int ldz = (int)slots;
-    SKD_CUDA(c, sx.alloc(&dW, h.size()));
+    if (pack_coef(c, sx, (int)slots, coef + (size_t)b0 * K * dp, d, ldx, &dW)) return 1;
     SKD_CUDA(c, sx.alloc(&Z, (size_t)n * ldz));
     SKD_CUDA(c, sx.alloc(&dcode, (size_t)Bb));
     SKD_CUDA(c, sx.alloc(&dpos, (size_t)Bb));
     SKD_CUDA(c, sx.alloc(&dloss, (size_t)nz * Bb));
     SKD_CUDA(c, sx.alloc(&dcount, (size_t)Bb));
-    SKD_CUDA(c, cudaMemcpyAsync(dW, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaMemcpyAsync(dcode, col_fold + b0, Bb * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     if (col_pos) SKD_CUDA(c, cudaMemcpyAsync(dpos, col_pos + b0, Bb * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaMemsetAsync(dcount, 0, Bb * sizeof(unsigned long long), c->stream));
-    c->h2d += (int64_t)h.size() * 4;
     if (simt_raw_prediction(c, (int)slots, dW, dW + slots * ldx, Z, ldz)) return 1;
     mn_logloss_kernel<<<dim3(Bb, nz), 256, 0, c->stream>>>(Z, ldz, n, rpc, K, Bb, dcode, dpos, c->ycls, c->fold, dloss,
                                                           dcount);

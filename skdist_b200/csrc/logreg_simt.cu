@@ -159,10 +159,7 @@ fwd_kernel(const float* __restrict__ X, int64_t n, int ldx, const float* __restr
             gout[j] = gf;
           }
         } else if (MODE == MODE_SCORE) {
-          // fold code: f >= 0 -> rows of fold f; -2 -> all rows; -3-f -> rows NOT in fold f
-          bool test = rvalid && sfold[j] != -100 &&
-                      (sfold[j] == -2 || (sfold[j] >= 0 && fd == sfold[j]) ||
-                       (sfold[j] <= -3 && fd != (-3 - sfold[j])));
+          bool test = rvalid && sfold[j] != -100 && score_code_selects(sfold[j], fd);
           if (test) {
             bool pred = raw > 0.f;
             bool y = (yc == spos[j]);
@@ -170,9 +167,7 @@ fwd_kernel(const float* __restrict__ X, int64_t n, int ldx, const float* __restr
             acc_n[j] += 1;
           }
         } else if (MODE == MODE_R2) {
-          bool test = rvalid && sfold[j] != -100 &&
-                      (sfold[j] == -2 || (sfold[j] >= 0 && fd == sfold[j]) ||
-                       (sfold[j] <= -3 && fd != (-3 - sfold[j])));
+          bool test = rvalid && sfold[j] != -100 && score_code_selects(sfold[j], fd);
           if (test) {
             double r = (double)yr - (double)raw;
             acc_loss[j] += r * r;

@@ -217,7 +217,6 @@ struct TcParams {
   const uint32_t* ybits;     // TC_FIT: per-column row label bits (nullptr: class id == pos), see LogregWork
   const uint32_t* mbits;     // TC_FIT: per-column training-row bits (nullptr: every row of the training folds)
   long long rb_words;
-  int g_passes;              // MMA passes of the gradient product: 3 = G_hi X_hi + G_lo X_hi + G_hi X_lo, 2 = without G_lo X_hi
   int32_t* deal_log;         // nullptr, or {live groups, groups whose second half is padding, CTAs, CTAs whose
                              // range spans two or more groups} of this launch (the last entry zeroed by the caller)
   const float2* cw;          // TC_FIT_W / TC_FIT_UNI_W: per-column {label-0, label-1} class weights, largest <= 1
@@ -430,7 +429,6 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
   const uint64_t desc_mn = make_desc(smem_u32(s_ring), SM::X_CHUNK, 1024);    // X as MN-major (GEMM2)
   constexpr uint32_t WL_OFF = (NCHUNK * SM::W_CHUNK) >> 4;
   constexpr uint32_t XL_OFF = (NCHUNK * SM::X_CHUNK) >> 4;
-  const bool g3 = prm.g_passes >= 3;
 
   uint32_t h = 0;          // running sub-tile counter (ring position), identical in both consumers
   int w_loads = 0, g_prev = -1;
@@ -515,15 +513,15 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
     };
     // GEMM2 of a sub-tile: dW += G_hi X_hi + G_lo X_hi + G_hi X_lo   [64 slots x dpad per warpgroup],
     // one batch with every A fragment formed beforehand
-    auto gemm2 = [&](const uint32_t (&ahi)[2][4], const uint32_t (&alo)[2][4], uint32_t stage, bool three) {
+    auto gemm2 = [&](const uint32_t (&ahi)[2][4], const uint32_t (&alo)[2][4], uint32_t stage) {
       if constexpr (IS_FIT) {
         const uint64_t bm = desc_mn + (uint64_t)((stage * SM::STAGE) >> 4);
         const uint64_t bh0 = bm, bh1 = bm + (uint64_t)((16 * 128) >> 4);
         wgmma_grad<NCHUNK>(grad, ahi[0], bh0);
-        if (three) wgmma_grad<NCHUNK>(grad, alo[0], bh0);
+        wgmma_grad<NCHUNK>(grad, alo[0], bh0);
         wgmma_grad<NCHUNK>(grad, ahi[0], bh0 + XL_OFF);
         wgmma_grad<NCHUNK>(grad, ahi[1], bh1);
-        if (three) wgmma_grad<NCHUNK>(grad, alo[1], bh1);
+        wgmma_grad<NCHUNK>(grad, alo[1], bh1);
         wgmma_grad<NCHUNK>(grad, ahi[1], bh1 + XL_OFF);
         wgmma_commit();
       }
@@ -548,8 +546,7 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
       // straight-line issue in every branch (no control flow between a wgmma_fence and its products,
       // so ptxas needs no warpgroup.arrive between the instructions)
       if (IS_FIT && j > 0) {
-        if (g3) { wgmma_fence(); gemm1(zf, slu); gemm2(pa, pl, psl, true); }
-        else { wgmma_fence(); gemm1(zf, slu); gemm2(pa, pl, psl, false); }
+        wgmma_fence(); gemm1(zf, slu); gemm2(pa, pl, psl);
       } else {
         wgmma_fence(); gemm1(zf, slu);
       }
@@ -660,9 +657,7 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
           const uint32_t m = rm[rr];
           const float zv = fmaf(zf[i], zi[s], zb0[s]);
           const int fr = (int)(m >> 24);
-          // fold code: f >= 0 rows of fold f; -2 all rows; -3-f rows NOT in fold f
-          const bool in = (fr != 0xFF) && (sp[s].fold == -2 || (sp[s].fold >= 0 && fr == sp[s].fold) ||
-                                           (sp[s].fold <= -3 && fr != (-3 - sp[s].fold)));
+          const bool in = (fr != 0xFF) && score_code_selects(sp[s].fold, fr);
           if (MODE == TC_R2) {
             const float r = yv[rr] - zv;
             if (in) two_sum_add(ls_hi[s], ls_lo[s], r * r);
@@ -679,8 +674,7 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
     if constexpr (IS_FIT) {   // the item's last GEMM2 (nsub >= 2: empty chunks are skipped)
       reg_fence(grad);
       turn_begin();
-      if (g3) { wgmma_fence(); gemm2(pa, pl, psl, true); }
-      else { wgmma_fence(); gemm2(pa, pl, psl, false); }
+      wgmma_fence(); gemm2(pa, pl, psl);
       turn_end();
       wgmma_wait_all();
       reg_fence(grad);
@@ -948,7 +942,6 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
   prm.groups = groups;
   prm.n_tiles = n_tiles;
   prm.ldw = w.ldw;
-  { const char* gp = getenv("SKDIST_B200_TC_GPASSES"); prm.g_passes = gp ? atoi(gp) : 3; }
   prm.ybits = mode == TC_FIT ? w.ybits : nullptr;
   prm.mbits = mode == TC_FIT ? w.mbits : nullptr;
   prm.rb_words = w.rb_words;

@@ -66,6 +66,33 @@ struct SkdTreeView {
 };
 typedef void (*ForestSink)(void* arg, int tree_index, const SkdTreeView* view);
 
+// Scoring codes: the per-column col_fold of the scoring entries.  f >= 0 selects the rows of fold f, -2
+// every row, -3 - f the rows outside fold f; -1 is not a code.  row_fold is -1 when no folds are staged.
+__host__ __device__ __forceinline__ bool score_code_selects(int code, int row_fold) {
+  return code == -2 || (code >= 0 && row_fold == code) || (code <= -3 && row_fold != (-3 - code));
+}
+// the fold a scoring code names (-1: none)
+__host__ __device__ __forceinline__ int score_code_fold(int code) {
+  return code >= 0 ? code : (code <= -3 ? -3 - code : -1);
+}
+
+// One-shot inputs staged for the next call that reads them.  That call takes them off the context
+// (std::exchange) before any check, so they never outlive it, whether it succeeds or fails.
+struct StagedMasks {          // skd_stage_column_masks: per-column feature masks [cols x d]
+  std::vector<uint8_t> mask;
+  int32_t cols = 0;
+};
+struct StagedRowBits {        // skd_stage_row_bits: label of row r in column j / row r trains column j,
+  std::vector<uint32_t> y, m; // packed little-endian, `words` 32-bit words per column
+  int32_t cols = 0;
+  int64_t words = 0;
+};
+struct StagedClassWeights {   // skd_stage_class_weights: w [cols x k] weight of each class (binary calls:
+  std::vector<float> w;       // label 0, label 1), sw_sum [cols] the sum of the column's per-row weights
+  std::vector<double> sw_sum; // over its training rows
+  int32_t cols = 0, k = 0;
+};
+
 struct Ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -89,21 +116,12 @@ struct Ctx {
   ForestData forest;
   int64_t ycls_cap = 0, yreal_cap = 0, fold_cap = 0;   // allocated rows of the staged vectors (reused when large enough)
   int64_t vec_n = 0;        // row count the staged labels / targets / folds belong to (dropped when X changes it)
-  // per-column feature masks staged for the next skd_logreg_fit_batch (skd_stage_column_masks)
-  std::vector<uint8_t> h_fmask;
-  int32_t fmask_cols = 0;
-  // per-column row bit matrices staged for the next skd_logreg_fit_batch (skd_stage_row_bits):
-  // label of row r in column j / row r trains column j; packed little-endian, rb_words 32-bit words per column
-  std::vector<uint32_t> h_ybits, h_mbits;
-  int32_t rb_cols = 0;
-  int64_t rb_words = 0;
-  // per-column class weights staged for the next fit / loss-gradient call (skd_stage_class_weights):
-  // h_cw [cw_cols x cw_k] weight of each class (binary calls: label 0, label 1), h_swsum [cw_cols] the
-  // sum of the column's per-row weights over its training rows
-  std::vector<float> h_cw;
-  std::vector<double> h_swsum;
-  int32_t cw_cols = 0, cw_k = 0;
-  // class weights for the next forest fit (skd_stage_forest_class_weights; n_classes == 0: none)
+  // one-shot staged inputs: read by skd_logreg_fit_batch (all three), skd_logreg_loss_grad (class
+  // weights), skd_logreg_multinomial_fit_batch (masks, class weights) and skd_forest_fit (forest_cw,
+  // n_classes == 0: none)
+  StagedMasks fmask;
+  StagedRowBits row_bits;
+  StagedClassWeights cw;
   ForestClassWeights forest_cw;
   // scratch pool: device blocks released by finished calls, reused by the next ones (Scratch below)
   std::vector<std::pair<void*, size_t>> pool_free;
@@ -280,6 +298,8 @@ int forest_predict_device(Ctx* c, const float* dX, int64_t m, int ldx, int n_tre
                           const void* d_node, const double* d_thr, const double* d_val, int C, double* d_out);
 int ridge_fit_batch(Ctx* c, int B, const double* alpha, const int32_t* hold, int fit_intercept,
                     float* coef_out, int32_t* status_out);
+// Caller coefficients [rows x (d+1)] to the kernel layout on the device: weights [rows x ldx], then bias [rows]
+int pack_coef(Ctx* c, Scratch& sx, int rows, const float* coef, int64_t d, int64_t ldx, float** dW);
 
 // ---- multinomial logistic regression (logreg_multi.cu / lbfgs_dev.cu) -------------------
 // One optimiser problem per candidate with K * (d + 1) variables, variable (k, j) at k * dp + j;
@@ -308,9 +328,9 @@ struct MultiWork {
 int multi_lbfgs_init(Ctx* c, MultiWork& w, const int32_t* d_col_fold, double tol, int max_iter);
 int multi_lbfgs_enqueue(Ctx* c, MultiWork& w, int n_act_in, int fit_intercept, int32_t* hist);
 int multi_lbfgs_finish(Ctx* c, MultiWork& w, float* dcoef, int32_t* dniter, int32_t* dstatus, double* dloss);
-int multi_fit(Ctx* c, int B, int K, const double* C, const int32_t* col_fold, int fit_intercept, double tol,
-              int max_iter, const uint8_t* fmask /*[B x d] or nullptr*/,
-              const float* cw /*[B x K] or nullptr*/, const double* sw_sum /*[B] or nullptr*/, float* coef_out, int32_t* n_iter_out,
+int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold, int fit_intercept,
+              double tol, int max_iter, const uint8_t* fmask /*[B x d] or nullptr*/,
+              const float* cw /*[B x K] or nullptr*/, float* coef_out, int32_t* n_iter_out,
               int32_t* status_out, double* loss_out, int32_t* n_evals_out);
 int multi_score(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold, int64_t* conf_out);
 int logloss_batch(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold, const int32_t* col_pos,
@@ -322,7 +342,6 @@ int simt_backward(Ctx* c, const float* G, int ldg, int n_slots, int nz, int64_t 
 // ROC-AUC counts of linear binary classifiers (auc.cu): 2U, n_pos, n_neg per column
 int auc_batch(Ctx* c, int B, const float* coef, const int32_t* col_fold, const int32_t* col_pos, int64_t* u2_out,
               int64_t* n_pos_out, int64_t* n_neg_out);
-int simt_decision(Ctx* c, int B, const float* dW, float* dout);
 
 // tensor-core evaluation (logreg_tc.cu)
 bool tc_supported(const Ctx* c);

@@ -29,6 +29,12 @@ def _fold_ids(cv_splitted, n_samples):
     return fold
 
 
+def _train_codes(fold):
+    """Scoring codes of the device scoring calls that select the training rows of every column (the rows
+    outside its held-out fold `fold`): -3 - fold, as int32."""
+    return (-3 - fold).astype(np.int32)
+
+
 class _TargetCodes:
     """One hash pass over a 1-d integer / bool target: `codes` numbers the classes by order of first
     appearance (what StratifiedKFold's `_make_test_folds` works on), `classes` are the sorted labels and

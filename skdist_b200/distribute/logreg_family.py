@@ -15,7 +15,7 @@ import numpy as np
 
 from .. import parallel
 from .base import _clone, _merged_params
-from .folds import _classes_and_ids
+from .folds import _classes_and_ids, _train_codes
 
 _LOGREG_SEARCHABLE = {"C", "tol", "max_iter", "fit_intercept", "class_weight"}
 
@@ -330,7 +330,7 @@ class _LogRegFamily:
             out["n_iter"][idx] = res["n_iter"]
             out["status"][idx] = res["status"]
             if return_train_score:
-                vals, _ = self._scores(eng, res["coef"], (-3 - fold[idx]).astype(np.int32), pos,
+                vals, _ = self._scores(eng, res["coef"], _train_codes(fold[idx]), pos,
                                        self.total_pos - self.pos_in_fold[fold[idx]])
                 for name, v in vals.items():
                     v = np.asarray(v, dtype=np.float64).copy()
@@ -449,10 +449,10 @@ class _MultinomialFamily(_LogRegFamily):
             out["n_iter"][idx] = res["n_iter"]
             out["status"][idx] = res["status"]
             if return_train_score:
-                conf = eng.multinomial_confusion_batch(res["coef"], (-3 - fold[idx]).astype(np.int32))
+                train = _train_codes(fold[idx])
+                conf = eng.multinomial_confusion_batch(res["coef"], train)
                 for name, (kind, average) in self.metrics.items():
-                    out["train_%s" % name][idx] = self._metric(eng, kind, average, conf, res["coef"],
-                                                               (-3 - fold[idx]).astype(np.int32))
+                    out["train_%s" % name][idx] = self._metric(eng, kind, average, conf, res["coef"], train)
         return out
 
     @staticmethod

@@ -11,6 +11,7 @@ import numpy as np
 
 from .. import parallel
 from .base import _clone, _merged_params
+from .folds import _train_codes
 
 _RIDGE_SEARCHABLE = {"alpha", "fit_intercept"}
 
@@ -134,7 +135,7 @@ class _RidgeFamily:
             out["score_time"][idx] = (t2 - t1) / len(idx)
             out["status"][idx] = res["status"]
             if return_train_score:
-                sse2, n2 = eng.linear_r2_batch(res["coef"], (-3 - fold[idx]).astype(np.int32))
+                sse2, n2 = eng.linear_r2_batch(res["coef"], _train_codes(fold[idx]))
                 for name, kind in self.metrics.items():
                     out["train_%s" % name][idx] = self._metric(kind, sse2, n2, self.sst_train[fold[idx]])
         return out

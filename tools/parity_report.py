@@ -1,7 +1,7 @@
 """Predictions that differ from the reference (`flips` per held-out fold) on every logistic fixture,
 for the fp32 CUDA-core kernels and for the tensor-core kernel separately, next to the reference's own
 run-to-run envelope stored with the fixture.  One JSON line per (fixture, kernel); DESIGN.md section 4
-quotes them.   python tools/parity_report.py [--gpasses 2]"""
+quotes them.   python tools/parity_report.py"""
 import json, os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -27,8 +27,7 @@ for name in ["search_logreg_g1_4000x16", "search_logreg_g1_20000x64", "search_lo
         flips = np.abs(correct - np.rint(gold * count))
         rel = np.abs(res["coef"] - gc).max(1) / np.abs(gc).max(1)
         mean = np.average((correct / count).reshape(len(Cs), cv), axis=1, weights=count[:cv])
-        print(json.dumps({"fixture": name, "kernel": kname, "gpasses": os.environ.get("SKDIST_B200_TC_GPASSES", "3"),
-                          "test_rows_per_fold": int(count[0]), "columns": len(C),
+        print(json.dumps({"fixture": name, "kernel": kname, "test_rows_per_fold": int(count[0]), "columns": len(C),
                           "flips_max": int(flips.max()), "flips_mean": float(flips.mean()),
                           "reference_envelope_flips_max": int(nf.max()), "reference_envelope_flips_mean": float(nf.mean()),
                           "excess_over_envelope_max": int(np.max(flips - nf)), "columns_above_envelope": int(np.sum(flips > nf)),
