@@ -228,12 +228,16 @@ int skd_bootstrap_counts(int32_t n_trees, const uint32_t* seeds, int64_t n, int3
                          uint8_t* counts_out, uint32_t* rand_r_out, int32_t n_threads);
 
 /* Forest classifier trees, one persistent CTA per tree (depth-first, exact scikit-learn
- * splitter semantics on <= 256 distinct values per feature).  sample_counts[t*n + i] is the
+ * splitter semantics).  sample_counts[t*n + i] is the
  * bootstrap multiplicity of row i in tree t (the reference's sample_weight, uint8; NULL = no
  * bootstrap, every row once), rand_states[t] the splitter's xorshift seed; both are derived by the
- * host exactly as the reference does.  splitter: 0 = best split of the drawn features
- * (RandomForest, SK/tree/_splitter.pyx:262-504), 1 = one uniformly drawn threshold per drawn
- * feature (ExtraTrees, node_split_random :507-736).
+ * host exactly as the reference does.  splitter:
+ *   0 = best split of the drawn features (RandomForest, SK/tree/_splitter.pyx:262-504) on per-feature
+ *       value histograms: every feature must have <= 256 distinct values, else the call fails;
+ *   1 = one uniformly drawn threshold per drawn feature (ExtraTrees, node_split_random :507-736),
+ *       any finite values;
+ *   2 = as 0, and a feature with more than 256 distinct values is split by sorting the node's raw
+ *       float32 values (the same trees; when every feature has <= 256 distinct values, exactly 0).
  * Trees come back through an opaque handle: sizes first, then caller-allocated arrays.
  * ref: replaces n_trees invocations of ensemble.py:68-109 (_build_trees -> tree.fit):
  * SK/tree/_tree.pyx:139-337, SK/tree/_splitter.pyx:262-504, SK/tree/_criterion.pyx:605-680. */

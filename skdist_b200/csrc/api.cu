@@ -1367,7 +1367,7 @@ int skd_forest_fit(skd_ctx* ctx, int32_t n_trees, const uint8_t* sample_counts, 
   *out = nullptr;
   if (!c->X || (!y_regression && !c->ycls)) return fail(c, "skd_forest_fit: stage X and labels first");
   if (n_trees <= 0 || !rand_states || max_features < 1 || min_samples_split < 2 || min_samples_leaf < 1 ||
-      splitter < 0 || splitter > 1)
+      splitter < 0 || splitter > 2)
     return fail(c, "skd_forest_fit: bad arguments");
   SKD_CUDA(c, cudaSetDevice(c->device));
   std::unique_ptr<skd_forest> f(new skd_forest());
@@ -1376,7 +1376,7 @@ int skd_forest_fit(skd_ctx* ctx, int32_t n_trees, const uint8_t* sample_counts, 
   DeviceTimer timer(c);
   if (timer.start()) return 1;
   if (forest_fit(c, n_trees, sample_counts, rand_states, n_classes, max_features, max_depth, min_samples_split,
-                 min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter, y_regression,
+                 min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter == 1, splitter == 2, y_regression,
                  cw.n_classes ? &cw : nullptr, forest_sink, f.get()))
     return 1;
   f->binval = c->forest.h_binval;

@@ -16,8 +16,11 @@
 // RNG consumption and therefore every later draw are bit-identical to scikit-learn's.
 // The random splitter (node_split_random, ExtraTrees) uses the same histograms when every feature has
 // codes, and otherwise reads the raw float32 values (min / max pass, drawn threshold, left-side pass),
-// so it takes continuous features.
+// so it takes continuous features.  The best splitter on features without codes (splitter 2) sorts the
+// node's raw values per drawn feature -- a CTA radix sort in shared memory for small nodes, an LSD radix
+// sort in per-tree global scratch for large ones -- and scans the sorted order as the reference does.
 // No tensor cores: the work is integer histogramming, bound by gather bandwidth / latency.
+#include <cub/block/block_radix_sort.cuh>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -91,6 +94,17 @@ struct FoParams {
   int cw_bs;
   const double* cw;
   double min_weight_fraction;
+  // sort-based best splitter (FO_SORT): [slots][2][n] ping-pong (key, node position) buffers of the
+  // large-node radix sort, else nullptr
+  uint2* srt;
+};
+
+// What the general builder reads for a split (one kernel instantiation each, so that the histogram
+// instantiations keep their register allocation)
+enum FoMode : int {
+  FO_HIST = 0,   // bin codes and per-feature value histograms (best and random splitter)
+  FO_RAW = 1,    // random splitter over the raw float32 values (P.xval)
+  FO_SORT = 2,   // best splitter over the raw float32 values: sort the node's values, scan the runs
 };
 
 __device__ __forceinline__ uint32_t fo_rand_r(uint32_t* seed) {   // SK/utils/_random.pxd:20-34
@@ -170,9 +184,272 @@ __device__ __forceinline__ void fo_children_mse(const unsigned long long* sl, co
 // counts; the float64 statistics are w_c * count (one rounding), in scikit-learn's operation order.
 #define FO_TICK(ph) do { if (P.o_prof && tid == 0) { const long long _t = clock64(); prof[ph] += _t - tlast; tlast = _t; } } while (0)
 #define FOR_C(c) _Pragma("unroll") for (int c = 0; c < CM; ++c) if (c < C)
-// RAW: random splitter over the raw values (P.xval), a separate instantiation so that the histogram
-// instantiations keep their register allocation.
-template <int CM, bool REG, bool W, bool RAW>
+// ---------------- FO_SORT: node_split_best over the raw float32 values of one feature ----------------
+// (SK/tree/_splitter.pyx:262-504 with DensePartitioner.sort_samples_and_feature_values and next_p,
+// SK/tree/_partitioner.pyx:100-108, 209-215).  The node's values are sorted as order-preserving uint32
+// keys; only the bits below the highest bit in which the node's min and max keys differ take part, so
+// deep nodes with narrow value ranges need fewer radix passes.  Equal keys keep their node order
+// (both sorts are stable); the reference's introsort does not, but every statistic is a sum over a run
+// of equal values, so the candidates and their left sides are the same.
+constexpr int FO_SORT_IPT = 16;                         // sorted elements per thread and scan tile
+constexpr int FO_SORT_S = FO_THREADS * FO_SORT_IPT;     // S = 4096: nodes of up to S samples sort in shared memory
+using FoBlockSort = cub::BlockRadixSort<uint32_t, FO_THREADS, FO_SORT_IPT, int>;
+static_assert(sizeof(FoBlockSort::TempStorage) <= FO_HIST_WORDS * 4, "the CTA sort lives in the histogram words");
+static_assert(FO_MAXC * FO_THREADS * 2 <= FO_HIST_WORDS, "the scan's per-thread prefixes live in the histogram words");
+
+// order-preserving uint32 image of a float32; -0.0 maps to +0.0's key (equal values, one run)
+__device__ __forceinline__ uint32_t fo_fkey(float x) {
+  uint32_t u = __float_as_uint(x);
+  if (u == 0x80000000u) u = 0;
+  return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
+}
+__device__ __forceinline__ float fo_kval(uint32_t k) { return __uint_as_float(k ^ ((k >> 31) ? 0x80000000u : 0xFFFFFFFFu)); }
+
+// Proxy of the split whose left child has the statistics sl (the node: st, w_node), with the left and
+// right impurities; -inf when a child is lighter than min_weight_leaf.  The histogram scan's float64
+// operations, in the same order.
+template <int CM, bool REG, bool W>
+__device__ __forceinline__ double fo_split_proxy(const unsigned long long* sl, const unsigned long long* st,
+                                                 const double* cw, int C, double w_node, double mwl,
+                                                 double* il, double* ir) {
+  double wl = 0.0;
+  if constexpr (REG) wl = st_d(sl[0]);
+  else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(cw[c], (double)sl[c])); }
+  else { FOR_C(c) wl += (double)sl[c]; }
+  const double wr = w_node - wl;
+  if (wl < mwl || wr < mwl) return -INFINITY;
+  if constexpr (REG) {
+    fo_children_mse(sl, st, wl, wr, il, ir);
+    const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(st[1]), sum_l);
+    return __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
+  } else if constexpr (W) {
+    fo_children_impurity_w<CM>(sl, st, cw, C, wl, wr, il, ir);
+    return __dsub_rn(__dmul_rn(-wr, *ir), __dmul_rn(wl, *il));
+  } else {
+    fo_children_impurity<CM>(sl, st, C, wl, wr, il, ir);
+    return __dsub_rn(__dmul_rn(-wr, *ir), __dmul_rn(wl, *il));
+  }
+}
+
+// Best split of one non-constant feature (values col[samp[i].x], node positions start .. start+m-1,
+// min lo < max hi) into *R, filled as the histogram scan fills it.  Called by the whole block; hist is
+// free on entry and is overwritten.  bufA / bufB: this tree's two [n] scratch buffers.
+template <int CM, bool REG, bool W>
+__device__ void fo_sort_split(const FoParams& P, const uint2* __restrict__ samp, const float* __restrict__ col,
+                              uint2* bufA, uint2* bufB, unsigned int* hist, int start, int m, float lo, float hi,
+                              const unsigned long long* st, const double* cw, double w_node, double mwl,
+                              FoResult* R) {
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int C = REG ? 3 : P.n_classes;
+  __shared__ unsigned long long s_wt[FO_THREADS / 32][FO_MAXC];   // per-warp statistics of a scan tile
+  __shared__ unsigned long long s_carry[FO_MAXC];                 // statistics of the earlier tiles
+  __shared__ uint32_t s_first[FO_THREADS / 32 + 1];               // first key of each warp's elements, then of the next tile
+  __shared__ double s_amp[FO_THREADS / 32];                       // per-warp best proxy ...
+  __shared__ int s_amq[FO_THREADS / 32];                          // ... and its split position
+  __shared__ unsigned s_ws[FO_THREADS / 32];
+
+  const uint32_t kmin = fo_fkey(lo), kmax = fo_fkey(hi);
+  const int nbits = 32 - __clz(kmin ^ kmax);       // >= 1: the keys of min and max differ
+  const uint32_t mask = nbits == 32 ? 0xFFFFFFFFu : (1u << nbits) - 1u;
+  const uint32_t hib = kmin & ~mask;               // the bits every key of the node shares
+  uint32_t key[FO_SORT_IPT];
+  int pos[FO_SORT_IPT];
+  const uint2* srt = nullptr;                      // large nodes: the sorted (key, node position) pairs
+  __syncthreads();                                 // hist and the state above are free (earlier feature)
+  if (tid == 0) { R->is_const = 0; R->proxy = -INFINITY; R->pos = start + m; R->bin = -1; }
+  if (tid < FO_MAXC) s_carry[tid] = 0;
+  if (m <= FO_SORT_S) {
+    // ---- small node: one CTA radix sort of (key, position) in registers, blocked arrangement ----
+#pragma unroll
+    for (int j = 0; j < FO_SORT_IPT; ++j) {
+      const int e = tid * FO_SORT_IPT + j;
+      pos[j] = e;
+      key[j] = e < m ? fo_fkey(__ldg(col + samp[start + e].x)) & mask : mask;   // padding sorts after every key
+    }
+    FoBlockSort(*reinterpret_cast<typename FoBlockSort::TempStorage*>(hist)).Sort(key, pos, 0, nbits);
+    __syncthreads();
+  } else {
+    // ---- large node: LSD radix sort, 8-bit digits, ping-pong between bufB and bufA ----
+    uint16_t* wcnt = reinterpret_cast<uint16_t*>(hist);   // [32 rows][256 digits] element counts of a tile's rows
+    uint16_t* woff = wcnt + 32 * 256;                     // [32][256] their offsets within the tile's digit
+    unsigned* dcnt = hist + 32 * 256;                     // [4 passes][256] digit counts of the node
+    unsigned* s_tb = dcnt + 4 * 256;                      // [256] where the tile's elements of a digit start
+    const int npass = (nbits + 7) / 8;
+    for (int i = tid; i < 32 * 256 / 2; i += FO_THREADS) hist[i] = 0;
+    for (int i = tid; i < 4 * 256; i += FO_THREADS) dcnt[i] = 0;
+    __syncthreads();
+    for (int i = tid; i < m; i += FO_THREADS) {   // keys in node order, and the digit counts of every pass
+      const uint32_t k = fo_fkey(__ldg(col + samp[start + i].x)) & mask;
+      bufB[i] = make_uint2(k, (unsigned)i);
+      for (int p = 0; p < npass; ++p) atomicAdd(&dcnt[p * 256 + ((k >> (8 * p)) & 255)], 1u);
+    }
+    const uint2* src = bufB;
+    uint2* dst = bufA;
+    for (int p = 0; p < npass; ++p) {
+      __syncthreads();
+      // thread t: where digit t starts (exclusive scan of the counts)
+      const unsigned c0 = dcnt[p * 256 + tid];
+      unsigned incl = c0;
+      for (int o = 1; o < 32; o <<= 1) { const unsigned v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+      if (lane == 31) s_ws[wid] = incl;
+      __syncthreads();
+      unsigned gb = incl - c0;
+      for (int w = 0; w < wid; ++w) gb += s_ws[w];
+      const int sh = 8 * p;
+      // stable scatter: tiles of 4 x 256 elements in order; an element's rank among the equal digits of
+      // its warp row comes from __match_any_sync, the rows are counted and offset in element order
+      for (int t0 = 0; t0 < m; t0 += 4 * FO_THREADS) {
+        uint2 u[4];
+        unsigned dg[4], rk[4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const int e = t0 + r * FO_THREADS + tid;
+          const bool ok = e < m;
+          u[r] = ok ? src[e] : make_uint2(0, 0);
+          dg[r] = ok ? (u[r].x >> sh) & 255 : 0xFFFFu;
+          const unsigned peers = __match_any_sync(0xffffffffu, dg[r]);
+          rk[r] = __popc(peers & ((1u << lane) - 1u));
+          if (ok && rk[r] == 0) wcnt[(r * 8 + wid) * 256 + dg[r]] = (uint16_t)__popc(peers);
+        }
+        __syncthreads();
+        {
+          unsigned acc = 0;
+          for (int row = 0; row < 32; ++row) {
+            const unsigned cnt = wcnt[row * 256 + tid];
+            wcnt[row * 256 + tid] = 0;            // cleared for the next tile
+            woff[row * 256 + tid] = (uint16_t)acc;
+            acc += cnt;
+          }
+          s_tb[tid] = gb;
+          gb += acc;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+          if (t0 + r * FO_THREADS + tid < m) dst[s_tb[dg[r]] + woff[(r * 8 + wid) * 256 + dg[r]] + rk[r]] = u[r];
+      }
+      uint2* t = const_cast<uint2*>(src);
+      src = dst;
+      dst = t;
+    }
+    __syncthreads();
+    srt = src;
+  }
+
+  // ---- scan the sorted order in tiles of S elements, FO_SORT_IPT consecutive ones per thread ----
+  // Left-side statistics are prefix sums in a fixed order (thread, warp, tiles): no float atomics.
+  // A candidate follows element e when the next value exceeds v[e] + 1e-7 in float32 (next_p).
+  unsigned long long* s_ex = reinterpret_cast<unsigned long long*>(hist);   // [c][thread] statistics before a thread's elements
+  auto add = [&](unsigned long long* a, int p) {   // statistics of the sample at node position p
+    const uint2 sv = samp[start + p];
+    const unsigned wgt = sv.y >> 8;
+    if constexpr (REG) {
+      const double yv = __ldg(P.yreal + sv.x), wy = __dmul_rn((double)wgt, yv);
+      a[0] = d_st(__dadd_rn(st_d(a[0]), (double)wgt));
+      a[1] = d_st(__dadd_rn(st_d(a[1]), wy));
+      a[2] = d_st(__dadd_rn(st_d(a[2]), __dmul_rn(wy, yv)));
+    } else {
+      const int cls = (int)(sv.y & 0xFF);
+      FOR_C(c) if (cls == c) a[c] += wgt;
+    }
+  };
+  double run_bp = -INFINITY;   // best proxy of the earlier tiles (the same in every thread)
+  for (int t0 = 0; t0 < m; t0 += FO_SORT_S) {
+    const int e0 = t0 + tid * FO_SORT_IPT;   // this thread's first element
+    if (srt) {
+#pragma unroll
+      for (int j = 0; j < FO_SORT_IPT; ++j) {
+        const int e = e0 + j;
+        const uint2 u = e < m ? srt[e] : make_uint2(mask, 0);
+        key[j] = u.x; pos[j] = (int)u.y;
+      }
+    }
+    unsigned long long sl[CM];
+#pragma unroll
+    for (int c = 0; c < CM; ++c) sl[c] = 0;
+#pragma unroll
+    for (int j = 0; j < FO_SORT_IPT; ++j) if (e0 + j < m) add(sl, pos[j]);
+    FOR_C(c) {   // exclusive prefix over the warp
+      unsigned long long incl = sl[c];
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl = st_add<REG>(v, incl);
+      }
+      if (lane == 31) s_wt[wid][c] = incl;
+      const unsigned long long up = __shfl_up_sync(0xffffffffu, incl, 1);
+      sl[c] = lane > 0 ? up : 0ull;
+    }
+    if (lane == 0) s_first[wid] = key[0];
+    if (tid == 0) s_first[FO_THREADS / 32] = t0 + FO_SORT_S < m ? srt[t0 + FO_SORT_S].x : 0u;
+    __syncthreads();
+    unsigned long long carry_next = 0;   // thread c < C: the carry of the next tile
+    if (tid < C) {
+      carry_next = s_carry[tid];
+      for (int w = 0; w < FO_THREADS / 32; ++w) carry_next = st_add<REG>(carry_next, s_wt[w][tid]);
+    }
+    FOR_C(c) {
+      unsigned long long pre = s_carry[c];
+      for (int w = 0; w < wid; ++w) pre = st_add<REG>(pre, s_wt[w][c]);
+      sl[c] = st_add<REG>(pre, sl[c]);
+      s_ex[c * FO_THREADS + tid] = sl[c];
+    }
+    const uint32_t nk_lane = __shfl_down_sync(0xffffffffu, key[0], 1);
+    const uint32_t nk_last = lane < 31 ? nk_lane : s_first[wid + 1];   // key after this thread's last element
+    double bp = -INFINITY;
+    int bj = -1;
+    uint32_t bk = 0, bnk = 0;
+#pragma unroll
+    for (int j = 0; j < FO_SORT_IPT; ++j) {
+      const int e = e0 + j;
+      if (e + 1 < m) {   // the last element has no split after it
+        add(sl, pos[j]);
+        const uint32_t nk = j + 1 < FO_SORT_IPT ? key[j + 1] : nk_last;
+        const int n_left = e + 1;
+        if (fo_kval(hib | nk) > fo_kval(hib | key[j]) + FEATURE_THRESHOLD &&
+            n_left >= P.min_samples_leaf && m - n_left >= P.min_samples_leaf) {
+          double il, ir;
+          const double proxy = fo_split_proxy<CM, REG, W>(sl, st, cw, C, w_node, mwl, &il, &ir);
+          if (proxy > bp) { bp = proxy; bj = j; bk = key[j]; bnk = nk; }
+        }
+      }
+    }
+    // block arg-max: larger proxy, then smaller position (the sequential scan's strict '>')
+    const int myq = bj >= 0 ? e0 + bj + 1 : 0x7fffffff;
+    double wp = bp;
+    int wq = myq;
+    for (int o = 16; o > 0; o >>= 1) {
+      const double op = __shfl_xor_sync(0xffffffffu, wp, o);
+      const int oq = __shfl_xor_sync(0xffffffffu, wq, o);
+      if (op > wp || (op == wp && oq < wq)) { wp = op; wq = oq; }
+    }
+    if (lane == 0) { s_amp[wid] = wp; s_amq[wid] = wq; }
+    __syncthreads();
+    if (tid < C) s_carry[tid] = carry_next;
+    double gp = s_amp[0];
+    int gq = s_amq[0];
+    for (int w = 1; w < FO_THREADS / 32; ++w)
+      if (s_amp[w] > gp || (s_amp[w] == gp && s_amq[w] < gq)) { gp = s_amp[w]; gq = s_amq[w]; }
+    if (gp > run_bp) {   // later tiles hold larger positions: strictly better only
+      run_bp = gp;
+      if (myq == gq) {   // the one thread holding the winner: its left statistics again, then *R
+        unsigned long long a[CM];
+        FOR_C(c) a[c] = s_ex[c * FO_THREADS + tid];
+#pragma unroll
+        for (int j = 0; j < FO_SORT_IPT; ++j) if (j <= bj) add(a, pos[j]);
+        double il, ir;
+        R->proxy = fo_split_proxy<CM, REG, W>(a, st, cw, C, w_node, mwl, &il, &ir);
+        R->pos = start + gq; R->il = il; R->ir = ir;
+        R->thr = (double)fo_kval(hib | bk) / 2.0 + (double)fo_kval(hib | bnk) / 2.0;
+        FOR_C(c) R->sl[c] = a[c];
+      }
+    }
+  }
+}
+
+// MODE (FoMode): FO_HIST reads bin codes; FO_RAW (random splitter) and FO_SORT (best splitter) read the
+// raw values (P.xval).  Each is a separate instantiation so that the histogram instantiations keep their
+// register allocation.
+template <int CM, bool REG, bool W, int MODE>
 __global__ void __launch_bounds__(FO_THREADS)
 forest_build_kernel(const FoParams P) {
   static_assert(!(REG && W), "class weights are a classification feature");
@@ -211,7 +488,8 @@ forest_build_kernel(const FoParams P) {
   // histogram words per feature: classification [C][256] u32 weights + [256] counts; regression
   // [3][256] float64 statistics + [256] counts
   const int hstride = REG ? (3 * 2 + 1) * FO_BINS : (C + 1) * FO_BINS;
-  const int KB = min(FO_KB_MAX, FO_HIST_WORDS / hstride);
+  // (FO_SORT sorts the batch features one after another and keeps nothing per feature in hist)
+  const int KB = MODE == FO_SORT ? FO_KB_MAX : min(FO_KB_MAX, FO_HIST_WORDS / hstride);
 
   // ---- initialise the tree: samples with non-zero weight in ascending order (Splitter.init) ----
   __shared__ int base_s;
@@ -386,7 +664,7 @@ forest_build_kernel(const FoParams P) {
           // keep the simulated end state for the no-rollback case
           s_ctrl[1] = s_fi; s_ctrl[7] = s_nv; s_sim_nd = s_nd; s_sim_rs = s_rs; s_sim_ulen = ulen;
           if (nbatch == 0) { f_i = s_fi; n_visited = s_nv; n_drawn = s_nd; rstate = s_rs; }
-        } else if (tid >= 32) {
+        } else if (MODE != FO_SORT && tid >= 32) {
           // meanwhile the other warps clear the histograms (random splitter: the per-thread left
           // statistics, KB * C * FO_THREADS words, 64-bit when REG, which this covers) of a full batch
           for (int i = tid - 32; i < KB * hstride; i += FO_THREADS - 32) hist[i] = 0;
@@ -395,8 +673,8 @@ forest_build_kernel(const FoParams P) {
         FO_TICK(1);
         const int nbatch = s_ctrl[0];
         if (nbatch == 0) break;
-        if constexpr (RAW) {
-          // ------------------- node_split_random over the raw float32 values -------------------
+        if constexpr (MODE != FO_HIST) {
+          // ---------- node_split_random / node_split_best over the raw float32 values ----------
           // (SK/tree/_splitter.pyx node_split_random, DensePartitioner find_min_max / partition_samples)
           int fk[FO_KB_MAX];   // batch item k reads the column P.xval + fk[k] * n
 #pragma unroll
@@ -424,6 +702,21 @@ forest_build_kernel(const FoParams P) {
           }
           __syncthreads();
           FO_TICK(3);
+          if constexpr (MODE == FO_SORT) {
+            // node_split_best: the batch features one after another.  The commit discards every result
+            // after the first constant feature, so the batch stops there.
+            uint2* sbuf = P.srt + (size_t)slot * 2 * n;
+            for (int k = 0; k < nbatch; ++k) {
+              float lo = s_mm[0][0][k], hi = s_mm[1][0][k];
+              for (int w = 1; w < FO_THREADS / 32; ++w) { lo = fminf(lo, s_mm[0][w][k]); hi = fmaxf(hi, s_mm[1][w][k]); }
+              if (hi <= lo + FEATURE_THRESHOLD) {   // SK/tree/_splitter.pyx:373-377, the same in every thread
+                if (tid == 0) results[k].is_const = 1;
+                break;
+              }
+              fo_sort_split<CM, REG, W>(P, samp, P.xval + (size_t)items[k].f * n, sbuf, sbuf + n, hist, start, n_node,
+                                        lo, hi, rec.sums, s_cw, w_node, MIN_WEIGHT_LEAF, &results[k]);
+            }
+          } else {
           // every thread forms the same decisions: constant test in float32, threshold
           // rand_uniform(min, max) in float64 (SK/tree/_utils.pyx), and min if it lands on max
           double thr[FO_KB_MAX];
@@ -524,6 +817,7 @@ forest_build_kernel(const FoParams P) {
                 }
               }
             }
+          }
           }
         } else {
           // --- histograms of all batch features in one pass over the node's samples ---
@@ -813,7 +1107,7 @@ forest_build_kernel(const FoParams P) {
       if (best_pos < end) {
         // --- partition_samples_final: stable partition (keeps sample indices ascending) ---
         // (random splitter over raw values: the value against the drawn threshold, as partition_samples)
-        constexpr bool raw = RAW;
+        constexpr bool raw = MODE != FO_HIST;
         const uint8_t* xb = raw ? nullptr : P.xbin + (size_t)best_feature * n;
         const float* xv = raw ? P.xval + (size_t)best_feature * n : nullptr;
         __shared__ int loff, roff;
@@ -1049,20 +1343,25 @@ int forest_prepare(Ctx* c, bool values) {
 
 // Build `n_trees` trees.  counts: [n_trees][n] uint8 host array of bootstrap multiplicities,
 // rand_states: [n_trees] splitter seeds.  Results are delivered tree by tree through `sink`.
+// random_split: node_split_random (ExtraTrees), else node_split_best (RandomForest).  sort_split (best
+// splitter only): a feature without bin codes is split by sorting its raw values (FO_SORT) instead of
+// being refused; when every feature has codes the fit is the same as without it.
 // Two builders: forest_fast.cu (classification, best splitter, <= 4 classes: seven trees per SM)
 // and the general kernel above (two per SM).  Trees are built in rounds of `slots` concurrent
 // trees; the node arrays of a slot hold `node_cap` nodes, sized from the free device memory; a tree
 // that outgrows them (status 1) is rebuilt in a later round with the worst-case capacity 2n - 1.
 int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_states, int n_classes,
                int max_features, int max_depth, int min_samples_split, int min_samples_leaf,
-               double min_weight_leaf, double min_impurity_decrease, int random_split, const double* h_yreal,
-               const ForestClassWeights* cw, ForestSink sink, void* sink_arg) {
+               double min_weight_leaf, double min_impurity_decrease, bool random_split, bool sort_split,
+               const double* h_yreal, const ForestClassWeights* cw, ForestSink sink, void* sink_arg) {
   if (forest_prepare(c, false)) return 1;
   // the random splitter reads raw values when a feature has no bin codes; on codes alone its histogram
-  // form is faster (config-4 lattice, H100: profiles/README.md)
+  // form is faster (config-4 lattice, H100: profiles/README.md).  The sort-based best splitter, too,
+  // runs only when a feature has no codes.
   const bool raw_values = random_split && !c->forest.all_coded;
-  if (raw_values && forest_prepare(c, true)) return 1;
-  if (!random_split && !c->forest.all_coded) {
+  const bool sort_values = !random_split && sort_split && !c->forest.all_coded;
+  if ((raw_values || sort_values) && forest_prepare(c, true)) return 1;
+  if (!random_split && !sort_split && !c->forest.all_coded) {
     char b[220];
     snprintf(b, sizeof(b), "forest: feature %d has %d distinct values; the histogram splitter needs <= %d "
              "(continuous features need the sort-based splitter, not built yet)", c->forest.uncoded_feature,
@@ -1090,7 +1389,8 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
   const int stack_cap = 4096;
   const size_t rec_bytes = fast ? forest_fast_record_bytes(n_classes) : sizeof(FoRecord);
   const size_t node_bytes = fast ? 32 : (size_t)(4 * 4 + 1 + 8 * 3 + 8 * n_classes);   // fast builder: compact records
-  const size_t slot_fixed = (size_t)n * 17 + (size_t)stack_cap * rec_bytes + 64;   // two sample buffers + counts + stack
+  // two sample buffers + counts + stack (+ the two (key, position) buffers of the sort-based splitter)
+  const size_t slot_fixed = (size_t)n * (sort_values ? 33 : 17) + (size_t)stack_cap * rec_bytes + 64;
   const int64_t node_cap_max = std::max<int64_t>(2 * n, 16);
   int64_t node_cap = node_cap_max;
   if (const char* e = getenv("SKDIST_B200_FOREST_NODECAP")) {   // experiments / tests: smaller output arrays per tree
@@ -1118,7 +1418,9 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
                               (size_t)FO_KB_MAX * FO_BINS * sizeof(float) + (size_t)FO_SSTK * sizeof(FoRecord);
   // the general builder for this fit (CM: class-count bound; W: class weights)
   void (*general)(const FoParams) = nullptr;
-#define FO_PICK(CM, REG, W) (raw_values ? forest_build_kernel<CM, REG, W, true> : forest_build_kernel<CM, REG, W, false>)
+#define FO_PICK(CM, REG, W) (raw_values ? forest_build_kernel<CM, REG, W, FO_RAW>    \
+                            : sort_values ? forest_build_kernel<CM, REG, W, FO_SORT> \
+                                          : forest_build_kernel<CM, REG, W, FO_HIST>)
   if (reg) general = FO_PICK(4, true, false);
   else if (n_classes <= 2) general = weighted ? FO_PICK(2, false, true) : FO_PICK(2, false, false);
   else if (n_classes <= 4) general = weighted ? FO_PICK(4, false, true) : FO_PICK(4, false, false);
@@ -1174,10 +1476,11 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
     SKD_CUDA(c, sx.alloc(&P.o_count, (size_t)slots));
     SKD_CUDA(c, sx.alloc(&P.o_maxdepth, (size_t)slots));
     SKD_CUDA(c, sx.alloc(&P.o_status, (size_t)slots));
+    if (sort_values) SKD_CUDA(c, sx.alloc(&P.srt, (size_t)slots * 2 * n));
     long long* d_prof = nullptr;
     if (want_prof) SKD_CUDA(c, sx.alloc(&d_prof, (size_t)slots * 16));
     P.stack = (FoRecord*)dstack;
-    P.xbin = c->forest.xbin; P.binval = c->forest.binval; P.xval = raw_values ? c->forest.xval : nullptr; P.ycls = c->ycls; P.yreal = dy;
+    P.xbin = c->forest.xbin; P.binval = c->forest.binval; P.xval = raw_values || sort_values ? c->forest.xval : nullptr; P.ycls = c->ycls; P.yreal = dy;
     P.n = n; P.d = d; P.n_classes = n_classes;
     P.max_features = max_features; P.max_depth = max_depth; P.min_samples_split = min_samples_split;
     P.min_samples_leaf = min_samples_leaf; P.min_weight_leaf = min_weight_leaf;

@@ -291,8 +291,8 @@ int tc_make_map_2d(Ctx* c, CUtensorMap* map, const void* ptr, uint64_t rows, uin
 void forest_free(Ctx* c);
 int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_states, int n_classes,
                int max_features, int max_depth, int min_samples_split, int min_samples_leaf,
-               double min_weight_leaf, double min_impurity_decrease, int random_split, const double* h_yreal,
-               const ForestClassWeights* cw, ForestSink sink, void* sink_arg);
+               double min_weight_leaf, double min_impurity_decrease, bool random_split, bool sort_split,
+               const double* h_yreal, const ForestClassWeights* cw, ForestSink sink, void* sink_arg);
 int predict_device(Ctx* c, const float* dX, int64_t m, int ldx, int d, int B, const float* dW, float* dout);
 int forest_predict_device(Ctx* c, const float* dX, int64_t m, int ldx, int n_trees, const int64_t* d_off,
                           const void* d_node, const double* d_thr, const double* d_val, int C, double* d_out);

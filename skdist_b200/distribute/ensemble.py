@@ -151,6 +151,17 @@ def _remap_thresholds(arrays, table):
     return arrays
 
 
+def _sort_switch():
+    """SKDIST_B200_FOREST_SORT: unset (the best splitter refuses a feature with more than 256 distinct values)
+    or 1 (such features are split by sorting their values on the device: scikit-learn's trees)."""
+    v = os.environ.get("SKDIST_B200_FOREST_SORT")
+    if v is None:
+        return False
+    if v != "1":
+        raise ValueError("SKDIST_B200_FOREST_SORT must be unset or 1, not %r" % v)
+    return True
+
+
 def _finish_tree(t, template_params, state, n_features, n_classes, max_features_, tree_cls):
     est = tree_cls(**template_params)
     est.set_params(random_state=int(state))
@@ -167,12 +178,14 @@ def _finish_tree(t, template_params, state, n_features, n_classes, max_features_
 _LIMITS = """
 
     Limits of the device path (checked when the trees are built; `NotImplementedError` otherwise, there
-    is no CPU fallback): with the best splitter (RandomForest) every feature may take at most 256 distinct
+    is no CPU fallback): by default the best splitter (RandomForest) takes features with at most 256 distinct
     values (it works on per-feature value histograms: data on a lattice, counts, categorical codes, quantised
-    measurements -- continuous float features need a sort-based splitter that is not built; the opt-in
-    histogram mode `SKDIST_B200_FOREST_MAX_BINS=<2..256>` replaces such features by equal-count bin codes and
-    maps the thresholds back to raw units -- the trees scikit-learn builds on the coded matrix, not
-    bit-identical to the reference on the raw one); the random splitter (ExtraTrees, RandomTreesEmbedding)
+    measurements).  `SKDIST_B200_FOREST_SORT=1` lets it take continuous float features too: a feature with
+    more distinct values is split by sorting the node's raw float32 values on the device, which gives
+    scikit-learn's trees (features with at most 256 distinct values still take the histograms).  The
+    histogram mode `SKDIST_B200_FOREST_MAX_BINS=<2..256>` instead replaces such features by equal-count bin
+    codes and maps the thresholds back to raw units -- the trees scikit-learn builds on the coded matrix, not
+    bit-identical to the reference on the raw one; the two switches exclude each other.  The random splitter (ExtraTrees, RandomTreesEmbedding)
     reads the raw float32 values and takes any finite X (with the switch set it, too, is fitted on the coded
     matrix), at most 16 classes, at most
     384 features, bootstrap multiplicities up to 255, no missing values, `criterion` gini / squared
@@ -345,6 +358,12 @@ class _DistForestClassifier(_ScParamMixin):
         max_bins = int(os.environ.get("SKDIST_B200_FOREST_MAX_BINS", "0"))
         if max_bins and not 2 <= max_bins <= 256:
             raise ValueError("SKDIST_B200_FOREST_MAX_BINS must be between 2 and 256")
+        exact_sort = _sort_switch()
+        if exact_sort and max_bins:
+            raise ValueError("SKDIST_B200_FOREST_SORT and SKDIST_B200_FOREST_MAX_BINS ask for different trees "
+                             "(scikit-learn's exact ones, the histogram approximation); set one of them")
+        # the best splitter also takes features with more than 256 distinct values (sort-based splitter)
+        splitter = 2 if exact_sort and self._splitter == 0 else self._splitter
         X_dev, bin_table = _quantile_codes(X, max_bins) if max_bins else (X, None)
         try:
             parallel.stage_x_replicated(eng, X_dev)
@@ -386,11 +405,13 @@ class _DistForestClassifier(_ScParamMixin):
                     eng.stage_forest_class_weights(self.n_classes_, cw, cw_subsample, self.min_weight_fraction_leaf)
                 return eng.forest_fit(counts, rs, self.n_classes_, mf_i, max_depth, int(mss), int(msl),
                                       float(min_weight_leaf), float(self.min_impurity_decrease),
-                                      splitter=self._splitter, y_regression=y_reg)
+                                      splitter=splitter, y_regression=y_reg)
             except NotImplementedError as e:
                 if "distinct values" in str(e) and not max_bins:
-                    raise NotImplementedError(str(e) + "; SKDIST_B200_FOREST_MAX_BINS=256 selects the histogram "
-                                              "approximation (equal-count bins, see the class docstring)") from None
+                    raise NotImplementedError(str(e) + "; SKDIST_B200_FOREST_SORT=1 selects scikit-learn's exact "
+                                              "trees (sort-based splitter), SKDIST_B200_FOREST_MAX_BINS=256 the "
+                                              "histogram approximation (equal-count bins, see the class "
+                                              "docstring)") from None
                 raise
 
         def wrap(sts, arrays):

@@ -361,7 +361,8 @@ class Engine:
                    min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter=0, y_regression=None):
         """Build len(rand_states) classifier trees.  sample_counts [n_trees, n] uint8 (bootstrap
         multiplicities = the reference's sample_weight; None = every row once), rand_states [n_trees]
-        uint32 splitter seeds, splitter 0 = best (RandomForest) / 1 = random (ExtraTrees).
+        uint32 splitter seeds, splitter 0 = best (RandomForest) / 1 = random (ExtraTrees) / 2 = best, also on
+        features with more than 256 distinct values (sorts their raw values; otherwise the same as 0).
         y_regression: float64 targets [n] -> regression trees (MSE), one value per node.
         Returns a list of dicts with the sklearn Tree arrays of every tree."""
         yreg = None
