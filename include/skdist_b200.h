@@ -107,6 +107,14 @@ int skd_stage_class_weights(skd_ctx* ctx, int32_t B, int32_t K, const float* w, 
 int skd_stage_forest_class_weights(skd_ctx* ctx, int32_t n_classes, const double* w, int32_t balanced_subsample,
                                    double min_weight_fraction_leaf);
 
+/* Split criterion of the NEXT skd_forest_fit (one-shot, cleared by that call even when it fails): 0 = Gini
+ * (classification) / squared error (regression), the default; 1 = entropy in bits (classification only:
+ * the fit fails with a regression target).  Entropy fits always run the general tree builder.  The forest's
+ * `impurity` arrays are formed on the host with the host's log from the nodes' class sums, as scikit-learn
+ * forms them.  ref: `criterion="entropy"` / "log_loss" of the forest classifiers (SK/tree/_criterion.pyx
+ * Entropy). */
+int skd_stage_forest_criterion(skd_ctx* ctx, int32_t criterion);
+
 /* Batched binary L2 logistic regression (lbfgs), B independent columns sharing X.
  * Column j: positives = rows with y_class == col_pos[j]; training rows = rows whose fold id
  * != col_fold[j] (col_fold[j] < 0: all rows); l2 strength = 1 / (C[j] * n_train_j).

@@ -634,6 +634,16 @@ int skd_stage_forest_class_weights(skd_ctx* ctx, int32_t n_classes, const double
   return 0;
 }
 
+int skd_stage_forest_criterion(skd_ctx* ctx, int32_t criterion) {
+  if (!ctx) return fail(nullptr, "skd_stage_forest_criterion: ctx is NULL");
+  Ctx* c = &ctx->c;
+  c->forest_criterion = 0;
+  if (criterion != 0 && criterion != 1)
+    return fail(c, "skd_stage_forest_criterion: criterion must be 0 (gini / squared error) or 1 (entropy)");
+  c->forest_criterion = criterion;
+  return 0;
+}
+
 // Staged class weights of binary columns: weights scaled by the power of two 2^-e that brings the larger one
 // into (1/2, 1], so that |G| <= 2^14 holds in the fp16 operand of the tensor-core gradient product; 2^e goes
 // into inv_n.  Both scalings are exact.  l2 = 1 / (C sw_sum), inv_n = 2^e / sw_sum
@@ -1329,8 +1339,58 @@ struct skd_forest {
   };
   std::vector<Tree> trees;
   ForestClassWeights cw;               // staged for the fit (n_classes == 0: unweighted)
+  int32_t criterion = 0;               // staged for the fit: 0 Gini / MSE, 1 entropy
   std::vector<float> binval;           // [d][256] distinct feature values (thresholds of compact records)
 };
+
+// Entropy of one node in bits, as scikit-learn forms it (SK/tree/_criterion.pyx Entropy: e -= p * log(p),
+// p = s_c / w in class order, zero sums skipped; SK/tree/_utils.pyx: log(x) = ln(x) / ln(2.0)) with this
+// process's libm, the one scikit-learn calls
+static double entropy_bits(const double* s, int C, double w) {
+  const volatile double ln2 = std::log(2.0);
+  volatile double e = 0.0;
+  for (int c = 0; c < C; ++c) {
+    if (!(s[c] > 0.0)) continue;
+    const volatile double p = s[c] / w;
+    const volatile double lg = std::log(p) / ln2;
+    const volatile double t = p * lg;      // volatile: no contraction of the product into the difference
+    e = e - t;
+  }
+  return e;
+}
+
+// The impurity array of an entropy tree of the general builder, from its integer class sums [m][C].  The
+// builder ranks candidates with CUDA's log, which differs from the host's in the last bit on a few inputs;
+// the tree reports the impurity scikit-learn computes.  A node's impurity is the one its parent's
+// children_impurity formed: for the root (node_impurity) and a left child from the node's own sums
+// s_c = cw_c * count_c (one rounding) and w = sum_c s_c; for a right child from sum_right = cw_c * t_c -
+// cw_c * l_c and w_right = w_node - w_left, the builder's (and scikit-learn's) operations, which with
+// non-dyadic class weights can differ in the last bits from the child's own sums (the rule
+// skd_forest_tree_copy applies to the Gini trees of the throughput builder).  cw: nullptr when unweighted.
+static void forest_entropy_impurity(int m, int C, const int32_t* left, const int32_t* right,
+                                    const unsigned long long* sums, const double* cw, double* imp) {
+  std::vector<double> s(C), t(C);
+  auto weighted = [&](const unsigned long long* cnt, double* out) {
+    volatile double w = 0.0;
+    for (int c = 0; c < C; ++c) {
+      const volatile double a = cw ? cw[c] * (double)cnt[c] : (double)cnt[c];
+      out[c] = a;
+      w = w + a;
+    }
+    return (double)w;
+  };
+  imp[0] = entropy_bits(s.data(), C, weighted(sums, s.data()));
+  for (int i = 0; i < m; ++i) {
+    const int l = left[i], r = right[i];
+    if (l < 0) continue;
+    const double wn = weighted(sums + (size_t)i * C, t.data());
+    const double wl = weighted(sums + (size_t)l * C, s.data());
+    imp[l] = entropy_bits(s.data(), C, wl);
+    for (int c = 0; c < C; ++c) { const volatile double b = t[c] - s[c]; s[c] = b; }
+    const volatile double wr = wn - wl;
+    imp[r] = entropy_bits(s.data(), C, wr);
+  }
+}
 
 static void forest_sink(void* arg, int t, const SkdTreeView* v) {
   skd_forest* f = (skd_forest*)arg;
@@ -1354,6 +1414,19 @@ static void forest_sink(void* arg, int t, const SkdTreeView* v) {
   tr.thr.assign(v->threshold, v->threshold + m); tr.imp.assign(v->impurity, v->impurity + m);
   tr.wn.assign(v->weighted_n_node_samples, v->weighted_n_node_samples + m);
   tr.val.assign(v->value, v->value + (size_t)m * v->n_classes);
+  if (v->class_sums && m > 0) {
+    std::vector<double> cw;
+    if (f->cw.n_classes) {
+      cw = f->cw.w;
+      if (f->cw.balanced_subsample) {   // the root's class sums are the bootstrap class counts
+        std::vector<uint32_t> root(v->class_sums, v->class_sums + v->n_classes);
+        cw.resize(v->n_classes);
+        forest_subsample_weights(root.data(), v->n_classes, cw.data());
+      }
+    }
+    forest_entropy_impurity(m, v->n_classes, v->left, v->right, v->class_sums, cw.empty() ? nullptr : cw.data(),
+                            tr.imp.data());
+  }
 }
 
 int skd_forest_fit(skd_ctx* ctx, int32_t n_trees, const uint8_t* sample_counts, const uint32_t* rand_states,
@@ -1363,6 +1436,7 @@ int skd_forest_fit(skd_ctx* ctx, int32_t n_trees, const uint8_t* sample_counts, 
   if (!ctx) return fail(nullptr, "skd_forest_fit: ctx is NULL");
   Ctx* c = &ctx->c;
   const ForestClassWeights cw = std::exchange(c->forest_cw, {});
+  const int32_t criterion = std::exchange(c->forest_criterion, 0);
   if (!out) return fail(c, "skd_forest_fit: out is NULL");
   *out = nullptr;
   if (!c->X || (!y_regression && !c->ycls)) return fail(c, "skd_forest_fit: stage X and labels first");
@@ -1373,11 +1447,12 @@ int skd_forest_fit(skd_ctx* ctx, int32_t n_trees, const uint8_t* sample_counts, 
   std::unique_ptr<skd_forest> f(new skd_forest());
   f->trees.resize(n_trees);
   f->cw = cw;
+  f->criterion = criterion;
   DeviceTimer timer(c);
   if (timer.start()) return 1;
   if (forest_fit(c, n_trees, sample_counts, rand_states, n_classes, max_features, max_depth, min_samples_split,
-                 min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter == 1, splitter == 2, y_regression,
-                 cw.n_classes ? &cw : nullptr, forest_sink, f.get()))
+                 min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter == 1, splitter == 2,
+                 criterion == 1, y_regression, cw.n_classes ? &cw : nullptr, forest_sink, f.get()))
     return 1;
   f->binval = c->forest.h_binval;
   if (timer.stop(gpu_seconds_out)) return 1;

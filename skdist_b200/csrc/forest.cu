@@ -97,6 +97,9 @@ struct FoParams {
   // sort-based best splitter (FO_SORT): [slots][2][n] ping-pong (key, node position) buffers of the
   // large-node radix sort, else nullptr
   uint2* srt;
+  // entropy (ENT): [slots][node_cap][n_classes] integer class sums of every node, from which the host forms
+  // the impurity with its own log (api.cu), else nullptr
+  unsigned long long* o_sums;
 };
 
 // What the general builder reads for a split (one kernel instantiation each, so that the histogram
@@ -151,6 +154,47 @@ __device__ __forceinline__ void fo_children_impurity_w(const unsigned long long*
   }
   *il = __dsub_rn(1.0, __ddiv_rn(sql, __dmul_rn(wl, wl)));
   *ir = __dsub_rn(1.0, __ddiv_rn(sqr, __dmul_rn(wr, wr)));
+}
+
+// Entropy in bits (SK/tree/_criterion.pyx Entropy: e -= p * log(p), p = sum_c / w, classes with a zero sum
+// skipped; SK/tree/_utils.pyx: log(x) = ln(x) / ln(2.0)), one class's term, no FMA contraction.  CUDA's
+// log is not the host libm's: these values only rank candidates, the impurity of the finished tree is
+// formed on the host from the class sums (api.cu: forest_entropy_impurity).
+constexpr double FO_LN2 = 0.6931471805599453;   // == the host's log(2.0)
+__device__ __forceinline__ double fo_entropy_term(double e, double s, double w) {
+  if (s > 0.0) {
+    const double p = __ddiv_rn(s, w);
+    e = __dsub_rn(e, __dmul_rn(p, __ddiv_rn(log(p), FO_LN2)));
+  }
+  return e;
+}
+// Entropy children impurity; W: with class weights, the statistics of fo_children_impurity_w
+template <int CM, bool W>
+__device__ __forceinline__ void fo_children_entropy(const unsigned long long* sl, const unsigned long long* st,
+                                                    const double* cw, int C, double wl, double wr, double* il,
+                                                    double* ir) {
+  double el = 0.0, er = 0.0;
+#pragma unroll
+  for (int c = 0; c < CM; ++c) {
+    if (c < C) {
+      double a, b;
+      if constexpr (W) { a = __dmul_rn(cw[c], (double)sl[c]); b = __dsub_rn(__dmul_rn(cw[c], (double)st[c]), a); }
+      else { a = (double)sl[c]; b = (double)(st[c] - sl[c]); }
+      el = fo_entropy_term(el, a, wl);
+      er = fo_entropy_term(er, b, wr);
+    }
+  }
+  *il = el;
+  *ir = er;
+}
+// children impurity of a classification split under the fit's criterion (ENT: entropy, else Gini)
+template <int CM, bool W, bool ENT>
+__device__ __forceinline__ void fo_children_class(const unsigned long long* sl, const unsigned long long* st,
+                                                  const double* cw, int C, double wl, double wr, double* il,
+                                                  double* ir) {
+  if constexpr (ENT) fo_children_entropy<CM, W>(sl, st, cw, C, wl, wr, il, ir);
+  else if constexpr (W) fo_children_impurity_w<CM>(sl, st, cw, C, wl, wr, il, ir);
+  else fo_children_impurity<CM>(sl, st, C, wl, wr, il, ir);
 }
 
 // Node statistics are kept as 64-bit patterns so that the classification path (integer class
@@ -208,7 +252,7 @@ __device__ __forceinline__ float fo_kval(uint32_t k) { return __uint_as_float(k 
 // Proxy of the split whose left child has the statistics sl (the node: st, w_node), with the left and
 // right impurities; -inf when a child is lighter than min_weight_leaf.  The histogram scan's float64
 // operations, in the same order.
-template <int CM, bool REG, bool W>
+template <int CM, bool REG, bool W, bool ENT>
 __device__ __forceinline__ double fo_split_proxy(const unsigned long long* sl, const unsigned long long* st,
                                                  const double* cw, int C, double w_node, double mwl,
                                                  double* il, double* ir) {
@@ -222,11 +266,8 @@ __device__ __forceinline__ double fo_split_proxy(const unsigned long long* sl, c
     fo_children_mse(sl, st, wl, wr, il, ir);
     const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(st[1]), sum_l);
     return __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
-  } else if constexpr (W) {
-    fo_children_impurity_w<CM>(sl, st, cw, C, wl, wr, il, ir);
-    return __dsub_rn(__dmul_rn(-wr, *ir), __dmul_rn(wl, *il));
   } else {
-    fo_children_impurity<CM>(sl, st, C, wl, wr, il, ir);
+    fo_children_class<CM, W, ENT>(sl, st, cw, C, wl, wr, il, ir);
     return __dsub_rn(__dmul_rn(-wr, *ir), __dmul_rn(wl, *il));
   }
 }
@@ -234,7 +275,7 @@ __device__ __forceinline__ double fo_split_proxy(const unsigned long long* sl, c
 // Best split of one non-constant feature (values col[samp[i].x], node positions start .. start+m-1,
 // min lo < max hi) into *R, filled as the histogram scan fills it.  Called by the whole block; hist is
 // free on entry and is overwritten.  bufA / bufB: this tree's two [n] scratch buffers.
-template <int CM, bool REG, bool W>
+template <int CM, bool REG, bool W, bool ENT>
 __device__ void fo_sort_split(const FoParams& P, const uint2* __restrict__ samp, const float* __restrict__ col,
                               uint2* bufA, uint2* bufB, unsigned int* hist, int start, int m, float lo, float hi,
                               const unsigned long long* st, const double* cw, double w_node, double mwl,
@@ -408,7 +449,7 @@ __device__ void fo_sort_split(const FoParams& P, const uint2* __restrict__ samp,
         if (fo_kval(hib | nk) > fo_kval(hib | key[j]) + FEATURE_THRESHOLD &&
             n_left >= P.min_samples_leaf && m - n_left >= P.min_samples_leaf) {
           double il, ir;
-          const double proxy = fo_split_proxy<CM, REG, W>(sl, st, cw, C, w_node, mwl, &il, &ir);
+          const double proxy = fo_split_proxy<CM, REG, W, ENT>(sl, st, cw, C, w_node, mwl, &il, &ir);
           if (proxy > bp) { bp = proxy; bj = j; bk = key[j]; bnk = nk; }
         }
       }
@@ -437,7 +478,7 @@ __device__ void fo_sort_split(const FoParams& P, const uint2* __restrict__ samp,
 #pragma unroll
         for (int j = 0; j < FO_SORT_IPT; ++j) if (j <= bj) add(a, pos[j]);
         double il, ir;
-        R->proxy = fo_split_proxy<CM, REG, W>(a, st, cw, C, w_node, mwl, &il, &ir);
+        R->proxy = fo_split_proxy<CM, REG, W, ENT>(a, st, cw, C, w_node, mwl, &il, &ir);
         R->pos = start + gq; R->il = il; R->ir = ir;
         R->thr = (double)fo_kval(hib | bk) / 2.0 + (double)fo_kval(hib | bnk) / 2.0;
         FOR_C(c) R->sl[c] = a[c];
@@ -448,11 +489,12 @@ __device__ void fo_sort_split(const FoParams& P, const uint2* __restrict__ samp,
 
 // MODE (FoMode): FO_HIST reads bin codes; FO_RAW (random splitter) and FO_SORT (best splitter) read the
 // raw values (P.xval).  Each is a separate instantiation so that the histogram instantiations keep their
-// register allocation.
-template <int CM, bool REG, bool W, int MODE>
+// register allocation.  ENT: criterion="entropy" (classification), else Gini / MSE.
+template <int CM, bool REG, bool W, int MODE, bool ENT>
 __global__ void __launch_bounds__(FO_THREADS)
 forest_build_kernel(const FoParams P) {
   static_assert(!(REG && W), "class weights are a classification feature");
+  static_assert(!(REG && ENT), "entropy is a classification criterion");
   const int slot = blockIdx.x;
   if (slot >= P.n_trees) return;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -603,6 +645,10 @@ forest_build_kernel(const FoParams P) {
       if constexpr (REG) {   // MSE.node_impurity
         const double mean = __ddiv_rn(st_d(rec.sums[1]), w_node);
         impurity = __dsub_rn(__ddiv_rn(st_d(rec.sums[2]), w_node), __dmul_rn(mean, mean));
+      } else if constexpr (ENT) {   // Entropy.node_impurity
+        double e = 0.0;
+        FOR_C(c) e = fo_entropy_term(e, W ? __dmul_rn(s_cw[c], (double)rec.sums[c]) : (double)rec.sums[c], w_node);
+        impurity = e;
       } else if constexpr (W) {
         double sq = 0.0;
         FOR_C(c) { const double a = __dmul_rn(s_cw[c], (double)rec.sums[c]); sq = __dadd_rn(sq, __dmul_rn(a, a)); }
@@ -713,7 +759,7 @@ forest_build_kernel(const FoParams P) {
                 if (tid == 0) results[k].is_const = 1;
                 break;
               }
-              fo_sort_split<CM, REG, W>(P, samp, P.xval + (size_t)items[k].f * n, sbuf, sbuf + n, hist, start, n_node,
+              fo_sort_split<CM, REG, W, ENT>(P, samp, P.xval + (size_t)items[k].f * n, sbuf, sbuf + n, hist, start, n_node,
                                         lo, hi, rec.sums, s_cw, w_node, MIN_WEIGHT_LEAF, &results[k]);
             }
           } else {
@@ -804,11 +850,8 @@ forest_build_kernel(const FoParams P) {
                       fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
                       const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
                       R->proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
-                    } else if constexpr (W) {
-                      fo_children_impurity_w<CM>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
-                      R->proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
                     } else {
-                      fo_children_impurity<CM>(sl, rec.sums, C, wl, wr, &il, &ir);
+                      fo_children_class<CM, W, ENT>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
                       R->proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
                     }
                     R->pos = start + n_left; R->il = il; R->ir = ir;
@@ -963,11 +1006,8 @@ forest_build_kernel(const FoParams P) {
                         fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
                         const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
                         R->proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
-                      } else if constexpr (W) {
-                        fo_children_impurity_w<CM>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
-                        R->proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
                       } else {
-                        fo_children_impurity<CM>(sl, rec.sums, C, wl, wr, &il, &ir);
+                        fo_children_class<CM, W, ENT>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
                         R->proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
                       }
                       R->pos = start + n_left; R->il = il; R->ir = ir;
@@ -1010,11 +1050,8 @@ forest_build_kernel(const FoParams P) {
                   fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
                   const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
                   proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
-                } else if constexpr (W) {
-                  fo_children_impurity_w<CM>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
-                  proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
-                } else {
-                  fo_children_impurity<CM>(sl, rec.sums, C, wl, wr, &il, &ir);
+                } else {                 // Criterion.proxy_impurity_improvement: -w_r * imp_r - w_l * imp_l
+                  fo_children_class<CM, W, ENT>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
                   proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
                 }
                 if (proxy > bproxy) {
@@ -1169,6 +1206,7 @@ forest_build_kernel(const FoParams P) {
         FOR_C(c)
           P.o_val[(nb + node_id) * C + c] = __ddiv_rn((double)rec.sums[c], w_node);   // class fractions
       }
+      if constexpr (ENT) { FOR_C(c) P.o_sums[(nb + node_id) * C + c] = rec.sums[c]; }
     }
     node_count += 1;
     if (!is_leaf) {
@@ -1345,15 +1383,18 @@ int forest_prepare(Ctx* c, bool values) {
 // rand_states: [n_trees] splitter seeds.  Results are delivered tree by tree through `sink`.
 // random_split: node_split_random (ExtraTrees), else node_split_best (RandomForest).  sort_split (best
 // splitter only): a feature without bin codes is split by sorting its raw values (FO_SORT) instead of
-// being refused; when every feature has codes the fit is the same as without it.
-// Two builders: forest_fast.cu (classification, best splitter, <= 4 classes: seven trees per SM)
+// being refused; when every feature has codes the fit is the same as without it.  entropy: criterion
+// "entropy" (classification, general builder only); the trees come with their integer class sums.
+// Two builders: forest_fast.cu (classification, Gini, best splitter, <= 4 classes: seven trees per SM)
 // and the general kernel above (two per SM).  Trees are built in rounds of `slots` concurrent
 // trees; the node arrays of a slot hold `node_cap` nodes, sized from the free device memory; a tree
 // that outgrows them (status 1) is rebuilt in a later round with the worst-case capacity 2n - 1.
 int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_states, int n_classes,
                int max_features, int max_depth, int min_samples_split, int min_samples_leaf,
                double min_weight_leaf, double min_impurity_decrease, bool random_split, bool sort_split,
-               const double* h_yreal, const ForestClassWeights* cw, ForestSink sink, void* sink_arg) {
+               bool entropy, const double* h_yreal, const ForestClassWeights* cw, ForestSink sink,
+               void* sink_arg) {
+  if (entropy && h_yreal) return fail(c, "forest: criterion entropy is staged but this is a regression fit");
   if (forest_prepare(c, false)) return 1;
   // the random splitter reads raw values when a feature has no bin codes; on codes alone its histogram
   // form is faster (config-4 lattice, H100: profiles/README.md).  The sort-based best splitter, too,
@@ -1378,7 +1419,7 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
   const int64_t n = c->n;
   const int d = (int)c->d;
   if ((size_t)4 * d * sizeof(int) > 6 * 1024) return fail(c, "forest: device path supports up to 384 features (shared-memory feature permutation)");
-  bool fast = forest_fast_supported(c, n_classes, reg, random_split);
+  bool fast = forest_fast_supported(c, n_classes, reg, random_split, entropy);
   if (fast && weighted && !cw->balanced_subsample) {
     // the float32 rank value of the fast builder needs the positive weights within 2^40 of each other
     // (balanced_subsample weights are within n of each other)
@@ -1388,7 +1429,8 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
   }
   const int stack_cap = 4096;
   const size_t rec_bytes = fast ? forest_fast_record_bytes(n_classes) : sizeof(FoRecord);
-  const size_t node_bytes = fast ? 32 : (size_t)(4 * 4 + 1 + 8 * 3 + 8 * n_classes);   // fast builder: compact records
+  // fast builder: compact records; entropy: the class sums too
+  const size_t node_bytes = fast ? 32 : (size_t)(4 * 4 + 1 + 8 * 3 + 8 * n_classes * (entropy ? 2 : 1));
   // two sample buffers + counts + stack (+ the two (key, position) buffers of the sort-based splitter)
   const size_t slot_fixed = (size_t)n * (sort_values ? 33 : 17) + (size_t)stack_cap * rec_bytes + 64;
   const int64_t node_cap_max = std::max<int64_t>(2 * n, 16);
@@ -1416,22 +1458,25 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
   }
   const size_t smem_general = (size_t)2 * d * sizeof(int) + (size_t)(d + 16) * sizeof(int2) +
                               (size_t)FO_KB_MAX * FO_BINS * sizeof(float) + (size_t)FO_SSTK * sizeof(FoRecord);
-  // the general builder for this fit (CM: class-count bound; W: class weights)
+  // the general builder for this fit (CM: class-count bound; W: class weights; ENT: entropy)
   void (*general)(const FoParams) = nullptr;
-#define FO_PICK(CM, REG, W) (raw_values ? forest_build_kernel<CM, REG, W, FO_RAW>    \
-                            : sort_values ? forest_build_kernel<CM, REG, W, FO_SORT> \
-                                          : forest_build_kernel<CM, REG, W, FO_HIST>)
-  if (reg) general = FO_PICK(4, true, false);
-  else if (n_classes <= 2) general = weighted ? FO_PICK(2, false, true) : FO_PICK(2, false, false);
-  else if (n_classes <= 4) general = weighted ? FO_PICK(4, false, true) : FO_PICK(4, false, false);
-  else if (n_classes <= 8) general = weighted ? FO_PICK(8, false, true) : FO_PICK(8, false, false);
-  else general = weighted ? FO_PICK(FO_MAXC, false, true) : FO_PICK(FO_MAXC, false, false);
+#define FO_PICK_M(CM, REG, W, ENT) (raw_values ? forest_build_kernel<CM, REG, W, FO_RAW, ENT>    \
+                                   : sort_values ? forest_build_kernel<CM, REG, W, FO_SORT, ENT> \
+                                                 : forest_build_kernel<CM, REG, W, FO_HIST, ENT>)
+#define FO_PICK(CM, W) (entropy ? FO_PICK_M(CM, false, W, true) : FO_PICK_M(CM, false, W, false))
+  if (reg) general = FO_PICK_M(4, true, false, false);
+  else if (n_classes <= 2) general = weighted ? FO_PICK(2, true) : FO_PICK(2, false);
+  else if (n_classes <= 4) general = weighted ? FO_PICK(4, true) : FO_PICK(4, false);
+  else if (n_classes <= 8) general = weighted ? FO_PICK(8, true) : FO_PICK(8, false);
+  else general = weighted ? FO_PICK(FO_MAXC, true) : FO_PICK(FO_MAXC, false);
 #undef FO_PICK
+#undef FO_PICK_M
   if (!fast) SKD_CUDA(c, cudaFuncSetAttribute(general, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_general));
   std::vector<int> pending(n_trees);
   for (int t = 0; t < n_trees; ++t) pending[t] = t;
   c->forest_kernel_ms = 0.0;
   std::vector<int32_t> hl, hr, hf, hn; std::vector<uint8_t> hm; std::vector<double> ht, hi, hw, hv;
+  std::vector<unsigned long long> hs;
   for (int round = 0; !pending.empty(); ++round) {
     // slots: concurrent trees of this round, bounded by the resident builders and by memory
     size_t free_b = 0, total_b = 0;
@@ -1472,6 +1517,7 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
       SKD_CUDA(c, sx.alloc(&P.o_imp, (size_t)slots * node_cap));
       SKD_CUDA(c, sx.alloc(&P.o_wn, (size_t)slots * node_cap));
       SKD_CUDA(c, sx.alloc(&P.o_val, (size_t)slots * node_cap * n_classes));
+      if (entropy) SKD_CUDA(c, sx.alloc(&P.o_sums, (size_t)slots * node_cap * n_classes));
     }
     SKD_CUDA(c, sx.alloc(&P.o_count, (size_t)slots));
     SKD_CUDA(c, sx.alloc(&P.o_maxdepth, (size_t)slots));
@@ -1633,12 +1679,17 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
         SKD_CUDA(c, cudaMemcpyAsync(hi.data(), P.o_imp + o, m * 8, cudaMemcpyDeviceToHost, c->stream));
         SKD_CUDA(c, cudaMemcpyAsync(hw.data(), P.o_wn + o, m * 8, cudaMemcpyDeviceToHost, c->stream));
         SKD_CUDA(c, cudaMemcpyAsync(hv.data(), P.o_val + o * n_classes, (size_t)m * n_classes * 8, cudaMemcpyDeviceToHost, c->stream));
+        if (entropy) {
+          hs.resize((size_t)m * n_classes);
+          SKD_CUDA(c, cudaMemcpyAsync(hs.data(), P.o_sums + o * n_classes, (size_t)m * n_classes * 8, cudaMemcpyDeviceToHost, c->stream));
+        }
         SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-        c->d2h += (int64_t)m * (4 * 4 + 1 + 8 * 3 + 8 * n_classes);
+        c->d2h += (int64_t)m * node_bytes;
         view.node_count = m; view.max_depth = hdepth[s]; view.n_classes = n_classes;
         view.left = hl.data(); view.right = hr.data(); view.feature = hf.data(); view.n_node_samples = hn.data();
         view.missing_go_to_left = hm.data(); view.threshold = ht.data(); view.impurity = hi.data();
         view.weighted_n_node_samples = hw.data(); view.value = hv.data();
+        view.class_sums = entropy ? hs.data() : nullptr;
         sink(sink_arg, pending[p0 + s], &view);
       }
     }

@@ -60,7 +60,7 @@ inline void forest_subsample_weights(const uint32_t* sums, int C, double* w) {
   }
 }
 
-bool forest_fast_supported(const Ctx* c, int n_classes, bool reg, int random_split);
+bool forest_fast_supported(const Ctx* c, int n_classes, bool reg, int random_split, bool entropy);
 int forest_fast_slots_per_sm();
 size_t forest_fast_record_bytes(int n_classes);
 int forest_fast_launch(Ctx* c, FfParams& P, int nt);

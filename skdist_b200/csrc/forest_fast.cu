@@ -998,8 +998,10 @@ static int ff_stage_rows(int d, int n_classes, int* ws_out) {
   return S >= 64 ? S : 0;
 }
 
-bool forest_fast_supported(const Ctx* c, int n_classes, bool reg, int random_split) {
-  if (reg || random_split || n_classes > 4 || c->d > 255 || !c->forest.all_coded || !c->forest.well_separated)
+// entropy: never (the candidate screening's float32 rank value and its error bound are Gini's)
+bool forest_fast_supported(const Ctx* c, int n_classes, bool reg, int random_split, bool entropy) {
+  if (reg || random_split || entropy || n_classes > 4 || c->d > 255 || !c->forest.all_coded ||
+      !c->forest.well_separated)
     return false;
   if ((double)c->n * 255.0 >= 4294967296.0) return false;
   if (const char* e = getenv("SKDIST_B200_FOREST_KERNEL")) if (!strcmp(e, "general")) return false;

@@ -63,6 +63,9 @@ struct SkdTreeView {
   const int32_t *left, *right, *feature, *n_node_samples;
   const uint8_t* missing_go_to_left;
   const double *threshold, *impurity, *weighted_n_node_samples, *value;
+  // criterion entropy: [node_count][n_classes] integer class sums of every node, else nullptr; the
+  // consumer forms the impurity from them (`impurity` then holds the builder's ranking values)
+  const unsigned long long* class_sums = nullptr;
 };
 typedef void (*ForestSink)(void* arg, int tree_index, const SkdTreeView* view);
 
@@ -118,11 +121,12 @@ struct Ctx {
   int64_t vec_n = 0;        // row count the staged labels / targets / folds belong to (dropped when X changes it)
   // one-shot staged inputs: read by skd_logreg_fit_batch (all three), skd_logreg_loss_grad (class
   // weights), skd_logreg_multinomial_fit_batch (masks, class weights) and skd_forest_fit (forest_cw,
-  // n_classes == 0: none)
+  // n_classes == 0: none; forest_criterion, 0: Gini / MSE, 1: entropy)
   StagedMasks fmask;
   StagedRowBits row_bits;
   StagedClassWeights cw;
   ForestClassWeights forest_cw;
+  int32_t forest_criterion = 0;
   // scratch pool: device blocks released by finished calls, reused by the next ones (Scratch below)
   std::vector<std::pair<void*, size_t>> pool_free;
   size_t pool_bytes = 0;
@@ -292,7 +296,8 @@ void forest_free(Ctx* c);
 int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_states, int n_classes,
                int max_features, int max_depth, int min_samples_split, int min_samples_leaf,
                double min_weight_leaf, double min_impurity_decrease, bool random_split, bool sort_split,
-               const double* h_yreal, const ForestClassWeights* cw, ForestSink sink, void* sink_arg);
+               bool entropy, const double* h_yreal, const ForestClassWeights* cw, ForestSink sink,
+               void* sink_arg);
 int predict_device(Ctx* c, const float* dX, int64_t m, int ldx, int d, int B, const float* dW, float* dout);
 int forest_predict_device(Ctx* c, const float* dX, int64_t m, int ldx, int n_trees, const int64_t* d_off,
                           const void* d_node, const double* d_thr, const double* d_val, int C, double* d_out);

@@ -175,6 +175,9 @@ def _finish_tree(t, template_params, state, n_features, n_classes, max_features_
     return est
 
 
+# classifier criteria with a device path -> the library's criterion code (skd_stage_forest_criterion)
+_CLASS_CRITERIA = {"gini": 0, "entropy": 1, "log_loss": 1}
+
 _LIMITS = """
 
     Limits of the device path (checked when the trees are built; `NotImplementedError` otherwise, there
@@ -188,8 +191,9 @@ _LIMITS = """
     bit-identical to the reference on the raw one; the two switches exclude each other.  The random splitter (ExtraTrees, RandomTreesEmbedding)
     reads the raw float32 values and takes any finite X (with the switch set it, too, is fitted on the coded
     matrix), at most 16 classes, at most
-    384 features, bootstrap multiplicities up to 255, no missing values, `criterion` gini / squared
-    error, no `max_leaf_nodes`, `sample_weight` or multi-output targets; `class_weight` (classifiers) may
+    384 features, bootstrap multiplicities up to 255, no missing values, `criterion` gini, entropy or
+    log_loss (classifiers; the entropy alias, fitted by the general tree builder, whose `impurity` arrays are
+    formed on the host with scikit-learn's log) or squared error (regressors), no `max_leaf_nodes`, `sample_weight` or multi-output targets; `class_weight` (classifiers) may
     be a dict, "balanced" or "balanced_subsample", not "subsample" or a list of dicts."""
 
 _CLASS_WEIGHT = """
@@ -258,8 +262,8 @@ class _DistForestClassifier(_ScParamMixin):
         if self._regression:
             if self.criterion not in ("mse", "squared_error"):   # "mse" is the reference era's name
                 bad.append("criterion=%r (only 'squared_error' / 'mse')" % self.criterion)
-        elif self.criterion != "gini":
-            bad.append("criterion=%r (only 'gini')" % self.criterion)
+        elif not (isinstance(self.criterion, str) and self.criterion in _CLASS_CRITERIA):
+            bad.append("criterion=%r (only 'gini', 'entropy' / 'log_loss')" % (self.criterion,))
         if self.max_leaf_nodes is not None:
             bad.append("max_leaf_nodes (best-first builder)")
         cw = self.class_weight
@@ -385,7 +389,11 @@ class _DistForestClassifier(_ScParamMixin):
         # of chunk k-1 into scikit-learn trees (ctypes releases the GIL during the device call).
         # (the throughput builder of csrc/forest_fast.cu keeps seven trees per SM resident, the general
         # one two: a chunk is one full wave of the builder that will run)
-        fast = not self._regression and self._splitter == 0 and self.n_classes_ <= 4 and d <= 255
+        # criterion code of the library: 1 = entropy ("log_loss" is scikit-learn's other name for it), which
+        # only the general builder runs
+        entropy = not self._regression and _CLASS_CRITERIA[self.criterion] == 1
+        fast = (not self._regression and not entropy and self._splitter == 0 and self.n_classes_ <= 4
+                and d <= 255)
         if cw is not None and fast:       # the library keeps positive dict weights within 2^40 on the throughput builder
             pos = cw[cw > 0]
             fast = bool(pos.max() <= 2.0 ** 40 * pos.min())
@@ -403,6 +411,8 @@ class _DistForestClassifier(_ScParamMixin):
             try:
                 if weighted:      # one-shot: staged for each chunk's fit (min_weight_leaf per tree: fraction * sum w)
                     eng.stage_forest_class_weights(self.n_classes_, cw, cw_subsample, self.min_weight_fraction_leaf)
+                if entropy:       # one-shot as well; Gini fits stage nothing (the library's default)
+                    eng.stage_forest_criterion(1)
                 return eng.forest_fit(counts, rs, self.n_classes_, mf_i, max_depth, int(mss), int(msl),
                                       float(min_weight_leaf), float(self.min_impurity_decrease),
                                       splitter=splitter, y_regression=y_reg)

@@ -357,6 +357,11 @@ class Engine:
         check(self._lib.skd_stage_forest_class_weights(self._h, int(n_classes), ptr(w), 0,
                                                        float(min_weight_fraction_leaf)), self._h)
 
+    def stage_forest_criterion(self, criterion):
+        """Split criterion of the next forest_fit: 0 Gini / squared error, 1 entropy (classification only;
+        the general tree builder, impurity in bits formed on the host as scikit-learn forms it)."""
+        check(self._lib.skd_stage_forest_criterion(self._h, int(criterion)), self._h)
+
     def forest_fit(self, sample_counts, rand_states, n_classes, max_features, max_depth, min_samples_split,
                    min_samples_leaf, min_weight_leaf, min_impurity_decrease, splitter=0, y_regression=None):
         """Build len(rand_states) classifier trees.  sample_counts [n_trees, n] uint8 (bootstrap
