@@ -225,6 +225,25 @@ int skd_sgd_fit_batch(skd_ctx* ctx, int32_t B, const int32_t* col_pos, int32_t l
                       int32_t n_iter_no_change, float* coef_out, double* intercept_out,
                       int32_t* n_iter_out, double* t_out, int32_t* status_out, double* gpu_seconds_out);
 
+/* The same exact-order SGD for cross-validation: B binary columns in G order groups.  Column j fits
+ * group col_group[j] with its own col_alpha[j] (> 0) and col_optimal_init[j] (computed by the host per alpha,
+ * as for skd_sgd_fit_batch); positives = rows with y_class == col_pos[j].  Group g walks the rows
+ * group_rows[group_offsets[g] .. group_offsets[g+1]) (a fold's training rows, in the splitter's order; int32
+ * row ids, every group non-empty, group_offsets[0] = 0) and shuffles that list every epoch with its own
+ * group_seeds[g]; its t and per-epoch objective use n_g = its row count, so t_out = 1 + n_iter * n_g.
+ * Every other argument and output as skd_sgd_fit_batch.  All groups run side by side in one launch per epoch
+ * on the warp-per-column kernels (never on the tensor cores).
+ * ref: replaces B invocations of search.py:180-288 (_fit_and_score: estimator.fit(X[train], y[train])) with
+ * estimator = SGDClassifier: SK/linear_model/_stochastic_gradient.py:387-515 (binary) and :795-830 (one
+ * seed per class, seeds = RandomState(random_state).randint(MAX_INT, size=K)),
+ * SK/linear_model/_sgd_fast.pyx.tp:274-640. */
+int skd_sgd_fit_groups(skd_ctx* ctx, int32_t B, const int32_t* col_pos, const int32_t* col_group,
+                       const double* col_alpha, const double* col_optimal_init, int32_t G, const int64_t* group_offsets,
+                       const int32_t* group_rows, const uint32_t* group_seeds, int32_t loss, int32_t fit_intercept,
+                       int32_t max_iter, double tol, int32_t shuffle, int32_t lr_type, double eta0, double power_t,
+                       int32_t n_iter_no_change, float* coef_out, double* intercept_out, int32_t* n_iter_out,
+                       double* t_out, int32_t* status_out, double* gpu_seconds_out);
+
 /* Host-only helper (no CUDA, no context): bootstrap multiplicities and splitter seeds of n_trees trees
  * from their integer seeds, spread over host threads (n_threads <= 0: all cores, at most 64).
  * counts_out[t * n + i] = how often row i is drawn by RandomState(seeds[t]).randint(0, n, n) (needed only

@@ -68,6 +68,11 @@ SYMBOLS = {
                                      _c.c_int32, _c.c_double, _c.c_int32, _c.c_uint32, _c.c_int32, _c.c_double,
                                      _c.c_double, _c.c_double, _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_void_p,
                                      _c.c_void_p, _c.c_void_p, _c.POINTER(_c.c_double)]),
+    "skd_sgd_fit_groups": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_void_p,
+                                      _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_int32, _c.c_int32,
+                                      _c.c_int32, _c.c_double, _c.c_int32, _c.c_int32, _c.c_double, _c.c_double,
+                                      _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_void_p,
+                                      _c.POINTER(_c.c_double)]),
     "skd_bootstrap_counts": (_c.c_int, [_c.c_int32, _c.c_void_p, _c.c_int64, _c.c_int32, _c.c_void_p, _c.c_void_p,
                                         _c.c_int32]),
     "skd_forest_fit": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_int32, _c.c_int32,

@@ -1328,6 +1328,46 @@ int skd_sgd_fit_batch(skd_ctx* ctx, int32_t B, const int32_t* col_pos, int32_t l
   return timer.stop(gpu_seconds_out);
 }
 
+int skd_sgd_fit_groups(skd_ctx* ctx, int32_t B, const int32_t* col_pos, const int32_t* col_group,
+                       const double* col_alpha, const double* col_optimal_init, int32_t G, const int64_t* group_offsets,
+                       const int32_t* group_rows, const uint32_t* group_seeds, int32_t loss, int32_t fit_intercept,
+                       int32_t max_iter, double tol, int32_t shuffle, int32_t lr_type, double eta0, double power_t,
+                       int32_t n_iter_no_change, float* coef_out, double* intercept_out, int32_t* n_iter_out,
+                       double* t_out, int32_t* status_out, double* gpu_seconds_out) {
+  if (!ctx) return fail(nullptr, "skd_sgd_fit_groups: ctx is NULL");
+  Ctx* c = &ctx->c;
+  if (!c->X || !c->ycls) return fail(c, "skd_sgd_fit_groups: stage X and labels first");
+  if (B <= 0 || G <= 0 || !col_pos || !col_group || !col_alpha || !col_optimal_init || !group_offsets || !group_rows ||
+      !group_seeds || !coef_out || !intercept_out || !n_iter_out || !t_out || !status_out)
+    return fail(c, "skd_sgd_fit_groups: bad arguments");
+  if (loss < 0 || loss > 1 || lr_type < 0 || lr_type > 2 || max_iter < 1)
+    return fail(c, "skd_sgd_fit_groups: unsupported loss / learning rate / max_iter");
+  if (c->n >= ((int64_t)1 << 31)) return fail(c, "skd_sgd_fit_groups: row ids are int32, n must be < 2^31");
+  for (int32_t j = 0; j < B; ++j) {
+    if (col_group[j] < 0 || col_group[j] >= G)
+      return fail(c, "skd_sgd_fit_groups: column " + std::to_string(j) + " names group " +
+                         std::to_string(col_group[j]) + ", not in [0, G)");
+    if (!(col_alpha[j] > 0.0))
+      return fail(c, "skd_sgd_fit_groups: column " + std::to_string(j) + " has alpha <= 0");
+  }
+  if (group_offsets[0] != 0) return fail(c, "skd_sgd_fit_groups: group_offsets[0] must be 0");
+  for (int32_t g = 0; g < G; ++g)
+    if (group_offsets[g + 1] <= group_offsets[g])
+      return fail(c, "skd_sgd_fit_groups: group " + std::to_string(g) + " is empty");
+  for (int64_t i = 0; i < group_offsets[G]; ++i)
+    if (group_rows[i] < 0 || group_rows[i] >= c->n)
+      return fail(c, "skd_sgd_fit_groups: row id " + std::to_string(group_rows[i]) + " at position " +
+                         std::to_string(i) + " is outside [0, n)");
+  SKD_CUDA(c, cudaSetDevice(c->device));
+  DeviceTimer timer(c);
+  if (timer.start()) return 1;
+  if (sgd_fit_groups(c, B, col_pos, col_group, col_alpha, col_optimal_init, G, group_offsets, group_rows,
+                     group_seeds, loss, fit_intercept, max_iter, tol, shuffle, lr_type, eta0, power_t,
+                     n_iter_no_change, coef_out, intercept_out, n_iter_out, t_out, status_out))
+    return 1;
+  return timer.stop(gpu_seconds_out);
+}
+
 struct skd_forest {
   struct Tree {
     int32_t max_depth = 0, n_classes = 0, node_count = 0;

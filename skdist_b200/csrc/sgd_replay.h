@@ -76,18 +76,25 @@ __device__ __forceinline__ void sgd_end_epoch(SgdState& st, const float (&w)[DPL
   st.objective_sum = 0.0;
 }
 
-// What one fit shares between its epochs and between the two paths (device pointers).
+// What one fit shares between its epochs and between the two paths (device pointers).  The columns form
+// order groups: group g walks its own n_g rows order[goff[g] .. goff[g+1]) (its own shuffle), and column j
+// belongs to group col_group[j] with its own alpha.  The tensor-core path runs one group of all n rows with
+// one alpha and reads the per-sample tables eta / cfac; the warp kernels form each column's rates themselves.
 struct SgdFit {
   int B, dpl, ldw;          // columns; weights per lane; leading dimension of W (32 * dpl)
   float* W;                 // [B x ldw] stored weights (times wscale = the coefficients)
   SgdState* state;          // [B]
   const int32_t* col_pos;   // [B] positive class of each column
-  const int32_t* order;     // [n] sample order of the epoch
+  const int32_t* col_group; // [B] order group of each column
+  const double* col_alpha;  // [B] alpha of each column
+  const double* col_oi;     // [B] its optimal_init ("optimal" rate)
+  const int64_t* goff;      // [G + 1] start of each group's rows in order (and in eta)
+  const int32_t* order;     // [goff[G]] sample order of the epoch, group by group
   const int32_t* active;    // [n_active] columns still running
-  const double* eta;        // [n] learning rate of each sample of the epoch
-  const float* cfac;        // [n] its weight-decay factor max(0, 1 - eta * alpha), as float
-  double alpha, tol;
-  int fit_intercept, n_iter_no_change;
+  const double* eta;        // [goff[G]] learning rate of each sample of the epoch (tensor cores; warp kernels: invscaling only)
+  const float* cfac;        // [n] its weight-decay factor max(0, 1 - eta * alpha), as float (tensor cores only)
+  double alpha, tol, eta0;  // alpha: the tensor-core path's one alpha
+  int fit_intercept, n_iter_no_change, lr_type;
 };
 
 // whether a fit runs its epochs on SgdTc: hinge, d <= 1024 and n >= 2 blocks of samples, unless

@@ -290,6 +290,12 @@ int sgd_fit_batch(Ctx* c, int B, const int32_t* col_pos, int loss, double alpha,
                   int max_iter, double tol, int shuffle, uint32_t seed, int lr_type, double eta0,
                   double power_t, double optimal_init, int n_iter_no_change, float* coef_out,
                   double* intercept_out, int32_t* n_iter_out, double* t_out, int32_t* status_out);
+// the same fit with per-column alpha / optimal_init and G order groups (rows grows[goff[g] .. goff[g+1]), seed gseed[g])
+int sgd_fit_groups(Ctx* c, int B, const int32_t* col_pos, const int32_t* col_group, const double* col_alpha,
+                   const double* col_oi, int G, const int64_t* goff, const int32_t* grows, const uint32_t* gseed,
+                   int loss, int fit_intercept, int max_iter, double tol, int shuffle, int lr_type, double eta0,
+                   double power_t, int n_iter_no_change, float* coef_out, double* intercept_out,
+                   int32_t* n_iter_out, double* t_out, int32_t* status_out);
 // 2-D fp16 row-major [rows x cols] TMA descriptor, box = [box_rows x 64 cols], 128B swizzle (logreg_tc.cu)
 int tc_make_map_2d(Ctx* c, CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows);
 void forest_free(Ctx* c);

@@ -16,7 +16,8 @@ of a batched solve on the GPU(s):
   cv_results_ assembly, best_*, refit          same arithmetic as search.py:461-550 (host)
 
 Base estimators with a device path: ``LogisticRegression`` (binary y, penalty l2, solver
-lbfgs) and ``Ridge`` (dense, single target).  Anything else raises NotImplementedError: by
+lbfgs), ``Ridge`` (dense, single target) and ``SGDClassifier`` (hinge / log_loss, penalty l2,
+searched over alpha; sgd_family.py).  Anything else raises NotImplementedError: by
 design there is no CPU fallback (the reference's joblib branch, search.py:388-409, is what
 the CPU baseline in bench.py times).
 """
@@ -30,7 +31,7 @@ from sklearn.utils.metaestimators import available_if
 from numpy.ma import MaskedArray
 from scipy.stats import rankdata
 from sklearn.base import BaseEstimator, is_classifier
-from sklearn.linear_model import LogisticRegression, Ridge
+from sklearn.linear_model import LogisticRegression, Ridge, SGDClassifier
 from sklearn.model_selection import (GridSearchCV, ParameterGrid, ParameterSampler,
                                      RandomizedSearchCV, check_cv)
 from sklearn.utils.validation import indexable
@@ -60,9 +61,12 @@ def _pick_family(estimator, candidate_params, X, y, scorers, enc=None):
     if type(estimator) is Ridge:
         from .ridge_family import _RidgeFamily
         return _RidgeFamily(estimator, candidate_params, X, y, scorers)
+    if type(estimator) is SGDClassifier:
+        from .sgd_family import _SGDFamily
+        return _SGDFamily(estimator, candidate_params, X, y, scorers, enc)
     raise NotImplementedError(
         "%s has no device path; supported base estimators: LogisticRegression(solver='lbfgs'), "
-        "Ridge.  (No CPU fallback by design.)" % type(estimator).__name__)
+        "Ridge, SGDClassifier.  (No CPU fallback by design.)" % type(estimator).__name__)
 
 
 # ----------------------------------------------------------------------------------------
@@ -118,6 +122,8 @@ class DistBaseSearchCV(_ScParamMixin):
                 layouts, n_splits = _cv_fold_groups(cv, X, y_arr, groups, n_samples, enc, train_orders)
                 fold = layouts[0][0]
                 family = _pick_family(estimator, candidate_params, X_arr, y_arr, scorers, enc)
+                if self.refit and self.preds and not hasattr(family, "fold_proba"):
+                    raise NotImplementedError("preds=True has no device path for %s" % type(estimator).__name__)
                 if hasattr(family, "prepare"):      # host-only statistics of the folds (no engine calls)
                     family.prepare(fold, layouts[0][1])
             finally:

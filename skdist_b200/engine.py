@@ -298,51 +298,55 @@ class Engine:
         `est` is the template SGDClassifier; host-side constants are derived exactly as
         SK/linear_model/_stochastic_gradient.py:455-473 and _sgd_fast.pyx.tp:447-452 do."""
         p = est.get_params(deep=False)
-        bad = []
-        loss = {"hinge": 0, "log_loss": 1}.get(p["loss"])
-        if loss is None:
-            bad.append("loss=%r" % p["loss"])
-        if p["penalty"] != "l2":
-            bad.append("penalty=%r" % (p["penalty"],))
-        lr = {"optimal": 0, "constant": 1, "invscaling": 2}.get(p["learning_rate"])
-        if lr is None:
-            bad.append("learning_rate=%r" % p["learning_rate"])
-        for k in ("average", "early_stopping", "warm_start"):
-            if p.get(k):
-                bad.append("%s=%r" % (k, p[k]))
-        if p.get("class_weight") is not None:
-            bad.append("class_weight")
-        if bad:
-            raise NotImplementedError("SGDClassifier configuration without a device path: " + ", ".join(bad))
-        from sklearn.utils import check_random_state
-        max_int = np.iinfo(np.int32).max
-        rs = check_random_state(p["random_state"])
-        rs.randint(1, max_int)                 # make_dataset() draws the dataset seed first
-        seed = int(rs.randint(max_int))
+        loss, lr = sgd_config(p)
+        seed = sgd_seed(p["random_state"])
         alpha = float(p["alpha"])
-        typw = np.sqrt(1.0 / np.sqrt(alpha))
-        if loss == 0:
-            g0 = -1.0 if -typw <= 1.0 else 0.0      # Hinge.cy_gradient(1.0, -typw)
-        else:
-            g0 = -1.0 / (1.0 + np.exp(-typw))       # CyHalfBinomialLoss.cy_gradient(1.0, -typw) < 0
-        optimal_init = 1.0 / ((typw / max(1.0, g0)) * alpha)
         col_pos = np.ascontiguousarray(col_pos, dtype=np.int32)
         B = col_pos.shape[0]
-        coef = np.empty((B, self.d), dtype=np.float32)
-        intercept = np.empty(B, dtype=np.float64)
-        n_iter = np.empty(B, dtype=np.int32)
-        t = np.empty(B, dtype=np.float64)
-        status = np.empty(B, dtype=np.int32)
+        out = _sgd_outputs(B, self.d)
         secs = ctypes.c_double(0.0)
         tol = -np.inf if p["tol"] is None else float(p["tol"])
         check(self._lib.skd_sgd_fit_batch(
             self._h, B, ptr(col_pos), loss, alpha, int(bool(p["fit_intercept"])), int(p["max_iter"]), tol,
-            int(bool(p["shuffle"])), seed, lr, float(p["eta0"]), float(p["power_t"]), float(optimal_init),
-            int(p["n_iter_no_change"]), ptr(coef), ptr(intercept), ptr(n_iter), ptr(t), ptr(status),
+            int(bool(p["shuffle"])), seed, lr, float(p["eta0"]), float(p["power_t"]), sgd_optimal_init(loss, alpha),
+            int(p["n_iter_no_change"]), ptr(out["coef32"]), ptr(out["intercept"]), ptr(out["n_iter"]), ptr(out["t"]),
+            ptr(out["status"]), ctypes.byref(secs)), self._h)
+        return _sgd_result(out, secs.value)
+
+    def sgd_fit_groups(self, params, col_pos, col_group, col_alpha, group_rows, group_seeds):
+        """Binary SGDClassifier fits in order groups: column j fits the rows group_rows[col_group[j]] (int row ids,
+        in the order the fit walks them before its first shuffle) with alpha col_alpha[j] and positives y_class ==
+        col_pos[j]; group g shuffles with its own seed group_seeds[g] (the `seed` _plain_sgd receives, see
+        sgd_seed).  `params` are the SGDClassifier parameters shared by every column (their alpha is unused)."""
+        loss, lr = sgd_config(params)
+        p = params
+        col_pos = np.ascontiguousarray(col_pos, dtype=np.int32)
+        col_group = np.ascontiguousarray(col_group, dtype=np.int32)
+        col_alpha = np.ascontiguousarray(col_alpha, dtype=np.float64)
+        B = col_pos.shape[0]
+        assert col_group.shape == (B,) and col_alpha.shape == (B,)
+        if self.n >= 2 ** 31:
+            raise NotImplementedError("sgd_fit_groups: the device path supports n < 2^31 rows (int32 row ids)")
+        col_oi = np.array([sgd_optimal_init(loss, a) if a > 0 else 1.0 for a in col_alpha], dtype=np.float64)
+        sizes = np.array([len(r) for r in group_rows], dtype=np.int64)
+        offsets = np.ascontiguousarray(np.concatenate([[0], np.cumsum(sizes)]), dtype=np.int64)
+        rows = np.ascontiguousarray(np.concatenate([np.asarray(r, dtype=np.int64) for r in group_rows])
+                                    if len(group_rows) else np.zeros(0, np.int64))
+        if rows.size and (rows.min() < 0 or rows.max() >= self.n):
+            raise ValueError("sgd_fit_groups: row ids outside [0, %d)" % self.n)
+        rows = rows.astype(np.int32)
+        seeds = np.ascontiguousarray(group_seeds, dtype=np.uint32)
+        assert seeds.shape == (len(group_rows),)
+        out = _sgd_outputs(B, self.d)
+        secs = ctypes.c_double(0.0)
+        tol = -np.inf if p["tol"] is None else float(p["tol"])
+        check(self._lib.skd_sgd_fit_groups(
+            self._h, B, ptr(col_pos), ptr(col_group), ptr(col_alpha), ptr(col_oi), len(group_rows), ptr(offsets),
+            ptr(rows), ptr(seeds), loss, int(bool(p["fit_intercept"])), int(p["max_iter"]), tol,
+            int(bool(p["shuffle"])), lr, float(p["eta0"]), float(p["power_t"]), int(p["n_iter_no_change"]),
+            ptr(out["coef32"]), ptr(out["intercept"]), ptr(out["n_iter"]), ptr(out["t"]), ptr(out["status"]),
             ctypes.byref(secs)), self._h)
-        return {"coef": np.concatenate([coef.astype(np.float64), intercept[:, None]], axis=1),
-                "coef32": coef, "intercept": intercept, "n_iter": n_iter, "t": t, "status": status,
-                "gpu_seconds": secs.value}
+        return _sgd_result(out, secs.value)
 
     def stage_forest_class_weights(self, n_classes, w=None, balanced_subsample=False, min_weight_fraction_leaf=0.0):
         """Class weights of the next forest_fit: w [n_classes] float64 (the same for every tree), or
@@ -493,6 +497,65 @@ class Engine:
         out = np.empty((self.n, B), dtype=np.float32)
         check(self._lib.skd_linear_decision(self._h, B, ptr(coef), ptr(out)), self._h)
         return out
+
+
+# -- SGDClassifier on the device ------------------------------------------------------------------
+SGD_LOSSES = {"hinge": 0, "log_loss": 1}
+SGD_LEARNING_RATES = {"optimal": 0, "constant": 1, "invscaling": 2}
+_MAX_INT = np.iinfo(np.int32).max
+
+
+def sgd_config(p):
+    """(loss code, learning-rate code) of SGDClassifier parameters `p` (get_params(deep=False)), or
+    NotImplementedError naming every setting the exact-order SGD kernels do not reproduce."""
+    bad = []
+    loss = SGD_LOSSES.get(p["loss"])
+    if loss is None:
+        bad.append("loss=%r" % p["loss"])
+    if p["penalty"] != "l2":
+        bad.append("penalty=%r" % (p["penalty"],))
+    lr = SGD_LEARNING_RATES.get(p["learning_rate"])
+    if lr is None:
+        bad.append("learning_rate=%r" % p["learning_rate"])
+    for k in ("average", "early_stopping", "warm_start"):
+        if p.get(k):
+            bad.append("%s=%r" % (k, p[k]))
+    if p.get("class_weight") is not None:
+        bad.append("class_weight")
+    if bad:
+        raise NotImplementedError("SGDClassifier configuration without a device path: " + ", ".join(bad))
+    return loss, lr
+
+
+def sgd_seed(random_state):
+    """The shuffle seed one binary fit hands to _plain_sgd (SK/linear_model/_stochastic_gradient.py:455-473):
+    make_dataset() draws the dataset seed first, then seed = randint(MAX_INT)."""
+    from sklearn.utils import check_random_state
+    rs = check_random_state(random_state)
+    rs.randint(1, _MAX_INT)
+    return int(rs.randint(_MAX_INT))
+
+
+def sgd_optimal_init(loss, alpha):
+    """optimal_init of the "optimal" schedule for loss code `loss` (SK/linear_model/_sgd_fast.pyx.tp:447-452)."""
+    typw = np.sqrt(1.0 / np.sqrt(alpha))
+    if loss == 0:
+        g0 = -1.0 if -typw <= 1.0 else 0.0      # Hinge.cy_gradient(1.0, -typw)
+    else:
+        g0 = -1.0 / (1.0 + np.exp(-typw))       # CyHalfBinomialLoss.cy_gradient(1.0, -typw) < 0
+    return float(1.0 / ((typw / max(1.0, g0)) * alpha))
+
+
+def _sgd_outputs(B, d):
+    return {"coef32": np.empty((B, d), dtype=np.float32), "intercept": np.empty(B, dtype=np.float64),
+            "n_iter": np.empty(B, dtype=np.int32), "t": np.empty(B, dtype=np.float64),
+            "status": np.empty(B, dtype=np.int32)}
+
+
+def _sgd_result(out, secs):
+    out["coef"] = np.concatenate([out["coef32"].astype(np.float64), out["intercept"][:, None]], axis=1)
+    out["gpu_seconds"] = secs
+    return out
 
 
 # -- per-process singleton -------------------------------------------------------------------
