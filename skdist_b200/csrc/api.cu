@@ -205,6 +205,74 @@ __global__ void finite_check_kernel(const float* __restrict__ X, int64_t total, 
   if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicOr(flag, 1);
 }
 
+// Entropy of one node in bits, as scikit-learn forms it (SK/tree/_criterion.pyx Entropy: e -= p * log(p),
+// p = s_c / w in class order, zero sums skipped; SK/tree/_utils.pyx: log(x) = ln(x) / ln(2.0)) with this
+// process's libm, the one scikit-learn calls
+static double entropy_bits(const double* s, int C, double w) {
+  const volatile double ln2 = std::log(2.0);
+  volatile double e = 0.0;
+  for (int c = 0; c < C; ++c) {
+    if (!(s[c] > 0.0)) continue;
+    const volatile double p = s[c] / w;
+    const volatile double lg = std::log(p) / ln2;
+    const volatile double t = p * lg;      // volatile: no contraction of the product into the difference
+    e = e - t;
+  }
+  return e;
+}
+
+// Gini of one node, 1 - sum_c s_c^2 / w^2 (SK/tree/_criterion.pyx:650-680)
+static double gini(const double* s, int C, double w) {
+  volatile double sq = 0.0;
+  for (int c = 0; c < C; ++c) {
+    const volatile double aa = s[c] * s[c];      // volatile: no contraction of the product into the sum
+    sq = sq + aa;
+  }
+  const volatile double ww = w * w;
+  const volatile double q = sq / ww;
+  return 1.0 - q;
+}
+
+// A node's float64 class sums s_c = cw_c * count_c (one rounding; cw: nullptr when unweighted) and their
+// total, weighted_n_node_samples, in class order (SK/tree/_criterion.pyx:483-486)
+template <class T>
+static double weighted_class_sums(const T* count, int C, const double* cw, double* s) {
+  volatile double w = 0.0;
+  for (int c = 0; c < C; ++c) {
+    const volatile double a = cw ? cw[c] * (double)count[c] : (double)count[c];
+    s[c] = a;
+    w = w + a;
+  }
+  return w;
+}
+
+// The impurity array of a classification tree (Gini, or entropy in bits) from its integer class sums, as the
+// builders and scikit-learn form it.  A node's impurity is the one its parent's children_impurity formed: for
+// the root (node_impurity) and a left child from the node's own sums; for a right child from sum_right_c =
+// cw_c * t_c - cw_c * l_c and w_right = w_node - w_left.  With non-dyadic class weights those can differ in
+// the last bits from the right child's own sums; the tree reports the impurity the builder compared with
+// EPSILON and used in the improvement.  Entropy uses this process's libm, the one scikit-learn calls: the
+// builder ranks candidates with CUDA's log, which differs from the host's in the last bit on a few inputs.
+// sums(i): node i's C class sums; children(i, l, r): node i's children, false for a leaf.
+template <class Sums, class Children>
+static void forest_class_impurity(int m, int C, const double* cw, bool entropy, Sums sums, Children children,
+                                  double* imp) {
+  if (m <= 0) return;
+  auto impurity = [&](const double* s, double w) { return entropy ? entropy_bits(s, C, w) : gini(s, C, w); };
+  std::vector<double> s(C), t(C);
+  imp[0] = impurity(s.data(), weighted_class_sums(sums(0), C, cw, s.data()));
+  for (int i = 0; i < m; ++i) {
+    int l, r;
+    if (!children(i, l, r)) continue;
+    const double wn = weighted_class_sums(sums(i), C, cw, t.data());
+    const double wl = weighted_class_sums(sums(l), C, cw, s.data());
+    imp[l] = impurity(s.data(), wl);
+    for (int c = 0; c < C; ++c) { const volatile double b = t[c] - s[c]; s[c] = b; }
+    const volatile double wr = wn - wl;
+    imp[r] = impurity(s.data(), wr);
+  }
+}
+
 extern "C" {
 
 int skd_version(void) { return 100; }
@@ -1383,69 +1451,25 @@ struct skd_forest {
   std::vector<float> binval;           // [d][256] distinct feature values (thresholds of compact records)
 };
 
-// Entropy of one node in bits, as scikit-learn forms it (SK/tree/_criterion.pyx Entropy: e -= p * log(p),
-// p = s_c / w in class order, zero sums skipped; SK/tree/_utils.pyx: log(x) = ln(x) / ln(2.0)) with this
-// process's libm, the one scikit-learn calls
-static double entropy_bits(const double* s, int C, double w) {
-  const volatile double ln2 = std::log(2.0);
-  volatile double e = 0.0;
-  for (int c = 0; c < C; ++c) {
-    if (!(s[c] > 0.0)) continue;
-    const volatile double p = s[c] / w;
-    const volatile double lg = std::log(p) / ln2;
-    const volatile double t = p * lg;      // volatile: no contraction of the product into the difference
-    e = e - t;
-  }
-  return e;
-}
-
-// The impurity array of an entropy tree of the general builder, from its integer class sums [m][C].  The
-// builder ranks candidates with CUDA's log, which differs from the host's in the last bit on a few inputs;
-// the tree reports the impurity scikit-learn computes.  A node's impurity is the one its parent's
-// children_impurity formed: for the root (node_impurity) and a left child from the node's own sums
-// s_c = cw_c * count_c (one rounding) and w = sum_c s_c; for a right child from sum_right = cw_c * t_c -
-// cw_c * l_c and w_right = w_node - w_left, the builder's (and scikit-learn's) operations, which with
-// non-dyadic class weights can differ in the last bits from the child's own sums (the rule
-// skd_forest_tree_copy applies to the Gini trees of the throughput builder).  cw: nullptr when unweighted.
-static void forest_entropy_impurity(int m, int C, const int32_t* left, const int32_t* right,
-                                    const unsigned long long* sums, const double* cw, double* imp) {
-  std::vector<double> s(C), t(C);
-  auto weighted = [&](const unsigned long long* cnt, double* out) {
-    volatile double w = 0.0;
-    for (int c = 0; c < C; ++c) {
-      const volatile double a = cw ? cw[c] * (double)cnt[c] : (double)cnt[c];
-      out[c] = a;
-      w = w + a;
-    }
-    return (double)w;
-  };
-  imp[0] = entropy_bits(s.data(), C, weighted(sums, s.data()));
-  for (int i = 0; i < m; ++i) {
-    const int l = left[i], r = right[i];
-    if (l < 0) continue;
-    const double wn = weighted(sums + (size_t)i * C, t.data());
-    const double wl = weighted(sums + (size_t)l * C, s.data());
-    imp[l] = entropy_bits(s.data(), C, wl);
-    for (int c = 0; c < C; ++c) { const volatile double b = t[c] - s[c]; s[c] = b; }
-    const volatile double wr = wn - wl;
-    imp[r] = entropy_bits(s.data(), C, wr);
-  }
-}
-
 static void forest_sink(void* arg, int t, const SkdTreeView* v) {
   skd_forest* f = (skd_forest*)arg;
   skd_forest::Tree& tr = f->trees[t];
   const int m = v->node_count;
   tr.max_depth = v->max_depth; tr.n_classes = v->n_classes; tr.node_count = m;
+  // the class weights the tree was built with, for the impurity formed from its class sums
+  std::vector<double> cw;
+  if (f->cw.n_classes && m > 0 && (v->compact || v->class_sums)) {
+    cw = f->cw.w;
+    if (f->cw.balanced_subsample) {   // the root's class sums are the bootstrap class counts
+      std::vector<uint32_t> root(v->n_classes);
+      for (int c = 0; c < v->n_classes; ++c) root[c] = v->compact ? v->compact[4 + c] : (uint32_t)v->class_sums[c];
+      cw.resize(v->n_classes);
+      forest_subsample_weights(root.data(), v->n_classes, cw.data());
+    }
+  }
   if (v->compact) {
     tr.compact.assign(v->compact, v->compact + (size_t)m * 8);
-    if (f->cw.n_classes) {
-      tr.cw = f->cw.w;
-      if (f->cw.balanced_subsample) {   // the root record's class sums are the bootstrap class counts
-        tr.cw.resize(v->n_classes);
-        forest_subsample_weights(v->compact + 4, v->n_classes, tr.cw.data());
-      }
-    }
+    tr.cw = std::move(cw);
     return;
   }
   tr.left.assign(v->left, v->left + m); tr.right.assign(v->right, v->right + m);
@@ -1454,18 +1478,11 @@ static void forest_sink(void* arg, int t, const SkdTreeView* v) {
   tr.thr.assign(v->threshold, v->threshold + m); tr.imp.assign(v->impurity, v->impurity + m);
   tr.wn.assign(v->weighted_n_node_samples, v->weighted_n_node_samples + m);
   tr.val.assign(v->value, v->value + (size_t)m * v->n_classes);
-  if (v->class_sums && m > 0) {
-    std::vector<double> cw;
-    if (f->cw.n_classes) {
-      cw = f->cw.w;
-      if (f->cw.balanced_subsample) {   // the root's class sums are the bootstrap class counts
-        std::vector<uint32_t> root(v->class_sums, v->class_sums + v->n_classes);
-        cw.resize(v->n_classes);
-        forest_subsample_weights(root.data(), v->n_classes, cw.data());
-      }
-    }
-    forest_entropy_impurity(m, v->n_classes, v->left, v->right, v->class_sums, cw.empty() ? nullptr : cw.data(),
-                            tr.imp.data());
+  if (v->class_sums) {   // entropy trees: the builder's impurity was formed with CUDA's log
+    const int C = v->n_classes;
+    forest_class_impurity(
+        m, C, cw.empty() ? nullptr : cw.data(), true, [&](int i) { return v->class_sums + (size_t)i * C; },
+        [&](int i, int& l, int& r) { l = v->left[i]; r = v->right[i]; return l >= 0; }, tr.imp.data());
   }
 }
 
@@ -1522,15 +1539,9 @@ int skd_forest_tree_copy(skd_forest* f, int32_t tree, int32_t* left, int32_t* ri
     // Compact records of the throughput builder: {right child, feature | bin_a << 16 | bin_b << 24,
     // n_node_samples, depth, class sums[4]}, nodes in depth-first order (left child = id + 1).  The
     // float64 fields are formed here with the builder's (= scikit-learn's) operations:
-    //   weighted_n = sum_c (double)s_c;  value_c = s_c / weighted_n            (SK/tree/_criterion.pyx:483-486)
-    //   impurity   = 1 - (sum_c s_c^2) / (weighted_n * weighted_n)             (Gini, :650-680; what the parent's
-    //                children_impurity computed from the same integers)
+    //   weighted_n = sum_c s_c;  value_c = s_c / weighted_n                     (weighted_class_sums)
+    //   impurity   = Gini, as forest_class_impurity forms it
     //   threshold  = v[a] / 2 + v[b] / 2                                        (SK/tree/_splitter.pyx:459-461)
-    // With class weights every s_c above is the weighted sum cw_c * s_c (one rounding), as in the builder,
-    // except the impurity of a right child: the builder (like scikit-learn) forms it at the parent from
-    // sum_right = cw_c * t_c - cw_c * l_c and w_right = w_node - w_left (ff_proxy4w), which with non-dyadic
-    // weights can differ in the last bits from the child's own sums; it is recomputed that way below, so the
-    // tree reports the impurity the builder compared with EPSILON and used in the improvement.
     const size_t m = (size_t)t.node_count;
     const int C = t.n_classes;
     const uint32_t* r = t.compact.data();
@@ -1552,47 +1563,25 @@ int skd_forest_tree_copy(skd_forest* f, int32_t tree, int32_t* left, int32_t* ri
           threshold[i] = ha + hb;
         }
       }
-      volatile double w = 0.0, sq = 0.0;
-      double s[4];
-      for (int c = 0; c < C; ++c) {
-        const volatile double a = cw ? cw[c] * (double)r[4 + c] : (double)r[4 + c];
-        s[c] = a;
-        w = w + a;
-        const volatile double aa = a * a;      // volatile: no contraction of the product into the sum
-        sq = sq + aa;
-      }
       if (n_node_samples) n_node_samples[i] = (int32_t)r[2];
-      if (weighted_n_node_samples) weighted_n_node_samples[i] = w;
-      if (impurity) { const volatile double ww = w * w; const volatile double q = sq / ww; impurity[i] = 1.0 - q; }
-      if (value) for (int c = 0; c < C; ++c) value[i * C + c] = s[c] / w;
       if (missing_go_to_left) missing_go_to_left[i] = 0;
+      double s[4];
+      const double w = weighted_class_sums(r + 4, C, cw, s);
+      if (weighted_n_node_samples) weighted_n_node_samples[i] = w;
+      if (value) for (int c = 0; c < C; ++c) value[i * C + c] = s[c] / w;
     }
-    if (impurity && cw) {
-      r = t.compact.data();
-      for (size_t i = 0; i < m; ++i) {
-        const int32_t rc = (int32_t)r[i * 8];
-        if ((r[i * 8 + 1] & 0xFFFFu) == 0xFFFFu || rc <= 0) continue;
-        const uint32_t* tp = r + i * 8 + 4;           // the parent's class sums
-        const uint32_t* lp = r + (i + 1) * 8 + 4;     // the left child's
-        volatile double wn = 0.0, wl = 0.0, sqr = 0.0;
-        for (int c = 0; c < C; ++c) { const volatile double st = cw[c] * (double)tp[c]; wn = wn + st; }
-        for (int c = 0; c < C; ++c) {
-          const volatile double st = cw[c] * (double)tp[c], a = cw[c] * (double)lp[c];
-          const volatile double b = st - a, bb = b * b;
-          wl = wl + a;
-          sqr = sqr + bb;
-        }
-        const volatile double wr = wn - wl, ww = wr * wr, q = sqr / ww;
-        impurity[rc] = 1.0 - q;
-      }
-    }
+    const uint32_t* rec = t.compact.data();
+    auto children = [&](int i, int& l, int& rc) {
+      rc = (int32_t)rec[(size_t)i * 8];
+      l = i + 1;
+      return (rec[(size_t)i * 8 + 1] & 0xFFFFu) != 0xFFFFu && rc > 0;
+    };
+    if (impurity)
+      forest_class_impurity((int)m, C, cw, false, [&](int i) { return rec + (size_t)i * 8 + 4; }, children, impurity);
     if (missing_go_to_left) {      // n_left > n_right (SK/tree/_splitter.pyx: best_split.missing_go_to_left with no missing values)
-      r = t.compact.data();
-      for (size_t i = 0; i < m; ++i) {
-        const int32_t rc = (int32_t)r[i * 8];
-        if ((r[i * 8 + 1] & 0xFFFFu) != 0xFFFFu && rc > 0)
-          missing_go_to_left[i] = r[(i + 1) * 8 + 2] > r[(size_t)rc * 8 + 2] ? 1 : 0;
-      }
+      int l, rc;
+      for (size_t i = 0; i < m; ++i)
+        if (children((int)i, l, rc)) missing_go_to_left[i] = rec[(size_t)l * 8 + 2] > rec[(size_t)rc * 8 + 2] ? 1 : 0;
     }
     return 0;
   }

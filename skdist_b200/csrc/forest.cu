@@ -121,36 +121,32 @@ __device__ __forceinline__ int fo_rand_int(int low, int high, uint32_t* seed) {
   return low + (int)(fo_rand_r(seed) % (uint32_t)(high - low));
 }
 
-// Gini children impurity, float64 with scikit-learn's operation order (no FMA contraction)
-template <int CM>
-__device__ __forceinline__ void fo_children_impurity(const unsigned long long* sl, const unsigned long long* st,
-                                                     int C, double wl, double wr, double* il, double* ir) {
-  double sql = 0.0, sqr = 0.0;
-#pragma unroll
-  for (int c = 0; c < CM; ++c) {
-    if (c < C) {
-      const double a = (double)sl[c], b = (double)(st[c] - sl[c]);
-      sql = __dadd_rn(sql, __dmul_rn(a, a));
-      sqr = __dadd_rn(sqr, __dmul_rn(b, b));
-    }
-  }
-  *il = __dsub_rn(1.0, __ddiv_rn(sql, __dmul_rn(wl, wl)));
-  *ir = __dsub_rn(1.0, __ddiv_rn(sqr, __dmul_rn(wr, wr)));
+// CM: compile-time bound on the class count (3 statistics when REG), so the per-class arrays of a thread live in registers.
+// W: class weights (classification only).  Histograms, records and the partition keep the integer
+// counts; the float64 statistics are w_c * count (one rounding), in scikit-learn's operation order.
+#define FOR_C(c) _Pragma("unroll") for (int c = 0; c < CM; ++c) if (c < C)
+
+// Class c's float64 sums of the left child (a) and of the right child (b) of a split: with class weights
+// sum_left[c] = w_c * count, sum_right[c] = sum_total[c] - sum_left[c] (ClassificationCriterion.update,
+// SK/tree/_criterion.pyx)
+template <bool W>
+__device__ __forceinline__ void fo_class_sums(const unsigned long long* sl, const unsigned long long* st,
+                                              const double* cw, int c, double* a, double* b) {
+  if constexpr (W) { *a = __dmul_rn(cw[c], (double)sl[c]); *b = __dsub_rn(__dmul_rn(cw[c], (double)st[c]), *a); }
+  else { *a = (double)sl[c]; *b = (double)(st[c] - sl[c]); }
 }
-// ... with class weights: sum_left[c] = w_c * count, sum_right[c] = sum_total[c] - sum_left[c]
-// (ClassificationCriterion.update, SK/tree/_criterion.pyx)
-template <int CM>
-__device__ __forceinline__ void fo_children_impurity_w(const unsigned long long* sl, const unsigned long long* st,
-                                                       const double* cw, int C, double wl, double wr, double* il,
-                                                       double* ir) {
+
+// Gini children impurity, float64 with scikit-learn's operation order (no FMA contraction)
+template <int CM, bool W>
+__device__ __forceinline__ void fo_children_gini(const unsigned long long* sl, const unsigned long long* st,
+                                                 const double* cw, int C, double wl, double wr, double* il,
+                                                 double* ir) {
   double sql = 0.0, sqr = 0.0;
-#pragma unroll
-  for (int c = 0; c < CM; ++c) {
-    if (c < C) {
-      const double a = __dmul_rn(cw[c], (double)sl[c]), b = __dsub_rn(__dmul_rn(cw[c], (double)st[c]), a);
-      sql = __dadd_rn(sql, __dmul_rn(a, a));
-      sqr = __dadd_rn(sqr, __dmul_rn(b, b));
-    }
+  FOR_C(c) {
+    double a, b;
+    fo_class_sums<W>(sl, st, cw, c, &a, &b);
+    sql = __dadd_rn(sql, __dmul_rn(a, a));
+    sqr = __dadd_rn(sqr, __dmul_rn(b, b));
   }
   *il = __dsub_rn(1.0, __ddiv_rn(sql, __dmul_rn(wl, wl)));
   *ir = __dsub_rn(1.0, __ddiv_rn(sqr, __dmul_rn(wr, wr)));
@@ -159,7 +155,7 @@ __device__ __forceinline__ void fo_children_impurity_w(const unsigned long long*
 // Entropy in bits (SK/tree/_criterion.pyx Entropy: e -= p * log(p), p = sum_c / w, classes with a zero sum
 // skipped; SK/tree/_utils.pyx: log(x) = ln(x) / ln(2.0)), one class's term, no FMA contraction.  CUDA's
 // log is not the host libm's: these values only rank candidates, the impurity of the finished tree is
-// formed on the host from the class sums (api.cu: forest_entropy_impurity).
+// formed on the host from the class sums (api.cu: forest_class_impurity).
 constexpr double FO_LN2 = 0.6931471805599453;   // == the host's log(2.0)
 __device__ __forceinline__ double fo_entropy_term(double e, double s, double w) {
   if (s > 0.0) {
@@ -168,33 +164,20 @@ __device__ __forceinline__ double fo_entropy_term(double e, double s, double w) 
   }
   return e;
 }
-// Entropy children impurity; W: with class weights, the statistics of fo_children_impurity_w
+// Entropy children impurity
 template <int CM, bool W>
 __device__ __forceinline__ void fo_children_entropy(const unsigned long long* sl, const unsigned long long* st,
                                                     const double* cw, int C, double wl, double wr, double* il,
                                                     double* ir) {
   double el = 0.0, er = 0.0;
-#pragma unroll
-  for (int c = 0; c < CM; ++c) {
-    if (c < C) {
-      double a, b;
-      if constexpr (W) { a = __dmul_rn(cw[c], (double)sl[c]); b = __dsub_rn(__dmul_rn(cw[c], (double)st[c]), a); }
-      else { a = (double)sl[c]; b = (double)(st[c] - sl[c]); }
-      el = fo_entropy_term(el, a, wl);
-      er = fo_entropy_term(er, b, wr);
-    }
+  FOR_C(c) {
+    double a, b;
+    fo_class_sums<W>(sl, st, cw, c, &a, &b);
+    el = fo_entropy_term(el, a, wl);
+    er = fo_entropy_term(er, b, wr);
   }
   *il = el;
   *ir = er;
-}
-// children impurity of a classification split under the fit's criterion (ENT: entropy, else Gini)
-template <int CM, bool W, bool ENT>
-__device__ __forceinline__ void fo_children_class(const unsigned long long* sl, const unsigned long long* st,
-                                                  const double* cw, int C, double wl, double wr, double* il,
-                                                  double* ir) {
-  if constexpr (ENT) fo_children_entropy<CM, W>(sl, st, cw, C, wl, wr, il, ir);
-  else if constexpr (W) fo_children_impurity_w<CM>(sl, st, cw, C, wl, wr, il, ir);
-  else fo_children_impurity<CM>(sl, st, C, wl, wr, il, ir);
 }
 
 // Node statistics are kept as 64-bit patterns so that the classification path (integer class
@@ -223,11 +206,61 @@ __device__ __forceinline__ void fo_children_mse(const unsigned long long* sl, co
   *ir = __dsub_rn(__ddiv_rn(sq_r, wr), __dmul_rn(mr, mr));
 }
 
-// CM: compile-time bound on the class count (3 statistics when REG), so the per-class arrays of a thread live in registers.
-// W: class weights (classification only).  Histograms, records and the partition keep the integer
-// counts; the float64 statistics are w_c * count (one rounding), in scikit-learn's operation order.
+// children impurity of a split under the fit's criterion (REG: MSE; ENT: entropy; else Gini)
+template <int CM, bool REG, bool W, bool ENT>
+__device__ __forceinline__ void fo_children(const unsigned long long* sl, const unsigned long long* st,
+                                            const double* cw, int C, double wl, double wr, double* il, double* ir) {
+  if constexpr (REG) fo_children_mse(sl, st, wl, wr, il, ir);
+  else if constexpr (ENT) fo_children_entropy<CM, W>(sl, st, cw, C, wl, wr, il, ir);
+  else fo_children_gini<CM, W>(sl, st, cw, C, wl, wr, il, ir);
+}
+
+// node_impurity (SK/tree/_criterion.pyx:620-640): the left-child impurity of the split that sends the whole
+// node left -- the same operations; the right half is dead code
+template <int CM, bool REG, bool W, bool ENT>
+__device__ __forceinline__ double fo_node_impurity(const unsigned long long* s, const double* cw, int C, double w) {
+  double imp, unused;
+  fo_children<CM, REG, W, ENT>(s, s, cw, C, w, w, &imp, &unused);
+  return imp;
+}
+
+// weighted_n of a node or child from its statistics s (REG: sum w; W: sum_c w_c * count_c)
+template <int CM, bool REG, bool W>
+__device__ __forceinline__ double fo_weight(const unsigned long long* s, const double* cw, int C) {
+  double w = 0.0;
+  if constexpr (REG) w = st_d(s[0]);
+  else if constexpr (W) { FOR_C(c) w = __dadd_rn(w, __dmul_rn(cw[c], (double)s[c])); }
+  else { FOR_C(c) w += (double)s[c]; }
+  return w;
+}
+
+// The split whose left child has the statistics sl (the node: st, w_node): false when a child is lighter
+// than min_weight_leaf (mwl), else its proxy_impurity_improvement and the children impurities.
+template <int CM, bool REG, bool W, bool ENT>
+__device__ __forceinline__ bool fo_eval_split(const unsigned long long* sl, const unsigned long long* st,
+                                              const double* cw, int C, double w_node, double mwl, double* proxy,
+                                              double* il, double* ir) {
+  const double wl = fo_weight<CM, REG, W>(sl, cw, C);
+  const double wr = w_node - wl;
+  if (wl < mwl || wr < mwl) return false;
+  fo_children<CM, REG, W, ENT>(sl, st, cw, C, wl, wr, il, ir);
+  if constexpr (REG) {   // MSE.proxy_impurity_improvement: sum_l^2 / w_l + sum_r^2 / w_r
+    const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(st[1]), sum_l);
+    *proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
+  } else {               // Criterion.proxy_impurity_improvement: -w_r * imp_r - w_l * imp_l
+    *proxy = __dsub_rn(__dmul_rn(-wr, *ir), __dmul_rn(wl, *il));
+  }
+  return true;
+}
+
+// node_split_random's threshold rand_uniform(lo, hi) from the drawn rand_r value (SK/tree/_utils.pyx:57-61),
+// and lo if it lands on hi (SK/tree/_splitter.pyx)
+__device__ __forceinline__ double fo_draw_threshold(double lo, double hi, uint32_t rnd) {
+  const double t = __dadd_rn(__ddiv_rn(__dmul_rn(__dsub_rn(hi, lo), (double)rnd), 2147483647.0), lo);
+  return t == hi ? lo : t;
+}
+
 #define FO_TICK(ph) do { if (P.o_prof && tid == 0) { const long long _t = clock64(); prof[ph] += _t - tlast; tlast = _t; } } while (0)
-#define FOR_C(c) _Pragma("unroll") for (int c = 0; c < CM; ++c) if (c < C)
 // ---------------- FO_SORT: node_split_best over the raw float32 values of one feature ----------------
 // (SK/tree/_splitter.pyx:262-504 with DensePartitioner.sort_samples_and_feature_values and next_p,
 // SK/tree/_partitioner.pyx:100-108, 209-215).  The node's values are sorted as order-preserving uint32
@@ -248,29 +281,6 @@ __device__ __forceinline__ uint32_t fo_fkey(float x) {
   return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
 }
 __device__ __forceinline__ float fo_kval(uint32_t k) { return __uint_as_float(k ^ ((k >> 31) ? 0x80000000u : 0xFFFFFFFFu)); }
-
-// Proxy of the split whose left child has the statistics sl (the node: st, w_node), with the left and
-// right impurities; -inf when a child is lighter than min_weight_leaf.  The histogram scan's float64
-// operations, in the same order.
-template <int CM, bool REG, bool W, bool ENT>
-__device__ __forceinline__ double fo_split_proxy(const unsigned long long* sl, const unsigned long long* st,
-                                                 const double* cw, int C, double w_node, double mwl,
-                                                 double* il, double* ir) {
-  double wl = 0.0;
-  if constexpr (REG) wl = st_d(sl[0]);
-  else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(cw[c], (double)sl[c])); }
-  else { FOR_C(c) wl += (double)sl[c]; }
-  const double wr = w_node - wl;
-  if (wl < mwl || wr < mwl) return -INFINITY;
-  if constexpr (REG) {
-    fo_children_mse(sl, st, wl, wr, il, ir);
-    const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(st[1]), sum_l);
-    return __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
-  } else {
-    fo_children_class<CM, W, ENT>(sl, st, cw, C, wl, wr, il, ir);
-    return __dsub_rn(__dmul_rn(-wr, *ir), __dmul_rn(wl, *il));
-  }
-}
 
 // Best split of one non-constant feature (values col[samp[i].x], node positions start .. start+m-1,
 // min lo < max hi) into *R, filled as the histogram scan fills it.  Called by the whole block; hist is
@@ -448,8 +458,8 @@ __device__ void fo_sort_split(const FoParams& P, const uint2* __restrict__ samp,
         const int n_left = e + 1;
         if (fo_kval(hib | nk) > fo_kval(hib | key[j]) + FEATURE_THRESHOLD &&
             n_left >= P.min_samples_leaf && m - n_left >= P.min_samples_leaf) {
-          double il, ir;
-          const double proxy = fo_split_proxy<CM, REG, W, ENT>(sl, st, cw, C, w_node, mwl, &il, &ir);
+          double proxy = -INFINITY, il, ir;
+          fo_eval_split<CM, REG, W, ENT>(sl, st, cw, C, w_node, mwl, &proxy, &il, &ir);
           if (proxy > bp) { bp = proxy; bj = j; bk = key[j]; bnk = nk; }
         }
       }
@@ -477,8 +487,8 @@ __device__ void fo_sort_split(const FoParams& P, const uint2* __restrict__ samp,
         FOR_C(c) a[c] = s_ex[c * FO_THREADS + tid];
 #pragma unroll
         for (int j = 0; j < FO_SORT_IPT; ++j) if (j <= bj) add(a, pos[j]);
-        double il, ir;
-        R->proxy = fo_split_proxy<CM, REG, W, ENT>(a, st, cw, C, w_node, mwl, &il, &ir);
+        double il, ir;   // the winner: a valid split
+        fo_eval_split<CM, REG, W, ENT>(a, st, cw, C, w_node, mwl, &R->proxy, &il, &ir);
         R->pos = start + gq; R->il = il; R->ir = ir;
         R->thr = (double)fo_kval(hib | bk) / 2.0 + (double)fo_kval(hib | bnk) / 2.0;
         FOR_C(c) R->sl[c] = a[c];
@@ -587,9 +597,7 @@ forest_build_kernel(const FoParams P) {
     red[tid] = v;
   }
   __syncthreads();
-  double w_samples = 0.0;
-  if constexpr (REG) w_samples = st_d(red[0]);
-  else if constexpr (W) {
+  if constexpr (W) {
     if (P.cw_bs) {   // compute_class_weight("balanced") of the bootstrap sample: n / (K_present * N_c)
       if (tid < C) {
         unsigned long long nt = 0; int kp = 0;
@@ -598,9 +606,8 @@ forest_build_kernel(const FoParams P) {
       }
       __syncthreads();
     }
-    FOR_C(c) w_samples = __dadd_rn(w_samples, __dmul_rn(s_cw[c], (double)red[c]));
   }
-  else { FOR_C(c) w_samples += (double)red[c]; }    // weighted_n_samples (integer valued)
+  const double w_samples = fo_weight<CM, REG, W>(red, s_cw, C);   // weighted_n_samples
   // BaseDecisionTree._fit: min_weight_leaf = min_weight_fraction_leaf * sum(sample_weight)
   const double mwl_w = W ? __dmul_rn(P.min_weight_fraction, w_samples) : 0.0;
 #define MIN_WEIGHT_LEAF (W ? mwl_w : P.min_weight_leaf)
@@ -634,30 +641,12 @@ forest_build_kernel(const FoParams P) {
     FO_TICK(0);
     const int start = rec.start, end = rec.end, depth = rec.depth;
     const int n_node = end - start;
-    double w_node = 0.0;
-    if constexpr (REG) w_node = st_d(rec.sums[0]);
-    else if constexpr (W) { FOR_C(c) w_node = __dadd_rn(w_node, __dmul_rn(s_cw[c], (double)rec.sums[c])); }
-    else { FOR_C(c) w_node += (double)rec.sums[c]; }
+    const double w_node = fo_weight<CM, REG, W>(rec.sums, s_cw, C);
     double impurity = rec.impurity;
     bool is_leaf = depth >= P.max_depth || n_node < P.min_samples_split || n_node < 2 * P.min_samples_leaf ||
                    w_node < 2.0 * MIN_WEIGHT_LEAF;
-    if (first) {   // root: node_impurity()  (SK/tree/_criterion.pyx:620-640)
-      if constexpr (REG) {   // MSE.node_impurity
-        const double mean = __ddiv_rn(st_d(rec.sums[1]), w_node);
-        impurity = __dsub_rn(__ddiv_rn(st_d(rec.sums[2]), w_node), __dmul_rn(mean, mean));
-      } else if constexpr (ENT) {   // Entropy.node_impurity
-        double e = 0.0;
-        FOR_C(c) e = fo_entropy_term(e, W ? __dmul_rn(s_cw[c], (double)rec.sums[c]) : (double)rec.sums[c], w_node);
-        impurity = e;
-      } else if constexpr (W) {
-        double sq = 0.0;
-        FOR_C(c) { const double a = __dmul_rn(s_cw[c], (double)rec.sums[c]); sq = __dadd_rn(sq, __dmul_rn(a, a)); }
-        impurity = __dsub_rn(1.0, __ddiv_rn(sq, __dmul_rn(w_node, w_node)));
-      } else {
-        double sq = 0.0;
-        FOR_C(c) { const double a = (double)rec.sums[c]; sq = __dadd_rn(sq, __dmul_rn(a, a)); }
-        impurity = __dsub_rn(1.0, __ddiv_rn(sq, __dmul_rn(w_node, w_node)));
-      }
+    if (first) {   // root: node_impurity()
+      impurity = fo_node_impurity<CM, REG, W, ENT>(rec.sums, s_cw, C, w_node);
       first = false;
     }
     is_leaf = is_leaf || impurity <= FO_EPSILON;
@@ -748,13 +737,17 @@ forest_build_kernel(const FoParams P) {
           }
           __syncthreads();
           FO_TICK(3);
+          auto block_minmax = [&](int k, float& lo, float& hi) {   // over the warps' min / max of feature k
+            lo = s_mm[0][0][k]; hi = s_mm[1][0][k];
+            for (int w = 1; w < FO_THREADS / 32; ++w) { lo = fminf(lo, s_mm[0][w][k]); hi = fmaxf(hi, s_mm[1][w][k]); }
+          };
           if constexpr (MODE == FO_SORT) {
             // node_split_best: the batch features one after another.  The commit discards every result
             // after the first constant feature, so the batch stops there.
             uint2* sbuf = P.srt + (size_t)slot * 2 * n;
             for (int k = 0; k < nbatch; ++k) {
-              float lo = s_mm[0][0][k], hi = s_mm[1][0][k];
-              for (int w = 1; w < FO_THREADS / 32; ++w) { lo = fminf(lo, s_mm[0][w][k]); hi = fmaxf(hi, s_mm[1][w][k]); }
+              float lo, hi;
+              block_minmax(k, lo, hi);
               if (hi <= lo + FEATURE_THRESHOLD) {   // SK/tree/_splitter.pyx:373-377, the same in every thread
                 if (tid == 0) results[k].is_const = 1;
                 break;
@@ -763,20 +756,15 @@ forest_build_kernel(const FoParams P) {
                                         lo, hi, rec.sums, s_cw, w_node, MIN_WEIGHT_LEAF, &results[k]);
             }
           } else {
-          // every thread forms the same decisions: constant test in float32, threshold
-          // rand_uniform(min, max) in float64 (SK/tree/_utils.pyx), and min if it lands on max
+          // every thread forms the same decisions: constant test in float32, drawn threshold in float64
           double thr[FO_KB_MAX];
 #pragma unroll
           for (int k = 0; k < FO_KB_MAX; ++k) {
-            float lo = s_mm[0][0][k], hi = s_mm[1][0][k];
-            for (int w = 1; w < FO_THREADS / 32; ++w) { lo = fminf(lo, s_mm[0][w][k]); hi = fmaxf(hi, s_mm[1][w][k]); }
+            float lo, hi;
+            block_minmax(k, lo, hi);
             thr[k] = -INFINITY;    // constant (or not in the batch): no sample goes left
-            if (k < nbatch && !(hi <= lo + FEATURE_THRESHOLD)) {
-              const double dlo = (double)lo, dhi = (double)hi;
-              double t = __dadd_rn(__ddiv_rn(__dmul_rn(__dsub_rn(dhi, dlo), (double)items[k].rnd), 2147483647.0), dlo);
-              if (t == dhi) t = dlo;
-              thr[k] = t;
-            }
+            if (k < nbatch && !(hi <= lo + FEATURE_THRESHOLD))
+              thr[k] = fo_draw_threshold((double)lo, (double)hi, items[k].rnd);
             if (tid == 0 && k < nbatch) { results[k].is_const = thr[k] == -INFINITY; results[k].thr = thr[k]; }
           }
           // pass B: (double)x <= threshold goes left (DensePartitioner.partition_samples); every thread
@@ -838,25 +826,11 @@ forest_build_kernel(const FoParams P) {
                 int n_left = 0;
                 for (int w = 0; w < FO_THREADS / 32; ++w) n_left += s_nl[w][k];
                 const int n_right = n_node - n_left;
-                if (n_left >= P.min_samples_leaf && n_right >= P.min_samples_leaf) {
-                  double wl = 0.0;
-                  if constexpr (REG) wl = st_d(sl[0]);
-                  else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(s_cw[c], (double)sl[c])); }
-                  else { FOR_C(c) wl += (double)sl[c]; }
-                  const double wr = w_node - wl;
-                  if (!(wl < MIN_WEIGHT_LEAF || wr < MIN_WEIGHT_LEAF)) {
-                    double il, ir;
-                    if constexpr (REG) {
-                      fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
-                      const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
-                      R->proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
-                    } else {
-                      fo_children_class<CM, W, ENT>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
-                      R->proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
-                    }
-                    R->pos = start + n_left; R->il = il; R->ir = ir;
-                    FOR_C(c) R->sl[c] = sl[c];
-                  }
+                double il, ir;
+                if (n_left >= P.min_samples_leaf && n_right >= P.min_samples_leaf &&
+                    fo_eval_split<CM, REG, W, ENT>(sl, rec.sums, s_cw, C, w_node, MIN_WEIGHT_LEAF, &R->proxy, &il, &ir)) {
+                  R->pos = start + n_left; R->il = il; R->ir = ir;
+                  FOR_C(c) R->sl[c] = sl[c];
                 }
               }
             }
@@ -966,9 +940,7 @@ forest_build_kernel(const FoParams P) {
               FOR_C(c) sl[c] = 0;
               int nin = 0;
               if (!is_const) {
-                const double lo = (double)bv[gfirst], hi = (double)bv[glast];
-                thr = __dadd_rn(__ddiv_rn(__dmul_rn(__dsub_rn(hi, lo), (double)items[k].rnd), 2147483647.0), lo);
-                if (thr == hi) thr = lo;
+                thr = fo_draw_threshold((double)bv[gfirst], (double)bv[glast], items[k].rnd);
   #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                   const int bb = lane * 8 + j;
@@ -994,25 +966,11 @@ forest_build_kernel(const FoParams P) {
                 R->is_const = is_const; R->proxy = -INFINITY; R->pos = end; R->bin = cutbin; R->thr = thr;
                 if (!is_const) {
                   const int n_left = (int)n_left_u, n_right = n_node - n_left;
-                  if (n_left >= P.min_samples_leaf && n_right >= P.min_samples_leaf) {
-                    double wl = 0.0;
-                    if constexpr (REG) wl = st_d(sl[0]);
-                    else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(s_cw[c], (double)sl[c])); }
-                    else { FOR_C(c) wl += (double)sl[c]; }
-                    const double wr = w_node - wl;
-                    if (!(wl < MIN_WEIGHT_LEAF || wr < MIN_WEIGHT_LEAF)) {
-                      double il, ir;
-                      if constexpr (REG) {
-                        fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
-                        const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
-                        R->proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
-                      } else {
-                        fo_children_class<CM, W, ENT>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
-                        R->proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
-                      }
-                      R->pos = start + n_left; R->il = il; R->ir = ir;
-                      FOR_C(c) R->sl[c] = sl[c];
-                    }
+                  double il, ir;
+                  if (n_left >= P.min_samples_leaf && n_right >= P.min_samples_leaf &&
+                      fo_eval_split<CM, REG, W, ENT>(sl, rec.sums, s_cw, C, w_node, MIN_WEIGHT_LEAF, &R->proxy, &il, &ir)) {
+                    R->pos = start + n_left; R->il = il; R->ir = ir;
+                    FOR_C(c) R->sl[c] = sl[c];
                   }
                 }
               }
@@ -1039,19 +997,17 @@ forest_build_kernel(const FoParams P) {
                 if (!(bv[nb2] > bv[bb] + FEATURE_THRESHOLD)) continue;       // values within 1e-7: same run
                 const int n_left = (int)run_cnt, n_right = n_node - n_left;
                 if (n_left < P.min_samples_leaf || n_right < P.min_samples_leaf) continue;
-                double wl = 0.0;
-                if constexpr (REG) wl = st_d(sl[0]);
-                else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(s_cw[c], (double)sl[c])); }
-                else { FOR_C(c) wl += (double)sl[c]; }
+                // fo_eval_split's operations, written out: through the helper the histogram instantiations
+                // spill more (profiles/README.md)
+                const double wl = fo_weight<CM, REG, W>(sl, s_cw, C);
                 const double wr = w_node - wl;
                 if (wl < MIN_WEIGHT_LEAF || wr < MIN_WEIGHT_LEAF) continue;
                 double il, ir, proxy;
-                if constexpr (REG) {     // MSE.proxy_impurity_improvement: sum_l^2 / w_l + sum_r^2 / w_r
-                  fo_children_mse(sl, rec.sums, wl, wr, &il, &ir);
+                fo_children<CM, REG, W, ENT>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
+                if constexpr (REG) {
                   const double sum_l = st_d(sl[1]), sum_r = __dsub_rn(st_d(rec.sums[1]), sum_l);
                   proxy = __dadd_rn(__ddiv_rn(__dmul_rn(sum_l, sum_l), wl), __ddiv_rn(__dmul_rn(sum_r, sum_r), wr));
-                } else {                 // Criterion.proxy_impurity_improvement: -w_r * imp_r - w_l * imp_l
-                  fo_children_class<CM, W, ENT>(sl, rec.sums, s_cw, C, wl, wr, &il, &ir);
+                } else {
                   proxy = __dsub_rn(__dmul_rn(-wr, ir), __dmul_rn(wl, il));
                 }
                 if (proxy > bproxy) {
@@ -1117,10 +1073,7 @@ forest_build_kernel(const FoParams P) {
         s_ctrl[6] = best_mgl;
         s_dbl[0] = best_thr; s_dbl[1] = best_il; s_dbl[2] = best_ir;
         if (best_pos < end) {
-          double wl = 0.0;
-          if constexpr (REG) wl = st_d(best_sl[0]);
-          else if constexpr (W) { FOR_C(c) wl = __dadd_rn(wl, __dmul_rn(s_cw[c], (double)best_sl[c])); }
-          else { FOR_C(c) wl += (double)best_sl[c]; }
+          const double wl = fo_weight<CM, REG, W>(best_sl, s_cw, C);
           const double wr = w_node - wl;
           // impurity_improvement (SK/tree/_criterion.pyx:163-190)
           const double a = __dmul_rn(__ddiv_rn(wr, w_node), best_ir);
