@@ -203,7 +203,8 @@ int skd_linear_logloss_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, const f
 /* Batched Ridge: B independent (alpha, fold) columns from one pass over the staged X and the
  * staged real targets.  Column j trains on rows whose fold id != col_fold[j] (col_fold[j] < 0: all
  * rows).  coef_out[j*(d+1)+k] (k<d weights, k==d intercept); status_out[j] 1 = ok, 4 = matrix not
- * positive definite.
+ * positive definite.  Supports d <= 338 (each column's Cholesky factor is held in shared memory);
+ * larger d fails with an error before any work is launched.
  * ref: replaces B invocations of search.py:180-288 with estimator = Ridge (dense, solver
  * auto->cholesky): SK/linear_model/_base.py:113-220 (centring), SK/linear_model/_ridge.py:215-234
  * (_solve_cholesky: X^T X, X^T y, LAPACK posv). */

@@ -4,12 +4,16 @@
 // Ridge.fit): centring (SK/linear_model/_base.py:189-199), A = Xc^T Xc and Xc^T yc by sgemm
 // (SK/linear_model/_ridge.py:215-221), scipy.linalg.solve(assume_a="pos") (:223-234).
 // The reference recomputes the same Gram matrix for every alpha and every fold; here
+//       colsum / colmean         : global shifts mu = mean(X) and yg = mean(y) (with an intercept;
+//                                  0 without), float64 slab partials added in slab order
 //   K4  gram_kernel / xty_kernel : per-fold-block  S_f = X_f^T X_f,  v_f = X_f^T y_f,  s_f = sum x,
-//                                  sum y, sum y^2  in one pass (rows visited fold by fold through a
-//                                  permutation; fp32 products, fp32 accumulation inside a chunk of
-//                                  <= 2048 rows, float64 across chunks)
+//                                  sum y, sum y^2  in one pass, all on x - mu and y - yg (rows visited
+//                                  fold by fold through a permutation; fp32 products summed per block of
+//                                  16 rows, fp32 over the blocks of a chunk of <= 2048 rows, float64
+//                                  across chunks)
 //       ridge_prepare_kernel     : training statistics of fold f = total - block f, centred in
-//                                  float64:  A_f = S - n xbar xbar^T,  b_f = v - n xbar ybar
+//                                  float64:  A_f = S - n xbar xbar^T,  b_f = v - n xbar ybar; the
+//                                  intercept's ybar gets yg back
 //   K5  ridge_solve_kernel       : one CTA per (alpha, fold): A_f + alpha I -> fp32 Cholesky in
 //                                  shared memory (packed lower triangle) -> two triangular solves
 //                                  (the arithmetic class of LAPACK sposv)
@@ -28,24 +32,46 @@ struct GramChunk {
   int32_t fold;
 };
 
-// Global column means (float64 atomics over 4096-row slabs).  All block statistics below are taken
-// on x - mu so that "S - n xbar xbar^T" never cancels leading digits on uncentred data (the
-// reference centres X before forming the Gram matrix, SK/linear_model/_base.py:196).
-__global__ void colsum_kernel(const float* __restrict__ X, int64_t n, int ldx, int d, double* __restrict__ sum) {
-  int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= d) return;
-  int64_t r0 = (int64_t)blockIdx.y * 4096, r1 = r0 + 4096 < n ? r0 + 4096 : n;
+// The packed Cholesky factor and the right-hand side of one column live in shared memory; the largest
+// d whose buffer fits the 226 KB the solve kernel opts into is 338 (230 516 B; d = 339 needs 231 876 B).
+constexpr size_t ridge_smem_bytes(int64_t d) { return ((size_t)d * (d + 1) / 2 + (size_t)d) * sizeof(float); }
+constexpr int RIDGE_MAX_D = 338;
+constexpr size_t RIDGE_SMEM_CAP = 226 * 1024;
+static_assert(ridge_smem_bytes(RIDGE_MAX_D) <= RIDGE_SMEM_CAP && ridge_smem_bytes(RIDGE_MAX_D + 1) > RIDGE_SMEM_CAP,
+              "RIDGE_MAX_D must be the largest d whose solve buffer fits RIDGE_SMEM_CAP");
+constexpr int CS_SLAB = 4096;  // rows per column-sum partial
+
+// Global column means of X and, in column d, the mean of y: float64 partials over 4096-row slabs,
+// added in slab order by colmean_kernel (so mu and the target shift are the same on every run).
+// All block statistics below are taken on x - mu and y - ybar_g, so that "S - n xbar xbar^T" and
+// "v - n xbar ybar" never cancel leading digits on uncentred features or targets (the reference
+// centres X and y before forming X^T X and X^T y, SK/linear_model/_base.py:196-199).
+__global__ void colsum_kernel(const float* __restrict__ X, const float* __restrict__ y, int64_t n, int ldx, int d,
+                              double* __restrict__ part /*[slab][d + 1]*/) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k > d) return;
+  const int64_t r0 = (int64_t)blockIdx.y * CS_SLAB, r1 = r0 + CS_SLAB < n ? r0 + CS_SLAB : n;
   double a = 0.0;
-  for (int64_t r = r0; r < r1; ++r) a += (double)X[r * ldx + k];
-  atomicAdd(&sum[k], a);
+  if (k < d)
+    for (int64_t r = r0; r < r1; ++r) a += (double)X[r * ldx + k];
+  else
+    for (int64_t r = r0; r < r1; ++r) a += (double)y[r];
+  part[(size_t)blockIdx.y * (d + 1) + k] = a;
 }
-__global__ void colmean_kernel(const double* __restrict__ sum, int64_t n, int d, int ldx, float* __restrict__ mu) {
-  int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k < ldx) mu[k] = k < d ? (float)(sum[k] / (double)n) : 0.f;
+// mu[0..ldx) = column means (0 on the padding), mu[ldx] = mean of y
+__global__ void colmean_kernel(const double* __restrict__ part, int nslab, int64_t n, int d, int ldx,
+                               float* __restrict__ mu) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k > ldx) return;
+  if (k >= d && k < ldx) { mu[k] = 0.f; return; }
+  const int col = k < d ? k : d;
+  double a = 0.0;
+  for (int s = 0; s < nslab; ++s) a += part[(size_t)s * (d + 1) + col];
+  mu[k] = (float)(a / (double)n);
 }
 
 // Partial Gram of one chunk for one (ti <= tj) tile pair: Gp[(chunk * npairs + pair)][64][64]
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, 4)   // 64 registers: four CTAs per SM
 gram_kernel(const float* __restrict__ X, int ldx, const float* __restrict__ mu,
             const int32_t* __restrict__ perm, const GramChunk* __restrict__ chunks, int ntile,
             float* __restrict__ Gp) {
@@ -84,6 +110,14 @@ gram_kernel(const float* __restrict__ X, int ldx, const float* __restrict__ mu,
       *reinterpret_cast<float4*>(&Bs[r][q]) = b;
     }
     __syncthreads();
+    // products of the 16 rows summed on their own, then added to the chunk sum: the fp32 rounding error
+    // grows with 16 + len/16 additions instead of len (sequentially over 2048 rows it exceeds that of a
+    // float32 GEMM and shows in the coefficients)
+    float blk[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) blk[i][j] = 0.f;
 #pragma unroll
     for (int k = 0; k < GR_K; ++k) {
       float a[4], b[4];
@@ -94,8 +128,12 @@ gram_kernel(const float* __restrict__ X, int ldx, const float* __restrict__ mu,
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+        for (int j = 0; j < 4; ++j) blk[i][j] = fmaf(a[i], b[j], blk[i][j]);
     }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) acc[i][j] += blk[i][j];
     __syncthreads();
   }
   float* out = Gp + ((size_t)blockIdx.y * npairs + pair) * (GR_T * GR_T);
@@ -105,7 +143,9 @@ gram_kernel(const float* __restrict__ X, int ldx, const float* __restrict__ mu,
         make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
 }
 
-// X^T y, sum x per chunk (threads over features), sum y / sum y^2 / count per chunk
+// (X - mu)^T (y - yg), sum (x - mu) per chunk (threads over features), sum (y - yg) / sum (y - yg)^2 per
+// chunk.  yg = mu[ldx] is the global mean of y with an intercept and 0 without one: the fp32 products
+// and chunk sums then carry the spread of y, not its offset.
 __global__ void __launch_bounds__(256)
 xty_kernel(const float* __restrict__ X, int ldx, int d, const float* __restrict__ mu,
            const float* __restrict__ y,
@@ -114,15 +154,22 @@ xty_kernel(const float* __restrict__ X, int ldx, int d, const float* __restrict_
            double* __restrict__ yp /*[chunk][2]*/) {
   __shared__ double red[2][8];
   const GramChunk ch = chunks[blockIdx.x];
+  const float yg = mu[ldx];
   for (int k0 = 0; k0 < ldx; k0 += 256) {
     const int k = k0 + threadIdx.x;
     float av = 0.f, as = 0.f;
     if (k < ldx) {
-      for (int r = 0; r < ch.len; ++r) {
-        const int32_t row = perm[ch.start + r];
-        const float xv = X[(int64_t)row * ldx + k] - mu[k];
-        av = fmaf(xv, y[row], av);
-        as += xv;
+      for (int r0 = 0; r0 < ch.len; r0 += GR_K) {     // blocks of 16 rows, as gram_kernel
+        const int r1 = r0 + GR_K < ch.len ? r0 + GR_K : ch.len;
+        float bv = 0.f, bs = 0.f;
+        for (int r = r0; r < r1; ++r) {
+          const int32_t row = perm[ch.start + r];
+          const float xv = X[(int64_t)row * ldx + k] - mu[k];
+          bv = fmaf(xv, y[row] - yg, bv);
+          bs += xv;
+        }
+        av += bv;
+        as += bs;
       }
       vp[(size_t)blockIdx.x * ldx + k] = av;
       sp[(size_t)blockIdx.x * ldx + k] = as;
@@ -130,7 +177,7 @@ xty_kernel(const float* __restrict__ X, int ldx, int d, const float* __restrict_
   }
   double sy = 0.0, syy = 0.0;
   for (int r = threadIdx.x; r < ch.len; r += 256) {
-    const double v = (double)y[perm[ch.start + r]];
+    const double v = (double)(y[perm[ch.start + r]] - yg);
     sy += v;
     syy += v * v;
   }
@@ -192,7 +239,8 @@ __global__ void gram_reduce_kernel(const float* __restrict__ Gp, const float* __
 }
 
 // Training statistics for "hold out fold h" (h == n_folds: hold out nothing), centred.
-// A[h][dG x dG] fp32, b[h][dG] fp32, xbar[h][dG] fp32, misc[h] = {ybar, n_train}
+// A[h][dG x dG] fp32, b[h][dG] fp32, xbar[h][dG] fp32, misc[h] = {ybar, n_train}.  The block sums are on
+// y - yg; centring removes yg from b, and misc gets it back so that ybar is the mean of the original y.
 __global__ void ridge_prepare_kernel(const double* __restrict__ S, const double* __restrict__ v,
                                      const double* __restrict__ s, const double* __restrict__ ys,
                                      const float* __restrict__ mu, int ldx,
@@ -227,7 +275,10 @@ __global__ void ridge_prepare_kernel(const double* __restrict__ S, const double*
       xbar[(size_t)h * dG + r] = fit_intercept && ntr > 0 ? (float)((double)(r < ldx ? mu[r] : 0.f) + sr / ntr) : 0.f;
     }
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0) { misc[h * 2] = ybar; misc[h * 2 + 1] = ntr; }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    misc[h * 2] = fit_intercept && ntr > 0 ? ybar + (double)mu[ldx] : 0.0;
+    misc[h * 2 + 1] = ntr;
+  }
 }
 
 // One CTA per column: fp32 Cholesky of (A_h + alpha I) on the packed lower triangle in shared
@@ -312,8 +363,8 @@ int ridge_fit_batch(Ctx* c, int B, const double* alpha, const int32_t* hold, int
   const int d = (int)c->d, ldx = (int)c->ldx;
   if (!c->yreal) return fail(c, "ridge: stage real-valued targets first (skd_stage_targets)");
   const int ntile = (d + GR_T - 1) / GR_T, dG = ntile * GR_T;
-  const size_t smem = ((size_t)d * (d + 1) / 2 + d) * sizeof(float);
-  if (smem > 226 * 1024) return fail(c, "ridge: device path supports d <= 330 (Cholesky in shared memory)");
+  if (d > RIDGE_MAX_D) return fail(c, "ridge: device path supports d <= 338 (Cholesky in shared memory)");
+  const size_t smem = ridge_smem_bytes(d);
   const int n_folds = c->fold ? c->n_folds : 1;
   // host: permutation of rows by fold + chunk table (chunks never straddle a fold)
   std::vector<int8_t> hfold;
@@ -339,14 +390,15 @@ int ridge_fit_batch(Ctx* c, int B, const double* alpha, const int32_t* hold, int
   int32_t* dperm; GramChunk* dchunks; float *Gp, *vp, *sp; double* yp;
   double *S, *v, *s, *ys, *misc; float *A, *bv, *xbar;
   double* dalpha; int32_t* dhold; float* dcoef; int32_t* dstatus;
-  double* colsum; float* mu;
-  SKD_CUDA(c, sx.alloc(&colsum, (size_t)ldx));
-  SKD_CUDA(c, sx.alloc(&mu, (size_t)ldx));
-  SKD_CUDA(c, cudaMemsetAsync(colsum, 0, (size_t)ldx * sizeof(double), c->stream));
-  SKD_CUDA(c, cudaMemsetAsync(mu, 0, (size_t)ldx * sizeof(float), c->stream));
+  // mu[0..ldx): feature shift, mu[ldx]: target shift; all zero without an intercept
+  double* colpart; float* mu;
+  const int nslab = (int)((n + CS_SLAB - 1) / CS_SLAB);
+  SKD_CUDA(c, sx.alloc(&mu, (size_t)ldx + 1));
+  SKD_CUDA(c, cudaMemsetAsync(mu, 0, ((size_t)ldx + 1) * sizeof(float), c->stream));
   if (fit_intercept) {
-    colsum_kernel<<<dim3((d + 127) / 128, (unsigned)((n + 4095) / 4096)), 128, 0, c->stream>>>(c->X, n, ldx, d, colsum);
-    colmean_kernel<<<(ldx + 127) / 128, 128, 0, c->stream>>>(colsum, n, d, ldx, mu);
+    SKD_CUDA(c, sx.alloc(&colpart, (size_t)nslab * (d + 1)));
+    colsum_kernel<<<dim3((d + 1 + 127) / 128, (unsigned)nslab), 128, 0, c->stream>>>(c->X, c->yreal, n, ldx, d, colpart);
+    colmean_kernel<<<(ldx + 1 + 127) / 128, 128, 0, c->stream>>>(colpart, nslab, n, d, ldx, mu);
     c->launches += 2;
   }
   SKD_CUDA(c, sx.alloc(&dperm, (size_t)n));

@@ -14,6 +14,8 @@ from .base import _clone, _merged_params
 from .folds import _train_codes
 
 _RIDGE_SEARCHABLE = {"alpha", "fit_intercept"}
+# each column's packed Cholesky factor lives in one CTA's shared memory (csrc/ridge.cu RIDGE_MAX_D)
+_RIDGE_MAX_FEATURES = 338
 
 
 def _resolve(estimator, params):
@@ -51,6 +53,9 @@ class _RidgeFamily:
         self.cands = [_check_ridge(q) for q in _merged_params(estimator, candidate_params)]
         if np.ndim(y) != 1:
             raise NotImplementedError("multi-target Ridge has no device path")
+        if X.shape[1] > _RIDGE_MAX_FEATURES:
+            raise NotImplementedError("Ridge with %d features has no device path (supported: n_features <= %d)"
+                                      % (X.shape[1], _RIDGE_MAX_FEATURES))
         self.y = np.asarray(y, dtype=np.float32)
         # scorers that are functions of the per-column (sum of squared residuals, row count):
         # r2 (also estimator.score), neg_mean_squared_error, neg_root_mean_squared_error

@@ -85,6 +85,23 @@ def test_ridge_randomized_matches_oracle(fake_engine):
     pickle.loads(pickle.dumps(rs))
 
 
+def test_ridge_feature_bound_is_checked_up_front(fake_engine):
+    """The device solve holds d <= 338 (one CTA's shared memory per Cholesky factor): one more feature is a
+    NotImplementedError before any fit, like every other configuration without a device path."""
+    from sklearn.linear_model import Ridge
+    from skdist_b200 import engine
+    from tests.fake_engine import FakeEngine
+    made = []
+    engine.set_engine_factory(lambda: made.append(FakeEngine()) or made[-1])
+    rng = np.random.default_rng(0)
+    X, y = rng.standard_normal((400, 339)).astype(np.float32), rng.standard_normal(400).astype(np.float32)
+    with pytest.raises(NotImplementedError, match="n_features <= 338"):
+        DistGridSearchCV(Ridge(), {"alpha": [1.0]}, None, cv=3).fit(X, y)
+    assert not any(call[0] == "ridge" for e in made for call in e.calls)
+    gs = DistGridSearchCV(Ridge(), {"alpha": [1.0, 10.0]}, None, cv=3).fit(X[:, :338], y)
+    assert gs.best_estimator_.coef_.shape == (338,)
+
+
 @pytest.mark.filterwarnings("ignore")
 def test_multi_model_search_matches_reference_semantics(fake_engine):
     """DistMultiModelSearch: per-model ParameterSampler draws with the shared random_state, plain
