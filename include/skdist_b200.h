@@ -154,8 +154,8 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
 int skd_linear_score_batch(skd_ctx* ctx, int32_t B, const float* coef, const int32_t* col_fold,
                            const int32_t* col_pos, int64_t* correct_out, int64_t* count_out);
 
-/* B multinomial (n_classes > 2) L2 logistic regressions sharing the staged X and class ids
- * 0..n_classes-1: candidate j minimises mean_i[logsumexp(W x_i + b) - (W x_i + b)_{y_i}] +
+/* B multinomial (n_classes >= 2) L2 logistic regressions sharing the staged X and class ids
+ * 0..n_classes-1 (the call fails, naming the staged range, when a class id lies outside it): candidate j minimises mean_i[logsumexp(W x_i + b) - (W x_i + b)_{y_i}] +
  * 0.5 / (C[j] * n_train) * ||W||^2 over the rows whose fold id != col_fold[j] (col_fold[j] < 0: all
  * rows) with L-BFGS-B from W = 0 (m = 10, maxls = 50, gtol = tol, ftol = 64 eps, like scikit-learn's
  * call).  coef_out[(j * n_classes + k) * (d+1) + i]: i < d weights of class k, i == d its intercept.
@@ -168,9 +168,23 @@ int skd_logreg_multinomial_fit_batch(skd_ctx* ctx, int32_t B, int32_t n_classes,
                                      float* coef_out, int32_t* n_iter_out, int32_t* status_out, double* loss_out,
                                      int32_t* n_evals_out, double* gpu_seconds_out);
 
+/* Objective and gradient of B multinomial candidates at caller-supplied points
+ * w_in[(j * n_classes + k) * (d+1) + i] (float64, the layout of coef_out above; cast to fp32 for the products as
+ * scikit-learn does, intercepts read as 0 without fit_intercept).  loss_out[j], grad_out (same layout as w_in)
+ * follow SK/linear_model/_linear_loss.py:291-379, multiclass branch (mean loss + 0.5*l2*|W|^2, intercepts
+ * unpenalised).  Staged class weights and column masks apply as in skd_logreg_multinomial_fit_batch and are
+ * consumed by this call.  Diagnostic / test entry: it runs the passes, buffers, evaluation kernels and gradient
+ * reduction of one round of skd_logreg_multinomial_fit_batch on the same batch, every candidate active.  Fails
+ * like the fit on class ids outside 0..n_classes-1, C <= 0, an empty training set or staged inputs that do not
+ * match B (x d, x n_classes). */
+int skd_logreg_multinomial_loss_grad(skd_ctx* ctx, int32_t B, int32_t n_classes, const double* w_in, const double* C,
+                                     const int32_t* col_fold, int32_t fit_intercept, double* loss_out,
+                                     double* grad_out);
+
 /* Accuracy counts of B multiclass linear classifiers (coef laid out as above): prediction =
  * first arg max_k (W x + b)_k compared with the staged class id, on the rows selected by the fold
- * codes of skd_linear_score_batch.
+ * codes of skd_linear_score_batch.  This entry, the confusion counts below and the multiclass log loss fail
+ * when a staged class id lies outside 0..n_classes-1.
  * ref: replaces search.py:264 (_score -> ClassifierMixin.score -> accuracy_score). */
 int skd_multinomial_score_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, const float* coef,
                                 const int32_t* col_fold, int64_t* correct_out, int64_t* count_out);

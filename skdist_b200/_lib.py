@@ -54,6 +54,8 @@ SYMBOLS = {
     "skd_logreg_multinomial_fit_batch": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_int32, _c.c_void_p, _c.c_void_p,
                                                     _c.c_int32, _c.c_double, _c.c_int32, _c.c_void_p, _c.c_void_p,
                                                     _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.POINTER(_c.c_double)]),
+    "skd_logreg_multinomial_loss_grad": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_int32, _c.c_void_p, _c.c_void_p,
+                                                    _c.c_void_p, _c.c_int32, _c.c_void_p, _c.c_void_p]),
     "skd_multinomial_score_batch": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_int32, _c.c_void_p, _c.c_void_p,
                                                _c.c_void_p, _c.c_void_p]),
     "skd_multinomial_confusion_batch": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_int32, _c.c_void_p, _c.c_void_p,

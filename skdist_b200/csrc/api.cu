@@ -466,6 +466,7 @@ static void drop_stale_row_vectors(Ctx* c, int64_t n_new) {
   c->fold_count.clear();
   c->h_fold.clear();
   c->h_ycls.clear();
+  c->ycls_min = 0; c->ycls_max = -1;
   c->row_bits = {};
   c->tc.meta_valid = false;
   c->vec_n = n_new;
@@ -587,6 +588,8 @@ int skd_stage_labels(skd_ctx* ctx, const int32_t* y, int64_t n) {
   SKD_CUDA(c, cudaSetDevice(c->device));
   if (stage_device_vector(c, c->ycls, c->ycls_cap, y, n)) return 1;
   c->h_ycls.assign(y, y + n);
+  const auto mm = std::minmax_element(y, y + n);
+  c->ycls_min = *mm.first; c->ycls_max = *mm.second;
   c->tc.meta_valid = false;
   return 0;
 }
@@ -1205,6 +1208,35 @@ int skd_linear_score_batch(skd_ctx* ctx, int32_t B, const float* coef, const int
   return 0;
 }
 
+// The entries that take n_classes read class ids 0..n_classes-1.  A row with any other id would still count in
+// n_train (so in 1/n_train and l2) while the kernels leave it out of the loss, the gradient and the scores.
+static int check_class_ids(Ctx* c, const char* who, int n_classes) {
+  if (c->ycls_min < 0 || c->ycls_max >= n_classes)
+    return fail(c, std::string(who) + ": staged class ids span " + std::to_string(c->ycls_min) + ".." +
+                       std::to_string(c->ycls_max) + ", outside 0..n_classes-1 = 0.." + std::to_string(n_classes - 1));
+  return 0;
+}
+
+// l2 and inv_n of every multinomial candidate, with the staged masks and class weights checked against the batch:
+// the sum of a candidate's per-row weights takes the place of n_train (SK/linear_model/_logistic.py:474).
+static int multinomial_constants(Ctx* c, const char* who, int B, int n_classes, const double* C, const int32_t* col_fold,
+                                 const StagedMasks& masks, const StagedClassWeights& cw, std::vector<double>& l2,
+                                 std::vector<double>& inv_n) {
+  if (check_class_ids(c, who, n_classes)) return 1;
+  if (column_train_sizes(c, who, B, C, col_fold, nullptr, nullptr, nullptr, l2, inv_n)) return 1;
+  if (masks.cols > 0 && (masks.cols != B || (int64_t)masks.mask.size() != (int64_t)B * c->d))
+    return fail(c, std::string(who) + ": staged column masks do not match the batch");
+  if (cw.cols > 0) {
+    if (cw.cols != B || cw.k != n_classes)
+      return fail(c, std::string(who) + ": staged class weights do not match this batch (B x n_classes)");
+    for (int j = 0; j < B; ++j) {
+      l2[j] = 1.0 / (C[j] * cw.sw_sum[j]);
+      inv_n[j] = 1.0 / cw.sw_sum[j];
+    }
+  }
+  return 0;
+}
+
 int skd_logreg_multinomial_fit_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, const double* C,
                                      const int32_t* col_fold, int32_t fit_intercept, double tol, int32_t max_iter,
                                      float* coef_out, int32_t* n_iter_out, int32_t* status_out, double* loss_out,
@@ -1218,19 +1250,9 @@ int skd_logreg_multinomial_fit_batch(skd_ctx* ctx, int32_t B, int32_t n_classes,
     return fail(c, "skd_logreg_multinomial_fit_batch: bad arguments");
   if (max_iter < 1) return fail(c, "skd_logreg_multinomial_fit_batch: max_iter must be >= 1");
   std::vector<double> l2, inv_n;
-  if (column_train_sizes(c, "skd_logreg_multinomial_fit_batch", B, C, col_fold, nullptr, nullptr, nullptr, l2, inv_n))
+  if (multinomial_constants(c, "skd_logreg_multinomial_fit_batch", B, n_classes, C, col_fold, staged_masks, staged_cw,
+                            l2, inv_n))
     return 1;
-  if (staged_masks.cols > 0 && (staged_masks.cols != B || (int64_t)staged_masks.mask.size() != (int64_t)B * c->d))
-    return fail(c, "skd_logreg_multinomial_fit_batch: staged column masks do not match the batch");
-  if (staged_cw.cols > 0) {
-    if (staged_cw.cols != B || staged_cw.k != n_classes)
-      return fail(c, "skd_logreg_multinomial_fit_batch: staged class weights do not match this batch (B x n_classes)");
-    // the sum of the per-row weights takes the place of n_train (SK/linear_model/_logistic.py:474)
-    for (int j = 0; j < B; ++j) {
-      l2[j] = 1.0 / (C[j] * staged_cw.sw_sum[j]);
-      inv_n[j] = 1.0 / staged_cw.sw_sum[j];
-    }
-  }
   SKD_CUDA(c, cudaSetDevice(c->device));
   Trace tr(c, "multinomial_fit");
   DeviceTimer timer(c);
@@ -1240,6 +1262,31 @@ int skd_logreg_multinomial_fit_batch(skd_ctx* ctx, int32_t B, int32_t n_classes,
                 staged_cw.cols > 0 ? staged_cw.w.data() : nullptr, coef_out, n_iter_out, status_out, loss_out, n_evals_out))
     return 1;
   return timer.stop(gpu_seconds_out);
+}
+
+int skd_logreg_multinomial_loss_grad(skd_ctx* ctx, int32_t B, int32_t n_classes, const double* w_in, const double* C,
+                                     const int32_t* col_fold, int32_t fit_intercept, double* loss_out,
+                                     double* grad_out) {
+  if (!ctx) return fail(nullptr, "skd_logreg_multinomial_loss_grad: ctx is NULL");
+  Ctx* c = &ctx->c;
+  const StagedClassWeights staged_cw = std::exchange(c->cw, {});
+  const StagedMasks staged_masks = std::exchange(c->fmask, {});
+  if (!c->X || !c->ycls) return fail(c, "skd_logreg_multinomial_loss_grad: stage X and labels first");
+  if (B <= 0 || n_classes < 2 || !w_in || !C || !col_fold || !loss_out || !grad_out)
+    return fail(c, "skd_logreg_multinomial_loss_grad: bad arguments");
+  std::vector<double> l2, inv_n;
+  if (multinomial_constants(c, "skd_logreg_multinomial_loss_grad", B, n_classes, C, col_fold, staged_masks, staged_cw,
+                            l2, inv_n))
+    return 1;
+  SKD_CUDA(c, cudaSetDevice(c->device));
+  const int dp = (int)c->d + 1;
+  std::vector<double> x(w_in, w_in + (size_t)B * n_classes * dp);
+  if (!fit_intercept)   // the fit's intercepts stay at 0 without one
+    for (size_t r = 0; r < (size_t)B * n_classes; ++r) x[r * dp + dp - 1] = 0.0;
+  Trace tr(c, "multinomial_loss_grad");
+  return multi_loss_grad(c, B, n_classes, l2.data(), inv_n.data(), col_fold, fit_intercept,
+                         staged_masks.cols > 0 ? staged_masks.mask.data() : nullptr,
+                         staged_cw.cols > 0 ? staged_cw.w.data() : nullptr, x.data(), loss_out, grad_out);
 }
 
 static int multinomial_check(Ctx* c, const char* who, int32_t B, int32_t n_classes, const float* coef,
@@ -1255,6 +1302,7 @@ int skd_multinomial_confusion_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, 
   Ctx* c = &ctx->c;
   if (multinomial_check(c, "skd_multinomial_confusion_batch", B, n_classes, coef, col_fold)) return 1;
   if (!confusion_out) return fail(c, "skd_multinomial_confusion_batch: bad arguments");
+  if (check_class_ids(c, "skd_multinomial_confusion_batch", n_classes)) return 1;
   SKD_CUDA(c, cudaSetDevice(c->device));
   Trace tr(c, "multinomial_confusion");
   return multi_score(c, B, n_classes, coef, col_fold, confusion_out);
@@ -1266,6 +1314,7 @@ int skd_multinomial_score_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, cons
   Ctx* c = &ctx->c;
   if (multinomial_check(c, "skd_multinomial_score_batch", B, n_classes, coef, col_fold)) return 1;
   if (!correct_out || !count_out) return fail(c, "skd_multinomial_score_batch: bad arguments");
+  if (check_class_ids(c, "skd_multinomial_score_batch", n_classes)) return 1;
   SKD_CUDA(c, cudaSetDevice(c->device));
   Trace tr(c, "multinomial_score");
   const size_t KK = (size_t)n_classes * n_classes;
@@ -1306,6 +1355,7 @@ int skd_linear_logloss_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, const f
   if (multinomial_check(c, "skd_linear_logloss_batch", B, n_classes == 1 ? 2 : n_classes, coef, col_fold)) return 1;
   if (!loss_sum_out || !count_out || (n_classes == 1 && !col_pos))
     return fail(c, "skd_linear_logloss_batch: bad arguments");
+  if (n_classes > 2 && check_class_ids(c, "skd_linear_logloss_batch", n_classes)) return 1;
   SKD_CUDA(c, cudaSetDevice(c->device));
   Trace tr(c, "logloss");
   return logloss_batch(c, B, n_classes, coef, col_fold, col_pos, loss_sum_out, count_out);

@@ -445,9 +445,40 @@ int lbfgs_dev_finish(Ctx* c, LogregWork& w, float* dcoef, int32_t* dniter, int32
 }
 
 // ---- multinomial problems: one CTA per active candidate, K * dp variables ------------------
-// f, g from the evaluation partials (SK/linear_model/_linear_loss.py:349-372, multiclass branch:
-// loss = sum(loss_i) / n + 0.5 * l2 * ||W||^2, grad[:, :d] = G^T X / n + l2 * W, grad[:, d] = sum_i G / n),
-// then one step of the optimiser state machine.
+// f, g of active candidate a from the evaluation partials, added in chunk order (SK/linear_model/_linear_loss.py:349-372,
+// multiclass branch: loss = sum(loss_i) / n + 0.5 * l2 * ||W||^2, grad[:, :d] = G^T X / n + l2 * W,
+// grad[:, d] = sum_i G / n).  fmask: the candidate's feature mask or null.
+template <class Par>
+__device__ __forceinline__ double mn_gather_fg(const Par& P, int a, int n_act_in, int K, int d, int ldx, int nz,
+                                               int fit_intercept, const double* __restrict__ lossp,
+                                               const double* __restrict__ gsump, const float* __restrict__ gradp,
+                                               double l2, double inv_n, const double* x, double* g,
+                                               const uint8_t* __restrict__ fmask) {
+  const int dp = d + 1, n = K * dp;
+  const size_t n_slots = (size_t)n_act_in * K;
+  double lsum = 0.0;
+  for (int z = 0; z < nz; ++z) lsum += lossp[(size_t)z * n_act_in + a];
+  double wsq = 0.0;
+  for (int idx = P.tid(); idx < n; idx += P.nthr()) {
+    const int k = idx / dp, j = idx - k * dp;
+    const size_t slot = (size_t)a * K + k;
+    double acc = 0.0;
+    if (j < d) {
+      for (int z = 0; z < nz; ++z) acc += (double)gradp[((size_t)z * n_slots + slot) * ldx + j];
+      const double xk = x[idx];
+      // a feature masked out of this candidate keeps weight 0 in every class row (zero gradient entry)
+      g[idx] = (fmask && !fmask[j]) ? 0.0 : acc * inv_n + l2 * xk;
+      wsq += xk * xk;
+    } else {
+      for (int z = 0; z < nz; ++z) acc += gsump[(size_t)z * n_slots + slot];
+      g[idx] = fit_intercept ? acc * inv_n : 0.0;
+    }
+  }
+  wsq = P.block_sum(wsq);
+  return lsum * inv_n + 0.5 * l2 * wsq;
+}
+
+// f, g, then one step of the optimiser state machine.
 __global__ void __launch_bounds__(LB_THREADS)
 mn_step_kernel(LbfgsScalars* sc, double* vec, size_t vec_stride, const SlotMeta* cand, int n_act_in,
                const int32_t* __restrict__ n_act_dev, int K, int d, int ldx, int nz, int fit_intercept,
@@ -459,31 +490,11 @@ mn_step_kernel(LbfgsScalars* sc, double* vec, size_t vec_stride, const SlotMeta*
   if (a >= n_act_in || a >= *n_act_dev) return;
   const int col = cand[a].col;
   LbfgsScalars st = sc[col];
-  const int n = st.n, m = st.m, dp = d + 1;
+  const int n = st.n, m = st.m;
   LbfgsVectors v = col_vectors(vec + (size_t)col * vec_stride, n, m);
   CtaPar P{red};
-  const double l2 = l2v[col], inv_n = inv_nv[col];
-  const size_t n_slots = (size_t)n_act_in * K;
-  double lsum = 0.0;
-  for (int z = 0; z < nz; ++z) lsum += lossp[(size_t)z * n_act_in + a];
-  double wsq = 0.0;
-  for (int idx = threadIdx.x; idx < n; idx += LB_THREADS) {
-    const int k = idx / dp, j = idx - k * dp;
-    const size_t slot = (size_t)a * K + k;
-    double acc = 0.0;
-    if (j < d) {
-      for (int z = 0; z < nz; ++z) acc += (double)gradp[((size_t)z * n_slots + slot) * ldx + j];
-      const double xk = v.x[idx];
-      // a feature masked out of this candidate keeps weight 0 in every class row (zero gradient entry)
-      v.g[idx] = (fmask && !fmask[(size_t)col * d + j]) ? 0.0 : acc * inv_n + l2 * xk;
-      wsq += xk * xk;
-    } else {
-      for (int z = 0; z < nz; ++z) acc += gsump[(size_t)z * n_slots + slot];
-      v.g[idx] = fit_intercept ? acc * inv_n : 0.0;
-    }
-  }
-  wsq = P.block_sum(wsq);
-  const double f = lsum * inv_n + 0.5 * l2 * wsq;
+  const double f = mn_gather_fg(P, a, n_act_in, K, d, ldx, nz, fit_intercept, lossp, gsump, gradp, l2v[col],
+                                inv_nv[col], v.x, v.g, fmask ? fmask + (size_t)col * d : nullptr);
   __syncthreads();
   lbfgs_advance(P, st, v, f);
   __syncthreads();
@@ -491,6 +502,25 @@ mn_step_kernel(LbfgsScalars* sc, double* vec, size_t vec_stride, const SlotMeta*
     sc[col] = st;
     n_evals[col] += 1;
   }
+}
+
+// Test entry: objective and gradient of every active candidate at caller points xin [B][K][dp]; the partials
+// are indexed by active index, the constants, point and outputs by cand[a].col.
+__global__ void __launch_bounds__(LB_THREADS)
+mn_gather_kernel(const SlotMeta* cand, int n_act_in, int K, int d, int ldx, int nz, int fit_intercept,
+                 const double* __restrict__ lossp, const double* __restrict__ gsump,
+                 const float* __restrict__ gradp, const double* __restrict__ l2v,
+                 const double* __restrict__ inv_nv, const uint8_t* __restrict__ fmask,
+                 const double* __restrict__ xin, double* __restrict__ fout, double* __restrict__ gout) {
+  __shared__ double red[8];
+  const int a = blockIdx.x;
+  if (a >= n_act_in) return;
+  const int col = cand[a].col;
+  const size_t n = (size_t)K * (d + 1);
+  CtaPar P{red};
+  const double f = mn_gather_fg(P, a, n_act_in, K, d, ldx, nz, fit_intercept, lossp, gsump, gradp, l2v[col],
+                                inv_nv[col], xin + col * n, gout + col * n, fmask ? fmask + (size_t)col * d : nullptr);
+  if (threadIdx.x == 0) fout[col] = f;
 }
 
 __global__ void mn_init_kernel(LbfgsScalars* sc, double* vec, size_t vec_stride, int B, int n, int m,
@@ -558,6 +588,23 @@ int multi_lbfgs_enqueue(Ctx* c, MultiWork& w, int n_act_in, int fit_intercept, i
   mn_export_kernel<<<n_act_in * w.K, 128, 0, c->stream>>>(w.vec, w.vec_stride, w.cand, w.n_act, w.K, d, ldx,
                                                           (size_t)w.B * w.K * ldx, w.W);
   c->launches += 3;
+  SKD_CUDA(c, cudaGetLastError());
+  return 0;
+}
+
+// caller points dx [B][K][dp] (device, float64) to the fp32 slot rows, by the export of the optimiser's trial points
+int multi_export_points(Ctx* c, MultiWork& w, const double* dx) {
+  mn_export_kernel<<<w.B * w.K, 128, 0, c->stream>>>(dx, (size_t)w.K * w.dp, w.cand, w.n_act, w.K, (int)c->d,
+                                                     (int)c->ldx, (size_t)w.B * w.K * c->ldx, w.W);
+  c->launches += 1;
+  SKD_CUDA(c, cudaGetLastError());
+  return 0;
+}
+
+int multi_gather(Ctx* c, MultiWork& w, int fit_intercept, const double* dx, double* df, double* dg) {
+  mn_gather_kernel<<<w.B, LB_THREADS, 0, c->stream>>>(w.cand, w.B, w.K, (int)c->d, (int)c->ldx, w.nz, fit_intercept,
+                                                      w.lossp, w.gsump, w.gradp, w.l2, w.inv_n, w.fmask, dx, df, dg);
+  c->launches += 1;
   SKD_CUDA(c, cudaGetLastError());
   return 0;
 }

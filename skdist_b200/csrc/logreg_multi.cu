@@ -158,53 +158,76 @@ static int64_t candidates_per_pass(const Ctx* c, int K, int nz) {
   return b < 1 ? 1 : b;
 }
 
+// Device buffers of one pass over candidates b0 .. b0 + Bb - 1 and the uploads of their constants (l2, inv_n,
+// held-out folds into *d_fold, feature masks, class weights), shared by multi_fit and multi_loss_grad.
+static int multi_pass_setup(Ctx* c, Scratch& sx, MultiWork& w, int64_t b0, int Bb, int K, int nz, int64_t rpc,
+                            const double* l2, const double* inv_n, const int32_t* col_fold, const uint8_t* fmask,
+                            const float* cw, int32_t** d_fold) {
+  const int64_t n = c->n, ldx = c->ldx;
+  const int dp = (int)c->d + 1, m = 10;
+  w.B = Bb; w.K = K; w.dp = dp; w.nz = nz; w.rpc = rpc;
+  const size_t slots = (size_t)Bb * K;
+  w.ldg = (int)((slots + 63) / 64 * 64);
+  w.vec_stride = (size_t)(5 + 2 * m) * K * dp + 2 * m;
+  SKD_CUDA(c, sx.alloc(&w.sc, (size_t)Bb));
+  SKD_CUDA(c, sx.alloc(&w.vec, (size_t)Bb * w.vec_stride));
+  SKD_CUDA(c, sx.alloc(&w.l2, (size_t)Bb));
+  SKD_CUDA(c, sx.alloc(&w.inv_n, (size_t)Bb));
+  SKD_CUDA(c, sx.alloc(&w.n_evals, (size_t)Bb));
+  SKD_CUDA(c, sx.alloc(&w.cand, (size_t)Bb));
+  SKD_CUDA(c, sx.alloc(d_fold, (size_t)Bb));
+  SKD_CUDA(c, sx.alloc(&w.W, slots * ldx + slots));
+  SKD_CUDA(c, sx.alloc(&w.G, (size_t)n * w.ldg));
+  SKD_CUDA(c, sx.alloc(&w.lossp, (size_t)nz * Bb));
+  SKD_CUDA(c, sx.alloc(&w.gsump, (size_t)nz * slots));
+  SKD_CUDA(c, sx.alloc(&w.gradp, (size_t)nz * slots * ldx));
+  SKD_CUDA(c, sx.alloc(&w.n_act, 1));
+  SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2 + b0, Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n + b0, Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(*d_fold, col_fold + b0, Bb * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  c->h2d += (int64_t)Bb * 20;
+  if (fmask) {     // per-candidate feature masks (DistFeatureEliminator): masked weights stay exactly 0
+    SKD_CUDA(c, sx.alloc(&w.fmask, (size_t)Bb * c->d));
+    SKD_CUDA(c, cudaMemcpyAsync(w.fmask, fmask + (size_t)b0 * c->d, (size_t)Bb * c->d, cudaMemcpyHostToDevice, c->stream));
+    c->h2d += (int64_t)Bb * c->d;
+  }
+  if (cw) {
+    float* dcw;
+    SKD_CUDA(c, sx.alloc(&dcw, (size_t)Bb * K));
+    SKD_CUDA(c, cudaMemcpyAsync(dcw, cw + (size_t)b0 * K, (size_t)Bb * K * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    c->h2d += (int64_t)Bb * K * 4;
+    w.cw = dcw;
+  }
+  return 0;
+}
+
+// One evaluation of the n_act active candidates at the slot rows in w.W: raw predictions, pointwise loss and
+// gradient in place, per-chunk intercept and weight gradient partials (w.lossp, w.gsump, w.gradp).
+static int multi_eval(Ctx* c, MultiWork& w, int n_act) {
+  const size_t slots = (size_t)w.B * w.K;
+  const int ns = n_act * w.K;
+  if (simt_raw_prediction(c, ns, w.W, w.W + slots * c->ldx, w.G, w.ldg)) return 1;
+  mn_pointwise_kernel<<<dim3(n_act, w.nz), 256, 0, c->stream>>>(w.G, w.ldg, c->n, w.rpc, w.K, w.cand, w.n_act, n_act,
+                                                               c->ycls, c->fold, w.lossp, w.cw);
+  mn_colsum_kernel<<<dim3((ns + 63) / 64, w.nz), 256, 0, c->stream>>>(w.G, w.ldg, c->n, w.rpc, ns, w.gsump);
+  c->launches += 2;
+  return simt_backward(c, w.G, w.ldg, ns, w.nz, w.rpc, w.gradp);
+}
+
 int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold, int fit_intercept,
               double tol, int max_iter, const uint8_t* fmask, const float* cw, float* coef_out,
               int32_t* n_iter_out, int32_t* status_out, double* loss_out, int32_t* n_evals_out) {
-  const int64_t n = c->n, ldx = c->ldx;
-  const int dp = (int)c->d + 1, m = 10;
+  const int dp = (int)c->d + 1;
   int nz;
   int64_t rpc;
-  multi_chunks(n, &nz, &rpc);
+  multi_chunks(c->n, &nz, &rpc);
   const int64_t per_pass = candidates_per_pass(c, K, nz);
   for (int64_t b0 = 0; b0 < B; b0 += per_pass) {
     const int Bb = (int)std::min<int64_t>(per_pass, B - b0);
     Scratch sx(c);
     MultiWork w;
-    w.B = Bb; w.K = K; w.dp = dp; w.nz = nz; w.rpc = rpc;
-    const size_t slots = (size_t)Bb * K;
-    w.ldg = (int)((slots + 63) / 64 * 64);
-    w.vec_stride = (size_t)(5 + 2 * m) * K * dp + 2 * m;
     int32_t* d_fold;
-    SKD_CUDA(c, sx.alloc(&w.sc, (size_t)Bb));
-    SKD_CUDA(c, sx.alloc(&w.vec, (size_t)Bb * w.vec_stride));
-    SKD_CUDA(c, sx.alloc(&w.l2, (size_t)Bb));
-    SKD_CUDA(c, sx.alloc(&w.inv_n, (size_t)Bb));
-    SKD_CUDA(c, sx.alloc(&w.n_evals, (size_t)Bb));
-    SKD_CUDA(c, sx.alloc(&w.cand, (size_t)Bb));
-    SKD_CUDA(c, sx.alloc(&d_fold, (size_t)Bb));
-    SKD_CUDA(c, sx.alloc(&w.W, slots * ldx + slots));
-    SKD_CUDA(c, sx.alloc(&w.G, (size_t)n * w.ldg));
-    SKD_CUDA(c, sx.alloc(&w.lossp, (size_t)nz * Bb));
-    SKD_CUDA(c, sx.alloc(&w.gsump, (size_t)nz * slots));
-    SKD_CUDA(c, sx.alloc(&w.gradp, (size_t)nz * slots * ldx));
-    SKD_CUDA(c, sx.alloc(&w.n_act, 1));
-    SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2 + b0, Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n + b0, Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(d_fold, col_fold + b0, Bb * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    c->h2d += (int64_t)Bb * 20;
-    if (fmask) {     // per-candidate feature masks (DistFeatureEliminator): masked weights stay exactly 0
-      SKD_CUDA(c, sx.alloc(&w.fmask, (size_t)Bb * c->d));
-      SKD_CUDA(c, cudaMemcpyAsync(w.fmask, fmask + (size_t)b0 * c->d, (size_t)Bb * c->d, cudaMemcpyHostToDevice, c->stream));
-      c->h2d += (int64_t)Bb * c->d;
-    }
-    if (cw) {
-      float* dcw;
-      SKD_CUDA(c, sx.alloc(&dcw, (size_t)Bb * K));
-      SKD_CUDA(c, cudaMemcpyAsync(dcw, cw + (size_t)b0 * K, (size_t)Bb * K * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-      c->h2d += (int64_t)Bb * K * 4;
-      w.cw = dcw;
-    }
+    if (multi_pass_setup(c, sx, w, b0, Bb, K, nz, rpc, l2, inv_n, col_fold, fmask, cw, &d_fold)) return 1;
     if (multi_lbfgs_init(c, w, d_fold, tol, max_iter)) return 1;
 
     // several optimiser rounds per host round trip; the kernels read the live candidate count from
@@ -215,13 +238,7 @@ int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const
     long long round = 0;
     while (n_act > 0) {
       for (int q = 0; q < rounds_per_sync; ++q, ++round) {
-        const int ns = n_act * K;
-        if (simt_raw_prediction(c, ns, w.W, w.W + slots * ldx, w.G, w.ldg)) return 1;
-        mn_pointwise_kernel<<<dim3(n_act, nz), 256, 0, c->stream>>>(w.G, w.ldg, n, rpc, K, w.cand, w.n_act, n_act,
-                                                                   c->ycls, c->fold, w.lossp, w.cw);
-        mn_colsum_kernel<<<dim3((ns + 63) / 64, nz), 256, 0, c->stream>>>(w.G, w.ldg, n, rpc, ns, w.gsump);
-        c->launches += 2;
-        if (simt_backward(c, w.G, w.ldg, ns, nz, rpc, w.gradp)) return 1;
+        if (multi_eval(c, w, n_act)) return 1;
         if (multi_lbfgs_enqueue(c, w, n_act, fit_intercept, nullptr)) return 1;
       }
       int32_t na = 0;
@@ -246,6 +263,46 @@ int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const
       SKD_CUDA(c, cudaMemcpyAsync(n_evals_out + b0, w.n_evals, Bb * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
     SKD_CUDA(c, cudaStreamSynchronize(c->stream));
     c->d2h += (int64_t)Bb * (K * dp * 4 + 20);
+  }
+  return 0;
+}
+
+// Objective and gradient at caller points w_in [B][K][d+1] (float64): the passes, set-up, evaluation and
+// gather of multi_fit's first round, with every candidate active in column order.
+int multi_loss_grad(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold,
+                    int fit_intercept, const uint8_t* fmask, const float* cw, const double* w_in, double* loss_out,
+                    double* grad_out) {
+  const int dp = (int)c->d + 1;
+  int nz;
+  int64_t rpc;
+  multi_chunks(c->n, &nz, &rpc);
+  const int64_t per_pass = candidates_per_pass(c, K, nz);
+  for (int64_t b0 = 0; b0 < B; b0 += per_pass) {
+    const int Bb = (int)std::min<int64_t>(per_pass, B - b0);
+    Scratch sx(c);
+    MultiWork w;
+    int32_t* d_fold;
+    if (multi_pass_setup(c, sx, w, b0, Bb, K, nz, rpc, l2, inv_n, col_fold, fmask, cw, &d_fold)) return 1;
+    std::vector<SlotMeta> hc(Bb);
+    for (int j = 0; j < Bb; ++j) { hc[j].col = j; hc[j].fold = col_fold[b0 + j]; hc[j].pos = 0; hc[j].pad = 0; }
+    double *dx, *df, *dg;
+    const size_t nvar = (size_t)Bb * K * dp;
+    SKD_CUDA(c, sx.alloc(&dx, nvar));
+    SKD_CUDA(c, sx.alloc(&df, (size_t)Bb));
+    SKD_CUDA(c, sx.alloc(&dg, nvar));
+    SKD_CUDA(c, cudaMemcpyAsync(w.cand, hc.data(), Bb * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &Bb, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(dx, w_in + (size_t)b0 * K * dp, nvar * sizeof(double), cudaMemcpyHostToDevice,
+                                c->stream));
+    c->h2d += (int64_t)Bb * sizeof(SlotMeta) + 4 + (int64_t)nvar * 8;
+    if (multi_export_points(c, w, dx)) return 1;
+    if (multi_eval(c, w, Bb)) return 1;
+    if (multi_gather(c, w, fit_intercept, dx, df, dg)) return 1;
+    SKD_CUDA(c, cudaMemcpyAsync(loss_out + b0, df, Bb * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(grad_out + (size_t)b0 * K * dp, dg, nvar * sizeof(double), cudaMemcpyDeviceToHost,
+                                c->stream));
+    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+    c->d2h += (int64_t)Bb * 8 + (int64_t)nvar * 8;
   }
   return 0;
 }

@@ -112,6 +112,7 @@ struct Ctx {
   int8_t* fold = nullptr;   // [n]; nullptr = no folds staged (points into fold_store otherwise)
   int8_t* fold_store = nullptr;
   std::vector<int32_t> h_ycls; // host copy of the class ids (training-set sizes of one-vs-one pair columns)
+  int32_t ycls_min = 0, ycls_max = -1;  // range of the staged class ids (multinomial entries check it)
   std::vector<int8_t> h_fold;  // host copy of the fold ids (tile lists for fold-aware tile skipping)
   int32_t n_folds = 0;
   std::vector<int64_t> fold_count;  // rows per fold id
@@ -339,10 +340,16 @@ struct MultiWork {
 int multi_lbfgs_init(Ctx* c, MultiWork& w, const int32_t* d_col_fold, double tol, int max_iter);
 int multi_lbfgs_enqueue(Ctx* c, MultiWork& w, int n_act_in, int fit_intercept, int32_t* hist);
 int multi_lbfgs_finish(Ctx* c, MultiWork& w, float* dcoef, int32_t* dniter, int32_t* dstatus, double* dloss);
+// caller points dx [B][K][dp] (device) into w.W, and f, g of every candidate at them after one evaluation
+int multi_export_points(Ctx* c, MultiWork& w, const double* dx);
+int multi_gather(Ctx* c, MultiWork& w, int fit_intercept, const double* dx, double* df, double* dg);
 int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold, int fit_intercept,
               double tol, int max_iter, const uint8_t* fmask /*[B x d] or nullptr*/,
               const float* cw /*[B x K] or nullptr*/, float* coef_out, int32_t* n_iter_out,
               int32_t* status_out, double* loss_out, int32_t* n_evals_out);
+int multi_loss_grad(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold,
+                    int fit_intercept, const uint8_t* fmask, const float* cw, const double* w_in, double* loss_out,
+                    double* grad_out);
 int multi_score(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold, int64_t* conf_out);
 int logloss_batch(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold, const int32_t* col_pos,
                   double* loss_sum_out, int64_t* count_out);

@@ -240,6 +240,21 @@ class Engine:
         return {"coef": coef, "n_iter": n_iter, "status": status, "loss": loss,
                 "n_evals": n_evals, "gpu_seconds": secs.value}
 
+    def logreg_multinomial_loss_grad(self, w, C, col_fold, fit_intercept=True):
+        """Objective [B] and gradient [B, K, d + 1] of B multinomial candidates at the points w [B, K, d + 1],
+        by the evaluation of logreg_multinomial_fit_batch (class ids 0..K-1 staged)."""
+        w = np.ascontiguousarray(w, dtype=np.float64)
+        B, K = w.shape[0], w.shape[1]
+        assert w.shape[2] == self.d + 1
+        C = np.ascontiguousarray(C, dtype=np.float64)
+        col_fold = np.ascontiguousarray(col_fold, dtype=np.int32)
+        assert C.shape == (B,) and col_fold.shape == (B,)
+        loss = np.empty(B, dtype=np.float64)
+        grad = np.empty_like(w)
+        check(self._lib.skd_logreg_multinomial_loss_grad(self._h, B, K, ptr(w), ptr(C), ptr(col_fold),
+                                                         int(bool(fit_intercept)), ptr(loss), ptr(grad)), self._h)
+        return loss, grad
+
     def multinomial_score_batch(self, coef, col_fold):
         coef = np.ascontiguousarray(coef, dtype=np.float32)
         B, K = coef.shape[0], coef.shape[1]
