@@ -1676,14 +1676,16 @@ int skd_forest_tree_nodes(skd_forest* f, int32_t tree, void* nodes64, double* va
 
 void skd_forest_free(skd_forest* f) { delete f; }
 
-// Streams m new rows [m x d] (row pitch ld) through `kernel(dX, rows, ldx, dO)` in row chunks of <= 256 MiB:
-// threaded pinned-bounce H2D (stage_rows_h2d), one pass of the kernel, D2H of the (small) result of
-// out_row_bytes per row into out.  The copy engine is the bottleneck.  *seconds: wall time of the chunks.
+// Streams m new rows [m x d] (row pitch ld) through `kernel(dX, rows, ldx, dO)` in row chunks whose input
+// and output each take <= 256 MiB: threaded pinned-bounce H2D (stage_rows_h2d), one pass of the kernel, D2H
+// of the result of out_row_bytes per row into out.  The copy engine is the bottleneck.  *seconds: wall time
+// of the chunks.
 static int stream_rows(Ctx* c, Scratch& sx, const float* Xnew, int64_t m, int64_t d, int64_t ld, size_t out_row_bytes,
                        void* out, double* seconds,
                        const std::function<int(const float* dX, int64_t rows, int ldx, void* dO)>& kernel) {
   const int64_t ldx = round_up(d, 4);
-  int64_t rows_per_chunk = std::max<int64_t>(1, ((int64_t)256 << 20) / (ldx * 4));
+  const int64_t row_bytes = std::max<int64_t>(ldx * 4, (int64_t)out_row_bytes);
+  int64_t rows_per_chunk = std::max<int64_t>(1, ((int64_t)256 << 20) / row_bytes);
   if (rows_per_chunk > m) rows_per_chunk = m;
   float* dX; uint8_t* dO;
   SKD_CUDA(c, sx.alloc(&dX, (size_t)rows_per_chunk * ldx));
@@ -1775,7 +1777,9 @@ int skd_linear_decision(skd_ctx* ctx, int32_t B, const float* coef, float* out) 
   float *dW, *dout;
   if (pack_coef(c, sx, B, coef, c->d, c->ldx, &dW)) return 1;
   SKD_CUDA(c, sx.alloc(&dout, (size_t)c->n * B));
-  if (B <= 16 && c->ldx * 4 * 8 <= 48 * 1024) {
+  // up to 16 models whose rows fit the weight cache 8 at a time run on the row-per-warp kernel; more models
+  // or wider rows on the 64 x 64 tiled kernel
+  if (B <= 16 && predict_cache_rows(c->ldx) == 8) {
     if (predict_device(c, c->X, c->n, (int)c->ldx, (int)c->d, B, dW, dout)) return 1;
   } else if (simt_decision(c, B, dW, dout)) return 1;
   SKD_CUDA(c, cudaMemcpyAsync(out, dout, (size_t)c->n * B * sizeof(float), cudaMemcpyDeviceToHost, c->stream));

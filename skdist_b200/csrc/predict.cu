@@ -8,13 +8,20 @@
 
 namespace skd {
 
-template <int NB>
+constexpr size_t PREDICT_CACHE_BYTES = 48 * 1024;   // shared-memory weight cache of predict_kernel
+
+// CACHED: the NB weight rows are copied to shared memory once per CTA; otherwise (rows wider than the
+// cache) every warp reads them from global memory, where they stay L2-resident.
+template <int NB, bool CACHED>
 __global__ void __launch_bounds__(256)
 predict_kernel(const float* __restrict__ X, int64_t m, int ldx, int d, const float* __restrict__ W /*[NB][ldx]*/,
                const float* __restrict__ bias, float* __restrict__ out, int ldo, int col0) {
   extern __shared__ float sw[];   // NB * ldx
-  for (int i = threadIdx.x; i < NB * ldx; i += blockDim.x) sw[i] = W[i];
-  __syncthreads();
+  if (CACHED) {
+    for (int i = threadIdx.x; i < NB * ldx; i += blockDim.x) sw[i] = W[i];
+    __syncthreads();
+  }
+  const float* wsrc = CACHED ? sw : W;
   const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
   for (int64_t r = (int64_t)blockIdx.x * wpb + (threadIdx.x >> 5); r < m; r += (int64_t)gridDim.x * wpb) {
     const float4* row = reinterpret_cast<const float4*>(X + r * ldx);
@@ -25,7 +32,8 @@ predict_kernel(const float* __restrict__ X, int64_t m, int ldx, int d, const flo
       const float4 x = __ldg(row + q);
 #pragma unroll
       for (int b = 0; b < NB; ++b) {
-        const float4 w = *reinterpret_cast<const float4*>(sw + b * ldx + q * 4);
+        const float4* wp = reinterpret_cast<const float4*>(wsrc + b * ldx + q * 4);
+        const float4 w = CACHED ? *wp : __ldg(wp);
         acc[b] = fmaf(x.x, w.x, fmaf(x.y, w.y, fmaf(x.z, w.z, fmaf(x.w, w.w, acc[b]))));
       }
     }
@@ -39,23 +47,36 @@ predict_kernel(const float* __restrict__ X, int64_t m, int ldx, int d, const flo
   (void)d;
 }
 
+int predict_cache_rows(int64_t ldx) {
+  return (int)std::min<int64_t>(8, (int64_t)PREDICT_CACHE_BYTES / (ldx * (int64_t)sizeof(float)));
+}
+
+template <bool CACHED>
+static void predict_launch(Ctx* c, int nb, const float* dX, int64_t m, int ldx, int d, const float* w,
+                           const float* bias, float* dout, int B, int b0) {
+  const int grid = c->sm_count * 8;
+  const size_t smem = CACHED ? (size_t)nb * ldx * sizeof(float) : 0;
+  switch (nb) {
+    case 8: predict_kernel<8, CACHED><<<grid, 256, smem, c->stream>>>(dX, m, ldx, d, w, bias, dout, B, b0); break;
+    case 4: predict_kernel<4, CACHED><<<grid, 256, smem, c->stream>>>(dX, m, ldx, d, w, bias, dout, B, b0); break;
+    case 2: predict_kernel<2, CACHED><<<grid, 256, smem, c->stream>>>(dX, m, ldx, d, w, bias, dout, B, b0); break;
+    default: predict_kernel<1, CACHED><<<grid, 256, smem, c->stream>>>(dX, m, ldx, d, w, bias, dout, B, b0); break;
+  }
+}
+
 // dX: [m x ldx] device rows (ldx % 4 == 0, zero padded), dW: [B x ldx] + bias[B] packed as in
-// pack_coef (weights then bias block), dout: [m x B].
+// pack_coef (weights then bias block), dout: [m x B].  Each pass takes the largest of 8/4/2/1 models
+// that are left and fit the weight cache; rows wider than the cache run uncached, up to 8 models a pass.
 int predict_device(Ctx* c, const float* dX, int64_t m, int ldx, int d, int B, const float* dW, float* dout) {
   if (m <= 0) return 0;
-  int grid = c->sm_count * 8;
+  const int cache_rows = predict_cache_rows(ldx);
   for (int b0 = 0; b0 < B;) {
-    int nb = B - b0 >= 8 ? 8 : (B - b0 >= 4 ? 4 : (B - b0 >= 2 ? 2 : 1));
+    const int cap = std::min(B - b0, cache_rows > 0 ? cache_rows : 8);
+    const int nb = cap >= 8 ? 8 : (cap >= 4 ? 4 : (cap >= 2 ? 2 : 1));
     const float* w = dW + (size_t)b0 * ldx;
     const float* bias = dW + (size_t)B * ldx + b0;
-    size_t smem = (size_t)nb * ldx * sizeof(float);
-    if (smem > 48 * 1024) return fail(c, "predict: d too large for the shared-memory weight cache");
-    switch (nb) {
-      case 8: predict_kernel<8><<<grid, 256, smem, c->stream>>>(dX, m, ldx, d, w, bias, dout, B, b0); break;
-      case 4: predict_kernel<4><<<grid, 256, smem, c->stream>>>(dX, m, ldx, d, w, bias, dout, B, b0); break;
-      case 2: predict_kernel<2><<<grid, 256, smem, c->stream>>>(dX, m, ldx, d, w, bias, dout, B, b0); break;
-      default: predict_kernel<1><<<grid, 256, smem, c->stream>>>(dX, m, ldx, d, w, bias, dout, B, b0); break;
-    }
+    if (cache_rows > 0) predict_launch<true>(c, nb, dX, m, ldx, d, w, bias, dout, B, b0);
+    else predict_launch<false>(c, nb, dX, m, ldx, d, w, bias, dout, B, b0);
     c->launches += 1;
     b0 += nb;
   }

@@ -305,6 +305,8 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
                double min_weight_leaf, double min_impurity_decrease, bool random_split, bool sort_split,
                bool entropy, const double* h_yreal, const ForestClassWeights* cw, ForestSink sink,
                void* sink_arg);
+// weight rows of pitch ldx that predict_device's shared-memory cache holds, at most 8 (0: read from global)
+int predict_cache_rows(int64_t ldx);
 int predict_device(Ctx* c, const float* dX, int64_t m, int ldx, int d, int B, const float* dW, float* dout);
 int forest_predict_device(Ctx* c, const float* dX, int64_t m, int ldx, int n_trees, const int64_t* d_off,
                           const void* d_node, const double* d_thr, const double* d_val, int C, double* d_out);
