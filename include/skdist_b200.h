@@ -205,6 +205,24 @@ int skd_multinomial_confusion_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, 
 int skd_linear_auc_batch(skd_ctx* ctx, int32_t B, const float* coef, const int32_t* col_fold,
                          const int32_t* col_pos, int64_t* u2_out, int64_t* n_pos_out, int64_t* n_neg_out);
 
+/* Ranked counts of B linear classifiers on the rows selected by the fold codes of skd_linear_score_batch, per
+ * SEGMENT: u2_out = 2U (U = #{(p, q): s_p > s_q} + 0.5 * #{s_p == s_q} over positive rows p and negative rows q),
+ * n_pos_out, n_neg_out, and ap_out = average precision (sum over the tie groups in descending score of
+ * pos_g * tp_g / (tp_g + fp_g), divided by n_pos; 0 without positives).  auc = u2 / (2 * n_pos * n_neg).
+ *   n_classes == 1: coef [B][d+1] binary columns, one segment per column, positives y_class == col_pos[j].
+ *   n_classes = K > 2: coef [B][K][d+1], class ids 0..K-1; pairs == 0: K one-vs-rest segments per column
+ *     (segment k: positives y == k, score s_k); pairs == 1: K (K - 1) one-vs-one segments, ordered pair (a, b)
+ *     at a * (K - 1) + (b < a ? b : b - 1): the rows with y in {a, b}, positives y == a, score s_a.
+ * score_kind: 0 the fp32 decision values z = x.w + b, 1 their negation (pos_label = classes_[0]), 2 the float32
+ * predict_proba of LogisticRegression (expit for binary columns, softmax for K > 2; K <= 128), within
+ * (K + 10) * 2^-23 relative of numpy's (the device exp is correctly rounded, numpy's float32 exp within 4 ulp).
+ * Outputs are [B][segments].
+ * ref: replaces search.py:264 for scoring="roc_auc_ovr", "roc_auc_ovr_weighted", "roc_auc_ovo",
+ * "roc_auc_ovo_weighted" (predict_proba) and "average_precision" (decision_function). */
+int skd_linear_rank_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, const float* coef, const int32_t* col_fold,
+                          const int32_t* col_pos, int32_t score_kind, int32_t pairs, int64_t* u2_out,
+                          int64_t* n_pos_out, int64_t* n_neg_out, double* ap_out);
+
 /* Log loss of the predicted probabilities on the rows selected by the fold codes of
  * skd_linear_score_batch: loss_sum_out[j] = sum_i -log(clip(p_i[y_i], eps, 1 - eps)), eps = float32 epsilon,
  * p = softmax of the fp32 decision values; count_out[j] = rows.  n_classes == 1: B binary columns

@@ -62,6 +62,8 @@ SYMBOLS = {
                                                    _c.c_void_p]),
     "skd_linear_auc_batch": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_void_p,
                                         _c.c_void_p, _c.c_void_p, _c.c_void_p]),
+    "skd_linear_rank_batch": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_void_p,
+                                         _c.c_int32, _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_void_p]),
     "skd_linear_logloss_batch": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_int32, _c.c_void_p, _c.c_void_p,
                                             _c.c_void_p, _c.c_void_p, _c.c_void_p]),
     "skd_ridge_fit_batch": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_int32,

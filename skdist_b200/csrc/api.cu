@@ -1347,6 +1347,30 @@ int skd_linear_auc_batch(skd_ctx* ctx, int32_t B, const float* coef, const int32
   return auc_batch(c, B, coef, col_fold, col_pos, u2_out, n_pos_out, n_neg_out);
 }
 
+int skd_linear_rank_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, const float* coef, const int32_t* col_fold,
+                          const int32_t* col_pos, int32_t score_kind, int32_t pairs, int64_t* u2_out,
+                          int64_t* n_pos_out, int64_t* n_neg_out, double* ap_out) {
+  if (!ctx) return fail(nullptr, "skd_linear_rank_batch: ctx is NULL");
+  Ctx* c = &ctx->c;
+  if (n_classes == 2 || n_classes < 1)
+    return fail(c, "skd_linear_rank_batch: n_classes is 1 (binary columns) or > 2");
+  if (multinomial_check(c, "skd_linear_rank_batch", B, n_classes == 1 ? 2 : n_classes, coef, col_fold)) return 1;
+  if (!u2_out || !n_pos_out || !n_neg_out || !ap_out || (n_classes == 1 && !col_pos))
+    return fail(c, "skd_linear_rank_batch: bad arguments");
+  if (score_kind != RANK_DECISION && score_kind != RANK_NEG_DECISION && score_kind != RANK_PROBA)
+    return fail(c, "skd_linear_rank_batch: score_kind is 0 (decision), 1 (negated decision) or 2 (probability)");
+  if (pairs != 0 && (pairs != 1 || n_classes == 1))
+    return fail(c, "skd_linear_rank_batch: pairs is 0, or 1 with n_classes > 2");
+  if (score_kind == RANK_PROBA && n_classes > 128)
+    return fail(c, "skd_linear_rank_batch: probabilities of more than 128 classes have no device path");
+  if (n_classes > 2 && check_class_ids(c, "skd_linear_rank_batch", n_classes)) return 1;
+  if ((int64_t)rank_segments(n_classes, pairs) > 65536)
+    return fail(c, "skd_linear_rank_batch: more than 65536 segments per fit");
+  SKD_CUDA(c, cudaSetDevice(c->device));
+  Trace tr(c, "rank");
+  return rank_batch(c, B, n_classes, coef, col_fold, col_pos, score_kind, pairs, u2_out, n_pos_out, n_neg_out, ap_out);
+}
+
 int skd_linear_logloss_batch(skd_ctx* ctx, int32_t B, int32_t n_classes, const float* coef, const int32_t* col_fold,
                              const int32_t* col_pos, double* loss_sum_out, int64_t* count_out) {
   if (!ctx) return fail(nullptr, "skd_linear_logloss_batch: ctx is NULL");

@@ -359,7 +359,12 @@ int logloss_batch(Ctx* c, int B, int K, const float* coef, const int32_t* col_fo
 int simt_raw_prediction(Ctx* c, int n_slots, const float* dW, const float* dbias, float* dout, int ldd);
 int simt_backward(Ctx* c, const float* G, int ldg, int n_slots, int nz, int64_t rpc, float* gradp);
 
-// ROC-AUC counts of linear binary classifiers (auc.cu): 2U, n_pos, n_neg per column
+// Ranked counts of linear classifiers (auc.cu): 2U, n_pos, n_neg and average precision per segment
+enum RankScore { RANK_DECISION = 0, RANK_NEG_DECISION = 1, RANK_PROBA = 2 };
+int rank_segments(int K, int pairs);
+int rank_batch(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold, const int32_t* col_pos, int kind,
+               int pairs, int64_t* u2_out, int64_t* n_pos_out, int64_t* n_neg_out, double* ap_out);
+// ROC-AUC counts of linear binary classifiers on their decision values: rank_batch with one segment per column
 int auc_batch(Ctx* c, int B, const float* coef, const int32_t* col_fold, const int32_t* col_pos, int64_t* u2_out,
               int64_t* n_pos_out, int64_t* n_neg_out);
 

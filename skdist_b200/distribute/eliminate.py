@@ -12,8 +12,12 @@ so its weight stays exactly 0 and the L-BFGS iterates are those of the fit on th
 columns (csrc/lbfgs_dev.cu gather_fg).  No column-dropped copies of X are made; scoring uses the
 zero-padded coefficient rows on the full X.
 
-Base estimator with a device path: ``LogisticRegression(solver="lbfgs")`` (binary or multiclass target) with
-scoring=None / "accuracy" / "roc_auc".  Anything else raises NotImplementedError (no CPU fallback).
+Base estimator with a device path: ``LogisticRegression(solver="lbfgs")`` (binary or multiclass target).  The
+(feature set, fold) fits are scored by the search's LogisticRegression families (logreg_family.py), so every
+classifier scorer the search takes for the target works here too: accuracy, balanced accuracy, precision /
+recall / f1 with any averaging the target allows (the reference's examples/eliminate/covtype.py uses
+"f1_weighted"), roc_auc, roc_auc_ovr / roc_auc_ovo [_weighted], average_precision and neg_log_loss.  Anything
+else raises NotImplementedError (no CPU fallback).
 """
 import numpy as np
 from sklearn.utils.metaestimators import available_if
@@ -27,7 +31,7 @@ from .. import parallel
 from ..engine import get_engine
 from .base import _clone, _parse_partitions, _ScParamMixin
 from .folds import _fold_ids
-from .logreg_family import _check_logreg, _ClassWeights, _count_metric
+from .logreg_family import _check_engine_entries, _check_logreg, _ClassWeights, _LogRegFamily, _MultinomialFamily
 from .utils import _check_multimetric_scoring
 
 __all__ = ["DistFeatureEliminator"]
@@ -64,16 +68,13 @@ class DistFeatureEliminator(_ScParamMixin, ClassifierMixin, BaseEstimator):
                 "  (No CPU fallback by design.)" % type(self.estimator).__name__)
         p = _check_logreg(_clone(self.estimator), class_weight=True)
         scorers, _ = _check_multimetric_scoring(self.estimator, scoring=self.scoring)
-        metric = _count_metric(scorers["score"])
-        if metric is None or metric[0] not in ("accuracy", "roc_auc"):
-            raise NotImplementedError("scoring=None / 'accuracy' / 'roc_auc' are scored on the device")
         classes = np.unique(y)
         n_classes = len(classes)
         if n_classes < 2:
             raise ValueError("the target has a single class")
         multi = n_classes > 2          # LogisticRegression(lbfgs) is multinomial there (SK/linear_model/_logistic.py:523-547)
-        if multi and metric[0] == "roc_auc":
-            raise NotImplementedError("roc_auc on a multiclass target has no device path")
+        # the search's family for this target scores the fits (it raises for a scorer without a device path)
+        family = (_MultinomialFamily if multi else _LogRegFamily)(self.estimator, [{}], X, y, scorers)
         cv = check_cv(self.cv, y, classifier=is_classifier(self.estimator))
         n_samples, n_features = X.shape
         min_features_to_select = n_features // 2 if self.min_features_to_select is None \
@@ -84,13 +85,13 @@ class DistFeatureEliminator(_ScParamMixin, ClassifierMixin, BaseEstimator):
 
         rank, world, _ = parallel.dist_info()
         eng = get_engine()
+        _check_engine_entries(family, eng)
         ycls = np.searchsorted(classes, y).astype(np.int32)
         cv_splits = list(cv.split(X, y, groups))
         n_splits = len(cv_splits)
         fold = _fold_ids(cv_splits, n_samples)
         parallel.stage_x_replicated(eng, X)
-        eng.stage_labels(ycls)
-        eng.stage_folds(fold, n_splits)
+        family.stage(eng, X, fold, n_splits, x_staged=True)      # class ids (== ycls) and fold ids
         kw = dict(fit_intercept=p["fit_intercept"], tol=p["tol"], max_iter=p["max_iter"])
         one = np.ones(1, np.int32)
         weights = _ClassWeights(classes, ycls)
@@ -123,21 +124,17 @@ class DistFeatureEliminator(_ScParamMixin, ClassifierMixin, BaseEstimator):
         for i, col in enumerate(mine):
             masks[i, features_to_remove[col // n_splits]] = 0
         f_cols = (np.asarray(mine) % n_splits).astype(np.int32)
-        pos = np.ones(len(mine), np.int32)
         if len(mine):
             eng.stage_column_masks(masks)
             res = fit(np.full(len(mine), p["C"]), f_cols)
-            if multi:
-                correct, count = eng.multinomial_score_batch(res["coef"], f_cols)
-                loc = correct / np.maximum(count, 1)
-            elif metric[0] == "roc_auc":       # the reference's examples/eliminate/basic_usage.py scorer
-                loc, _ = eng.linear_auc_batch(res["coef"], f_cols, pos)
-            else:
-                correct, count = eng.linear_score_batch(res["coef"], f_cols, pos)
-                loc = correct / np.maximum(count, 1)
+            loc = np.asarray(family.score_columns(eng, res["coef"], f_cols)["score"], dtype=np.float64)
         else:
             loc = np.zeros(0)
         scores = np.asarray(parallel.all_gather_columns(loc, n_cols, rank, world), dtype=np.float64)
+        if not np.all(np.isfinite(scores)):
+            # the reference's _fit_and_score_one (ref :29-38) calls the scorer bare: its error propagates
+            raise ValueError("scoring=%r failed on a (feature set, fold) fit: scikit-learn's scorer raises there "
+                             "(for example a fold without every class)" % (self.scoring,))
         self.scores_ = [float(np.mean(s)) for s in scores.reshape(n_sets, n_splits)]   # ref :214-217
         best_set_ = int(np.argmax(self.scores_))
         self.best_score_ = self.scores_[best_set_]

@@ -6,8 +6,9 @@
   _MultinomialFamily   more than two classes: multinomial problems (csrc/logreg_multi.cu)
 
 Scorers are functions of device-side counts / sums: confusion counts (accuracy, balanced accuracy,
-precision / recall / f1 with any averaging), integer pair counts (roc_auc, csrc/auc.cu) and a sum of
--log p (neg_log_loss)."""
+precision / recall / f1 with any averaging), ranked counts per segment (csrc/auc.cu: roc_auc on the decision
+values, roc_auc_ovr / roc_auc_ovo [_weighted] on float32 predict_proba, average_precision on the decision
+values) and a sum of -log p (neg_log_loss)."""
 import time
 from collections import defaultdict
 
@@ -71,6 +72,10 @@ def _count_metric(scorer):
     if getattr(f, "__name__", "") == "roc_auc_score" and not kwargs and getattr(scorer, "_sign", 1) == 1:
         # scoring="roc_auc": roc_auc_score(y, decision_function(X)) -- exact pair counts on the device (csrc/auc.cu)
         return "roc_auc", None
+    rank = _ranking_metric(getattr(f, "__name__", ""), dict(kwargs), getattr(scorer, "_response_method", None),
+                           getattr(scorer, "_sign", 1))
+    if rank is not None:
+        return rank
     if kind is None or getattr(scorer, "_sign", 1) != 1:
         return None
     if kind in ("accuracy", "balanced_accuracy"):
@@ -82,6 +87,126 @@ def _count_metric(scorer):
     if pos_label != 1 and not (average != "binary" and pos_label is None):
         return None
     return kind, average
+
+
+# ranking scorers -> the score the device ranks: "proba" = float32 predict_proba, "decision" = decision_function
+_RANK_SCORE = {"roc_auc_ovr": "proba", "roc_auc_ovo": "proba", "average_precision": "decision"}
+SUPPORTED_CLASSIFIER_SCORERS = (
+    "accuracy, balanced_accuracy, precision / recall / f1 with average binary (binary target), micro, macro or "
+    "weighted, roc_auc (binary target), roc_auc_ovr, roc_auc_ovr_weighted, roc_auc_ovo, roc_auc_ovo_weighted, "
+    "average_precision, neg_log_loss")
+
+
+def _ranking_metric(func_name, kwargs, response_method, sign):
+    """(kind, average) of a ranking scorer the rank kernel serves, or None:
+      roc_auc_score(multi_class="ovr" | "ovo", average="macro" | "weighted") on predict_proba
+          -> ("roc_auc_ovr" | "roc_auc_ovo", average)
+      average_precision_score() on decision_function first -> ("average_precision", None)"""
+    if sign != 1:
+        return None
+    rm = tuple(response_method) if isinstance(response_method, (list, tuple)) else (response_method,)
+    if func_name == "roc_auc_score" and rm == ("predict_proba",):
+        multi_class = kwargs.pop("multi_class", "raise")
+        average = kwargs.pop("average", "macro")
+        if kwargs or multi_class not in ("ovr", "ovo") or average not in ("macro", "weighted"):
+            return None
+        return "roc_auc_" + multi_class, average
+    if func_name == "average_precision_score" and not kwargs and rm and rm[0] == "decision_function":
+        return "average_precision", None
+    return None
+
+
+def _is_rank(metric):
+    """True for the (kind, average) of a ranking scorer served by the rank kernel."""
+    return isinstance(metric, tuple) and metric[0] in _RANK_SCORE
+
+
+def _rank_entries(metrics):
+    """Engine entries the scorers in `metrics` call beyond the fit and count kernels."""
+    return ("linear_rank_batch",) if any(_is_rank(k) for k in metrics.values()) else ()
+
+
+def _check_engine_entries(family, eng):
+    """Raise NotImplementedError before any fit when the engine lacks an entry the family's scorers call: a
+    scorer whose kernel the engine does not provide has no device path (and no CPU fallback)."""
+    missing = [e for e in getattr(family, "engine_entries", ()) if not hasattr(eng, e)]
+    if missing:
+        raise NotImplementedError(
+            "scorers %s need %s, which %s does not provide: no device path on this engine"
+            % (sorted(family.metrics), ", ".join(missing), type(eng).__name__))
+
+
+def _label_one(classes):
+    """Class id of the label 1 (the pos_label of the average_precision scorer), or None when no class is 1."""
+    hits = [i for i, c in enumerate(classes) if not isinstance(c, (str, bytes)) and c == 1]
+    return hits[0] if hits else None
+
+
+def _auc(r):
+    """ROC-AUC per segment from {2U, n_pos, n_neg}: NaN where a class is missing."""
+    den = 2.0 * r["n_pos"].astype(np.float64) * r["n_neg"].astype(np.float64)
+    return np.divide(r["u2"].astype(np.float64), den, out=np.full(den.shape, np.nan), where=den > 0)
+
+
+def _rank_average(kind, average, r, K):
+    """Per-column score of a ranking scorer from the per-segment counts r ([B, S] arrays), averaged as
+    SK/metrics/_ranking.py averages them.  K == 1: binary columns, one segment each.  K > 2: a column whose
+    rows miss a class gets NaN (scikit-learn raises "Number of classes in y_true not equal to the number of
+    columns in 'y_score'", and y_true / y_score shapes differ for average_precision)."""
+    if K == 1:
+        return r["ap"][:, 0] if kind == "average_precision" else _auc(r)[:, 0]
+    if kind == "roc_auc_ovo":
+        # segment a * (K - 1) + (b < a ? b : b - 1): positives y == a, negatives y == b
+        n_cls = r["n_pos"][:, ::K - 1]                                   # rows of class a (segment (a, *))
+        auc = _auc(r)
+        a, b = np.triu_indices(K, 1)
+        ab = a * (K - 1) + b - 1
+        ba = b * (K - 1) + a
+        pair = (auc[:, ab] + auc[:, ba]) / 2.0
+        if average == "macro":
+            val = pair.mean(axis=1)
+        else:       # prevalence (n_a + n_b) / n of the pair
+            prev = (n_cls[:, a] + n_cls[:, b]) / n_cls.sum(axis=1, keepdims=True).astype(np.float64)
+            val = (pair * prev).sum(axis=1) / prev.sum(axis=1)
+    else:
+        n_cls = r["n_pos"]
+        per = r["ap"] if kind == "average_precision" else _auc(r)
+        if average == "weighted":
+            w = n_cls.astype(np.float64)
+            val = (per * w).sum(axis=1) / np.maximum(w.sum(axis=1), 1.0)
+        else:
+            val = per.mean(axis=1)
+    return np.where(np.all(n_cls > 0, axis=1), val, np.nan)
+
+
+class _RankScores:
+    """Ranking scorers of one scoring call: one rank-kernel call per (score, pairs) the scorers need.
+    binary_proba: the score that ranks as predict_proba[:, 1] does on binary columns."""
+
+    def __init__(self, eng, coef, codes, label_one=1, binary_proba="proba"):
+        self.eng, self.coef, self.codes, self.label_one = eng, coef, codes, label_one
+        self.binary_proba = binary_proba
+        self.cache = {}
+
+    def value(self, kind, average):
+        K = 1 if self.coef.ndim == 2 else self.coef.shape[1]
+        score, pos = _RANK_SCORE[kind], None
+        if K == 1:
+            if score == "proba":
+                score = self.binary_proba
+            pos = 1
+            if kind == "average_precision":     # pos_label=1: classes_[1] as usual, classes_[0] on -decision
+                if self.label_one is None:      # scikit-learn: "pos_label=1 is not a valid label"
+                    return np.full(len(self.codes), np.nan)
+                pos = self.label_one
+                score = "decision" if pos == 1 else "neg_decision"
+        pairs = kind == "roc_auc_ovo" and K > 1
+        key = (score, pairs, pos)
+        if key not in self.cache:
+            self.cache[key] = self.eng.linear_rank_batch(
+                self.coef, self.codes, None if K > 1 else np.full(len(self.codes), pos, dtype=np.int32),
+                score=score, pairs=pairs)
+        return _rank_average(kind, average, self.cache[key], K)
 
 
 def _metric_from_confusion(kind, average, conf):
@@ -222,17 +347,19 @@ class _LogRegFamily:
         self.weights = _ClassWeights(self.classes_, self.y_class)
         # every scorer must be a count-based metric (accuracy / precision / recall / f1 / balanced
         # accuracy on predict); scoring=None -> _PassthroughScorer -> estimator.score == accuracy
+        self.label_one = _label_one(self.classes_)
         self.metrics = {}
         for name, scorer in scorers.items():
             m = _count_metric(scorer)
             if m is None:
                 raise NotImplementedError(
-                    "scorer %r has no device path for classifiers (supported: accuracy, balanced_accuracy, "
-                    "precision / recall / f1 with average binary, micro, macro or weighted, roc_auc, "
-                    "neg_log_loss)" % (scorer,))
-            # binary averaging keeps the plain name; averaged variants carry (kind, average)
-            self.metrics[name] = m[0] if m[1] in (None, "binary") else m
-        self.needs_pred_pos = any(k not in ("accuracy", "roc_auc", "neg_log_loss") for k in self.metrics.values())
+                    "scorer %r has no device path for classifiers (supported: %s)"
+                    % (scorer, SUPPORTED_CLASSIFIER_SCORERS))
+            # binary averaging keeps the plain name; averaged variants and ranking scorers carry (kind, average)
+            self.metrics[name] = m if _is_rank(m) or m[1] not in (None, "binary") else m[0]
+        self.needs_pred_pos = any(k not in ("accuracy", "roc_auc", "neg_log_loss") and not _is_rank(k)
+                                  for k in self.metrics.values())
+        self.engine_entries = _rank_entries(self.metrics)
 
     def stage(self, eng, X, fold, n_splits, x_staged=False):
         if not x_staged:
@@ -261,11 +388,14 @@ class _LogRegFamily:
             neg_correct, _ = eng.linear_score_batch(coef, codes, np.full(len(pos), -7, dtype=np.int32))
             pred_pos = count - neg_correct
         out = {}
+        rank = _RankScores(eng, coef, codes, self.label_one)
         for name, kind in self.metrics.items():
             if kind == "roc_auc":
                 out[name], _ = eng.linear_auc_batch(coef, codes, pos)
             elif kind == "neg_log_loss":
                 out[name] = -eng.linear_logloss_batch(coef, codes, pos)[0]
+            elif _is_rank(kind):
+                out[name] = rank.value(*kind)
             elif isinstance(kind, tuple):      # micro / macro / weighted: 2 x 2 confusion [true, predicted]
                 tp = (pred_pos + actual_pos + correct - count) / 2.0
                 fp, fn = pred_pos - tp, actual_pos - tp
@@ -274,6 +404,14 @@ class _LogRegFamily:
             else:
                 out[name] = _metric_from_counts(kind, correct, count, pred_pos, actual_pos)
         return out, count
+
+    def score_columns(self, eng, coef, codes):
+        """{scorer name: per-column value} of fitted coefficients on the rows the scoring codes select."""
+        codes = np.asarray(codes, dtype=np.int32)
+        f = np.where(codes >= 0, codes, -3 - codes)
+        actual = np.where(codes >= 0, self.pos_in_fold[np.clip(f, 0, None)],
+                          np.where(codes == -2, self.total_pos, self.total_pos - self.pos_in_fold[np.clip(f, 0, None)]))
+        return self._scores(eng, coef, codes, np.ones(len(codes), dtype=np.int32), actual)[0]
 
     def column_cost(self, n_splits):
         """Expected relative duration of every (candidate, fold) column, for the multi-GPU block deal."""
@@ -403,9 +541,12 @@ class _MultinomialFamily(_LogRegFamily):
             if m is None or m[1] == "binary" or m[0] == "roc_auc":    # scikit-learn itself rejects these on a multiclass target
                 raise NotImplementedError(
                     "scorer %r has no device path for a multiclass target (supported: accuracy, "
-                    "balanced_accuracy, precision / recall / f1 with average micro, macro or weighted)" % (scorer,))
+                    "balanced_accuracy, precision / recall / f1 with average micro, macro or weighted, "
+                    "roc_auc_ovr, roc_auc_ovr_weighted, roc_auc_ovo, roc_auc_ovo_weighted, average_precision, "
+                    "neg_log_loss)" % (scorer,))
             self.metrics[name] = m
         self.needs_pred_pos = False
+        self.engine_entries = _rank_entries(self.metrics)
 
     def stage(self, eng, X, fold, n_splits, x_staged=False):
         if not x_staged:
@@ -440,9 +581,9 @@ class _MultinomialFamily(_LogRegFamily):
                                                    max_iter=mi)
             t1 = time.time()
             conf = eng.multinomial_confusion_batch(res["coef"], fold[idx])
+            for name, v in self._values(eng, conf, res["coef"], fold[idx]).items():
+                out["test_%s" % name][idx] = v
             t2 = time.time()
-            for name, (kind, average) in self.metrics.items():
-                out["test_%s" % name][idx] = self._metric(eng, kind, average, conf, res["coef"], fold[idx])
             out["n_test"][idx] = conf.sum(axis=(1, 2))
             out["fit_time"][idx] = (t1 - t0) / len(idx)
             out["score_time"][idx] = (t2 - t1) / len(idx)
@@ -451,15 +592,26 @@ class _MultinomialFamily(_LogRegFamily):
             if return_train_score:
                 train = _train_codes(fold[idx])
                 conf = eng.multinomial_confusion_batch(res["coef"], train)
-                for name, (kind, average) in self.metrics.items():
-                    out["train_%s" % name][idx] = self._metric(eng, kind, average, conf, res["coef"], train)
+                for name, v in self._values(eng, conf, res["coef"], train).items():
+                    out["train_%s" % name][idx] = v
         return out
 
-    @staticmethod
-    def _metric(eng, kind, average, conf, coef, codes):
-        if kind == "neg_log_loss":
-            return -eng.linear_logloss_batch(coef, codes)[0]
-        return _metric_from_confusion(kind, average, conf)
+    def _values(self, eng, conf, coef, codes):
+        """{scorer name: per-problem value} from the confusion counts conf of the rows the codes select."""
+        rank = _RankScores(eng, coef, codes)
+        out = {}
+        for name, (kind, average) in self.metrics.items():
+            if kind == "neg_log_loss":
+                out[name] = -eng.linear_logloss_batch(coef, codes)[0]
+            elif _is_rank((kind, average)):
+                out[name] = rank.value(kind, average)
+            else:
+                out[name] = _metric_from_confusion(kind, average, conf)
+        return out
+
+    def score_columns(self, eng, coef, codes):
+        """{scorer name: per-problem value} of fitted coefficients on the rows the scoring codes select."""
+        return self._values(eng, eng.multinomial_confusion_batch(coef, codes), coef, codes)
 
     def refit(self, eng, params, X_dtype, n_features):
         p = _check_logreg(_resolve(self.estimator, params), class_weight=True)

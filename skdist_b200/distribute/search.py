@@ -46,7 +46,7 @@ __all__ = ["DistGridSearchCV", "DistRandomizedSearchCV", "DistMultiModelSearch"]
 
 
 from .folds import _cv_fold_groups, _cv_fold_ids, _encode_target
-from .logreg_family import _LogRegFamily, _MultinomialFamily
+from .logreg_family import _check_engine_entries, _LogRegFamily, _MultinomialFamily
 
 
 # ----------------------------------------------------------------------------------------
@@ -122,6 +122,7 @@ class DistBaseSearchCV(_ScParamMixin):
                 layouts, n_splits = _cv_fold_groups(cv, X, y_arr, groups, n_samples, enc, train_orders)
                 fold = layouts[0][0]
                 family = _pick_family(estimator, candidate_params, X_arr, y_arr, scorers, enc)
+                _check_engine_entries(family, eng)
                 if self.refit and self.preds and not hasattr(family, "fold_proba"):
                     raise NotImplementedError("preds=True has no device path for %s" % type(estimator).__name__)
                 if hasattr(family, "prepare"):      # host-only statistics of the folds (no engine calls)
@@ -357,6 +358,7 @@ class DistMultiModelSearch(_ScParamMixin, BaseEstimator):
             cands = [param_sets[i]["param_set"] for i in rows]
             scorers, _ = _check_multimetric_scoring(estimator, scoring=self.scoring)
             family = _pick_family(estimator, cands, X_arr, y_arr, scorers)
+            _check_engine_entries(family, eng)
             families[index] = family
             family.stage(eng, X_arr, fold, n_splits)
             n_cols = len(cands) * n_splits

@@ -12,7 +12,10 @@ in alpha, so every (candidate, fold, class) column of a launch runs side by side
 
 Only alpha varies within a launch; the other searchable parameters group the launches.  Scores come from the
 device scoring kernels: confusion counts of the `decision > 0` rule (binary) or of the first arg-max of the K
-decision values (multiclass), exact pair counts (roc_auc) and, for binary log_loss, the expit log loss."""
+decision values (multiclass), exact pair counts (roc_auc) and, for binary log_loss, the expit log loss.  On a
+binary target the ranking scorers run on the rank kernel: average_precision on the decision values, and
+roc_auc_ovr / roc_auc_ovo [_weighted] (the AUC of predict_proba[:, 1], ranked as the decision values rank) when
+every candidate has loss="log_loss"."""
 import copy
 import time
 import warnings
@@ -24,7 +27,8 @@ from .. import parallel
 from ..engine import sgd_config, sgd_seed
 from .base import _clone, _merged_params
 from .folds import _classes_and_ids, _train_codes
-from .logreg_family import _count_metric, _metric_from_confusion, _metric_from_counts
+from .logreg_family import (_count_metric, _is_rank, _label_one, _metric_from_confusion, _metric_from_counts,
+                            _rank_entries, _RankScores)
 
 _MAX_INT = np.iinfo(np.int32).max
 # parameters that group the launches (one value per launch); alpha varies per column
@@ -90,24 +94,29 @@ class _SGDFamily:
         for name, scorer in scorers.items():
             m = _count_metric(scorer)
             ok = m is not None
-            if ok and self.binary and m[0] == "neg_log_loss":
+            if ok and self.binary and (m[0] == "neg_log_loss" or m[0] in ("roc_auc_ovr", "roc_auc_ovo")):
                 # predict_proba of log_loss is _predict_proba_lr's expit; hinge has none
                 ok = all(q["loss"] == "log_loss" for q in self.cands)
             elif ok and not self.binary:
                 # scikit-learn rejects binary averaging and roc_auc on a multiclass target; SGD's multiclass
-                # probabilities are one-vs-rest normalised, not the softmax the device log loss forms
-                ok = m[1] != "binary" and m[0] not in ("roc_auc", "neg_log_loss")
+                # probabilities are one-vs-rest normalised, not the softmax the device forms, and its
+                # average_precision stays with them
+                ok = m[1] != "binary" and m[0] not in ("roc_auc", "neg_log_loss") and not _is_rank(m)
             if not ok:
                 raise NotImplementedError(
                     "scorer %r has no device path for SGDClassifier (supported: accuracy, balanced_accuracy, "
                     "precision / recall / f1 with average binary (binary target), micro, macro or weighted, "
-                    "roc_auc (binary target), neg_log_loss (binary target, loss='log_loss'))" % (scorer,))
+                    "roc_auc and average_precision (binary target), neg_log_loss, roc_auc_ovr, "
+                    "roc_auc_ovr_weighted, roc_auc_ovo and roc_auc_ovo_weighted (binary target, "
+                    "loss='log_loss'))" % (scorer,))
             if self.binary:
-                self.metrics[name] = m[0] if m[1] in (None, "binary") else m
+                self.metrics[name] = m if _is_rank(m) or m[1] not in (None, "binary") else m[0]
             else:
                 self.metrics[name] = m
         self.needs_pred_pos = self.binary and any(
-            k not in ("accuracy", "roc_auc", "neg_log_loss") for k in self.metrics.values())
+            k not in ("accuracy", "roc_auc", "neg_log_loss") and not _is_rank(k) for k in self.metrics.values())
+        self.label_one = _label_one(self.classes_)
+        self.engine_entries = _rank_entries(self.metrics)
         self.fold, self.train_rows = None, None
 
     # -- layout -------------------------------------------------------------------------------------------
@@ -182,11 +191,16 @@ class _SGDFamily:
             neg_correct, _ = eng.linear_score_batch(coef, codes, np.full(len(pos), -7, dtype=np.int32))
             pred_pos = count - neg_correct
         out = {}
+        # binary SGDClassifier's predict_proba is expit of a float64 decision (float64 intercept_): strictly
+        # increasing in z until float64 saturates (|z| > 36), so it ranks the rows as the decision values do
+        rank = _RankScores(eng, coef, codes, self.label_one, binary_proba="decision")
         for name, kind in self.metrics.items():
             if kind == "roc_auc":
                 out[name], _ = eng.linear_auc_batch(coef, codes, pos)
             elif kind == "neg_log_loss":
                 out[name] = -eng.linear_logloss_batch(coef, codes, pos)[0]
+            elif _is_rank(kind):
+                out[name] = rank.value(*kind)
             elif isinstance(kind, tuple):
                 tp = (pred_pos + actual_pos + correct - count) / 2.0
                 fp, fn = pred_pos - tp, actual_pos - tp

@@ -292,6 +292,29 @@ class Engine:
         den = 2.0 * n_pos.astype(np.float64) * n_neg.astype(np.float64)
         return np.divide(u2.astype(np.float64), den, out=np.full(B, np.nan), where=den > 0), n_pos + n_neg
 
+    RANK_SCORES = {"decision": 0, "neg_decision": 1, "proba": 2}
+
+    def linear_rank_batch(self, coef, col_fold, col_pos=None, score="decision", pairs=False):
+        """Ranked counts per segment on the rows selected by the fold codes: {"u2", "n_pos", "n_neg", "ap"},
+        each [B, S].  coef [B, d+1] with col_pos: one binary segment per column; coef [B, K, d+1]: K
+        one-vs-rest segments per column, or K (K - 1) ordered one-vs-one pairs when `pairs`.  score:
+        "decision", "neg_decision" or "proba" (float32 predict_proba)."""
+        coef = np.ascontiguousarray(coef, dtype=np.float32)
+        B = coef.shape[0]
+        K = 1 if coef.ndim == 2 else coef.shape[1]
+        assert coef.shape[-1] == self.d + 1
+        col_fold = np.ascontiguousarray(col_fold, dtype=np.int32)
+        if K == 1:
+            col_pos = np.ascontiguousarray(col_pos, dtype=np.int32)
+        S = 1 if K == 1 else (K * (K - 1) if pairs else K)
+        out = {k: np.empty((B, S), dtype=np.int64) for k in ("u2", "n_pos", "n_neg")}
+        out["ap"] = np.empty((B, S), dtype=np.float64)
+        check(self._lib.skd_linear_rank_batch(self._h, B, K, ptr(coef), ptr(col_fold),
+                                              ptr(col_pos) if K == 1 else None, self.RANK_SCORES[score],
+                                              int(bool(pairs)), ptr(out["u2"]), ptr(out["n_pos"]),
+                                              ptr(out["n_neg"]), ptr(out["ap"])), self._h)
+        return out
+
     def linear_logloss_batch(self, coef, col_fold, col_pos=None):
         """Mean log loss of the predicted probabilities per column on the rows selected by the fold codes.
         coef [B, d+1] with col_pos: binary columns; coef [B, K, d+1]: multiclass."""
