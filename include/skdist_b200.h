@@ -383,7 +383,41 @@ double* skd_lbfgs_g(skd_lbfgs* h);
 int skd_lbfgs_advance(skd_lbfgs* h, double f); /* returns status (0 = evaluate at x again) */
 int skd_lbfgs_nit(skd_lbfgs* h);
 int skd_lbfgs_nfev(skd_lbfgs* h);
+/* the core's whole state, struct LbfgsScalars of csrc/lbfgs_core.h, as raw bytes; set_state writes it back
+ * (tests: a core that loses one pair update, to show that the device comparison would notice) */
+void skd_lbfgs_state(skd_lbfgs* h, void* out);
+void skd_lbfgs_set_state(skd_lbfgs* h, const void* in);
+int skd_lbfgs_state_bytes(void);
 void skd_lbfgs_free(skd_lbfgs* h);
+
+/* Diagnostic / test entry: the device optimiser of skd_logreg_fit_batch (K == 1) and
+ * skd_logreg_multinomial_fit_batch (K >= 2) driven by caller-supplied evaluation partials
+ * instead of an evaluation kernel.  It needs a staged X: d and the row pitch come from it.
+ * create: B columns of K * (d + 1) variables, x0 = 0, memory 10; grouped = 1 runs the fold-grouped
+ *   slot layout of the tensor-core fit (K == 1, d <= 256, labels staged; col_fold in -1..127),
+ *   grouped = 0 slot s = column s; nz partials per slot; use_reduce = 1 reduces the gradient partials
+ *   with the whole device first when nz > 8, as the tensor-core fit does; l2[B], inv_n[B];
+ *   gscale[d] (K == 1) or NULL; fmask[B x d] (1 = feature takes part) or NULL.
+ *   dims_out[4] = {variables per column, slot-list capacity, row pitch ldw, floats of rows_out}.
+ * step: one optimiser round.  loss_parts[B][nz] and gsum_parts[B*K][nz] (float64) and
+ *   grad_parts[B*K][nz][d] (fp32) are scattered by the current slot list into the partial buffers
+ *   with stride n_act_in (between the live slot count and the capacity); slots that hold no live
+ *   column get NaN.  Returns x_out[B][K*(d+1)], state_out[B] (struct LbfgsScalars), slot_out[cap][4]
+ *   ({col, fold, pos, pad}), counts_out[4] = {slots, running, round record} and, if not NULL and
+ *   dims_out[3] > 0, the exported fp32 rows (weights [slots x ldw], then one bias per slot).
+ * finish: coef[B][K*(d+1)] (fp32), n_iter, status and loss of every column. */
+typedef struct skd_lbfgs_dev skd_lbfgs_dev;
+skd_lbfgs_dev* skd_lbfgs_dev_create(skd_ctx* ctx, int32_t B, int32_t K, int32_t d, int32_t fit_intercept,
+                                    int32_t grouped, const int32_t* col_fold, int32_t nz, int32_t use_reduce,
+                                    int32_t maxiter, int32_t maxls, double pgtol, double ftol, const double* l2,
+                                    const double* inv_n, const double* gscale, const uint8_t* fmask,
+                                    int32_t* dims_out);
+int skd_lbfgs_dev_step(skd_lbfgs_dev* h, int32_t n_act_in, const double* loss_parts, const double* gsum_parts,
+                       const float* grad_parts, double* x_out, void* state_out, int32_t* slot_out,
+                       int32_t* counts_out, float* rows_out);
+int skd_lbfgs_dev_finish(skd_lbfgs_dev* h, float* coef_out, int32_t* n_iter_out, int32_t* status_out,
+                         double* loss_out);
+void skd_lbfgs_dev_free(skd_lbfgs_dev* h);
 
 #ifdef __cplusplus
 }

@@ -108,7 +108,17 @@ SYMBOLS = {
     "skd_lbfgs_advance": (_c.c_int, [_c.c_void_p, _c.c_double]),
     "skd_lbfgs_nit": (_c.c_int, [_c.c_void_p]),
     "skd_lbfgs_nfev": (_c.c_int, [_c.c_void_p]),
+    "skd_lbfgs_state": (None, [_c.c_void_p, _c.c_void_p]),
+    "skd_lbfgs_set_state": (None, [_c.c_void_p, _c.c_void_p]),
+    "skd_lbfgs_state_bytes": (_c.c_int, []),
     "skd_lbfgs_free": (None, [_c.c_void_p]),
+    "skd_lbfgs_dev_create": (_c.c_void_p, [_c.c_void_p, _c.c_int32, _c.c_int32, _c.c_int32, _c.c_int32, _c.c_int32,
+                                           _c.c_void_p, _c.c_int32, _c.c_int32, _c.c_int32, _c.c_int32, _c.c_double,
+                                           _c.c_double, _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_void_p,
+                                           _c.c_void_p]),
+    "skd_lbfgs_dev_step": (_c.c_int, [_c.c_void_p, _c.c_int32] + [_c.c_void_p] * 8),
+    "skd_lbfgs_dev_finish": (_c.c_int, [_c.c_void_p] + [_c.c_void_p] * 4),
+    "skd_lbfgs_dev_free": (None, [_c.c_void_p]),
 }
 
 

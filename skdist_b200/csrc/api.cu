@@ -155,29 +155,35 @@ static int alloc_eval_buffers(Ctx* c, Scratch& sx, LogregWork& w, int B, int slo
   return 0;
 }
 
+// The fold-grouped slot layout: columns stable-sorted by held-out fold, every fold segment padded with
+// col = -1 slots to a multiple of 128 (one MMA group = one fold -> tile skipping).
+static int grouped_slot_layout(Ctx* c, int B, const int32_t* col_fold, const int32_t* col_pos, const int32_t* col_neg,
+                               std::vector<SlotMeta>& hslots) {
+  hslots.clear();
+  std::vector<int> order(B);
+  for (int j = 0; j < B; ++j) order[j] = j;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return col_fold[a] < col_fold[b]; });
+  for (int i = 0; i < B;) {
+    const int f = col_fold[order[i]];
+    if (f > 127) return fail(c, "fold id above 127");
+    for (; i < B && col_fold[order[i]] == f; ++i) {
+      SlotMeta sm; sm.col = order[i]; sm.fold = f < 0 ? -1 : f; sm.pos = col_pos[order[i]];
+      sm.pad = (col_neg && col_neg[order[i]] >= 0) ? col_neg[order[i]] + 1 : 0;
+      hslots.push_back(sm);
+    }
+    while (hslots.size() % 128) { SlotMeta sm; sm.col = -1; sm.fold = f < 0 ? -1 : f; sm.pos = -1; sm.pad = 0; hslots.push_back(sm); }
+  }
+  return 0;
+}
+
 // Slot layout of a logistic batch, then its evaluation buffers (alloc_eval_buffers).  The tensor-core
-// path runs the fold-grouped layout: columns stable-sorted by held-out fold, every fold segment padded
-// with col = -1 slots to a multiple of 128 (one MMA group = one fold -> tile skipping), and w.uni_pos
-// set when every column is one-vs-rest with the same positive class.  hslots receives that layout;
-// it stays empty for the SIMT path, whose slot s is column s.
+// path runs the fold-grouped layout (grouped_slot_layout), with w.uni_pos set when every column is
+// one-vs-rest with the same positive class.  hslots receives that layout; it stays empty for the SIMT
+// path, whose slot s is column s.
 static int alloc_logreg_slots(Ctx* c, Scratch& sx, LogregWork& w, int B, const int32_t* col_fold,
                               const int32_t* col_pos, const int32_t* col_neg, std::vector<SlotMeta>& hslots) {
   hslots.clear();
-  if (want_tc(c) && tc_supported(c)) {
-    std::vector<int> order(B);
-    for (int j = 0; j < B; ++j) order[j] = j;
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return col_fold[a] < col_fold[b]; });
-    for (int i = 0; i < B;) {
-      const int f = col_fold[order[i]];
-      if (f > 127) return fail(c, "fold id above 127");
-      for (; i < B && col_fold[order[i]] == f; ++i) {
-        SlotMeta sm; sm.col = order[i]; sm.fold = f < 0 ? -1 : f; sm.pos = col_pos[order[i]];
-        sm.pad = (col_neg && col_neg[order[i]] >= 0) ? col_neg[order[i]] + 1 : 0;
-        hslots.push_back(sm);
-      }
-      while (hslots.size() % 128) { SlotMeta sm; sm.col = -1; sm.fold = f < 0 ? -1 : f; sm.pos = -1; sm.pad = 0; hslots.push_back(sm); }
-    }
-  }
+  if (want_tc(c) && tc_supported(c) && grouped_slot_layout(c, B, col_fold, col_pos, col_neg, hslots)) return 1;
   if (alloc_eval_buffers(c, sx, w, B, hslots.empty() ? B : (int)hslots.size())) return 1;
   w.grouped = !hslots.empty() && w.use_tc;
   if (!w.grouped) {
@@ -1812,6 +1818,247 @@ int skd_linear_decision(skd_ctx* ctx, int32_t B, const float* coef, float* out) 
   return 0;
 }
 
+// ---- device optimiser on caller-supplied evaluation partials (tests) ------------------------
+}  // extern "C"
+
+struct skd_lbfgs_dev {
+  Ctx* c = nullptr;
+  std::unique_ptr<Scratch> sx;
+  int B = 0, K = 1, d = 0, n = 0, nz = 0, fit_intercept = 1;
+  int slot_cap = 0;   // entries of the slot (binary) or candidate (multinomial) list
+  int ldw = 0;        // row pitch of the gradient partials and of the exported rows
+  size_t rows = 0;    // floats of the exported fp32 rows (0: the grouped layout exports fp16 hi / lo)
+  LogregWork w;       // K == 1
+  MultiWork mw;       // K >= 2
+  int32_t* hist = nullptr;   // device {slots, running} of the last round
+};
+
+static int lbfgs_dev_setup(skd_lbfgs_dev* h, int grouped, const int32_t* col_fold, int use_reduce, int maxiter,
+                           int maxls, double pgtol, double ftol, const double* l2, const double* inv_n,
+                           const double* gscale, const uint8_t* fmask) {
+  Ctx* c = h->c;
+  const int B = h->B, K = h->K, d = h->d, dp = d + 1, m = 10;
+  if (!c->X) return fail(c, "skd_lbfgs_dev_create: stage X first (d and the row pitch come from it)");
+  if (B <= 0 || K < 1 || d != (int)c->d || h->nz < 1 || !col_fold || !l2 || !inv_n || maxiter < 1 || maxls < 1)
+    return fail(c, "skd_lbfgs_dev_create: bad arguments");
+  if (K > 1 && (grouped || use_reduce || gscale))
+    return fail(c, "skd_lbfgs_dev_create: the multinomial optimiser has the dense layout and the direct gather only");
+  SKD_CUDA(c, cudaSetDevice(c->device));
+  h->sx.reset(new Scratch(c));
+  Scratch& sx = *h->sx;
+  h->n = K * dp;
+  SKD_CUDA(c, sx.alloc(&h->hist, 2));
+  uint8_t* dmask = nullptr;
+  if (fmask) {
+    SKD_CUDA(c, sx.alloc(&dmask, (size_t)B * d));
+    SKD_CUDA(c, cudaMemcpyAsync(dmask, fmask, (size_t)B * d, cudaMemcpyHostToDevice, c->stream));
+  }
+  int32_t* dfold;
+  SKD_CUDA(c, sx.alloc(&dfold, (size_t)B));
+  SKD_CUDA(c, cudaMemcpyAsync(dfold, col_fold, B * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  if (K > 1) {
+    MultiWork& w = h->mw;
+    const size_t slots = (size_t)B * K;
+    w.B = B; w.K = K; w.dp = dp; w.nz = h->nz;
+    w.vec_stride = (size_t)(5 + 2 * m) * K * dp + 2 * m;
+    h->slot_cap = B;
+    h->ldw = (int)c->ldx;
+    h->rows = slots * c->ldx + slots;
+    SKD_CUDA(c, sx.alloc(&w.sc, (size_t)B));
+    SKD_CUDA(c, sx.alloc(&w.vec, (size_t)B * w.vec_stride));
+    SKD_CUDA(c, sx.alloc(&w.l2, (size_t)B));
+    SKD_CUDA(c, sx.alloc(&w.inv_n, (size_t)B));
+    SKD_CUDA(c, sx.alloc(&w.n_evals, (size_t)B));
+    SKD_CUDA(c, sx.alloc(&w.cand, (size_t)B));
+    SKD_CUDA(c, sx.alloc(&w.W, h->rows));
+    SKD_CUDA(c, sx.alloc(&w.lossp, (size_t)h->nz * B));
+    SKD_CUDA(c, sx.alloc(&w.gsump, (size_t)h->nz * slots));
+    SKD_CUDA(c, sx.alloc(&w.gradp, (size_t)h->nz * slots * c->ldx));
+    SKD_CUDA(c, sx.alloc(&w.n_act, 1));
+    SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2, B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n, B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    w.fmask = dmask;
+    if (multi_lbfgs_init(c, w, dfold, pgtol, maxiter, maxls, ftol)) return 1;
+    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+    return 0;
+  }
+  LogregWork& w = h->w;
+  w.B = B; w.dp = dp; w.nz = h->nz;
+  w.vec_stride = (size_t)(5 + 2 * m) * dp + 2 * m;
+  std::vector<int32_t> zeros(B, 0);
+  std::vector<SlotMeta> hslots;
+  if (grouped) {   // the fit's tensor-core layout; its trial points leave through tc_export
+    if (!tc_supported(c)) return fail(c, "skd_lbfgs_dev_create: the grouped layout needs a staged X with d <= 256");
+    if (grouped_slot_layout(c, B, col_fold, zeros.data(), nullptr, hslots)) return 1;
+    if (tc_prepare(c)) return 1;
+    w.use_tc = true;
+    w.grouped = true;
+    h->slot_cap = (int)hslots.size();
+    if (alloc_tc_weights(c, sx, w, h->slot_cap)) return 1;
+  } else {
+    h->slot_cap = B;
+    w.ldw = (int)c->ldx;
+    h->rows = (size_t)B * c->ldx + B;
+    SKD_CUDA(c, sx.alloc(&w.Wact, h->rows));
+  }
+  h->ldw = w.ldw;
+  w.slot_cap = h->slot_cap;
+  const size_t cap = (size_t)h->nz * h->slot_cap;
+  SKD_CUDA(c, sx.alloc(&w.lossp, cap));
+  SKD_CUDA(c, sx.alloc(&w.gsump, cap));
+  SKD_CUDA(c, sx.alloc(&w.gradp, cap * w.ldw));
+  if (use_reduce) SKD_CUDA(c, sx.alloc(&w.gradr, (size_t)h->slot_cap * w.ldw));
+  SKD_CUDA(c, sx.alloc(&w.sc, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&w.vec, (size_t)B * w.vec_stride));
+  SKD_CUDA(c, sx.alloc(&w.l2, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&w.inv_n, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&w.col_pos, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&w.n_evals, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&w.slot, (size_t)h->slot_cap));
+  SKD_CUDA(c, sx.alloc(&w.n_act, 1));
+  SKD_CUDA(c, sx.alloc(&w.n_run, 1));
+  w.col_fold = dfold;
+  w.fmask = dmask;
+  if (gscale) {
+    double* dgs;
+    SKD_CUDA(c, sx.alloc(&dgs, (size_t)d));
+    SKD_CUDA(c, cudaMemcpyAsync(dgs, gscale, d * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    w.gscale = dgs;
+  }
+  SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2, B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n, B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(w.col_pos, zeros.data(), B * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  const int32_t nrun = B;
+  SKD_CUDA(c, cudaMemcpyAsync(w.n_run, &nrun, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  if (w.grouped) {
+    const int32_t ns = h->slot_cap;
+    SKD_CUDA(c, cudaMemcpyAsync(w.slot, hslots.data(), hslots.size() * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &ns, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  }
+  if (lbfgs_dev_init(c, w, h->fit_intercept, pgtol, maxiter, maxls, ftol)) return 1;
+  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+// One round: the caller's per-column parts scattered into the partial buffers by the current slot list with
+// stride n_act_in (NaN in every slot that holds no live column), then the fit's optimiser round itself.
+static int lbfgs_dev_round(skd_lbfgs_dev* h, int n_act_in, const double* loss_parts, const double* gsum_parts,
+                           const float* grad_parts, double* x_out, void* state_out, int32_t* slot_out,
+                           int32_t* counts_out, float* rows_out) {
+  Ctx* c = h->c;
+  const int B = h->B, K = h->K, d = h->d, nz = h->nz, ldw = h->ldw;
+  SlotMeta* dslot = K > 1 ? h->mw.cand : h->w.slot;
+  int32_t* dn_act = K > 1 ? h->mw.n_act : h->w.n_act;
+  std::vector<SlotMeta> hs(h->slot_cap);
+  int32_t live = 0;
+  SKD_CUDA(c, cudaMemcpyAsync(hs.data(), dslot, hs.size() * sizeof(SlotMeta), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(&live, dn_act, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  if (n_act_in < live || n_act_in > h->slot_cap)
+    return fail(c, "skd_lbfgs_dev_step: n_act_in must lie between the live slot count and the slot capacity");
+  const double nan = std::nan("");
+  const size_t ns = (size_t)n_act_in * K;   // partial rows per chunk
+  std::vector<double> lp((size_t)nz * n_act_in, nan), gs((size_t)nz * ns, nan);
+  std::vector<float> gp((size_t)nz * ns * ldw, std::nanf(""));
+  for (int s = 0; s < live; ++s) {
+    const int col = hs[s].col;
+    if (col < 0) continue;
+    for (int z = 0; z < nz; ++z) {
+      lp[(size_t)z * n_act_in + s] = loss_parts[(size_t)col * nz + z];
+      for (int k = 0; k < K; ++k) {
+        const size_t row = (size_t)z * ns + (size_t)s * K + k, src = ((size_t)col * K + k) * nz + z;
+        gs[row] = gsum_parts[src];
+        memcpy(&gp[row * ldw], grad_parts + src * d, d * sizeof(float));
+      }
+    }
+  }
+  double* dl = K > 1 ? h->mw.lossp : h->w.lossp;
+  double* dg = K > 1 ? h->mw.gsump : h->w.gsump;
+  float* dgp = K > 1 ? h->mw.gradp : h->w.gradp;
+  SKD_CUDA(c, cudaMemcpyAsync(dl, lp.data(), lp.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(dg, gs.data(), gs.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(dgp, gp.data(), gp.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  if (K > 1) {
+    if (multi_lbfgs_enqueue(c, h->mw, n_act_in, h->fit_intercept, h->hist)) return 1;
+  } else if (lbfgs_dev_enqueue(c, h->w, n_act_in, nz, h->fit_intercept, h->hist)) {
+    return 1;
+  }
+  const double* vec = K > 1 ? h->mw.vec : h->w.vec;
+  const size_t stride = K > 1 ? h->mw.vec_stride : h->w.vec_stride;
+  const LbfgsScalars* sc = K > 1 ? h->mw.sc : h->w.sc;
+  SKD_CUDA(c, cudaMemcpy2DAsync(x_out, h->n * sizeof(double), vec, stride * sizeof(double), h->n * sizeof(double), B,
+                                cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(state_out, sc, B * sizeof(LbfgsScalars), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(slot_out, dslot, h->slot_cap * sizeof(SlotMeta), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(counts_out, dn_act, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(counts_out + 1, K > 1 || !h->w.grouped ? dn_act : h->w.n_run, sizeof(int32_t),
+                              cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(counts_out + 2, h->hist, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  if (rows_out && h->rows)
+    SKD_CUDA(c, cudaMemcpyAsync(rows_out, K > 1 ? h->mw.W : h->w.Wact, h->rows * sizeof(float), cudaMemcpyDeviceToHost,
+                                c->stream));
+  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+static int lbfgs_dev_result(skd_lbfgs_dev* h, float* coef_out, int32_t* n_iter_out, int32_t* status_out,
+                            double* loss_out) {
+  Ctx* c = h->c;
+  const int B = h->B;
+  Scratch sx(c);
+  float* dcoef; int32_t *dniter, *dstatus; double* dloss;
+  SKD_CUDA(c, sx.alloc(&dcoef, (size_t)B * h->n));
+  SKD_CUDA(c, sx.alloc(&dniter, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&dstatus, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&dloss, (size_t)B));
+  if (h->K > 1) {
+    if (multi_lbfgs_finish(c, h->mw, dcoef, dniter, dstatus, dloss)) return 1;
+  } else if (lbfgs_dev_finish(c, h->w, dcoef, dniter, dstatus, dloss)) {
+    return 1;
+  }
+  SKD_CUDA(c, cudaMemcpyAsync(coef_out, dcoef, (size_t)B * h->n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(n_iter_out, dniter, B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(status_out, dstatus, B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(loss_out, dloss, B * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+extern "C" {
+
+skd_lbfgs_dev* skd_lbfgs_dev_create(skd_ctx* ctx, int32_t B, int32_t K, int32_t d, int32_t fit_intercept,
+                                    int32_t grouped, const int32_t* col_fold, int32_t nz, int32_t use_reduce,
+                                    int32_t maxiter, int32_t maxls, double pgtol, double ftol, const double* l2,
+                                    const double* inv_n, const double* gscale, const uint8_t* fmask,
+                                    int32_t* dims_out) {
+  if (!ctx) { fail(nullptr, "skd_lbfgs_dev_create: ctx is NULL"); return nullptr; }
+  std::unique_ptr<skd_lbfgs_dev> h(new skd_lbfgs_dev());
+  h->c = &ctx->c; h->B = B; h->K = K; h->d = d; h->nz = nz; h->fit_intercept = fit_intercept ? 1 : 0;
+  if (lbfgs_dev_setup(h.get(), grouped, col_fold, use_reduce, maxiter, maxls, pgtol, ftol, l2, inv_n, gscale, fmask))
+    return nullptr;
+  if (dims_out) { dims_out[0] = h->n; dims_out[1] = h->slot_cap; dims_out[2] = h->ldw; dims_out[3] = (int32_t)h->rows; }
+  return h.release();
+}
+
+int skd_lbfgs_dev_step(skd_lbfgs_dev* h, int32_t n_act_in, const double* loss_parts, const double* gsum_parts,
+                       const float* grad_parts, double* x_out, void* state_out, int32_t* slot_out,
+                       int32_t* counts_out, float* rows_out) {
+  if (!h) return fail(nullptr, "skd_lbfgs_dev_step: handle is NULL");
+  if (!loss_parts || !gsum_parts || !grad_parts || !x_out || !state_out || !slot_out || !counts_out)
+    return fail(h->c, "skd_lbfgs_dev_step: bad arguments");
+  return lbfgs_dev_round(h, n_act_in, loss_parts, gsum_parts, grad_parts, x_out, state_out, slot_out, counts_out,
+                         rows_out);
+}
+
+int skd_lbfgs_dev_finish(skd_lbfgs_dev* h, float* coef_out, int32_t* n_iter_out, int32_t* status_out,
+                         double* loss_out) {
+  if (!h) return fail(nullptr, "skd_lbfgs_dev_finish: handle is NULL");
+  if (!coef_out || !n_iter_out || !status_out || !loss_out) return fail(h->c, "skd_lbfgs_dev_finish: bad arguments");
+  return lbfgs_dev_result(h, coef_out, n_iter_out, status_out, loss_out);
+}
+
+void skd_lbfgs_dev_free(skd_lbfgs_dev* h) { delete h; }
+
 // ---- host-side L-BFGS object (tests) ----------------------------------------------------
 skd_lbfgs* skd_lbfgs_create(int32_t n, int32_t m, int32_t maxiter, int32_t maxls, double pgtol,
                             double ftol) {
@@ -1839,6 +2086,9 @@ int skd_lbfgs_advance(skd_lbfgs* h, double f) {
 }
 int skd_lbfgs_nit(skd_lbfgs* h) { return h->s.nit; }
 int skd_lbfgs_nfev(skd_lbfgs* h) { return h->s.nfev; }
+void skd_lbfgs_state(skd_lbfgs* h, void* out) { memcpy(out, &h->s, sizeof(LbfgsScalars)); }
+void skd_lbfgs_set_state(skd_lbfgs* h, const void* in) { memcpy(&h->s, in, sizeof(LbfgsScalars)); }
+int skd_lbfgs_state_bytes(void) { return (int)sizeof(LbfgsScalars); }
 void skd_lbfgs_free(skd_lbfgs* h) { delete h; }
 
 }  // extern "C"

@@ -352,7 +352,6 @@ SKD_HD void lbfgs_advance(Par& P, LbfgsScalars& s, LbfgsVectors& v, double f_new
   int task = dcsrch(s, s.f, s.gd, s.stp, LS_FG, 0.0, stpmx);
   if (task == LS_FG) {
     s.ifun += 1;
-    s.nfev += 1;
     s.iback = s.ifun - 1;
     if (s.iback >= s.maxls) {
       // line search failed: restore the previous iterate
@@ -364,6 +363,8 @@ SKD_HD void lbfgs_advance(Par& P, LbfgsScalars& s, LbfgsVectors& v, double f_new
       lbfgs_new_direction_or_fail(P, s, v);
       return;
     }
+    // counted here, not above: a line search that has run out of maxls requests no evaluation
+    s.nfev += 1;
     double stp = s.stp;
     for (int i = P.tid(); i < n; i += P.nthr()) v.x[i] = stp * v.d[i] + v.t[i];
     P.sync();

@@ -366,10 +366,8 @@ __global__ void lb_finish_kernel(const LbfgsScalars* sc, const double* vec, size
   }
 }
 
-int lbfgs_dev_init(Ctx* c, LogregWork& w, int fit_intercept, double tol, int max_iter) {
-  (void)fit_intercept;
-  const int m = 10, maxls = 50;
-  const double ftol = 64.0 * 2.220446049250313e-16;
+int lbfgs_dev_init(Ctx* c, LogregWork& w, int fit_intercept, double tol, int max_iter, int maxls, double ftol) {
+  const int m = 10;
   lb_init_kernel<<<w.B, 128, 0, c->stream>>>(w.sc, w.vec, w.vec_stride, w.B, w.dp, m, max_iter,
                                              maxls, tol, ftol, w.grouped ? nullptr : w.slot, w.col_fold,
                                              w.col_pos, w.col_neg1, w.n_evals, w.n_act);
@@ -567,9 +565,9 @@ __global__ void mn_finish_kernel(const LbfgsScalars* sc, const double* vec, size
   }
 }
 
-int multi_lbfgs_init(Ctx* c, MultiWork& w, const int32_t* d_col_fold, double tol, int max_iter) {
-  const int m = 10, maxls = 50;
-  const double ftol = 64.0 * 2.220446049250313e-16;
+int multi_lbfgs_init(Ctx* c, MultiWork& w, const int32_t* d_col_fold, double tol, int max_iter, int maxls,
+                     double ftol) {
+  const int m = 10;
   mn_init_kernel<<<w.B, 128, 0, c->stream>>>(w.sc, w.vec, w.vec_stride, w.B, w.K * w.dp, m, max_iter, maxls,
                                              tol, ftol, w.cand, d_col_fold, w.n_evals, w.n_act);
   c->launches += 1;

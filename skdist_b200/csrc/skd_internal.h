@@ -339,7 +339,9 @@ struct MultiWork {
   uint8_t* fmask = nullptr;      // [B x d] or nullptr: 1 = feature takes part in the candidate's fit
   const float* cw = nullptr;     // [B x K] or nullptr: weight of each class in the candidate's fit
 };
-int multi_lbfgs_init(Ctx* c, MultiWork& w, const int32_t* d_col_fold, double tol, int max_iter);
+// maxls and ftol: what scikit-learn passes to scipy (maxls = 50, ftol = 64 * eps) unless a test entry says otherwise
+int multi_lbfgs_init(Ctx* c, MultiWork& w, const int32_t* d_col_fold, double tol, int max_iter, int maxls = 50,
+                     double ftol = 64.0 * 2.220446049250313e-16);
 int multi_lbfgs_enqueue(Ctx* c, MultiWork& w, int n_act_in, int fit_intercept, int32_t* hist);
 int multi_lbfgs_finish(Ctx* c, MultiWork& w, float* dcoef, int32_t* dniter, int32_t* dstatus, double* dloss);
 // caller points dx [B][K][dp] (device) into w.W, and f, g of every candidate at them after one evaluation
@@ -380,7 +382,8 @@ size_t tc_slot_param_bytes();
 int tc_partials_per_slot();
 
 // device L-BFGS (lbfgs_dev.cu)
-int lbfgs_dev_init(Ctx* c, LogregWork& w, int fit_intercept, double tol, int max_iter);
+int lbfgs_dev_init(Ctx* c, LogregWork& w, int fit_intercept, double tol, int max_iter, int maxls = 50,
+                   double ftol = 64.0 * 2.220446049250313e-16);
 int lbfgs_dev_enqueue(Ctx* c, LogregWork& w, int n_act_in, int nz_used, int fit_intercept, int32_t* hist);
 int lbfgs_dev_readback(Ctx* c, LogregWork& w, int* n_act_out, int* n_run_out);  // advance + compact + export (synchronises)
 int lbfgs_dev_gather(Ctx* c, LogregWork& w, int n_act, int nz_used, int fit_intercept,
