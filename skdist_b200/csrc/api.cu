@@ -87,7 +87,7 @@ static int use_tensor_cores(Ctx* c, bool* use_tc) {
 
 // Tensor-core weights of `slots` slots: fp16 hi / lo coefficients (zeroed padding) and slot parameters.
 static int alloc_tc_weights(Ctx* c, Scratch& sx, LogregWork& w, int slots) {
-  w.ldw = c->tc.dpad;
+  w.lb.ldw = c->tc.dpad;
   w.slots_pad_cap = (int)round_up(slots, 128);
   const size_t wbytes = (size_t)w.slots_pad_cap * c->tc.dpad * 2;
   SKD_CUDA(c, sx.alloc((uint8_t**)&w.Wh, wbytes));
@@ -101,17 +101,17 @@ static int alloc_tc_weights(Ctx* c, Scratch& sx, LogregWork& w, int slots) {
 // Tensor-core setup of a scoring pass: slot s = column s of coef [B x (d+1)], exported into the weights.
 static int tc_scoring_setup(Ctx* c, Scratch& sx, LogregWork& w, int B, const float* coef, SlotMeta* dslot) {
   if (tc_prepare(c)) return 1;
-  w.B = B; w.dp = (int)c->d + 1; w.use_tc = true;
-  w.slot = dslot;
+  w.lb.B = B; w.lb.n = (int)c->d + 1; w.use_tc = true;
+  w.lb.slot = dslot;
   if (alloc_tc_weights(c, sx, w, B)) return 1;
-  SKD_CUDA(c, sx.alloc(&w.n_act, 1));
-  std::vector<double> hx((size_t)B * w.dp);
+  SKD_CUDA(c, sx.alloc(&w.lb.n_act, 1));
+  std::vector<double> hx((size_t)B * w.lb.n);
   for (size_t i = 0; i < hx.size(); ++i) hx[i] = (double)coef[i];
   double* dx;
   SKD_CUDA(c, sx.alloc(&dx, hx.size()));
   int32_t nb = B;
   SKD_CUDA(c, cudaMemcpyAsync(dx, hx.data(), hx.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &nb, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(w.lb.n_act, &nb, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaStreamSynchronize(c->stream));
   c->h2d += (int64_t)hx.size() * 8;
   return tc_export(c, w, B, dx, 1);
@@ -126,18 +126,19 @@ static int alloc_eval_buffers(Ctx* c, Scratch& sx, LogregWork& w, int B, int slo
   // partial sums per slot: row chunks of the SIMT grid, or the fixed chunk count of the tensor-core kernel
   w.cap_sc = w.use_tc ? (int64_t)tc_partials_per_slot() * round_up(slot_cap, 128)
                       : (int64_t)4 * c->sm_count * 64 + slot_cap + 64;
-  w.nz = 1024;
-  SKD_CUDA(c, sx.alloc(&w.lossp, (size_t)w.cap_sc));
-  SKD_CUDA(c, sx.alloc(&w.gsump, (size_t)w.cap_sc));
+  LbfgsBatch& b = w.lb;
+  b.nz = 1024;
+  SKD_CUDA(c, sx.alloc(&b.lossp, (size_t)w.cap_sc));
+  SKD_CUDA(c, sx.alloc(&b.gsump, (size_t)w.cap_sc));
   if (w.use_tc) {
     if (tc_prepare(c)) return 1;
-    w.gscale = c->tc.gscale;
+    b.gscale = c->tc.gscale;
     if (alloc_tc_weights(c, sx, w, slot_cap)) return 1;
-    SKD_CUDA(c, sx.alloc(&w.gradp, (size_t)w.cap_sc * w.ldw));
-    SKD_CUDA(c, sx.alloc(&w.gradr, (size_t)w.slots_pad_cap * w.ldw));
+    SKD_CUDA(c, sx.alloc(&b.gradp, (size_t)w.cap_sc * b.ldw));
+    SKD_CUDA(c, sx.alloc(&b.gradr, (size_t)w.slots_pad_cap * b.ldw));
   } else {
-    w.ldw = (int)ldx;
-    w.gscale = nullptr;
+    b.ldw = (int)ldx;
+    b.gscale = nullptr;
     w.ldg = (int)round_up(B, 64);
     // the n x B gradient-factor matrix must leave room for X and the solver state: at most 3/4 of the device
     size_t free_b = 0, total_b = 0;
@@ -148,9 +149,9 @@ static int alloc_eval_buffers(Ctx* c, Scratch& sx, LogregWork& w, int B, int slo
                "3/4 of the device); split the batch", 0.75 * (double)total_b / 1e9);
       return fail(c, b);
     }
-    SKD_CUDA(c, sx.alloc(&w.Wact, (size_t)B * ldx + B));
+    SKD_CUDA(c, sx.alloc(&b.W, (size_t)B * ldx + B));
     SKD_CUDA(c, sx.alloc(&w.G, (size_t)n * w.ldg));
-    SKD_CUDA(c, sx.alloc(&w.gradp, (size_t)w.cap_sc * ldx));
+    SKD_CUDA(c, sx.alloc(&b.gradp, (size_t)w.cap_sc * ldx));
   }
   return 0;
 }
@@ -185,8 +186,8 @@ static int alloc_logreg_slots(Ctx* c, Scratch& sx, LogregWork& w, int B, const i
   hslots.clear();
   if (want_tc(c) && tc_supported(c) && grouped_slot_layout(c, B, col_fold, col_pos, col_neg, hslots)) return 1;
   if (alloc_eval_buffers(c, sx, w, B, hslots.empty() ? B : (int)hslots.size())) return 1;
-  w.grouped = !hslots.empty() && w.use_tc;
-  if (!w.grouped) {
+  w.lb.grouped = !hslots.empty() && w.use_tc;
+  if (!w.lb.grouped) {
     hslots.clear();
     return 0;
   }
@@ -898,7 +899,7 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   if (max_iter < 1) return fail(c, "skd_logreg_fit_batch: max_iter must be >= 1");
   SKD_CUDA(c, cudaSetDevice(c->device));
   const int64_t d = c->d;
-  const int dp = (int)d + 1, m = 10;
+  const int dp = (int)d + 1;
 
   std::vector<double> l2, inv_n;
   double mean_ntrain = 0.0;
@@ -911,14 +912,11 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   Trace tr(c, "logreg_fit");
   Scratch sx(c);
   LogregWork w;
-  w.B = B; w.dp = dp;
-  w.vec_stride = (size_t)(5 + 2 * m) * dp + 2 * m;
+  LbfgsBatch& b = w.lb;
+  b.B = B; b.n = dp;
   std::vector<SlotMeta> hslots;
   if (alloc_logreg_slots(c, sx, w, B, col_fold, col_pos, col_neg, hslots)) return 1;
-  SKD_CUDA(c, sx.alloc(&w.sc, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&w.vec, (size_t)B * w.vec_stride));
-  SKD_CUDA(c, sx.alloc(&w.l2, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&w.inv_n, (size_t)B));
+  if (lbfgs_alloc(c, sx, b, w.slot_cap, true)) return 1;
   SKD_CUDA(c, sx.alloc(&w.col_fold, (size_t)B));
   SKD_CUDA(c, sx.alloc(&w.col_pos, (size_t)B));
   std::vector<int32_t> hneg1;
@@ -927,7 +925,6 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
     for (int j = 0; j < B; ++j) hneg1[j] = col_neg[j] >= 0 ? col_neg[j] + 1 : 0;
     SKD_CUDA(c, sx.alloc(&w.col_neg1, (size_t)B));
   }
-  SKD_CUDA(c, sx.alloc(&w.n_evals, (size_t)B));
   if (!hcw.empty()) {
     float2* dcw;
     SKD_CUDA(c, sx.alloc(&dcw, (size_t)B));
@@ -939,7 +936,7 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   if (use_fmask) {
     if (staged_masks.cols != B || (int64_t)staged_masks.mask.size() != (int64_t)B * d)
       return fail(c, "skd_logreg_fit_batch: staged column masks do not match this batch (B x d)");
-    SKD_CUDA(c, sx.alloc(&w.fmask, (size_t)B * d));
+    SKD_CUDA(c, sx.alloc(&b.fmask, (size_t)B * d));
   }
   if (staged_bits.cols > 0) {
     w.rb_words = staged_bits.words;
@@ -960,50 +957,33 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
     SKD_CUDA(c, cudaStreamSynchronize(c->stream));
     w.uni_pos = -1;
   }
-  SKD_CUDA(c, sx.alloc(&w.slot, (size_t)w.slot_cap));
-  SKD_CUDA(c, sx.alloc(&w.n_act, 1));
-  SKD_CUDA(c, sx.alloc(&w.n_run, 1));
-  float* dcoef; int32_t *dniter, *dstatus; double* dloss;
-  SKD_CUDA(c, sx.alloc(&dcoef, (size_t)B * dp));
-  SKD_CUDA(c, sx.alloc(&dniter, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&dstatus, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&dloss, (size_t)B));
 
   tr.mark("alloc");
   DeviceTimer timer(c);
   if (timer.start()) return 1;
-  SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(b.l2, l2.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(b.inv_n, inv_n.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(w.col_fold, col_fold, B * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(w.col_pos, col_pos, B * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   if (col_neg) SKD_CUDA(c, cudaMemcpyAsync(w.col_neg1, hneg1.data(), B * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   if (use_fmask) {
-    SKD_CUDA(c, cudaMemcpyAsync(w.fmask, staged_masks.mask.data(), (size_t)B * d, cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(b.fmask, staged_masks.mask.data(), (size_t)B * d, cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaStreamSynchronize(c->stream));
     c->h2d += (int64_t)B * d;
   }
   c->h2d += (int64_t)B * 24;
 
-  if (w.grouped) {
+  if (b.grouped) {
     int32_t ns = (int32_t)hslots.size();
-    SKD_CUDA(c, cudaMemcpyAsync(w.slot, hslots.data(), hslots.size() * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &ns, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(b.slot, hslots.data(), hslots.size() * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(b.n_act, &ns, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   }
-  if (lbfgs_dev_init(c, w, fit_intercept, tol, max_iter)) return 1;
+  if (lbfgs_init(c, b, b.grouped ? nullptr : w.col_fold, w.col_pos, w.col_neg1, tol, max_iter)) return 1;
+  if (w.use_tc && tc_export(c, w, b.grouped ? w.slot_cap : B, nullptr, fit_intercept)) return 1;
   tr.mark("init");
-  int n_act = w.grouped ? (int)hslots.size() : B;
-  int n_run = B;
-  const long max_rounds = (long)max_iter * 52 + 16;
-  long rounds = 0;
-  std::vector<double> round_flops;
-  std::vector<int> round_act, round_run;
-  size_t ev_used = 0;
-  // Several optimiser rounds are enqueued per host round trip: the kernels read the live slot count
-  // on the device, the host's n_act is only an upper bound that sizes the grids and strides.  Each
-  // round records {slots, running} in `hist` so the profile below uses the true counts.
-  const int rounds_per_sync = 4;
+  // Every round records {slots, running} in `hist` so the profile below uses the true counts.
+  const long hist_cap = lbfgs_max_rounds(max_iter) + 1;
   int32_t* hist = nullptr;
-  const long hist_cap = max_rounds + rounds_per_sync + 4;
   SKD_CUDA(c, sx.alloc(&hist, (size_t)2 * hist_cap));
   // SKDIST_B200_TRACE=2 on the tensor-core path: every evaluation also records its work deal
   const bool trace_rounds = tr.on && c->prof && getenv("SKDIST_B200_TRACE")[0] == '2';
@@ -1012,36 +992,35 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
     SKD_CUDA(c, sx.alloc(&deal_hist, (size_t)4 * hist_cap));
     SKD_CUDA(c, cudaMemsetAsync(deal_hist, 0, (size_t)4 * hist_cap * sizeof(int32_t), c->stream));
   }
+  size_t ev_used = 0;
   std::vector<int> ev_round;              // round index of every profiled evaluation
-  while (n_run > 0) {
-    for (int k = 0; k < rounds_per_sync; ++k) {
-      int nz_used = 0;
-      if (deal_hist) w.deal_log = rounds < hist_cap ? deal_hist + 4 * rounds : nullptr;
-      if (c->prof) {
-        if (c->prof_events.size() < ev_used + 2) {
-          cudaEvent_t a, b;
-          SKD_CUDA(c, cudaEventCreate(&a));
-          SKD_CUDA(c, cudaEventCreate(&b));
-          c->prof_events.push_back(a);
-          c->prof_events.push_back(b);
-        }
-        SKD_CUDA(c, cudaEventRecord(c->prof_events[ev_used], c->stream));
+  auto eval = [&](int n_act, long round, int* nz_used) -> int {
+    if (deal_hist) w.deal_log = round < hist_cap ? deal_hist + 4 * round : nullptr;
+    if (c->prof) {
+      if (c->prof_events.size() < ev_used + 2) {
+        cudaEvent_t e0, e1;
+        SKD_CUDA(c, cudaEventCreate(&e0));
+        SKD_CUDA(c, cudaEventCreate(&e1));
+        c->prof_events.push_back(e0);
+        c->prof_events.push_back(e1);
       }
-      if (eval_dispatch(c, w, n_act, &nz_used)) return 1;
-      if (c->prof) {
-        SKD_CUDA(c, cudaEventRecord(c->prof_events[ev_used + 1], c->stream));
-        ev_used += 2;
-        ev_round.push_back((int)rounds);
-      }
-      if (lbfgs_dev_enqueue(c, w, n_act, nz_used, fit_intercept, hist + 2 * rounds)) return 1;
-      if (++rounds > max_rounds) return fail(c, "skd_logreg_fit_batch: round limit exceeded (internal error)");
+      SKD_CUDA(c, cudaEventRecord(c->prof_events[ev_used], c->stream));
     }
-    int n_next = 0, r_next = 0;
-    if (lbfgs_dev_readback(c, w, &n_next, &r_next)) return 1;
-    n_act = n_next;
-    n_run = r_next;
-  }
+    if (eval_dispatch(c, w, n_act, nz_used)) return 1;
+    if (c->prof) {
+      SKD_CUDA(c, cudaEventRecord(c->prof_events[ev_used + 1], c->stream));
+      ev_used += 2;
+      ev_round.push_back((int)round);
+    }
+    return 0;
+  };
+  long rounds = 0;
+  if (lbfgs_run(c, b, b.grouped ? (int)hslots.size() : B, fit_intercept, max_iter, hist, w.use_tc ? &w : nullptr,
+                eval, &rounds))
+    return 1;
   // true per-round counts (columns evaluated in round r = running after round r - 1)
+  std::vector<double> round_flops;
+  std::vector<int> round_act, round_run;
   std::vector<int32_t> hhist((size_t)2 * std::max<long>(rounds, 1), 0);
   if (rounds > 0)
     SKD_CUDA(c, cudaMemcpyAsync(hhist.data(), hist, (size_t)2 * rounds * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
@@ -1056,7 +1035,7 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   for (size_t e = 0; e < ev_round.size(); ++e) {
     const int r = ev_round[e];
     const int running = r == 0 ? B : hhist[2 * (r - 1) + 1];
-    const int slots = r == 0 ? (w.grouped ? (int)hslots.size() : B) : hhist[2 * (r - 1)];
+    const int slots = r == 0 ? (b.grouped ? (int)hslots.size() : B) : hhist[2 * (r - 1)];
     round_flops.push_back(4.0 * (double)d * (double)running * mean_ntrain);
     round_act.push_back(slots);
     round_run.push_back(running);
@@ -1083,16 +1062,8 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
     }
     c->prof_rounds += live_rounds;
   }
-  if (lbfgs_dev_finish(c, w, dcoef, dniter, dstatus, dloss)) return 1;
-  SKD_CUDA(c, cudaMemcpyAsync(coef_out, dcoef, (size_t)B * dp * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(n_iter_out, dniter, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(status_out, dstatus, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  if (loss_out)
-    SKD_CUDA(c, cudaMemcpyAsync(loss_out, dloss, (size_t)B * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  if (n_evals_out)
-    SKD_CUDA(c, cudaMemcpyAsync(n_evals_out, w.n_evals, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  if (lbfgs_result(c, sx, b, 0, coef_out, n_iter_out, status_out, loss_out, n_evals_out)) return 1;
   if (timer.stop(gpu_seconds_out)) return 1;
-  c->d2h += (int64_t)B * (dp * 4 + 20);
   tr.mark("finish");
   return 0;
 }
@@ -1120,7 +1091,8 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
   if (staged_cw.cols > 0 && binary_class_weights(c, "skd_logreg_loss_grad", staged_cw, B, C, hcw, l2, inv_n)) return 1;
   Scratch sx(c);
   LogregWork w;
-  w.B = B; w.dp = dp;
+  LbfgsBatch& b = w.lb;
+  b.B = B; b.n = dp;
   if (!hcw.empty()) {
     float2* dcw;
     SKD_CUDA(c, sx.alloc(&dcw, (size_t)B));
@@ -1130,32 +1102,32 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
   // the slot layout of skd_logreg_fit_batch: fold-grouped on the tensor cores, slot s = column s on SIMT
   std::vector<SlotMeta> hs;
   if (alloc_logreg_slots(c, sx, w, B, col_fold, col_pos, nullptr, hs)) return 1;
-  if (!w.grouped) {
+  if (!b.grouped) {
     hs.resize(B);
     for (int j = 0; j < B; ++j) { hs[j].col = j; hs[j].fold = col_fold[j] < 0 ? -1 : col_fold[j]; hs[j].pos = col_pos[j]; hs[j].pad = 0; }
   }
   const int n_slots = (int)hs.size();
-  SKD_CUDA(c, sx.alloc(&w.l2, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&w.inv_n, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&w.slot, (size_t)n_slots));
-  SKD_CUDA(c, sx.alloc(&w.n_act, 1));
+  SKD_CUDA(c, sx.alloc(&b.l2, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&b.inv_n, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&b.slot, (size_t)n_slots));
+  SKD_CUDA(c, sx.alloc(&b.n_act, 1));
   double *dx, *df, *dg;
   SKD_CUDA(c, sx.alloc(&dx, (size_t)B * dp));
   SKD_CUDA(c, sx.alloc(&df, (size_t)B));
   SKD_CUDA(c, sx.alloc(&dg, (size_t)B * dp));
-  SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(w.slot, hs.data(), n_slots * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(b.l2, l2.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(b.inv_n, inv_n.data(), B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(b.slot, hs.data(), n_slots * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(dx, w_in, (size_t)B * dp * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   if (w.use_tc) {
-    SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &n_slots, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(b.n_act, &n_slots, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     if (tc_export(c, w, n_slots, dx, fit_intercept)) return 1;
   } else {
-    SKD_CUDA(c, cudaMemcpyAsync(w.Wact, hw.data(), hw.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(b.W, hw.data(), hw.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
   }
   int nz_used = 0;
   if (eval_dispatch(c, w, n_slots, &nz_used)) return 1;
-  if (lbfgs_dev_gather(c, w, n_slots, nz_used, fit_intercept, dx, df, dg)) return 1;
+  if (lbfgs_gather(c, b, n_slots, nz_used, fit_intercept, dx, df, dg)) return 1;
   SKD_CUDA(c, cudaMemcpyAsync(loss_out, df, B * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(grad_out, dg, (size_t)B * dp * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   SKD_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1440,8 +1412,8 @@ int skd_linear_r2_batch(skd_ctx* ctx, int32_t B, const float* coef, const int32_
     LogregWork w;
     if (tc_scoring_setup(c, sx, w, B, coef, dslot)) return 1;
     const size_t n_part = (size_t)tc_partials_per_slot() * B;   // per-chunk squared-error sums
-    SKD_CUDA(c, sx.alloc(&w.lossp, n_part));
-    SKD_CUDA(c, cudaMemsetAsync(w.lossp, 0, n_part * sizeof(double), c->stream));
+    SKD_CUDA(c, sx.alloc(&w.lb.lossp, n_part));
+    SKD_CUDA(c, cudaMemsetAsync(w.lb.lossp, 0, n_part * sizeof(double), c->stream));
     if (tc_r2(c, w, B, dsse, dcount)) return 1;
   } else {
     float* dW;
@@ -1824,20 +1796,18 @@ int skd_linear_decision(skd_ctx* ctx, int32_t B, const float* coef, float* out) 
 struct skd_lbfgs_dev {
   Ctx* c = nullptr;
   std::unique_ptr<Scratch> sx;
-  int B = 0, K = 1, d = 0, n = 0, nz = 0, fit_intercept = 1;
-  int slot_cap = 0;   // entries of the slot (binary) or candidate (multinomial) list
-  int ldw = 0;        // row pitch of the gradient partials and of the exported rows
+  int d = 0, nz = 0, fit_intercept = 1;
+  int slot_cap = 0;   // entries of the active list
   size_t rows = 0;    // floats of the exported fp32 rows (0: the grouped layout exports fp16 hi / lo)
-  LogregWork w;       // K == 1
-  MultiWork mw;       // K >= 2
+  LogregWork w;       // w.lb: the optimiser batch; the rest only for the grouped layout's tensor-core export
   int32_t* hist = nullptr;   // device {slots, running} of the last round
 };
 
-static int lbfgs_dev_setup(skd_lbfgs_dev* h, int grouped, const int32_t* col_fold, int use_reduce, int maxiter,
-                           int maxls, double pgtol, double ftol, const double* l2, const double* inv_n,
+static int lbfgs_dev_setup(skd_lbfgs_dev* h, int B, int K, int grouped, const int32_t* col_fold, int use_reduce,
+                           int maxiter, int maxls, double pgtol, double ftol, const double* l2, const double* inv_n,
                            const double* gscale, const uint8_t* fmask) {
   Ctx* c = h->c;
-  const int B = h->B, K = h->K, d = h->d, dp = d + 1, m = 10;
+  const int d = h->d, dp = d + 1;
   if (!c->X) return fail(c, "skd_lbfgs_dev_create: stage X first (d and the row pitch come from it)");
   if (B <= 0 || K < 1 || d != (int)c->d || h->nz < 1 || !col_fold || !l2 || !inv_n || maxiter < 1 || maxls < 1)
     return fail(c, "skd_lbfgs_dev_create: bad arguments");
@@ -1846,45 +1816,10 @@ static int lbfgs_dev_setup(skd_lbfgs_dev* h, int grouped, const int32_t* col_fol
   SKD_CUDA(c, cudaSetDevice(c->device));
   h->sx.reset(new Scratch(c));
   Scratch& sx = *h->sx;
-  h->n = K * dp;
-  SKD_CUDA(c, sx.alloc(&h->hist, 2));
-  uint8_t* dmask = nullptr;
-  if (fmask) {
-    SKD_CUDA(c, sx.alloc(&dmask, (size_t)B * d));
-    SKD_CUDA(c, cudaMemcpyAsync(dmask, fmask, (size_t)B * d, cudaMemcpyHostToDevice, c->stream));
-  }
-  int32_t* dfold;
-  SKD_CUDA(c, sx.alloc(&dfold, (size_t)B));
-  SKD_CUDA(c, cudaMemcpyAsync(dfold, col_fold, B * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-  if (K > 1) {
-    MultiWork& w = h->mw;
-    const size_t slots = (size_t)B * K;
-    w.B = B; w.K = K; w.dp = dp; w.nz = h->nz;
-    w.vec_stride = (size_t)(5 + 2 * m) * K * dp + 2 * m;
-    h->slot_cap = B;
-    h->ldw = (int)c->ldx;
-    h->rows = slots * c->ldx + slots;
-    SKD_CUDA(c, sx.alloc(&w.sc, (size_t)B));
-    SKD_CUDA(c, sx.alloc(&w.vec, (size_t)B * w.vec_stride));
-    SKD_CUDA(c, sx.alloc(&w.l2, (size_t)B));
-    SKD_CUDA(c, sx.alloc(&w.inv_n, (size_t)B));
-    SKD_CUDA(c, sx.alloc(&w.n_evals, (size_t)B));
-    SKD_CUDA(c, sx.alloc(&w.cand, (size_t)B));
-    SKD_CUDA(c, sx.alloc(&w.W, h->rows));
-    SKD_CUDA(c, sx.alloc(&w.lossp, (size_t)h->nz * B));
-    SKD_CUDA(c, sx.alloc(&w.gsump, (size_t)h->nz * slots));
-    SKD_CUDA(c, sx.alloc(&w.gradp, (size_t)h->nz * slots * c->ldx));
-    SKD_CUDA(c, sx.alloc(&w.n_act, 1));
-    SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2, B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n, B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    w.fmask = dmask;
-    if (multi_lbfgs_init(c, w, dfold, pgtol, maxiter, maxls, ftol)) return 1;
-    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-    return 0;
-  }
   LogregWork& w = h->w;
-  w.B = B; w.dp = dp; w.nz = h->nz;
-  w.vec_stride = (size_t)(5 + 2 * m) * dp + 2 * m;
+  LbfgsBatch& b = w.lb;
+  b.B = B; b.K = K; b.n = K * dp; b.nz = h->nz;
+  SKD_CUDA(c, sx.alloc(&h->hist, 2));
   std::vector<int32_t> zeros(B, 0);
   std::vector<SlotMeta> hslots;
   if (grouped) {   // the fit's tensor-core layout; its trial points leave through tc_export
@@ -1892,50 +1827,45 @@ static int lbfgs_dev_setup(skd_lbfgs_dev* h, int grouped, const int32_t* col_fol
     if (grouped_slot_layout(c, B, col_fold, zeros.data(), nullptr, hslots)) return 1;
     if (tc_prepare(c)) return 1;
     w.use_tc = true;
-    w.grouped = true;
+    b.grouped = true;
     h->slot_cap = (int)hslots.size();
     if (alloc_tc_weights(c, sx, w, h->slot_cap)) return 1;
   } else {
     h->slot_cap = B;
-    w.ldw = (int)c->ldx;
-    h->rows = (size_t)B * c->ldx + B;
-    SKD_CUDA(c, sx.alloc(&w.Wact, h->rows));
+    b.ldw = (int)c->ldx;
+    h->rows = (size_t)B * K * c->ldx + (size_t)B * K;
+    SKD_CUDA(c, sx.alloc(&b.W, h->rows));
   }
-  h->ldw = w.ldw;
   w.slot_cap = h->slot_cap;
   const size_t cap = (size_t)h->nz * h->slot_cap;
-  SKD_CUDA(c, sx.alloc(&w.lossp, cap));
-  SKD_CUDA(c, sx.alloc(&w.gsump, cap));
-  SKD_CUDA(c, sx.alloc(&w.gradp, cap * w.ldw));
-  if (use_reduce) SKD_CUDA(c, sx.alloc(&w.gradr, (size_t)h->slot_cap * w.ldw));
-  SKD_CUDA(c, sx.alloc(&w.sc, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&w.vec, (size_t)B * w.vec_stride));
-  SKD_CUDA(c, sx.alloc(&w.l2, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&w.inv_n, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&w.col_pos, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&w.n_evals, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&w.slot, (size_t)h->slot_cap));
-  SKD_CUDA(c, sx.alloc(&w.n_act, 1));
-  SKD_CUDA(c, sx.alloc(&w.n_run, 1));
-  w.col_fold = dfold;
-  w.fmask = dmask;
+  SKD_CUDA(c, sx.alloc(&b.lossp, cap));
+  SKD_CUDA(c, sx.alloc(&b.gsump, cap * K));
+  SKD_CUDA(c, sx.alloc(&b.gradp, cap * K * b.ldw));
+  if (use_reduce) SKD_CUDA(c, sx.alloc(&b.gradr, (size_t)h->slot_cap * b.ldw));
+  if (lbfgs_alloc(c, sx, b, h->slot_cap, K == 1)) return 1;
+  if (fmask) {
+    SKD_CUDA(c, sx.alloc(&b.fmask, (size_t)B * d));
+    SKD_CUDA(c, cudaMemcpyAsync(b.fmask, fmask, (size_t)B * d, cudaMemcpyHostToDevice, c->stream));
+  }
   if (gscale) {
     double* dgs;
     SKD_CUDA(c, sx.alloc(&dgs, (size_t)d));
     SKD_CUDA(c, cudaMemcpyAsync(dgs, gscale, d * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    w.gscale = dgs;
+    b.gscale = dgs;
   }
-  SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2, B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n, B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(w.col_pos, zeros.data(), B * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-  const int32_t nrun = B;
-  SKD_CUDA(c, cudaMemcpyAsync(w.n_run, &nrun, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-  if (w.grouped) {
+  int32_t* dfold;
+  SKD_CUDA(c, sx.alloc(&dfold, (size_t)B));
+  SKD_CUDA(c, cudaMemcpyAsync(dfold, col_fold, B * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(b.l2, l2, B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(b.inv_n, inv_n, B * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  if (b.n_run) SKD_CUDA(c, cudaMemcpyAsync(b.n_run, &B, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  if (b.grouped) {
     const int32_t ns = h->slot_cap;
-    SKD_CUDA(c, cudaMemcpyAsync(w.slot, hslots.data(), hslots.size() * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &ns, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(b.slot, hslots.data(), hslots.size() * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(b.n_act, &ns, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   }
-  if (lbfgs_dev_init(c, w, h->fit_intercept, pgtol, maxiter, maxls, ftol)) return 1;
+  if (lbfgs_init(c, b, b.grouped ? nullptr : dfold, nullptr, nullptr, pgtol, maxiter, maxls, ftol)) return 1;
+  if (w.use_tc && tc_export(c, w, h->slot_cap, nullptr, h->fit_intercept)) return 1;
   SKD_CUDA(c, cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -1946,13 +1876,12 @@ static int lbfgs_dev_round(skd_lbfgs_dev* h, int n_act_in, const double* loss_pa
                            const float* grad_parts, double* x_out, void* state_out, int32_t* slot_out,
                            int32_t* counts_out, float* rows_out) {
   Ctx* c = h->c;
-  const int B = h->B, K = h->K, d = h->d, nz = h->nz, ldw = h->ldw;
-  SlotMeta* dslot = K > 1 ? h->mw.cand : h->w.slot;
-  int32_t* dn_act = K > 1 ? h->mw.n_act : h->w.n_act;
+  LbfgsBatch& b = h->w.lb;
+  const int B = b.B, K = b.K, d = h->d, nz = h->nz, ldw = b.ldw;
   std::vector<SlotMeta> hs(h->slot_cap);
   int32_t live = 0;
-  SKD_CUDA(c, cudaMemcpyAsync(hs.data(), dslot, hs.size() * sizeof(SlotMeta), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(&live, dn_act, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(hs.data(), b.slot, hs.size() * sizeof(SlotMeta), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(&live, b.n_act, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
   SKD_CUDA(c, cudaStreamSynchronize(c->stream));
   if (n_act_in < live || n_act_in > h->slot_cap)
     return fail(c, "skd_lbfgs_dev_step: n_act_in must lie between the live slot count and the slot capacity");
@@ -1972,55 +1901,29 @@ static int lbfgs_dev_round(skd_lbfgs_dev* h, int n_act_in, const double* loss_pa
       }
     }
   }
-  double* dl = K > 1 ? h->mw.lossp : h->w.lossp;
-  double* dg = K > 1 ? h->mw.gsump : h->w.gsump;
-  float* dgp = K > 1 ? h->mw.gradp : h->w.gradp;
-  SKD_CUDA(c, cudaMemcpyAsync(dl, lp.data(), lp.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(dg, gs.data(), gs.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(dgp, gp.data(), gp.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  if (K > 1) {
-    if (multi_lbfgs_enqueue(c, h->mw, n_act_in, h->fit_intercept, h->hist)) return 1;
-  } else if (lbfgs_dev_enqueue(c, h->w, n_act_in, nz, h->fit_intercept, h->hist)) {
-    return 1;
-  }
-  const double* vec = K > 1 ? h->mw.vec : h->w.vec;
-  const size_t stride = K > 1 ? h->mw.vec_stride : h->w.vec_stride;
-  const LbfgsScalars* sc = K > 1 ? h->mw.sc : h->w.sc;
-  SKD_CUDA(c, cudaMemcpy2DAsync(x_out, h->n * sizeof(double), vec, stride * sizeof(double), h->n * sizeof(double), B,
+  SKD_CUDA(c, cudaMemcpyAsync(b.lossp, lp.data(), lp.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(b.gsump, gs.data(), gs.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(b.gradp, gp.data(), gp.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  if (lbfgs_enqueue(c, b, n_act_in, nz, h->fit_intercept, h->hist, b.grouped ? &h->w : nullptr)) return 1;
+  SKD_CUDA(c, cudaMemcpy2DAsync(x_out, b.n * sizeof(double), b.vec, b.stride * sizeof(double), b.n * sizeof(double), B,
                                 cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(state_out, sc, B * sizeof(LbfgsScalars), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(slot_out, dslot, h->slot_cap * sizeof(SlotMeta), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(counts_out, dn_act, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(counts_out + 1, K > 1 || !h->w.grouped ? dn_act : h->w.n_run, sizeof(int32_t),
-                              cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(state_out, b.sc, B * sizeof(LbfgsScalars), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(slot_out, b.slot, h->slot_cap * sizeof(SlotMeta), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(counts_out, b.n_act, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(counts_out + 1, b.n_run ? b.n_run : b.n_act, sizeof(int32_t), cudaMemcpyDeviceToHost,
+                              c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(counts_out + 2, h->hist, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
   if (rows_out && h->rows)
-    SKD_CUDA(c, cudaMemcpyAsync(rows_out, K > 1 ? h->mw.W : h->w.Wact, h->rows * sizeof(float), cudaMemcpyDeviceToHost,
-                                c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(rows_out, b.W, h->rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
   SKD_CUDA(c, cudaStreamSynchronize(c->stream));
   return 0;
 }
 
 static int lbfgs_dev_result(skd_lbfgs_dev* h, float* coef_out, int32_t* n_iter_out, int32_t* status_out,
                             double* loss_out) {
-  Ctx* c = h->c;
-  const int B = h->B;
-  Scratch sx(c);
-  float* dcoef; int32_t *dniter, *dstatus; double* dloss;
-  SKD_CUDA(c, sx.alloc(&dcoef, (size_t)B * h->n));
-  SKD_CUDA(c, sx.alloc(&dniter, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&dstatus, (size_t)B));
-  SKD_CUDA(c, sx.alloc(&dloss, (size_t)B));
-  if (h->K > 1) {
-    if (multi_lbfgs_finish(c, h->mw, dcoef, dniter, dstatus, dloss)) return 1;
-  } else if (lbfgs_dev_finish(c, h->w, dcoef, dniter, dstatus, dloss)) {
-    return 1;
-  }
-  SKD_CUDA(c, cudaMemcpyAsync(coef_out, dcoef, (size_t)B * h->n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(n_iter_out, dniter, B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(status_out, dstatus, B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(loss_out, dloss, B * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+  Scratch sx(h->c);
+  if (lbfgs_result(h->c, sx, h->w.lb, 0, coef_out, n_iter_out, status_out, loss_out, nullptr)) return 1;
+  SKD_CUDA(h->c, cudaStreamSynchronize(h->c->stream));
   return 0;
 }
 
@@ -2033,10 +1936,13 @@ skd_lbfgs_dev* skd_lbfgs_dev_create(skd_ctx* ctx, int32_t B, int32_t K, int32_t 
                                     int32_t* dims_out) {
   if (!ctx) { fail(nullptr, "skd_lbfgs_dev_create: ctx is NULL"); return nullptr; }
   std::unique_ptr<skd_lbfgs_dev> h(new skd_lbfgs_dev());
-  h->c = &ctx->c; h->B = B; h->K = K; h->d = d; h->nz = nz; h->fit_intercept = fit_intercept ? 1 : 0;
-  if (lbfgs_dev_setup(h.get(), grouped, col_fold, use_reduce, maxiter, maxls, pgtol, ftol, l2, inv_n, gscale, fmask))
+  h->c = &ctx->c; h->d = d; h->nz = nz; h->fit_intercept = fit_intercept ? 1 : 0;
+  if (lbfgs_dev_setup(h.get(), B, K, grouped, col_fold, use_reduce, maxiter, maxls, pgtol, ftol, l2, inv_n, gscale,
+                      fmask))
     return nullptr;
-  if (dims_out) { dims_out[0] = h->n; dims_out[1] = h->slot_cap; dims_out[2] = h->ldw; dims_out[3] = (int32_t)h->rows; }
+  if (dims_out) {
+    dims_out[0] = h->w.lb.n; dims_out[1] = h->slot_cap; dims_out[2] = h->w.lb.ldw; dims_out[3] = (int32_t)h->rows;
+  }
   return h.release();
 }
 
@@ -2064,17 +1970,8 @@ skd_lbfgs* skd_lbfgs_create(int32_t n, int32_t m, int32_t maxiter, int32_t maxls
                             double ftol) {
   skd_lbfgs* h = new skd_lbfgs();
   lbfgs_init(h->s, n, m, maxiter, maxls, pgtol, ftol);
-  h->buf.assign((size_t)5 * n + 2 * (size_t)m * n + 2 * m, 0.0);
-  double* p = h->buf.data();
-  h->v.x = p; p += n;
-  h->v.g = p; p += n;
-  h->v.t = p; p += n;
-  h->v.r = p; p += n;
-  h->v.d = p; p += n;
-  h->v.S = p; p += (size_t)m * n;
-  h->v.Y = p; p += (size_t)m * n;
-  h->v.rho = p; p += m;
-  h->v.alpha = p;
+  h->buf.assign(lbfgs_col_doubles(n, m), 0.0);
+  h->v = lbfgs_col_vectors(h->buf.data(), n, m);
   return h;
 }
 double* skd_lbfgs_x(skd_lbfgs* h) { return h->v.x; }

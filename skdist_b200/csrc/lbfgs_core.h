@@ -20,13 +20,14 @@
 // The direction is evaluated with the two-loop recursion, which is algebraically the
 // compact-representation product that subsm() forms (difference: rounding, ~1e-16 rel).
 //
-// The same code is compiled for the host (sequential `Seq` policy; used by the CPU-side
-// tests that pin it against scipy's setulb trajectories) and for the device (one CTA per
-// column, `Cta` policy in lbfgs_kernels.cu).  All threads of a CTA execute the scalar
-// logic redundantly; dot products are block reductions that return the same value to
-// every thread, so control flow stays uniform.
+// The same code is compiled for the host (sequential `SeqPar` policy; used by the CPU-side
+// tests that pin it against scipy's setulb trajectories) and for the device (lbfgs_dev.cu:
+// one warp per binary column, `WarpPar`; one CTA per multinomial candidate, `CtaPar`).  All
+// threads of a column's warp or CTA execute the scalar logic redundantly; dot products are
+// reductions that return the same value to every thread, so control flow stays uniform.
 #pragma once
 #include <math.h>
+#include <stddef.h>
 #include <stdint.h>
 
 #if defined(__CUDACC__)
@@ -86,6 +87,28 @@ struct LbfgsVectors {
   double* rho; // m : 1 / (s_i' y_i)
   double* alpha; // m scratch
 };
+
+// Memory of every device fit: scikit-learn leaves scipy's default, m = 10.
+constexpr int LBFGS_M = 10;
+
+// Doubles of one column's vector storage: x, g, t, r, d, then S, Y, then rho, alpha.
+SKD_HD size_t lbfgs_col_doubles(int n, int m) { return (size_t)(5 + 2 * m) * n + 2 * m; }
+
+// The column's vectors in the block of lbfgs_col_doubles(n, m) doubles at base.
+SKD_HD LbfgsVectors lbfgs_col_vectors(double* base, int n, int m) {
+  LbfgsVectors v;
+  double* p = base;
+  v.x = p; p += n;
+  v.g = p; p += n;
+  v.t = p; p += n;
+  v.r = p; p += n;
+  v.d = p; p += n;
+  v.S = p; p += (size_t)m * n;
+  v.Y = p; p += (size_t)m * n;
+  v.rho = p; p += m;
+  v.alpha = p;
+  return v;
+}
 
 // --- MINPACK-2 dcstep -------------------------------------------------------------------
 SKD_HD void dcstep(double& stx, double& fx, double& dx, double& sty, double& fy, double& dy,

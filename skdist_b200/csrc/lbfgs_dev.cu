@@ -1,11 +1,11 @@
-// lbfgs_dev.cu -- device-resident batched L-BFGS-B driver: one CTA per active column.
+// lbfgs_dev.cu -- device-resident batched L-BFGS-B driver for binary columns and multinomial candidates.
 //
 // Replaces the host loop scipy/optimize/_lbfgsb_py.py:406-437 (setulb reverse communication)
 // that each of the reference's tasks runs inside estimator.fit (ref search.py:230); the
 // optimiser arithmetic is csrc/lbfgs_core.h.  Per round:
-//   lb_step_kernel    : gather the slot's partial sums -> f, g (float64, adds the L2 term as
+//   lb_step_kernel    : gather the entry's partial sums -> f, g (float64, adds the L2 term as
 //                       SK/linear_model/_linear_loss.py:350,356-361), advance the state machine
-//   lb_compact_kernel : rebuild the list of still-running columns (stable order)
+//   lb_compact_kernel : rebuild the list of still-running problems (stable order)
 //   lb_export_kernel  : cast the new trial points to fp32 (SK/_linear_loss.py:216-217) into the
 //                       active-slot weight matrix for the next evaluation
 #include "skd_internal.h"
@@ -14,7 +14,9 @@ namespace skd {
 
 constexpr int LB_THREADS = 128;
 
+// One CTA per problem: reductions over the CTA's four warps.
 struct CtaPar {
+  static constexpr int PER_CTA = 1;   // problems per LB_THREADS-thread CTA
   double* red;  // shared, >= 4 doubles
   __device__ __forceinline__ int tid() const { return threadIdx.x; }
   __device__ __forceinline__ int nthr() const { return LB_THREADS; }
@@ -48,6 +50,8 @@ struct CtaPar {
 // operations are a few hundred elements long; a 128-thread CTA spent most of its time in the two
 // barriers of every reduction.
 struct WarpPar {
+  static constexpr int PER_CTA = LB_THREADS / 32;
+  double* red;  // not used: the reductions are shuffles
   __device__ __forceinline__ int tid() const { return threadIdx.x & 31; }
   __device__ __forceinline__ int nthr() const { return 32; }
   __device__ __forceinline__ void sync() const { __syncwarp(); }
@@ -70,69 +74,61 @@ struct WarpPar {
   }
 };
 
-__device__ __forceinline__ LbfgsVectors col_vectors(double* base, int n, int m) {
-  LbfgsVectors v;
-  double* p = base;
-  v.x = p; p += n;
-  v.g = p; p += n;
-  v.t = p; p += n;
-  v.r = p; p += n;
-  v.d = p; p += n;
-  v.S = p; p += (size_t)m * n;
-  v.Y = p; p += (size_t)m * n;
-  v.rho = p; p += m;
-  v.alpha = p;
-  return v;
-}
-
-
-// f, g of slot s from the evaluation partials, with the L2 term added in float64 exactly as
-// SK/linear_model/_linear_loss.py:349-361 does (penalty on the weights only).
+// f, g of active entry a from the evaluation partials, added in chunk order, with the L2 term in float64 as
+// SK/linear_model/_linear_loss.py:349-372 forms it (penalty on the weights only): loss = sum(loss_i) / n +
+// 0.5 * l2 * ||W||^2, grad[k, :d] = G^T X / n + l2 * W, grad[k, d] = sum_i G / n for the K class rows of the
+// problem (slot a * K + k).  fmask: the problem's feature mask or null.
 template <class Par>
-__device__ __forceinline__ double gather_fg(const Par& P, int s, int n_act, int nz_used, int d,
-                                            int ldx, int fit_intercept,
-                                            const double* __restrict__ lossp,
-                                            const double* __restrict__ gsump,
-                                            const float* __restrict__ gradp,
-                                            const double* __restrict__ gscale, double l2,
-                                            double inv_n, const double* x, double* g,
-                                            const uint8_t* __restrict__ fmask = nullptr,
-                                            const double* __restrict__ gradr = nullptr) {
-  double lsum = 0.0, gsum = 0.0;
-  for (int z = 0; z < nz_used; ++z) {
-    lsum += lossp[(size_t)z * n_act + s];
-    gsum += gsump[(size_t)z * n_act + s];
-  }
+__device__ __forceinline__ double gather_fg(const Par& P, int a, int n_act, int K, int nz_used, int d, int ldx,
+                                            int fit_intercept, const double* __restrict__ lossp,
+                                            const double* __restrict__ gsump, const float* __restrict__ gradp,
+                                            const double* __restrict__ gradr, const double* __restrict__ gscale,
+                                            const uint8_t* __restrict__ fmask, double l2, double inv_n,
+                                            const double* x, double* g) {
+  const int dp = d + 1;
+  const size_t n_slots = (size_t)n_act * K;
+  double lsum = 0.0;
+  for (int z = 0; z < nz_used; ++z) lsum += lossp[(size_t)z * n_act + a];
   double wsq = 0.0;
-  for (int k = P.tid(); k < d; k += P.nthr()) {
+  for (int idx = P.tid(); idx < K * dp; idx += P.nthr()) {
+    const int k = idx / dp, j = idx - k * dp;
+    const size_t s = (size_t)a * K + k;
     double acc = 0.0;
+    if (j == d) {
+      for (int z = 0; z < nz_used; ++z) acc += gsump[(size_t)z * n_slots + s];
+      g[idx] = fit_intercept ? acc * inv_n : 0.0;
+      continue;
+    }
     // the partials are added in chunk order (the result must not depend on anything else); eight
     // loads are put in flight at a time, the additions stay sequential
     int z = 0;
-    if (gradr) { acc = gradr[(size_t)s * ldx + k]; z = nz_used; }   // already reduced by lb_reduce_kernel
+    if (gradr) { acc = gradr[s * ldx + j]; z = nz_used; }   // already reduced by lb_reduce_kernel
     for (; z + 8 <= nz_used; z += 8) {
       float v[8];
 #pragma unroll
-      for (int q = 0; q < 8; ++q) v[q] = gradp[((size_t)(z + q) * n_act + s) * ldx + k];
+      for (int q = 0; q < 8; ++q) v[q] = gradp[((size_t)(z + q) * n_slots + s) * ldx + j];
 #pragma unroll
       for (int q = 0; q < 8; ++q) acc += (double)v[q];
     }
-    for (; z < nz_used; ++z) acc += (double)gradp[((size_t)z * n_act + s) * ldx + k];
-    double xk = x[k];
-    if (gscale) acc *= gscale[k];
-    // a feature masked out of this column (DistFeatureEliminator) keeps weight 0: with a zero
-    // gradient entry every L-BFGS direction is 0 there, i.e. the fit on the remaining columns of X
-    g[k] = (fmask && !fmask[k]) ? 0.0 : acc * inv_n + l2 * xk;
+    for (; z < nz_used; ++z) acc += (double)gradp[((size_t)z * n_slots + s) * ldx + j];
+    const double xk = x[idx];
+    if (gscale) acc *= gscale[j];
+    // acc * inv_n + l2 * xk with one product fused into the sum: the penalty's for binary columns, the data
+    // term's for multinomial candidates (the roundings each kind's fits have always had)
+    const double gk = K == 1 ? __fma_rn(l2, xk, __dmul_rn(acc, inv_n)) : __fma_rn(acc, inv_n, __dmul_rn(l2, xk));
+    // a feature masked out of this problem (DistFeatureEliminator) keeps weight 0 in every class row: with a
+    // zero gradient entry every L-BFGS direction is 0 there, i.e. the fit on the remaining columns of X
+    g[idx] = (fmask && !fmask[j]) ? 0.0 : gk;
     wsq += xk * xk;
   }
-  if (P.tid() == 0) g[d] = fit_intercept ? gsum * inv_n : 0.0;
   wsq = P.block_sum(wsq);
   return lsum * inv_n + 0.5 * l2 * wsq;
 }
 
 // Sum of the per-chunk gradient partials of every (slot, feature) in chunk order, float64, one
-// thread per element: the whole device streams the partial array once (one column's optimiser CTA
+// thread per element: the whole device streams the partial array once (one column's optimiser warp
 // alone cannot pull its 147 KB fast enough).  Same additions in the same order as gather_fg's loop.
+// Binary columns only (one slot per entry).
 __global__ void __launch_bounds__(256)
 lb_reduce_kernel(const float* __restrict__ gradp, int nz, int n_act, int ldx, const int32_t* __restrict__ n_act_dev,
                  double* __restrict__ gradr) {
@@ -153,41 +149,42 @@ lb_reduce_kernel(const float* __restrict__ gradp, int nz, int n_act, int ldx, co
   gradr[e] = acc;
 }
 
-// Diagnostic / test entry: objective and gradient of every column at caller-supplied points.  The
-// partials are indexed by slot, the column's constants, point and outputs by slot[s].col.
+// Test / diagnostic entries: objective and gradient of every problem at caller-supplied points xin [B][n].  The
+// partials are indexed by active entry, the problem's constants, point and outputs by slot[a].col.
 __global__ void __launch_bounds__(LB_THREADS)
-lb_gather_kernel(int n_act, int nz_used, int d, int ldx, int fit_intercept, const SlotMeta* __restrict__ slot,
+lb_gather_kernel(const SlotMeta* __restrict__ slot, int n_act, int K, int nz_used, int d, int ldx, int fit_intercept,
                  const double* __restrict__ lossp, const double* __restrict__ gsump,
                  const float* __restrict__ gradp, const double* __restrict__ gscale,
-                 const double* __restrict__ l2v,
+                 const uint8_t* __restrict__ fmask, const double* __restrict__ l2v,
                  const double* __restrict__ inv_nv, const double* __restrict__ xin,
                  double* __restrict__ fout, double* __restrict__ gout) {
   __shared__ double red[8];
-  const int s = blockIdx.x;
-  if (s >= n_act) return;
-  const int col = slot[s].col;
+  const int a = blockIdx.x;
+  if (a >= n_act) return;
+  const int col = slot[a].col;
   if (col < 0) return;   // padding slot of the fold-grouped layout
+  const size_t n = (size_t)K * (d + 1);
   CtaPar P{red};
-  double f = gather_fg(P, s, n_act, nz_used, d, ldx, fit_intercept, lossp, gsump, gradp, gscale,
-                       l2v[col], inv_nv[col], xin + (size_t)col * (d + 1), gout + (size_t)col * (d + 1));
+  const double f = gather_fg(P, a, n_act, K, nz_used, d, ldx, fit_intercept, lossp, gsump, gradp, nullptr, gscale,
+                             fmask ? fmask + (size_t)col * d : nullptr, l2v[col], inv_nv[col], xin + col * n,
+                             gout + col * n);
   if (threadIdx.x == 0) fout[col] = f;
 }
 
-__global__ void lb_init_kernel(LbfgsScalars* sc, double* vec, size_t vec_stride, int B, int n,
-                               int m, int maxiter, int maxls, double pgtol, double ftol,
-                               SlotMeta* slot, const int32_t* col_fold, const int32_t* col_pos,
-                               const int32_t* col_neg1, int32_t* n_evals, int32_t* n_act) {
-  int col = blockIdx.x;
+__global__ void lb_init_kernel(LbfgsScalars* sc, double* vec, size_t stride, int B, int n, int m, int maxiter,
+                               int maxls, double pgtol, double ftol, SlotMeta* slot, const int32_t* col_fold,
+                               const int32_t* col_pos, const int32_t* col_neg1, int32_t* n_evals, int32_t* n_act) {
+  const int col = blockIdx.x;
   if (col >= B) return;
-  double* base = vec + (size_t)col * vec_stride;
-  for (size_t i = threadIdx.x; i < vec_stride; i += blockDim.x) base[i] = 0.0;
+  double* base = vec + (size_t)col * stride;
+  for (size_t i = threadIdx.x; i < stride; i += blockDim.x) base[i] = 0.0;
   if (threadIdx.x == 0) {
     LbfgsScalars s;
     lbfgs_init(s, n, m, maxiter, maxls, pgtol, ftol);
     sc[col] = s;
-    if (slot) {   // dense layout: slot i = column i (the grouped layout is uploaded by the host)
+    if (slot) {   // dense layout: entry i = problem i (the grouped layout is uploaded by the host)
       SlotMeta sm;
-      sm.col = col; sm.fold = col_fold[col]; sm.pos = col_pos[col]; sm.pad = col_neg1 ? col_neg1[col] : 0;
+      sm.col = col; sm.fold = col_fold[col]; sm.pos = col_pos ? col_pos[col] : 0; sm.pad = col_neg1 ? col_neg1[col] : 0;
       slot[col] = sm;
       if (col == 0) *n_act = B;
     }
@@ -195,43 +192,70 @@ __global__ void lb_init_kernel(LbfgsScalars* sc, double* vec, size_t vec_stride,
   }
 }
 
-// one warp per slot, four slots per CTA
+// f, g, then one step of the optimiser state machine.  WarpPar: one warp per entry, four per CTA (binary
+// columns); CtaPar: one CTA per entry (multinomial candidates).  The policy fixes the order of the dot products.
+template <class Par>
 __global__ void __launch_bounds__(LB_THREADS)
-lb_step_kernel(LbfgsScalars* sc, double* vec, size_t vec_stride, const SlotMeta* slot, int n_act,
-               int nz_used, int d, int ldx, int fit_intercept, const double* __restrict__ lossp,
-               const double* __restrict__ gsump, const float* __restrict__ gradp,
-               const double* __restrict__ gscale,
-               const double* __restrict__ l2v, const double* __restrict__ inv_nv,
-               int32_t* n_evals, const uint8_t* __restrict__ fmask, const int32_t* __restrict__ n_act_dev,
-               const double* __restrict__ gradr) {
-  const int s = blockIdx.x * (LB_THREADS / 32) + (threadIdx.x >> 5);
+lb_step_kernel(LbfgsScalars* sc, double* vec, size_t stride, const SlotMeta* slot, int n_act,
+               const int32_t* __restrict__ n_act_dev, int K, int nz_used, int d, int ldx, int fit_intercept,
+               const double* __restrict__ lossp, const double* __restrict__ gsump, const float* __restrict__ gradp,
+               const double* __restrict__ gradr, const double* __restrict__ gscale,
+               const uint8_t* __restrict__ fmask, const double* __restrict__ l2v, const double* __restrict__ inv_nv,
+               int32_t* n_evals) {
+  __shared__ double red[8];
+  const int a = blockIdx.x * Par::PER_CTA + threadIdx.x / (LB_THREADS / Par::PER_CTA);
   // n_act (host) may be a stale upper bound when several rounds are enqueued per host round trip:
   // the partial sums are indexed with it, the live slot count is the device's
-  if (s >= n_act || s >= *n_act_dev) return;
-  const int col = slot[s].col;
+  if (a >= n_act || a >= *n_act_dev) return;
+  const int col = slot[a].col;
   if (col < 0) return;   // padding slot of the fold-grouped layout
   LbfgsScalars st = sc[col];
   const int n = st.n, m = st.m;
-  LbfgsVectors v = col_vectors(vec + (size_t)col * vec_stride, n, m);
-  WarpPar P;
-  const double l2 = l2v[col], inv_n = inv_nv[col];
-  double f = gather_fg(P, s, n_act, nz_used, d, ldx, fit_intercept, lossp, gsump, gradp, gscale, l2,
-                       inv_n, v.x, v.g, fmask ? fmask + (size_t)col * d : nullptr, gradr);
-  __syncwarp();
+  LbfgsVectors v = lbfgs_col_vectors(vec + (size_t)col * stride, n, m);
+  Par P{red};
+  const double f = gather_fg(P, a, n_act, K, nz_used, d, ldx, fit_intercept, lossp, gsump, gradp, gradr, gscale,
+                             fmask ? fmask + (size_t)col * d : nullptr, l2v[col], inv_nv[col], v.x, v.g);
+  P.sync();
   lbfgs_advance(P, st, v, f);
-  __syncwarp();
+  P.sync();
   if (P.tid() == 0) {
     sc[col] = st;
     n_evals[col] += 1;
   }
 }
 
-// Stable in-place compaction of the active slot list (single CTA).
-__global__ void lb_compact_kernel(const LbfgsScalars* sc, SlotMeta* slot, int n_act_in,
-                                  int32_t* n_act_out, int32_t* n_act_host) {
+// Exclusive prefix sum of keep over the CTA, in thread order; total receives the CTA's sum.  wsum: shared, 32
+// ints; the caller synchronises before the next call writes it again.
+__device__ __forceinline__ int block_scan(int keep, int* wsum, int& total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int x = keep;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) wsum[wid] = x;
+  __syncthreads();
+  if (wid == 0) {
+    int w = (lane < (int)(blockDim.x >> 5)) ? wsum[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      int y = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += y;
+    }
+    wsum[lane] = w;  // inclusive
+  }
+  __syncthreads();
+  total = wsum[(blockDim.x >> 5) - 1];
+  return x - keep + (wid > 0 ? wsum[wid - 1] : 0);
+}
+
+// Stable in-place compaction of the active list (single CTA).
+__global__ void lb_compact_kernel(const LbfgsScalars* sc, SlotMeta* slot, int n_act_in, int32_t* n_act_out,
+                                  int32_t* n_run_out, int32_t* hist) {
   __shared__ int wsum[32];
   __shared__ int base_s;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int tid = threadIdx.x;
   if (tid == 0) base_s = 0;
   { const int live = *n_act_out; if (live < n_act_in) n_act_in = live; }   // host value may be a stale upper bound
   __syncthreads();
@@ -243,27 +267,8 @@ __global__ void lb_compact_kernel(const LbfgsScalars* sc, SlotMeta* slot, int n_
       sm = slot[i];
       keep = sc[sm.col].status == LB_RUNNING ? 1 : 0;
     }
-    // block exclusive scan of keep
-    int x = keep;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int y = __shfl_up_sync(0xffffffffu, x, o);
-      if (lane >= o) x += y;
-    }
-    if (lane == 31) wsum[wid] = x;
-    __syncthreads();
-    if (wid == 0) {
-      int w = (lane < (int)(blockDim.x >> 5)) ? wsum[lane] : 0;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        int y = __shfl_up_sync(0xffffffffu, w, o);
-        if (lane >= o) w += y;
-      }
-      wsum[lane] = w;  // inclusive
-    }
-    __syncthreads();
-    int prefix = x - keep + (wid > 0 ? wsum[wid - 1] : 0);
-    int total = wsum[(blockDim.x >> 5) - 1];
+    int total;
+    const int prefix = block_scan(keep, wsum, total);
     int base = base_s;
     __syncthreads();
     if (keep) slot[base + prefix] = sm;
@@ -272,7 +277,8 @@ __global__ void lb_compact_kernel(const LbfgsScalars* sc, SlotMeta* slot, int n_
   }
   if (tid == 0) {
     *n_act_out = base_s;
-    if (n_act_host) { n_act_host[0] = base_s; n_act_host[1] = base_s; }   // per-round record
+    if (n_run_out) *n_run_out = base_s;
+    if (hist) { hist[0] = base_s; hist[1] = base_s; }   // per-round record
   }
 }
 
@@ -286,7 +292,7 @@ __global__ void lb_compact_grouped_kernel(const LbfgsScalars* sc, SlotMeta* slot
   __shared__ int before[130];    // kept in earlier fold keys
   __shared__ int wsum[32];
   __shared__ int run_s;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int tid = threadIdx.x;
   for (int i = tid; i < 130; i += blockDim.x) cnt[i] = 0;
   if (tid == 0) run_s = 0;
   { const int live = *n_slots_out; if (live < n_in) n_in = live; }         // host value may be a stale upper bound
@@ -310,20 +316,8 @@ __global__ void lb_compact_grouped_kernel(const LbfgsScalars* sc, SlotMeta* slot
     SlotMeta sm;
     int keep = 0;
     if (i < n_in) { sm = slot[i]; keep = (sm.col >= 0 && sc[sm.col].status == LB_RUNNING) ? 1 : 0; }
-    int x = keep;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) wsum[wid] = x;
-    __syncthreads();
-    if (wid == 0) {
-      int w = (lane < (int)(blockDim.x >> 5)) ? wsum[lane] : 0;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-      wsum[lane] = w;
-    }
-    __syncthreads();
-    const int rank = run_s + x - keep + (wid > 0 ? wsum[wid - 1] : 0);
-    const int total = wsum[(blockDim.x >> 5) - 1];
+    int total;
+    const int rank = run_s + block_scan(keep, wsum, total);
     __syncthreads();
     if (keep) slot[base[sm.fold + 1] + rank - before[sm.fold + 1]] = sm;
     if (tid == 0) run_s += total;
@@ -339,223 +333,23 @@ __global__ void lb_compact_grouped_kernel(const LbfgsScalars* sc, SlotMeta* slot
   }
 }
 
-__global__ void lb_export_kernel(const LbfgsScalars* sc, const double* vec, size_t vec_stride,
-                                 const SlotMeta* slot, const int32_t* n_act, int d, int ldx,
-                                 int Bcap, float* Wact) {
-  const int s = blockIdx.x;
-  if (s >= *n_act) return;
-  const int col = slot[s].col;
-  const double* x = vec + (size_t)col * vec_stride;
-  for (int k = threadIdx.x; k < ldx; k += blockDim.x)
-    Wact[(size_t)s * ldx + k] = k < d ? (float)x[k] : 0.f;
-  if (threadIdx.x == 0) Wact[(size_t)Bcap * ldx + s] = (float)x[d];
-}
-
-__global__ void lb_finish_kernel(const LbfgsScalars* sc, const double* vec, size_t vec_stride,
-                                 int B, int d, float* coef, int32_t* niter, int32_t* status,
-                                 double* loss) {
-  const int col = blockIdx.x;
-  if (col >= B) return;
-  const double* x = vec + (size_t)col * vec_stride;
-  for (int k = threadIdx.x; k <= d; k += blockDim.x) coef[(size_t)col * (d + 1) + k] = (float)x[k];
-  if (threadIdx.x == 0) {
-    const LbfgsScalars& s = sc[col];
-    niter[col] = s.nit < s.maxiter ? s.nit : s.maxiter;
-    status[col] = s.status;
-    loss[col] = s.f;
-  }
-}
-
-int lbfgs_dev_init(Ctx* c, LogregWork& w, int fit_intercept, double tol, int max_iter, int maxls, double ftol) {
-  const int m = 10;
-  lb_init_kernel<<<w.B, 128, 0, c->stream>>>(w.sc, w.vec, w.vec_stride, w.B, w.dp, m, max_iter,
-                                             maxls, tol, ftol, w.grouped ? nullptr : w.slot, w.col_fold,
-                                             w.col_pos, w.col_neg1, w.n_evals, w.n_act);
-  // initial iterate is w0 = 0 (SK/linear_model/_logistic.py:443): export zeros
-  c->launches += 1;
-  if (w.use_tc) {
-    if (tc_export(c, w, w.grouped ? w.slot_cap : w.B, nullptr, fit_intercept)) return 1;
-  } else {
-    SKD_CUDA(c, cudaMemsetAsync(w.Wact, 0, ((size_t)w.B * c->ldx + w.B) * sizeof(float), c->stream));
-  }
-  SKD_CUDA(c, cudaGetLastError());
-  return 0;
-}
-
-// One optimiser round on the stream, no host synchronisation: advance every live column, rebuild the
-// slot list, export the new trial points.  n_act_in may be a stale upper bound of the live slot count
-// (the kernels read the device-side count); hist (may be null) receives {slots, running} of the round.
-int lbfgs_dev_enqueue(Ctx* c, LogregWork& w, int n_act_in, int nz_used, int fit_intercept, int32_t* hist) {
-  const int d = (int)c->d, ldx = (int)c->ldx;
-  if (w.gradr && nz_used > 8) {   // many partials per slot (tensor-core path): reduce them with the whole device first
-    const int64_t total = (int64_t)n_act_in * w.ldw;
-    lb_reduce_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c->stream>>>(w.gradp, nz_used, n_act_in, w.ldw, w.n_act,
-                                                                          w.gradr);
-    c->launches += 1;
-  }
-  lb_step_kernel<<<(n_act_in + LB_THREADS / 32 - 1) / (LB_THREADS / 32), LB_THREADS, 0, c->stream>>>(
-      w.sc, w.vec, w.vec_stride, w.slot, n_act_in, nz_used, d, w.ldw, fit_intercept, w.lossp,
-      w.gsump, w.gradp, w.gscale, w.l2, w.inv_n, w.n_evals, w.fmask, w.n_act,
-      (w.gradr && nz_used > 8) ? w.gradr : nullptr);
-  if (w.grouped) lb_compact_grouped_kernel<<<1, 1024, 0, c->stream>>>(w.sc, w.slot, n_act_in, w.n_act, w.n_run, hist);
-  else lb_compact_kernel<<<1, 1024, 0, c->stream>>>(w.sc, w.slot, n_act_in, w.n_act, hist);
-  c->launches += 2;
-  if (w.use_tc) {
-    if (tc_export(c, w, n_act_in, nullptr, fit_intercept)) return 1;
-  } else {
-    lb_export_kernel<<<n_act_in, 128, 0, c->stream>>>(w.sc, w.vec, w.vec_stride, w.slot, w.n_act, d,
-                                                      ldx, w.B, w.Wact);
-    c->launches += 1;
-  }
-  SKD_CUDA(c, cudaGetLastError());
-  return 0;
-}
-
-// Host round trip: current slot count and number of running columns.
-int lbfgs_dev_readback(Ctx* c, LogregWork& w, int* n_act_out, int* n_run_out) {
-  int32_t na = 0, nr = 0;
-  SKD_CUDA(c, cudaMemcpyAsync(&na, w.n_act, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  if (w.grouped) SKD_CUDA(c, cudaMemcpyAsync(&nr, w.n_run, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->d2h += 2 * sizeof(int32_t);
-  *n_act_out = na;
-  *n_run_out = w.grouped ? nr : na;
-  return 0;
-}
-
-int lbfgs_dev_gather(Ctx* c, LogregWork& w, int n_act, int nz_used, int fit_intercept,
-                     const double* dx, double* df, double* dg) {
-  lb_gather_kernel<<<n_act, LB_THREADS, 0, c->stream>>>(n_act, nz_used, (int)c->d, w.ldw,
-                                                        fit_intercept, w.slot, w.lossp, w.gsump, w.gradp,
-                                                        w.gscale, w.l2, w.inv_n, dx, df, dg);
-  c->launches += 1;
-  SKD_CUDA(c, cudaGetLastError());
-  return 0;
-}
-
-int lbfgs_dev_finish(Ctx* c, LogregWork& w, float* dcoef, int32_t* dniter, int32_t* dstatus,
-                     double* dloss) {
-  lb_finish_kernel<<<w.B, 128, 0, c->stream>>>(w.sc, w.vec, w.vec_stride, w.B, (int)c->d, dcoef,
-                                               dniter, dstatus, dloss);
-  c->launches += 1;
-  SKD_CUDA(c, cudaGetLastError());
-  return 0;
-}
-
-// ---- multinomial problems: one CTA per active candidate, K * dp variables ------------------
-// f, g of active candidate a from the evaluation partials, added in chunk order (SK/linear_model/_linear_loss.py:349-372,
-// multiclass branch: loss = sum(loss_i) / n + 0.5 * l2 * ||W||^2, grad[:, :d] = G^T X / n + l2 * W,
-// grad[:, d] = sum_i G / n).  fmask: the candidate's feature mask or null.
-template <class Par>
-__device__ __forceinline__ double mn_gather_fg(const Par& P, int a, int n_act_in, int K, int d, int ldx, int nz,
-                                               int fit_intercept, const double* __restrict__ lossp,
-                                               const double* __restrict__ gsump, const float* __restrict__ gradp,
-                                               double l2, double inv_n, const double* x, double* g,
-                                               const uint8_t* __restrict__ fmask) {
-  const int dp = d + 1, n = K * dp;
-  const size_t n_slots = (size_t)n_act_in * K;
-  double lsum = 0.0;
-  for (int z = 0; z < nz; ++z) lsum += lossp[(size_t)z * n_act_in + a];
-  double wsq = 0.0;
-  for (int idx = P.tid(); idx < n; idx += P.nthr()) {
-    const int k = idx / dp, j = idx - k * dp;
-    const size_t slot = (size_t)a * K + k;
-    double acc = 0.0;
-    if (j < d) {
-      for (int z = 0; z < nz; ++z) acc += (double)gradp[((size_t)z * n_slots + slot) * ldx + j];
-      const double xk = x[idx];
-      // a feature masked out of this candidate keeps weight 0 in every class row (zero gradient entry)
-      g[idx] = (fmask && !fmask[j]) ? 0.0 : acc * inv_n + l2 * xk;
-      wsq += xk * xk;
-    } else {
-      for (int z = 0; z < nz; ++z) acc += gsump[(size_t)z * n_slots + slot];
-      g[idx] = fit_intercept ? acc * inv_n : 0.0;
-    }
-  }
-  wsq = P.block_sum(wsq);
-  return lsum * inv_n + 0.5 * l2 * wsq;
-}
-
-// f, g, then one step of the optimiser state machine.
-__global__ void __launch_bounds__(LB_THREADS)
-mn_step_kernel(LbfgsScalars* sc, double* vec, size_t vec_stride, const SlotMeta* cand, int n_act_in,
-               const int32_t* __restrict__ n_act_dev, int K, int d, int ldx, int nz, int fit_intercept,
-               const double* __restrict__ lossp, const double* __restrict__ gsump,
-               const float* __restrict__ gradp, const double* __restrict__ l2v,
-               const double* __restrict__ inv_nv, int32_t* n_evals, const uint8_t* __restrict__ fmask) {
-  __shared__ double red[8];
-  const int a = blockIdx.x;
-  if (a >= n_act_in || a >= *n_act_dev) return;
-  const int col = cand[a].col;
-  LbfgsScalars st = sc[col];
-  const int n = st.n, m = st.m;
-  LbfgsVectors v = col_vectors(vec + (size_t)col * vec_stride, n, m);
-  CtaPar P{red};
-  const double f = mn_gather_fg(P, a, n_act_in, K, d, ldx, nz, fit_intercept, lossp, gsump, gradp, l2v[col],
-                                inv_nv[col], v.x, v.g, fmask ? fmask + (size_t)col * d : nullptr);
-  __syncthreads();
-  lbfgs_advance(P, st, v, f);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    sc[col] = st;
-    n_evals[col] += 1;
-  }
-}
-
-// Test entry: objective and gradient of every active candidate at caller points xin [B][K][dp]; the partials
-// are indexed by active index, the constants, point and outputs by cand[a].col.
-__global__ void __launch_bounds__(LB_THREADS)
-mn_gather_kernel(const SlotMeta* cand, int n_act_in, int K, int d, int ldx, int nz, int fit_intercept,
-                 const double* __restrict__ lossp, const double* __restrict__ gsump,
-                 const float* __restrict__ gradp, const double* __restrict__ l2v,
-                 const double* __restrict__ inv_nv, const uint8_t* __restrict__ fmask,
-                 const double* __restrict__ xin, double* __restrict__ fout, double* __restrict__ gout) {
-  __shared__ double red[8];
-  const int a = blockIdx.x;
-  if (a >= n_act_in) return;
-  const int col = cand[a].col;
-  const size_t n = (size_t)K * (d + 1);
-  CtaPar P{red};
-  const double f = mn_gather_fg(P, a, n_act_in, K, d, ldx, nz, fit_intercept, lossp, gsump, gradp, l2v[col],
-                                inv_nv[col], xin + col * n, gout + col * n, fmask ? fmask + (size_t)col * d : nullptr);
-  if (threadIdx.x == 0) fout[col] = f;
-}
-
-__global__ void mn_init_kernel(LbfgsScalars* sc, double* vec, size_t vec_stride, int B, int n, int m,
-                               int maxiter, int maxls, double pgtol, double ftol, SlotMeta* cand,
-                               const int32_t* col_fold, int32_t* n_evals, int32_t* n_act) {
-  const int col = blockIdx.x;
-  if (col >= B) return;
-  double* base = vec + (size_t)col * vec_stride;
-  for (size_t i = threadIdx.x; i < vec_stride; i += blockDim.x) base[i] = 0.0;
-  if (threadIdx.x == 0) {
-    LbfgsScalars s;
-    lbfgs_init(s, n, m, maxiter, maxls, pgtol, ftol);
-    sc[col] = s;
-    SlotMeta sm;
-    sm.col = col; sm.fold = col_fold[col]; sm.pos = 0; sm.pad = 0;
-    cand[col] = sm;
-    n_evals[col] = 0;
-    if (col == 0) *n_act = B;
-  }
-}
-
-// trial points of the active candidates as fp32 slot rows (SK/_linear_loss.py:216-217 casts the same way)
-__global__ void mn_export_kernel(const double* vec, size_t vec_stride, const SlotMeta* cand,
-                                 const int32_t* n_act, int K, int d, int ldx, size_t bias_off, float* W) {
+// Points of the active entries as fp32 slot rows (SK/_linear_loss.py:216-217 casts the same way): one CTA per
+// slot a * K + k, row k of the point of problem slot[a].col in x (pitch x_stride).
+__global__ void lb_export_kernel(const double* x, size_t x_stride, const SlotMeta* slot, const int32_t* n_act, int K,
+                                 int d, int ldx, size_t bias_off, float* W) {
   const int a = blockIdx.x / K, k = blockIdx.x - a * K;
   if (a >= *n_act) return;
-  const double* x = vec + (size_t)cand[a].col * vec_stride + (size_t)k * (d + 1);
-  const size_t slot = (size_t)a * K + k;
-  for (int j = threadIdx.x; j < ldx; j += blockDim.x) W[slot * ldx + j] = j < d ? (float)x[j] : 0.f;
-  if (threadIdx.x == 0) W[bias_off + slot] = (float)x[d];
+  const double* xr = x + (size_t)slot[a].col * x_stride + (size_t)k * (d + 1);
+  const size_t s = (size_t)a * K + k;
+  for (int j = threadIdx.x; j < ldx; j += blockDim.x) W[s * ldx + j] = j < d ? (float)xr[j] : 0.f;
+  if (threadIdx.x == 0) W[bias_off + s] = (float)xr[d];
 }
 
-__global__ void mn_finish_kernel(const LbfgsScalars* sc, const double* vec, size_t vec_stride, int B, int n,
+__global__ void lb_finish_kernel(const LbfgsScalars* sc, const double* vec, size_t stride, int B, int n,
                                  float* coef, int32_t* niter, int32_t* status, double* loss) {
   const int col = blockIdx.x;
   if (col >= B) return;
-  const double* x = vec + (size_t)col * vec_stride;
+  const double* x = vec + (size_t)col * stride;
   for (int k = threadIdx.x; k < n; k += blockDim.x) coef[(size_t)col * n + k] = (float)x[k];
   if (threadIdx.x == 0) {
     const LbfgsScalars& s = sc[col];
@@ -565,53 +359,134 @@ __global__ void mn_finish_kernel(const LbfgsScalars* sc, const double* vec, size
   }
 }
 
-int multi_lbfgs_init(Ctx* c, MultiWork& w, const int32_t* d_col_fold, double tol, int max_iter, int maxls,
-                     double ftol) {
-  const int m = 10;
-  mn_init_kernel<<<w.B, 128, 0, c->stream>>>(w.sc, w.vec, w.vec_stride, w.B, w.K * w.dp, m, max_iter, maxls,
-                                             tol, ftol, w.cand, d_col_fold, w.n_evals, w.n_act);
+int lbfgs_alloc(Ctx* c, Scratch& sx, LbfgsBatch& b, int slot_cap, bool with_n_run) {
+  b.stride = lbfgs_col_doubles(b.n, LBFGS_M);
+  SKD_CUDA(c, sx.alloc(&b.sc, (size_t)b.B));
+  SKD_CUDA(c, sx.alloc(&b.vec, (size_t)b.B * b.stride));
+  SKD_CUDA(c, sx.alloc(&b.l2, (size_t)b.B));
+  SKD_CUDA(c, sx.alloc(&b.inv_n, (size_t)b.B));
+  SKD_CUDA(c, sx.alloc(&b.n_evals, (size_t)b.B));
+  if (slot_cap > 0) {
+    SKD_CUDA(c, sx.alloc(&b.slot, (size_t)slot_cap));
+    SKD_CUDA(c, sx.alloc(&b.n_act, 1));
+    if (with_n_run) SKD_CUDA(c, sx.alloc(&b.n_run, 1));
+  }
+  return 0;
+}
+
+// fp32 rows [B * K x ldx] then bias [B * K]
+static size_t export_bias_offset(const Ctx* c, const LbfgsBatch& b) { return (size_t)b.B * b.K * c->ldx; }
+
+int lbfgs_init(Ctx* c, LbfgsBatch& b, const int32_t* col_fold, const int32_t* col_pos, const int32_t* col_neg1,
+               double tol, int max_iter, int maxls, double ftol) {
+  lb_init_kernel<<<b.B, 128, 0, c->stream>>>(b.sc, b.vec, b.stride, b.B, b.n, LBFGS_M, max_iter, maxls, tol, ftol,
+                                             col_fold ? b.slot : nullptr, col_fold, col_pos, col_neg1, b.n_evals,
+                                             b.n_act);
   c->launches += 1;
-  // w0 = 0 (SK/linear_model/_logistic.py:443)
-  SKD_CUDA(c, cudaMemsetAsync(w.W, 0, ((size_t)w.B * w.K * c->ldx + (size_t)w.B * w.K) * sizeof(float), c->stream));
+  // initial iterate w0 = 0 (SK/linear_model/_logistic.py:443)
+  if (b.W)
+    SKD_CUDA(c, cudaMemsetAsync(b.W, 0, (export_bias_offset(c, b) + (size_t)b.B * b.K) * sizeof(float), c->stream));
   SKD_CUDA(c, cudaGetLastError());
   return 0;
 }
 
-int multi_lbfgs_enqueue(Ctx* c, MultiWork& w, int n_act_in, int fit_intercept, int32_t* hist) {
-  const int d = (int)c->d, ldx = (int)c->ldx;
-  mn_step_kernel<<<n_act_in, LB_THREADS, 0, c->stream>>>(w.sc, w.vec, w.vec_stride, w.cand, n_act_in, w.n_act,
-                                                         w.K, d, ldx, w.nz, fit_intercept, w.lossp, w.gsump,
-                                                         w.gradp, w.l2, w.inv_n, w.n_evals, w.fmask);
-  lb_compact_kernel<<<1, 1024, 0, c->stream>>>(w.sc, w.cand, n_act_in, w.n_act, hist);
-  mn_export_kernel<<<n_act_in * w.K, 128, 0, c->stream>>>(w.vec, w.vec_stride, w.cand, w.n_act, w.K, d, ldx,
-                                                          (size_t)w.B * w.K * ldx, w.W);
-  c->launches += 3;
+int lbfgs_enqueue(Ctx* c, LbfgsBatch& b, int n_act_in, int nz_used, int fit_intercept, int32_t* hist,
+                  LogregWork* tc) {
+  const int d = (int)c->d;
+  // many partials per slot (tensor-core path): reduce them with the whole device first
+  const double* gradr = (b.gradr && nz_used > 8) ? b.gradr : nullptr;
+  if (gradr) {
+    const int64_t total = (int64_t)n_act_in * b.ldw;
+    lb_reduce_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c->stream>>>(b.gradp, nz_used, n_act_in, b.ldw, b.n_act,
+                                                                          b.gradr);
+    c->launches += 1;
+  }
+  if (b.K == 1)
+    lb_step_kernel<WarpPar><<<(n_act_in + WarpPar::PER_CTA - 1) / WarpPar::PER_CTA, LB_THREADS, 0, c->stream>>>(
+        b.sc, b.vec, b.stride, b.slot, n_act_in, b.n_act, b.K, nz_used, d, b.ldw, fit_intercept, b.lossp, b.gsump,
+        b.gradp, gradr, b.gscale, b.fmask, b.l2, b.inv_n, b.n_evals);
+  else
+    lb_step_kernel<CtaPar><<<n_act_in, LB_THREADS, 0, c->stream>>>(
+        b.sc, b.vec, b.stride, b.slot, n_act_in, b.n_act, b.K, nz_used, d, b.ldw, fit_intercept, b.lossp, b.gsump,
+        b.gradp, gradr, b.gscale, b.fmask, b.l2, b.inv_n, b.n_evals);
+  if (b.grouped) lb_compact_grouped_kernel<<<1, 1024, 0, c->stream>>>(b.sc, b.slot, n_act_in, b.n_act, b.n_run, hist);
+  else lb_compact_kernel<<<1, 1024, 0, c->stream>>>(b.sc, b.slot, n_act_in, b.n_act, b.n_run, hist);
+  c->launches += 2;
+  if (tc) {
+    if (tc_export(c, *tc, n_act_in, nullptr, fit_intercept)) return 1;
+  } else {
+    lb_export_kernel<<<n_act_in * b.K, 128, 0, c->stream>>>(b.vec, b.stride, b.slot, b.n_act, b.K, d, (int)c->ldx,
+                                                           export_bias_offset(c, b), b.W);
+    c->launches += 1;
+  }
   SKD_CUDA(c, cudaGetLastError());
   return 0;
 }
 
-// caller points dx [B][K][dp] (device, float64) to the fp32 slot rows, by the export of the optimiser's trial points
-int multi_export_points(Ctx* c, MultiWork& w, const double* dx) {
-  mn_export_kernel<<<w.B * w.K, 128, 0, c->stream>>>(dx, (size_t)w.K * w.dp, w.cand, w.n_act, w.K, (int)c->d,
-                                                     (int)c->ldx, (size_t)w.B * w.K * c->ldx, w.W);
+int lbfgs_run(Ctx* c, LbfgsBatch& b, int n_act, int fit_intercept, int max_iter, int32_t* hist, LogregWork* tc,
+              const std::function<int(int n_act, long round, int* nz_used)>& eval, long* rounds_out) {
+  const long max_rounds = lbfgs_max_rounds(max_iter);
+  long rounds = 0;
+  int n_run = b.B;
+  // Several optimiser rounds are enqueued per host round trip: the kernels read the live slot count on the
+  // device, the host's n_act is only an upper bound that sizes the grids and strides.
+  while (n_run > 0) {
+    for (int q = 0; q < LBFGS_ROUNDS_PER_SYNC; ++q) {
+      int nz_used = b.nz;
+      if (eval(n_act, rounds, &nz_used)) return 1;
+      if (lbfgs_enqueue(c, b, n_act, nz_used, fit_intercept, hist ? hist + 2 * rounds : nullptr, tc)) return 1;
+      if (++rounds > max_rounds) return fail(c, "device L-BFGS-B: round limit exceeded (internal error)");
+    }
+    int32_t na = 0, nr = 0;
+    SKD_CUDA(c, cudaMemcpyAsync(&na, b.n_act, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+    if (b.n_run) SKD_CUDA(c, cudaMemcpyAsync(&nr, b.n_run, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+    SKD_CUDA(c, cudaStreamSynchronize(c->stream));
+    c->d2h += (b.n_run ? 2 : 1) * sizeof(int32_t);
+    n_act = na;
+    n_run = b.n_run ? nr : na;
+  }
+  if (rounds_out) *rounds_out = rounds;
+  return 0;
+}
+
+int lbfgs_export_points(Ctx* c, LbfgsBatch& b, int n_act_upper, const double* dx) {
+  lb_export_kernel<<<n_act_upper * b.K, 128, 0, c->stream>>>(dx, (size_t)b.n, b.slot, b.n_act, b.K, (int)c->d,
+                                                            (int)c->ldx, export_bias_offset(c, b), b.W);
   c->launches += 1;
   SKD_CUDA(c, cudaGetLastError());
   return 0;
 }
 
-int multi_gather(Ctx* c, MultiWork& w, int fit_intercept, const double* dx, double* df, double* dg) {
-  mn_gather_kernel<<<w.B, LB_THREADS, 0, c->stream>>>(w.cand, w.B, w.K, (int)c->d, (int)c->ldx, w.nz, fit_intercept,
-                                                      w.lossp, w.gsump, w.gradp, w.l2, w.inv_n, w.fmask, dx, df, dg);
+int lbfgs_gather(Ctx* c, LbfgsBatch& b, int n_act, int nz_used, int fit_intercept, const double* dx, double* df,
+                 double* dg) {
+  lb_gather_kernel<<<n_act, LB_THREADS, 0, c->stream>>>(b.slot, n_act, b.K, nz_used, (int)c->d, b.ldw, fit_intercept,
+                                                        b.lossp, b.gsump, b.gradp, b.gscale, b.fmask, b.l2, b.inv_n,
+                                                        dx, df, dg);
   c->launches += 1;
   SKD_CUDA(c, cudaGetLastError());
   return 0;
 }
 
-int multi_lbfgs_finish(Ctx* c, MultiWork& w, float* dcoef, int32_t* dniter, int32_t* dstatus, double* dloss) {
-  mn_finish_kernel<<<w.B, 128, 0, c->stream>>>(w.sc, w.vec, w.vec_stride, w.B, w.K * w.dp, dcoef, dniter,
-                                               dstatus, dloss);
+int lbfgs_result(Ctx* c, Scratch& sx, LbfgsBatch& b, int64_t b0, float* coef_out, int32_t* n_iter_out,
+                 int32_t* status_out, double* loss_out, int32_t* n_evals_out) {
+  const int B = b.B;
+  float* dcoef; int32_t *dniter, *dstatus; double* dloss;
+  SKD_CUDA(c, sx.alloc(&dcoef, (size_t)B * b.n));
+  SKD_CUDA(c, sx.alloc(&dniter, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&dstatus, (size_t)B));
+  SKD_CUDA(c, sx.alloc(&dloss, (size_t)B));
+  lb_finish_kernel<<<B, 128, 0, c->stream>>>(b.sc, b.vec, b.stride, B, b.n, dcoef, dniter, dstatus, dloss);
   c->launches += 1;
   SKD_CUDA(c, cudaGetLastError());
+  SKD_CUDA(c, cudaMemcpyAsync(coef_out + b0 * b.n, dcoef, (size_t)B * b.n * sizeof(float), cudaMemcpyDeviceToHost,
+                              c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(n_iter_out + b0, dniter, B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(status_out + b0, dstatus, B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  if (loss_out)
+    SKD_CUDA(c, cudaMemcpyAsync(loss_out + b0, dloss, B * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  if (n_evals_out)
+    SKD_CUDA(c, cudaMemcpyAsync(n_evals_out + b0, b.n_evals, B * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  c->d2h += (int64_t)B * (b.n * 4 + 20);
   return 0;
 }
 

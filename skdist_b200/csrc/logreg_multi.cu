@@ -5,7 +5,7 @@
 // 584-598):  minimise  mean_i[ logsumexp(z_i) - z_{i, y_i} ] + 0.5 * l2 * ||W||^2,  z_i = W x_i + b,
 // l2 = 1 / (C * n_train), intercepts unpenalised, L-BFGS-B from W = 0.
 //
-// One optimiser problem per candidate with K * (d + 1) variables (lbfgs_dev.cu mn_step_kernel); the
+// One optimiser problem per candidate with K * (d + 1) variables (lbfgs_dev.cu lb_step_kernel); the
 // evaluation treats the K class rows of every active candidate as K slots of one fp32 slot matrix:
 //   simt_raw_prediction  Z = X W^T + b                       (fp32 FMA, SK/_linear_loss.py:219)
 //   mn_pointwise_kernel  per training row: softmax, loss, p - onehot in place of Z
@@ -164,31 +164,25 @@ static int multi_pass_setup(Ctx* c, Scratch& sx, MultiWork& w, int64_t b0, int B
                             const double* l2, const double* inv_n, const int32_t* col_fold, const uint8_t* fmask,
                             const float* cw, int32_t** d_fold) {
   const int64_t n = c->n, ldx = c->ldx;
-  const int dp = (int)c->d + 1, m = 10;
-  w.B = Bb; w.K = K; w.dp = dp; w.nz = nz; w.rpc = rpc;
+  LbfgsBatch& b = w.lb;
+  b.B = Bb; b.K = K; b.n = K * ((int)c->d + 1); b.nz = nz; b.ldw = (int)ldx;
+  w.rpc = rpc;
   const size_t slots = (size_t)Bb * K;
   w.ldg = (int)((slots + 63) / 64 * 64);
-  w.vec_stride = (size_t)(5 + 2 * m) * K * dp + 2 * m;
-  SKD_CUDA(c, sx.alloc(&w.sc, (size_t)Bb));
-  SKD_CUDA(c, sx.alloc(&w.vec, (size_t)Bb * w.vec_stride));
-  SKD_CUDA(c, sx.alloc(&w.l2, (size_t)Bb));
-  SKD_CUDA(c, sx.alloc(&w.inv_n, (size_t)Bb));
-  SKD_CUDA(c, sx.alloc(&w.n_evals, (size_t)Bb));
-  SKD_CUDA(c, sx.alloc(&w.cand, (size_t)Bb));
+  if (lbfgs_alloc(c, sx, b, Bb, false)) return 1;
   SKD_CUDA(c, sx.alloc(d_fold, (size_t)Bb));
-  SKD_CUDA(c, sx.alloc(&w.W, slots * ldx + slots));
+  SKD_CUDA(c, sx.alloc(&b.W, slots * ldx + slots));
   SKD_CUDA(c, sx.alloc(&w.G, (size_t)n * w.ldg));
-  SKD_CUDA(c, sx.alloc(&w.lossp, (size_t)nz * Bb));
-  SKD_CUDA(c, sx.alloc(&w.gsump, (size_t)nz * slots));
-  SKD_CUDA(c, sx.alloc(&w.gradp, (size_t)nz * slots * ldx));
-  SKD_CUDA(c, sx.alloc(&w.n_act, 1));
-  SKD_CUDA(c, cudaMemcpyAsync(w.l2, l2 + b0, Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  SKD_CUDA(c, cudaMemcpyAsync(w.inv_n, inv_n + b0, Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, sx.alloc(&b.lossp, (size_t)nz * Bb));
+  SKD_CUDA(c, sx.alloc(&b.gsump, (size_t)nz * slots));
+  SKD_CUDA(c, sx.alloc(&b.gradp, (size_t)nz * slots * ldx));
+  SKD_CUDA(c, cudaMemcpyAsync(b.l2, l2 + b0, Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SKD_CUDA(c, cudaMemcpyAsync(b.inv_n, inv_n + b0, Bb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   SKD_CUDA(c, cudaMemcpyAsync(*d_fold, col_fold + b0, Bb * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   c->h2d += (int64_t)Bb * 20;
   if (fmask) {     // per-candidate feature masks (DistFeatureEliminator): masked weights stay exactly 0
-    SKD_CUDA(c, sx.alloc(&w.fmask, (size_t)Bb * c->d));
-    SKD_CUDA(c, cudaMemcpyAsync(w.fmask, fmask + (size_t)b0 * c->d, (size_t)Bb * c->d, cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, sx.alloc(&b.fmask, (size_t)Bb * c->d));
+    SKD_CUDA(c, cudaMemcpyAsync(b.fmask, fmask + (size_t)b0 * c->d, (size_t)Bb * c->d, cudaMemcpyHostToDevice, c->stream));
     c->h2d += (int64_t)Bb * c->d;
   }
   if (cw) {
@@ -201,23 +195,23 @@ static int multi_pass_setup(Ctx* c, Scratch& sx, MultiWork& w, int64_t b0, int B
   return 0;
 }
 
-// One evaluation of the n_act active candidates at the slot rows in w.W: raw predictions, pointwise loss and
-// gradient in place, per-chunk intercept and weight gradient partials (w.lossp, w.gsump, w.gradp).
+// One evaluation of the n_act active candidates at the slot rows in w.lb.W: raw predictions, pointwise loss and
+// gradient in place, per-chunk intercept and weight gradient partials (lossp, gsump, gradp of w.lb).
 static int multi_eval(Ctx* c, MultiWork& w, int n_act) {
-  const size_t slots = (size_t)w.B * w.K;
-  const int ns = n_act * w.K;
-  if (simt_raw_prediction(c, ns, w.W, w.W + slots * c->ldx, w.G, w.ldg)) return 1;
-  mn_pointwise_kernel<<<dim3(n_act, w.nz), 256, 0, c->stream>>>(w.G, w.ldg, c->n, w.rpc, w.K, w.cand, w.n_act, n_act,
-                                                               c->ycls, c->fold, w.lossp, w.cw);
-  mn_colsum_kernel<<<dim3((ns + 63) / 64, w.nz), 256, 0, c->stream>>>(w.G, w.ldg, c->n, w.rpc, ns, w.gsump);
+  const LbfgsBatch& b = w.lb;
+  const size_t slots = (size_t)b.B * b.K;
+  const int ns = n_act * b.K;
+  if (simt_raw_prediction(c, ns, b.W, b.W + slots * c->ldx, w.G, w.ldg)) return 1;
+  mn_pointwise_kernel<<<dim3(n_act, b.nz), 256, 0, c->stream>>>(w.G, w.ldg, c->n, w.rpc, b.K, b.slot, b.n_act, n_act,
+                                                               c->ycls, c->fold, b.lossp, w.cw);
+  mn_colsum_kernel<<<dim3((ns + 63) / 64, b.nz), 256, 0, c->stream>>>(w.G, w.ldg, c->n, w.rpc, ns, b.gsump);
   c->launches += 2;
-  return simt_backward(c, w.G, w.ldg, ns, w.nz, w.rpc, w.gradp);
+  return simt_backward(c, w.G, w.ldg, ns, b.nz, w.rpc, b.gradp);
 }
 
 int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold, int fit_intercept,
               double tol, int max_iter, const uint8_t* fmask, const float* cw, float* coef_out,
               int32_t* n_iter_out, int32_t* status_out, double* loss_out, int32_t* n_evals_out) {
-  const int dp = (int)c->d + 1;
   int nz;
   int64_t rpc;
   multi_chunks(c->n, &nz, &rpc);
@@ -228,41 +222,12 @@ int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const
     MultiWork w;
     int32_t* d_fold;
     if (multi_pass_setup(c, sx, w, b0, Bb, K, nz, rpc, l2, inv_n, col_fold, fmask, cw, &d_fold)) return 1;
-    if (multi_lbfgs_init(c, w, d_fold, tol, max_iter)) return 1;
-
-    // several optimiser rounds per host round trip; the kernels read the live candidate count from
-    // the device, the host's value is an upper bound that only sizes the grids and strides
-    int n_act = Bb;
-    const int rounds_per_sync = 4;
-    const long long max_rounds = (long long)max_iter * 60 + 64;   // maxls = 50 evaluations per iteration at most
-    long long round = 0;
-    while (n_act > 0) {
-      for (int q = 0; q < rounds_per_sync; ++q, ++round) {
-        if (multi_eval(c, w, n_act)) return 1;
-        if (multi_lbfgs_enqueue(c, w, n_act, fit_intercept, nullptr)) return 1;
-      }
-      int32_t na = 0;
-      SKD_CUDA(c, cudaMemcpyAsync(&na, w.n_act, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-      SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-      c->d2h += 4;
-      n_act = na;
-      if (round > max_rounds) return fail(c, "skd_logreg_multinomial_fit_batch: optimiser did not terminate");
-    }
-    float* dcoef; int32_t *dniter, *dstatus; double* dloss;
-    SKD_CUDA(c, sx.alloc(&dcoef, (size_t)Bb * K * dp));
-    SKD_CUDA(c, sx.alloc(&dniter, (size_t)Bb));
-    SKD_CUDA(c, sx.alloc(&dstatus, (size_t)Bb));
-    SKD_CUDA(c, sx.alloc(&dloss, (size_t)Bb));
-    if (multi_lbfgs_finish(c, w, dcoef, dniter, dstatus, dloss)) return 1;
-    SKD_CUDA(c, cudaMemcpyAsync(coef_out + (size_t)b0 * K * dp, dcoef, (size_t)Bb * K * dp * sizeof(float),
-                                cudaMemcpyDeviceToHost, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(n_iter_out + b0, dniter, Bb * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(status_out + b0, dstatus, Bb * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-    if (loss_out) SKD_CUDA(c, cudaMemcpyAsync(loss_out + b0, dloss, Bb * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    if (n_evals_out)
-      SKD_CUDA(c, cudaMemcpyAsync(n_evals_out + b0, w.n_evals, Bb * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+    if (lbfgs_init(c, w.lb, d_fold, nullptr, nullptr, tol, max_iter)) return 1;
+    if (lbfgs_run(c, w.lb, Bb, fit_intercept, max_iter, nullptr, nullptr,
+                  [&](int n_act, long, int*) { return multi_eval(c, w, n_act); }, nullptr))
+      return 1;
+    if (lbfgs_result(c, sx, w.lb, b0, coef_out, n_iter_out, status_out, loss_out, n_evals_out)) return 1;
     SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-    c->d2h += (int64_t)Bb * (K * dp * 4 + 20);
   }
   return 0;
 }
@@ -290,14 +255,14 @@ int multi_loss_grad(Ctx* c, int B, int K, const double* l2, const double* inv_n,
     SKD_CUDA(c, sx.alloc(&dx, nvar));
     SKD_CUDA(c, sx.alloc(&df, (size_t)Bb));
     SKD_CUDA(c, sx.alloc(&dg, nvar));
-    SKD_CUDA(c, cudaMemcpyAsync(w.cand, hc.data(), Bb * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
-    SKD_CUDA(c, cudaMemcpyAsync(w.n_act, &Bb, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(w.lb.slot, hc.data(), Bb * sizeof(SlotMeta), cudaMemcpyHostToDevice, c->stream));
+    SKD_CUDA(c, cudaMemcpyAsync(w.lb.n_act, &Bb, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     SKD_CUDA(c, cudaMemcpyAsync(dx, w_in + (size_t)b0 * K * dp, nvar * sizeof(double), cudaMemcpyHostToDevice,
                                 c->stream));
     c->h2d += (int64_t)Bb * sizeof(SlotMeta) + 4 + (int64_t)nvar * 8;
-    if (multi_export_points(c, w, dx)) return 1;
+    if (lbfgs_export_points(c, w.lb, Bb, dx)) return 1;
     if (multi_eval(c, w, Bb)) return 1;
-    if (multi_gather(c, w, fit_intercept, dx, df, dg)) return 1;
+    if (lbfgs_gather(c, w.lb, Bb, nz, fit_intercept, dx, df, dg)) return 1;
     SKD_CUDA(c, cudaMemcpyAsync(loss_out + b0, df, Bb * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
     SKD_CUDA(c, cudaMemcpyAsync(grad_out + (size_t)b0 * K * dp, dg, nvar * sizeof(double), cudaMemcpyDeviceToHost,
                                 c->stream));

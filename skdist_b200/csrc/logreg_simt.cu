@@ -299,17 +299,17 @@ int simt_eval(Ctx* c, LogregWork& w, int n_act, int* nz_used) {
   if (n_act <= 0) return 0;
   int nz;
   int64_t rpc;
-  pick_chunks(c, c->n, n_act, w.nz, &nz, &rpc);
+  pick_chunks(c, c->n, n_act, w.lb.nz, &nz, &rpc);
   const int ldx = (int)c->ldx;
   // SlotMeta / W are indexed by slot; G uses ldg columns.  Process slot ranges so that the
   // grid covers [0, n_act).
   dim3 gf((n_act + TN - 1) / TN, nz);
   fwd_kernel<MODE_FIT><<<gf, 256, 0, c->stream>>>(
-      c->X, c->n, ldx, w.Wact, w.Wact + (size_t)w.B * ldx /*bias block*/, w.slot, n_act, c->ycls,
-      c->fold, rpc, w.G, w.ldg, w.lossp, w.gsump, nullptr, nullptr, nullptr, 0, nullptr, w.ybits, w.mbits,
+      c->X, c->n, ldx, w.lb.W, w.lb.W + (size_t)w.lb.B * ldx /*bias block*/, w.lb.slot, n_act, c->ycls,
+      c->fold, rpc, w.G, w.ldg, w.lb.lossp, w.lb.gsump, nullptr, nullptr, nullptr, 0, nullptr, w.ybits, w.mbits,
       (long long)w.rb_words, w.cw);
   dim3 gb((ldx + 63) / 64, (n_act + TN - 1) / TN, nz);
-  bwd_kernel<<<gb, 256, 0, c->stream>>>(c->X, c->n, ldx, w.G, w.ldg, n_act, rpc, w.gradp);
+  bwd_kernel<<<gb, 256, 0, c->stream>>>(c->X, c->n, ldx, w.G, w.ldg, n_act, rpc, w.lb.gradp);
   c->launches += 2;
   *nz_used = nz;
   cudaError_t e = cudaGetLastError();

@@ -866,7 +866,7 @@ int tc_prepare(Ctx* c) {
 
 int tc_export(Ctx* c, LogregWork& w, int n_act_upper, const double* xin, int fit_intercept) {
   TcData& t = c->tc;
-  tc_export_kernel<<<n_act_upper, 128, 0, c->stream>>>(w.vec, w.vec_stride, w.slot, w.n_act, (int)c->d,
+  tc_export_kernel<<<n_act_upper, 128, 0, c->stream>>>(w.lb.vec, w.lb.stride, w.lb.slot, w.lb.n_act, (int)c->d,
                                                        t.dpad, t.xscale, (__half*)w.Wh, (__half*)w.Wl,
                                                        (TcSlotParam*)w.sp, xin, fit_intercept);
   c->launches += 1;
@@ -920,9 +920,9 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
     // every (chunk, slot) partial has exactly one writer; only chunks without tiles (fewer tiles
     // than chunks in some list) are never written and must read as zero
     if (t.min_list_tiles < TC_NCH) {
-      SKD_CUDA(c, cudaMemsetAsync(w.lossp, 0, (size_t)nz * n_act * sizeof(double), c->stream));
-      SKD_CUDA(c, cudaMemsetAsync(w.gsump, 0, (size_t)nz * n_act * sizeof(double), c->stream));
-      SKD_CUDA(c, cudaMemsetAsync(w.gradp, 0, (size_t)nz * n_act * w.ldw * sizeof(float), c->stream));
+      SKD_CUDA(c, cudaMemsetAsync(w.lb.lossp, 0, (size_t)nz * n_act * sizeof(double), c->stream));
+      SKD_CUDA(c, cudaMemsetAsync(w.lb.gsump, 0, (size_t)nz * n_act * sizeof(double), c->stream));
+      SKD_CUDA(c, cudaMemsetAsync(w.lb.gradp, 0, (size_t)nz * n_act * w.lb.ldw * sizeof(float), c->stream));
     }
   }
   CUtensorMap map_wh, map_wl;
@@ -932,23 +932,23 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
   prm.sp = (const TcSlotParam*)w.sp;
   prm.rowmeta = t.rowmeta;
   prm.yreal = t.yreal_pad;
-  prm.lossp = w.lossp;
-  prm.gsump = w.gsump;
-  prm.gradp = w.gradp;
+  prm.lossp = w.lb.lossp;
+  prm.gsump = w.lb.gsump;
+  prm.gradp = w.lb.gradp;
   prm.correct = dcorrect;
   prm.count = dcount;
   prm.n_act = n_act;
-  prm.n_act_dev = (mode == TC_FIT) ? w.n_act : nullptr;
+  prm.n_act_dev = (mode == TC_FIT) ? w.lb.n_act : nullptr;
   prm.groups = groups;
   prm.n_tiles = n_tiles;
-  prm.ldw = w.ldw;
+  prm.ldw = w.lb.ldw;
   prm.ybits = mode == TC_FIT ? w.ybits : nullptr;
   prm.mbits = mode == TC_FIT ? w.mbits : nullptr;
   prm.rb_words = w.rb_words;
   prm.deal_log = mode == TC_FIT ? w.deal_log : nullptr;
   // TC_FIT_UNI reads a row's sign from the list of the group's fold, so it needs one list per staged
   // fold (tc_prepare builds them for at most 32 folds); otherwise TC_FIT decodes the fold per element
-  const bool uni = mode == TC_FIT && w.grouped && w.uni_pos >= 0 && c->ycls && !w.ybits && !w.mbits &&
+  const bool uni = mode == TC_FIT && w.lb.grouped && w.uni_pos >= 0 && c->ycls && !w.ybits && !w.mbits &&
                    t.n_lists == c->n_folds + 1;
   if (uni && (!t.rowsg_valid || t.rowsg_pos != w.uni_pos)) {
     if (!t.rowsg) SKD_CUDA(c, cudaMalloc((void**)&t.rowsg, (size_t)t.n_lists * t.npad * sizeof(float)));
@@ -961,7 +961,7 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
   }
   prm.rowsg = uni ? t.rowsg : nullptr;
   prm.rowsg_ld = t.npad;
-  const bool lists = mode == TC_FIT && w.grouped && t.tilelist;
+  const bool lists = mode == TC_FIT && w.lb.grouped && t.tilelist;
   prm.tilelist = lists ? t.tilelist : nullptr;
   prm.tilecnt = lists ? t.tilecnt : nullptr;
   prm.n_lists = t.n_lists;
@@ -999,12 +999,12 @@ __global__ void tc_chunk_sum_kernel(const double* __restrict__ part, int n_act, 
 }
 
 // Sum of squared residuals / row counts of n_act regression slots (sp.fold = scoring code).  The kernel
-// writes one partial per (chunk, slot) into w.lossp ([TC_NCH x n_act], zeroed by the caller: chunks
+// writes one partial per (chunk, slot) into w.lb.lossp ([TC_NCH x n_act], zeroed by the caller: chunks
 // without tiles are not written); they are added here in chunk order, so the sums do not depend on
 // which CTA ran which chunk.
 int tc_r2(Ctx* c, LogregWork& w, int n_act, double* dsse, int64_t* dcount) {
   if (tc_run(c, w, n_act, TC_R2, nullptr, nullptr, (unsigned long long*)dcount)) return 1;
-  tc_chunk_sum_kernel<<<(n_act + 255) / 256, 256, 0, c->stream>>>(w.lossp, n_act, dsse);
+  tc_chunk_sum_kernel<<<(n_act + 255) / 256, 256, 0, c->stream>>>(w.lb.lossp, n_act, dsse);
   c->launches += 1;
   SKD_CUDA(c, cudaGetLastError());
   return 0;

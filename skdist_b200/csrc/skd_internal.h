@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <functional>
 #include <string>
 #include <utility>
 #include <vector>
@@ -231,51 +232,63 @@ struct SlotMeta {
                    // `pos` or class k take part (one-vs-one pair)
 };
 
+// One batch of device L-BFGS-B problems (lbfgs_dev.cu) and the evaluation partials they read.  Problem b
+// (a binary column, or a multinomial candidate) has n = K * (d + 1) variables, variable (k, j) at
+// k * (d + 1) + j; the evaluation sees K slots per entry a of the active list (slot a * K + k), K = 1 for
+// binary columns.
+struct LbfgsBatch {
+  int32_t B = 0;               // problems in the batch
+  int32_t K = 1;               // classes per problem (1: binary)
+  int32_t n = 0;               // variables per problem, K * (d + 1) (intercepts pinned to 0 if !fit_intercept)
+  // per problem (indexed by col)
+  LbfgsScalars* sc = nullptr;  // [B]
+  double* vec = nullptr;       // [B x stride] lbfgs_col_vectors blocks
+  size_t stride = 0;           // lbfgs_col_doubles(n, LBFGS_M)
+  double* l2 = nullptr;        // [B] l2 strength
+  double* inv_n = nullptr;     // [B] 1 / n_train
+  int32_t* n_evals = nullptr;  // [B]
+  uint8_t* fmask = nullptr;    // [B x d] or nullptr: 1 = feature takes part in the problem's fit
+  // active list
+  SlotMeta* slot = nullptr;    // [slot_cap] col = problem (-1: padding of the fold-grouped layout)
+  int32_t* n_act = nullptr;    // device scalar: entries of the active list
+  int32_t* n_run = nullptr;    // device scalar: problems still running, or nullptr (multinomial: n_act)
+  // fold-grouped layout (binary tensor-core path): every group of 128 slots holds columns of ONE fold,
+  // padded with col = -1 entries, so a group can skip the tiles made only of its held-out rows
+  bool grouped = false;
+  // evaluation partials of chunk z, indexed by active entry a or slot s = a * K + k
+  int32_t nz = 0;              // partials per slot at most
+  int32_t ldw = 0;             // row pitch of gradp (ldx, or dpad on the tensor-core path)
+  double* lossp = nullptr;     // z * n_act + a
+  double* gsump = nullptr;     // z * n_act * K + s
+  float* gradp = nullptr;      // (z * n_act * K + s) * ldw + j
+  double* gradr = nullptr;     // [slots x ldw] or nullptr: gradp reduced in chunk order (binary tensor-core path)
+  const double* gscale = nullptr;  // [d] or nullptr: per-feature un-scaling of gradp (tensor-core path)
+  // trial points as fp32 rows [B * K x ldx], then bias [B * K]; nullptr: the tensor-core weights (tc_export)
+  float* W = nullptr;
+};
+
 // Workspace of one skd_logreg_fit_batch call (device pointers).
 struct LogregWork {
-  int32_t B = 0;        // columns in the batch
-  int32_t dp = 0;       // d + 1 (intercept slot always present; pinned to 0 if !fit_intercept)
-  int32_t nz = 0;       // max row chunks per evaluation (partials per slot)
+  LbfgsBatch lb;        // B columns of d + 1 variables
   int64_t cap_sc = 0;   // capacity of the partial buffers in (chunk, slot) pairs
   int32_t ldg = 0;      // leading dimension of G (columns, padded)
   // per column (indexed by col)
-  LbfgsScalars* sc = nullptr;
-  double* vec = nullptr;       // per column block of (5 + 2m) * dp + 2m doubles
-  size_t vec_stride = 0;
-  double* l2 = nullptr;        // [B] l2 strength
-  double* inv_n = nullptr;     // [B] 1 / n_train
   int32_t* col_fold = nullptr; // [B]
   int32_t* col_pos = nullptr;  // [B]
   int32_t* col_neg1 = nullptr; // [B] or nullptr (see SlotMeta::pad)
-  uint8_t* fmask = nullptr;    // [B x d] or nullptr: 1 = feature takes part in the column's fit
   const uint32_t* ybits = nullptr;  // [B x rb_words] or nullptr: bit r of column j = its label of row r (instead of class id == pos)
   const uint32_t* mbits = nullptr;  // [B x rb_words] or nullptr: bit r of column j = row r trains the column
   int64_t rb_words = 0;
   const float2* cw = nullptr;  // [B] or nullptr: {label-0, label-1} weights of column j, largest <= 1
                                // (the power of two that normalised them is folded into inv_n)
-  int32_t* n_evals = nullptr;  // [B]
-  // per slot (active batch)
-  SlotMeta* slot = nullptr;    // [B]
-  float* Wact = nullptr;       // [B x ldx] fp32 weights of the active slots, then bias[B]
   float* G = nullptr;          // [n x ldg] pointwise gradients (SIMT path)
-  double* lossp = nullptr;     // [cap_sc]        indexed z * n_act + slot
-  double* gsump = nullptr;     // [cap_sc]
-  float* gradp = nullptr;      // [cap_sc x ldx]
-  double* gradr = nullptr;     // [slots x ldw] partials reduced in chunk order (tensor-core path)
-  int32_t* n_act = nullptr;    // device scalar
   // tensor-core path (logreg_tc.cu)
   bool use_tc = false;
-  int32_t ldw = 0;             // leading dimension of gradp rows (ldx for SIMT, dpad for TC)
-  const double* gscale = nullptr;  // per-feature un-scaling of gradp (TC) or nullptr
   void* Wh = nullptr;          // [slots_pad_cap x dpad] fp16
   void* Wl = nullptr;          // [slots_pad_cap x dpad] fp16
   void* sp = nullptr;          // [slots_pad_cap] TcSlotParam
   int32_t slots_pad_cap = 0;
-  // fold-grouped slot layout (TC path): every group of 128 slots holds columns of ONE fold, padded
-  // with col = -1 entries, so a group can skip the tiles made only of its held-out rows
-  bool grouped = false;
   int32_t slot_cap = 0;        // slots incl. padding at the start of the solve
-  int32_t* n_run = nullptr;    // device scalar: columns still running
   int32_t uni_pos = -1;        // >= 0: every column of the batch has this positive class (grouped layout only)
   int32_t* deal_log = nullptr; // device [4] or nullptr: the next evaluation's work deal (TcParams::deal_log)
 };
@@ -315,38 +328,16 @@ int ridge_fit_batch(Ctx* c, int B, const double* alpha, const int32_t* hold, int
 // Caller coefficients [rows x (d+1)] to the kernel layout on the device: weights [rows x ldx], then bias [rows]
 int pack_coef(Ctx* c, Scratch& sx, int rows, const float* coef, int64_t d, int64_t ldx, float** dW);
 
-// ---- multinomial logistic regression (logreg_multi.cu / lbfgs_dev.cu) -------------------
-// One optimiser problem per candidate with K * (d + 1) variables, variable (k, j) at k * dp + j;
-// the evaluation sees K slots per active candidate (slot = a * K + k for active index a).
+// ---- multinomial logistic regression (logreg_multi.cu) ------------------------------------
+// One optimiser problem per candidate with K * (d + 1) variables; active entry a = one candidate
+// (slot fold = its held-out fold, -1 none).
 struct MultiWork {
-  int32_t B = 0, K = 0, dp = 0;  // candidates of this solve, classes, d + 1
-  int32_t nz = 0;                // row chunks per evaluation (fixed by n alone)
-  int64_t rpc = 0;               // rows per chunk
+  LbfgsBatch lb;                 // B candidates of this solve, K classes, fp32 rows in lb.W
+  int64_t rpc = 0;               // rows per chunk (lb.nz chunks, fixed by n alone)
   int32_t ldg = 0;               // leading dimension of G
-  LbfgsScalars* sc = nullptr;    // [B]
-  double* vec = nullptr;         // [B x vec_stride]
-  size_t vec_stride = 0;
-  double* l2 = nullptr;          // [B]
-  double* inv_n = nullptr;       // [B]
-  int32_t* n_evals = nullptr;    // [B]
-  SlotMeta* cand = nullptr;      // [B] active candidates: col = candidate, fold = held-out fold (-1 none)
-  float* W = nullptr;            // [B*K x ldx] weights of the active slots, then bias [B*K]
   float* G = nullptr;            // [n x ldg] raw predictions, overwritten by the pointwise gradients
-  double* lossp = nullptr;       // [nz x B]    indexed z * n_act + a
-  double* gsump = nullptr;       // [nz x B*K]  indexed z * n_slots + slot
-  float* gradp = nullptr;        // [nz x B*K x ldx]
-  int32_t* n_act = nullptr;      // device scalar: active candidates
-  uint8_t* fmask = nullptr;      // [B x d] or nullptr: 1 = feature takes part in the candidate's fit
   const float* cw = nullptr;     // [B x K] or nullptr: weight of each class in the candidate's fit
 };
-// maxls and ftol: what scikit-learn passes to scipy (maxls = 50, ftol = 64 * eps) unless a test entry says otherwise
-int multi_lbfgs_init(Ctx* c, MultiWork& w, const int32_t* d_col_fold, double tol, int max_iter, int maxls = 50,
-                     double ftol = 64.0 * 2.220446049250313e-16);
-int multi_lbfgs_enqueue(Ctx* c, MultiWork& w, int n_act_in, int fit_intercept, int32_t* hist);
-int multi_lbfgs_finish(Ctx* c, MultiWork& w, float* dcoef, int32_t* dniter, int32_t* dstatus, double* dloss);
-// caller points dx [B][K][dp] (device) into w.W, and f, g of every candidate at them after one evaluation
-int multi_export_points(Ctx* c, MultiWork& w, const double* dx);
-int multi_gather(Ctx* c, MultiWork& w, int fit_intercept, const double* dx, double* df, double* dg);
 int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold, int fit_intercept,
               double tol, int max_iter, const uint8_t* fmask /*[B x d] or nullptr*/,
               const float* cw /*[B x K] or nullptr*/, float* coef_out, int32_t* n_iter_out,
@@ -382,13 +373,42 @@ size_t tc_slot_param_bytes();
 int tc_partials_per_slot();
 
 // device L-BFGS (lbfgs_dev.cu)
-int lbfgs_dev_init(Ctx* c, LogregWork& w, int fit_intercept, double tol, int max_iter, int maxls = 50,
-                   double ftol = 64.0 * 2.220446049250313e-16);
-int lbfgs_dev_enqueue(Ctx* c, LogregWork& w, int n_act_in, int nz_used, int fit_intercept, int32_t* hist);
-int lbfgs_dev_readback(Ctx* c, LogregWork& w, int* n_act_out, int* n_run_out);  // advance + compact + export (synchronises)
-int lbfgs_dev_gather(Ctx* c, LogregWork& w, int n_act, int nz_used, int fit_intercept,
-                     const double* dx, double* df, double* dg);
-int lbfgs_dev_finish(Ctx* c, LogregWork& w, float* dcoef, int32_t* dniter, int32_t* dstatus,
-                     double* dloss);
+// scikit-learn's line-search limit (maxls = 50) and ftol (64 * eps), which every fit passes to scipy
+constexpr int LBFGS_MAXLS = 50;
+constexpr double LBFGS_FTOL = 64.0 * 2.220446049250313e-16;
+constexpr int LBFGS_ROUNDS_PER_SYNC = 4;
+// Round cap of a fit (lbfgs_run) and size of its per-round record.  Every round is one evaluation of every
+// running problem.  lbfgs_advance consumes at most maxls evaluations per line search: the maxls-th trial
+// sets iback = maxls and fails it.  A failed line search with memory restarts once from steepest descent
+// (col = 0); a failure without memory ends the fit (LB_ABNORMAL).  So one iteration takes at most
+// 2 * maxls evaluations, a fit at most 1 + 2 * maxls * max_iter (the first evaluation consumes no line
+// search), and the rounds enqueued after the last problem stopped add fewer than LBFGS_ROUNDS_PER_SYNC.
+inline long lbfgs_max_rounds(int max_iter) {
+  return 2L * LBFGS_MAXLS * max_iter + 1 + LBFGS_ROUNDS_PER_SYNC;
+}
+// Allocates the batch's optimiser state and, for slot_cap > 0, its active list and counters (B, K, n set).
+int lbfgs_alloc(Ctx* c, Scratch& sx, LbfgsBatch& b, int slot_cap, bool with_n_run);
+// State of every problem at w = 0 (SK/linear_model/_logistic.py:443), the dense active list when col_fold is
+// given (slot b = problem b, pos col_pos[b] or 0, pad col_neg1[b] or 0), and zero fp32 rows b.W.
+int lbfgs_init(Ctx* c, LbfgsBatch& b, const int32_t* col_fold, const int32_t* col_pos, const int32_t* col_neg1,
+               double tol, int max_iter, int maxls = LBFGS_MAXLS, double ftol = LBFGS_FTOL);
+// One optimiser round on the stream: advance, compact the active list, export the new trial points (into b.W,
+// or through tc_export(*tc)).  n_act_in may be a stale upper bound; hist (may be null) receives {slots, running}.
+int lbfgs_enqueue(Ctx* c, LbfgsBatch& b, int n_act_in, int nz_used, int fit_intercept, int32_t* hist,
+                  LogregWork* tc = nullptr);
+// Host round loop of a fit: eval(n_act, round, &nz_used) fills the partials of the active list, then one
+// optimiser round; LBFGS_ROUNDS_PER_SYNC rounds per read back of the live counts, until no problem runs.
+// hist (may be null) receives {slots, running} of every round.  Returns the rounds enqueued in *rounds.
+int lbfgs_run(Ctx* c, LbfgsBatch& b, int n_act, int fit_intercept, int max_iter, int32_t* hist, LogregWork* tc,
+              const std::function<int(int n_act, long round, int* nz_used)>& eval, long* rounds);
+// caller points dx [rows][K][d+1] (device, float64; row = slot[a].col) as the fp32 rows b.W of n_act_upper entries
+int lbfgs_export_points(Ctx* c, LbfgsBatch& b, int n_act_upper, const double* dx);
+// f, g of every problem at caller points dx [B][n] from the partials of n_act active entries
+int lbfgs_gather(Ctx* c, LbfgsBatch& b, int n_act, int nz_used, int fit_intercept, const double* dx, double* df,
+                 double* dg);
+// Final coefficients [B][n], iteration counts, statuses, losses and (n_evals_out) evaluation counts copied
+// (not yet synchronised) to the host outputs of problems b0 .. b0 + B - 1; loss_out and n_evals_out may be null.
+int lbfgs_result(Ctx* c, Scratch& sx, LbfgsBatch& b, int64_t b0, float* coef_out, int32_t* n_iter_out, int32_t* status_out,
+                 double* loss_out, int32_t* n_evals_out);
 
 }  // namespace skd

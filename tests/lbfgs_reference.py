@@ -7,7 +7,7 @@ gradient sums in fp32) and forms
 
   f = (sum_z loss_z) * inv_n + 0.5 * l2 * |w|^2,   g_k = (sum_z grad_zk) * gscale_k * inv_n + l2 * w_k
 
-with the sums sequential in chunk order (gather_fg / mn_gather_fg).  `Problem.parts` turns a family's f, g * n
+with the sums sequential in chunk order (gather_fg).  `Problem.parts` turns a family's f, g * n
 into such partials -- every chunk holds a non-zero share of its value (`split`) -- and `Problem.effective` forms
 the f, g the device forms from them, which is what scipy and the host core are given.  With l2 = 0, power-of-two inv_n
 and gscale every device operation on them is exact (exact tier); otherwise FMA contraction and the order of
@@ -225,7 +225,7 @@ class Problem:
         return lp, gs, gp
 
     def effective(self, X, cols, lp, gs, gp):
-        """f [c], g [c, n] that gather_fg / mn_gather_fg form from the partials."""
+        """f [c], g [c, n] that gather_fg forms from the partials."""
         c = len(cols)
         inv, l2 = self.inv_n[cols], self.l2[cols]
         acc = chunk_sum(gp.transpose(0, 2, 1)).reshape(c, self.K, self.d)

@@ -1,4 +1,4 @@
-"""float64 reference of the multinomial evaluation (csrc/logreg_multi.cu, mn_gather_fg in csrc/lbfgs_dev.cu) and the
+"""float64 reference of the multinomial evaluation (csrc/logreg_multi.cu, gather_fg in csrc/lbfgs_dev.cu) and the
 first-order error bound of its fp32 arithmetic, shared by the GPU tests and their host rehearsal.
 
 With u = 2^-24 (one fp32 rounding), per training row i and class k of a candidate:

@@ -1,4 +1,4 @@
-"""The multinomial evaluation (csrc/logreg_multi.cu, mn_gather_fg / mn_step_kernel in csrc/lbfgs_dev.cu) against
+"""The multinomial evaluation (csrc/logreg_multi.cu, gather_fg / lb_step_kernel in csrc/lbfgs_dev.cu) against
 float64, through skd_logreg_multinomial_loss_grad, which runs the passes, buffers and kernels of one round of the
 multinomial fit.
 
