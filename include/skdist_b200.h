@@ -96,6 +96,17 @@ int skd_stage_row_bits(skd_ctx* ctx, int32_t B, const uint8_t* label_bits, const
  * 1 / (C sw_sum).  ref: `class_weight` of LogisticRegression (SK/linear_model/_logistic.py:429-474). */
 int skd_stage_class_weights(skd_ctx* ctx, int32_t B, int32_t K, const float* w, const double* sw_sum);
 
+/* Per-row sample weights for the NEXT skd_logreg_fit_batch, skd_logreg_loss_grad,
+ * skd_logreg_multinomial_fit_batch or skd_logreg_multinomial_loss_grad call (one-shot, cleared by that call
+ * even when it fails; w = NULL clears).  w [n] float32, one per staged row, finite and >= 0; the call fails
+ * unless n equals the staged row count.  Every column of that call weighs training row i by w[i] times the
+ * class weight of the row's label in that column (a float32 product), so the call also needs class weights
+ * staged for it (all ones without class_weight): their sw_sum must be the sum of those products over the
+ * column's training rows.  Rows of weight 0 add nothing to the loss or the gradient.  The scoring entries do
+ * not use sample weights: scores stay unweighted.  ref: `sample_weight` of LogisticRegression.fit
+ * (SK/linear_model/_logistic.py:409-474), indexed by each fit's training rows (ref search.py:208-211). */
+int skd_stage_sample_weights(skd_ctx* ctx, const float* w, int64_t n);
+
 /* Class weights for the NEXT skd_forest_fit (classification; one-shot, cleared by that call even when it
  * fails; n_classes <= 0, or w = NULL without balanced_subsample, clears).  Tree t is fitted with
  * sample_weight count_i * cw[y_i]: w [n_classes] float64, finite and >= 0, the same for every tree, or

@@ -42,6 +42,7 @@ SYMBOLS = {
     "skd_stage_column_masks": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_void_p]),
     "skd_stage_row_bits": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_int64]),
     "skd_stage_class_weights": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_int32, _c.c_void_p, _c.c_void_p]),
+    "skd_stage_sample_weights": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int64]),
     "skd_stage_forest_class_weights": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_void_p, _c.c_int32, _c.c_double]),
     "skd_stage_forest_criterion": (_c.c_int, [_c.c_void_p, _c.c_int32]),
     "skd_logreg_fit_batch": (_c.c_int, [_c.c_void_p, _c.c_int32, _c.c_void_p, _c.c_void_p, _c.c_void_p,

@@ -348,7 +348,9 @@ static void free_staged(Ctx& c) {
   if (c.ycls) cudaFree(c.ycls);
   if (c.yreal) cudaFree(c.yreal);
   if (c.fold_store) cudaFree(c.fold_store);
+  if (c.roww) cudaFree(c.roww);
   c.X = nullptr; c.ycls = nullptr; c.yreal = nullptr; c.fold = nullptr; c.fold_store = nullptr;
+  c.roww = nullptr; c.roww_cap = 0;
 }
 
 int skd_ctx_destroy(skd_ctx* ctx) {
@@ -654,7 +656,7 @@ int skd_stage_row_bits(skd_ctx* ctx, int32_t B, const uint8_t* label_bits, const
   if (B <= 0 || (!label_bits && !train_bits)) return 0;   // cleared
   if (!c->X) return fail(c, "skd_stage_row_bits: stage X first");
   if (bytes_per_col * 8 < c->n) return fail(c, "skd_stage_row_bits: fewer bits per column than staged rows");
-  const int64_t words = (c->n + 63) / 64 * 2;              // whole 64-row tiles of the tensor-core path
+  const int64_t words = tc_padded_rows(c->n) / 32;         // whole tiles of the tensor-core path
   const int64_t use = std::min<int64_t>(bytes_per_col, (c->n + 7) / 8);
   auto pack = [&](const uint8_t* src, std::vector<uint32_t>& dst) {
     dst.assign((size_t)B * words, 0u);
@@ -691,6 +693,18 @@ int skd_stage_class_weights(skd_ctx* ctx, int32_t B, int32_t K, const float* w, 
   return 0;
 }
 
+int skd_stage_sample_weights(skd_ctx* ctx, const float* w, int64_t n) {
+  if (!ctx) return fail(nullptr, "skd_stage_sample_weights: ctx is NULL");
+  Ctx* c = &ctx->c;
+  c->sw = {};
+  if (!w) return 0;   // cleared
+  if (!c->X || n != c->n) return fail(c, "skd_stage_sample_weights: n does not match the staged X");
+  for (int64_t i = 0; i < n; ++i)
+    if (!(std::isfinite(w[i]) && w[i] >= 0.f)) return fail(c, "skd_stage_sample_weights: weights must be finite and >= 0");
+  c->sw.w.assign(w, w + n);
+  return 0;
+}
+
 int skd_stage_forest_class_weights(skd_ctx* ctx, int32_t n_classes, const double* w, int32_t balanced_subsample,
                                    double min_weight_fraction_leaf) {
   if (!ctx) return fail(nullptr, "skd_stage_forest_class_weights: ctx is NULL");
@@ -722,17 +736,98 @@ int skd_stage_forest_criterion(skd_ctx* ctx, int32_t criterion) {
   return 0;
 }
 
-// Staged class weights of binary columns: weights scaled by the power of two 2^-e that brings the larger one
-// into (1/2, 1], so that |G| <= 2^14 holds in the fp16 operand of the tensor-core gradient product; 2^e goes
-// into inv_n.  Both scalings are exact.  l2 = 1 / (C sw_sum), inv_n = 2^e / sw_sum
-// (SK/linear_model/_logistic.py:474, 580).
+// Staged sample weights a call consumes: they need class weights staged for the same call (those carry each
+// column's sw_sum) and the staged row count.  They are copied into the context's device buffer, zero padded to
+// the whole tiles the tensor-core kernel reads (tc_padded_rows); *droww stays nullptr when none are staged.
+static int upload_sample_weights(Ctx* c, const char* who, const StagedSampleWeights& sw, const StagedClassWeights& cw,
+                                 const float** droww) {
+  *droww = nullptr;
+  if (sw.w.empty()) return 0;
+  if (cw.cols <= 0)
+    return fail(c, std::string(who) + ": sample weights need class weights staged for the same call "
+                                      "(all ones without class_weight: they carry each column's sw_sum)");
+  if ((int64_t)sw.w.size() != c->n) return fail(c, std::string(who) + ": staged sample weights do not match the staged rows");
+  const int64_t npad = tc_padded_rows(c->n);
+  std::vector<float> h(sw.w);
+  h.resize((size_t)npad, 0.f);
+  if (stage_device_vector(c, c->roww, c->roww_cap, h.data(), npad)) return 1;
+  *droww = c->roww;
+  return 0;
+}
+
+// Largest sample weight of the training rows of every binary column, {label 0, label 1}, with the column's rows and
+// labels as the kernels form them: rows outside the held-out fold col_fold[j]; label 1 = class col_pos[j]; with
+// col_neg (pair columns, col_neg[j] >= 0) only the rows of class col_pos[j] or col_neg[j]; staged row bits
+// replace the training rows (bits->m) and the labels (bits->y).
+static int column_row_weight_max(Ctx* c, int B, const std::vector<float>& rw, const int32_t* col_fold,
+                                 const int32_t* col_pos, const int32_t* col_neg, const StagedRowBits* bits,
+                                 std::vector<float2>& mx) {
+  const int64_t n = c->n;
+  const bool have_bits = bits && bits->cols > 0;
+  if ((!have_bits || bits->y.empty()) && (int64_t)c->h_ycls.size() != n)
+    return fail(c, "sample weights: labels not staged");
+  mx.assign(B, make_float2(0.f, 0.f));
+  // largest weight per (fold, class): the folds of a row are 0 without staged folds
+  const int nf = c->h_fold.empty() ? 1 : c->n_folds;
+  const int lo = c->ycls_min, ncls = std::max(0, c->ycls_max - c->ycls_min + 1);
+  std::vector<float> cell;
+  if (!have_bits) {
+    cell.assign((size_t)nf * ncls, 0.f);
+    for (int64_t i = 0; i < n; ++i) {
+      const int f = c->h_fold.empty() ? 0 : (int)c->h_fold[i];
+      float& m = cell[(size_t)f * ncls + (c->h_ycls[i] - lo)];
+      m = std::max(m, rw[i]);
+    }
+  }
+  auto bit = [](const std::vector<uint32_t>& v, int64_t words, int j, int64_t i) {
+    return (v[(size_t)j * words + (i >> 5)] >> (i & 31)) & 1u;
+  };
+  for (int j = 0; j < B; ++j) {
+    float m0 = 0.f, m1 = 0.f;
+    if (have_bits) {   // row bits: one scan of the rows (the bit matrices exclude folds and pair columns)
+      for (int64_t i = 0; i < n; ++i) {
+        if (!bits->m.empty() && !bit(bits->m, bits->words, j, i)) continue;
+        const bool y1 = bits->y.empty() ? c->h_ycls[i] == col_pos[j] : bit(bits->y, bits->words, j, i) != 0;
+        float& m = y1 ? m1 : m0;
+        m = std::max(m, rw[i]);
+      }
+    } else {
+      const int neg = col_neg && col_neg[j] >= 0 ? col_neg[j] : INT32_MIN;
+      for (int f = 0; f < nf; ++f) {
+        if (!c->h_fold.empty() && f == col_fold[j]) continue;
+        for (int k = 0; k < ncls; ++k) {
+          const int cls = lo + k;
+          float& m = cls == col_pos[j] ? m1 : m0;
+          if (cls == col_pos[j] || neg == INT32_MIN || cls == neg) m = std::max(m, cell[(size_t)f * ncls + k]);
+        }
+      }
+    }
+    mx[j] = make_float2(m0, m1);
+  }
+  return 0;
+}
+
+// Staged class weights of binary columns: weights scaled by the power of two 2^-e that brings the largest row
+// factor into (1/2, 1], so that |G| <= 2^14 holds in the fp16 operand of the tensor-core gradient product; 2^e
+// goes into inv_n.  Both scalings are exact.  The row factor is the class weight of the row's label, times the
+// row's sample weight when those are staged (rw, host copy; the largest product over the column's training rows,
+// so that a column whose rows all weigh little does not sink into fp16 subnormals).  l2 = 1 / (C sw_sum),
+// inv_n = 2^e / sw_sum (SK/linear_model/_logistic.py:474, 580).
 static int binary_class_weights(Ctx* c, const char* who, const StagedClassWeights& cw, int B, const double* C,
-                                std::vector<float2>& hcw, std::vector<double>& l2, std::vector<double>& inv_n) {
+                                std::vector<float2>& hcw, std::vector<double>& l2, std::vector<double>& inv_n,
+                                const std::vector<float>* rw = nullptr, const int32_t* col_fold = nullptr,
+                                const int32_t* col_pos = nullptr, const int32_t* col_neg = nullptr,
+                                const StagedRowBits* bits = nullptr) {
   if (cw.cols != B || cw.k != 2) return fail(c, std::string(who) + ": staged class weights do not match this batch (B x 2)");
+  std::vector<float2> rmax;
+  if (rw && !rw->empty() && column_row_weight_max(c, B, *rw, col_fold, col_pos, col_neg, bits, rmax)) return 1;
   hcw.resize(B);
   for (int j = 0; j < B; ++j) {
-    const float mx = std::max(cw.w[2 * j], cw.w[2 * j + 1]);
-    if (!(mx > 0.f)) return fail(c, std::string(who) + ": every class weight of a column is 0");
+    float mx = std::max(cw.w[2 * j], cw.w[2 * j + 1]);
+    if (!rmax.empty()) mx = std::max(cw.w[2 * j] * rmax[j].x, cw.w[2 * j + 1] * rmax[j].y);   // float32 products
+    if (!(mx > 0.f))
+      return fail(c, std::string(who) + (rmax.empty() ? ": every class weight of a column is 0"
+                                                       : ": every weight of a column's training rows is 0"));
     int e;
     const float f = frexpf(mx, &e);   // mx = f 2^e, f in [1/2, 1)
     if (f == 0.5f) e -= 1;             // a power of two becomes exactly 1
@@ -885,6 +980,7 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
   if (!ctx) return fail(nullptr, "skd_logreg_fit_batch: ctx is NULL");
   Ctx* c = &ctx->c;
   const StagedClassWeights staged_cw = std::exchange(c->cw, {});
+  const StagedSampleWeights staged_sw = std::exchange(c->sw, {});
   const StagedMasks staged_masks = std::exchange(c->fmask, {});
   const StagedRowBits staged_bits = std::exchange(c->row_bits, {});
   if (!c->X || !c->ycls) return fail(c, "skd_logreg_fit_batch: stage X and labels first");
@@ -907,7 +1003,11 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
                          &mean_ntrain))
     return 1;
   std::vector<float2> hcw;
-  if (staged_cw.cols > 0 && binary_class_weights(c, "skd_logreg_fit_batch", staged_cw, B, C, hcw, l2, inv_n)) return 1;
+  const float* droww = nullptr;
+  if (upload_sample_weights(c, "skd_logreg_fit_batch", staged_sw, staged_cw, &droww)) return 1;
+  if (staged_cw.cols > 0 && binary_class_weights(c, "skd_logreg_fit_batch", staged_cw, B, C, hcw, l2, inv_n, &staged_sw.w,
+                                                 col_fold, col_pos, col_neg, &staged_bits))
+    return 1;
 
   Trace tr(c, "logreg_fit");
   Scratch sx(c);
@@ -931,6 +1031,7 @@ int skd_logreg_fit_batch(skd_ctx* ctx, int32_t B, const double* C, const int32_t
     SKD_CUDA(c, cudaMemcpyAsync(dcw, hcw.data(), B * sizeof(float2), cudaMemcpyHostToDevice, c->stream));
     c->h2d += (int64_t)B * 8;
     w.cw = dcw;
+    w.roww = droww;
   }
   const bool use_fmask = staged_masks.cols > 0;
   if (use_fmask) {
@@ -1074,6 +1175,7 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
   if (!ctx) return fail(nullptr, "skd_logreg_loss_grad: ctx is NULL");
   Ctx* c = &ctx->c;
   const StagedClassWeights staged_cw = std::exchange(c->cw, {});
+  const StagedSampleWeights staged_sw = std::exchange(c->sw, {});
   if (!c->X || !c->ycls) return fail(c, "skd_logreg_loss_grad: stage X and labels first");
   if (B <= 0 || !w_in || !C || !col_fold || !col_pos || !loss_out || !grad_out)
     return fail(c, "skd_logreg_loss_grad: bad arguments");
@@ -1088,7 +1190,11 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
     hw[(size_t)B * ldx + j] = fit_intercept ? (float)w_in[(size_t)j * dp + d] : 0.f;
   }
   std::vector<float2> hcw;
-  if (staged_cw.cols > 0 && binary_class_weights(c, "skd_logreg_loss_grad", staged_cw, B, C, hcw, l2, inv_n)) return 1;
+  const float* droww = nullptr;
+  if (upload_sample_weights(c, "skd_logreg_loss_grad", staged_sw, staged_cw, &droww)) return 1;
+  if (staged_cw.cols > 0 && binary_class_weights(c, "skd_logreg_loss_grad", staged_cw, B, C, hcw, l2, inv_n, &staged_sw.w,
+                                                 col_fold, col_pos))
+    return 1;
   Scratch sx(c);
   LogregWork w;
   LbfgsBatch& b = w.lb;
@@ -1098,6 +1204,7 @@ int skd_logreg_loss_grad(skd_ctx* ctx, int32_t B, const double* w_in, const doub
     SKD_CUDA(c, sx.alloc(&dcw, (size_t)B));
     SKD_CUDA(c, cudaMemcpyAsync(dcw, hcw.data(), B * sizeof(float2), cudaMemcpyHostToDevice, c->stream));
     w.cw = dcw;
+    w.roww = droww;
   }
   // the slot layout of skd_logreg_fit_batch: fold-grouped on the tensor cores, slot s = column s on SIMT
   std::vector<SlotMeta> hs;
@@ -1222,6 +1329,7 @@ int skd_logreg_multinomial_fit_batch(skd_ctx* ctx, int32_t B, int32_t n_classes,
   if (!ctx) return fail(nullptr, "skd_logreg_multinomial_fit_batch: ctx is NULL");
   Ctx* c = &ctx->c;
   const StagedClassWeights staged_cw = std::exchange(c->cw, {});
+  const StagedSampleWeights staged_sw = std::exchange(c->sw, {});
   const StagedMasks staged_masks = std::exchange(c->fmask, {});
   if (!c->X || !c->ycls) return fail(c, "skd_logreg_multinomial_fit_batch: stage X and labels first");
   if (B <= 0 || n_classes < 2 || !C || !col_fold || !coef_out || !n_iter_out || !status_out)
@@ -1232,12 +1340,15 @@ int skd_logreg_multinomial_fit_batch(skd_ctx* ctx, int32_t B, int32_t n_classes,
                             l2, inv_n))
     return 1;
   SKD_CUDA(c, cudaSetDevice(c->device));
+  const float* droww = nullptr;
+  if (upload_sample_weights(c, "skd_logreg_multinomial_fit_batch", staged_sw, staged_cw, &droww)) return 1;
   Trace tr(c, "multinomial_fit");
   DeviceTimer timer(c);
   if (timer.start()) return 1;
   if (multi_fit(c, B, n_classes, l2.data(), inv_n.data(), col_fold, fit_intercept, tol, max_iter,
                 staged_masks.cols > 0 ? staged_masks.mask.data() : nullptr,
-                staged_cw.cols > 0 ? staged_cw.w.data() : nullptr, coef_out, n_iter_out, status_out, loss_out, n_evals_out))
+                staged_cw.cols > 0 ? staged_cw.w.data() : nullptr, droww, coef_out, n_iter_out, status_out, loss_out,
+                n_evals_out))
     return 1;
   return timer.stop(gpu_seconds_out);
 }
@@ -1248,6 +1359,7 @@ int skd_logreg_multinomial_loss_grad(skd_ctx* ctx, int32_t B, int32_t n_classes,
   if (!ctx) return fail(nullptr, "skd_logreg_multinomial_loss_grad: ctx is NULL");
   Ctx* c = &ctx->c;
   const StagedClassWeights staged_cw = std::exchange(c->cw, {});
+  const StagedSampleWeights staged_sw = std::exchange(c->sw, {});
   const StagedMasks staged_masks = std::exchange(c->fmask, {});
   if (!c->X || !c->ycls) return fail(c, "skd_logreg_multinomial_loss_grad: stage X and labels first");
   if (B <= 0 || n_classes < 2 || !w_in || !C || !col_fold || !loss_out || !grad_out)
@@ -1257,6 +1369,8 @@ int skd_logreg_multinomial_loss_grad(skd_ctx* ctx, int32_t B, int32_t n_classes,
                             l2, inv_n))
     return 1;
   SKD_CUDA(c, cudaSetDevice(c->device));
+  const float* droww = nullptr;
+  if (upload_sample_weights(c, "skd_logreg_multinomial_loss_grad", staged_sw, staged_cw, &droww)) return 1;
   const int dp = (int)c->d + 1;
   std::vector<double> x(w_in, w_in + (size_t)B * n_classes * dp);
   if (!fit_intercept)   // the fit's intercepts stay at 0 without one
@@ -1264,7 +1378,7 @@ int skd_logreg_multinomial_loss_grad(skd_ctx* ctx, int32_t B, int32_t n_classes,
   Trace tr(c, "multinomial_loss_grad");
   return multi_loss_grad(c, B, n_classes, l2.data(), inv_n.data(), col_fold, fit_intercept,
                          staged_masks.cols > 0 ? staged_masks.mask.data() : nullptr,
-                         staged_cw.cols > 0 ? staged_cw.w.data() : nullptr, x.data(), loss_out, grad_out);
+                         staged_cw.cols > 0 ? staged_cw.w.data() : nullptr, droww, x.data(), loss_out, grad_out);
 }
 
 static int multinomial_check(Ctx* c, const char* who, int32_t B, int32_t n_classes, const float* coef,

@@ -30,7 +30,7 @@ __global__ void __launch_bounds__(256)
 mn_pointwise_kernel(float* __restrict__ G, int ldg, int64_t n, int64_t rpc, int K,
                     const SlotMeta* __restrict__ cand, const int32_t* __restrict__ n_act_dev, int n_act_in,
                     const int32_t* __restrict__ ycls, const int8_t* __restrict__ fold,
-                    double* __restrict__ lossp, const float* __restrict__ cw) {
+                    double* __restrict__ lossp, const float* __restrict__ cw, const float* __restrict__ roww) {
   __shared__ double red[8];
   const int a = blockIdx.x, z = blockIdx.y;
   if (a >= *n_act_dev) return;
@@ -55,8 +55,9 @@ mn_pointwise_kernel(float* __restrict__ G, int ldg, int64_t n, int64_t rpc, int 
     const float sum_f = (float)sum;
     float loss = (float)(log((double)sum_f) + (double)mx);
     loss -= zr[y];
-    if (wk) {   // sample weight of the row: float32 products, as SK/_loss/_loss.pyx.tp:1348-1350
-      const float sw = wk[y];
+    if (wk) {   // sample weight of the row: float32 products, as SK/_loss/_loss.pyx.tp:1348-1350; the class
+                // weight times the staged sample weight, as SK/linear_model/_logistic.py:436 forms it
+      const float sw = roww ? wk[y] * roww[r] : wk[y];
       for (int k = 0; k < K; ++k) {
         float p = (float)exp((double)zr[k] - (double)mx);
         p /= sum_f;
@@ -162,7 +163,7 @@ static int64_t candidates_per_pass(const Ctx* c, int K, int nz) {
 // held-out folds into *d_fold, feature masks, class weights), shared by multi_fit and multi_loss_grad.
 static int multi_pass_setup(Ctx* c, Scratch& sx, MultiWork& w, int64_t b0, int Bb, int K, int nz, int64_t rpc,
                             const double* l2, const double* inv_n, const int32_t* col_fold, const uint8_t* fmask,
-                            const float* cw, int32_t** d_fold) {
+                            const float* cw, const float* roww, int32_t** d_fold) {
   const int64_t n = c->n, ldx = c->ldx;
   LbfgsBatch& b = w.lb;
   b.B = Bb; b.K = K; b.n = K * ((int)c->d + 1); b.nz = nz; b.ldw = (int)ldx;
@@ -191,6 +192,7 @@ static int multi_pass_setup(Ctx* c, Scratch& sx, MultiWork& w, int64_t b0, int B
     SKD_CUDA(c, cudaMemcpyAsync(dcw, cw + (size_t)b0 * K, (size_t)Bb * K * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     c->h2d += (int64_t)Bb * K * 4;
     w.cw = dcw;
+    w.roww = roww;
   }
   return 0;
 }
@@ -203,14 +205,14 @@ static int multi_eval(Ctx* c, MultiWork& w, int n_act) {
   const int ns = n_act * b.K;
   if (simt_raw_prediction(c, ns, b.W, b.W + slots * c->ldx, w.G, w.ldg)) return 1;
   mn_pointwise_kernel<<<dim3(n_act, b.nz), 256, 0, c->stream>>>(w.G, w.ldg, c->n, w.rpc, b.K, b.slot, b.n_act, n_act,
-                                                               c->ycls, c->fold, b.lossp, w.cw);
+                                                               c->ycls, c->fold, b.lossp, w.cw, w.roww);
   mn_colsum_kernel<<<dim3((ns + 63) / 64, b.nz), 256, 0, c->stream>>>(w.G, w.ldg, c->n, w.rpc, ns, b.gsump);
   c->launches += 2;
   return simt_backward(c, w.G, w.ldg, ns, b.nz, w.rpc, b.gradp);
 }
 
 int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold, int fit_intercept,
-              double tol, int max_iter, const uint8_t* fmask, const float* cw, float* coef_out,
+              double tol, int max_iter, const uint8_t* fmask, const float* cw, const float* roww, float* coef_out,
               int32_t* n_iter_out, int32_t* status_out, double* loss_out, int32_t* n_evals_out) {
   int nz;
   int64_t rpc;
@@ -221,7 +223,7 @@ int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const
     Scratch sx(c);
     MultiWork w;
     int32_t* d_fold;
-    if (multi_pass_setup(c, sx, w, b0, Bb, K, nz, rpc, l2, inv_n, col_fold, fmask, cw, &d_fold)) return 1;
+    if (multi_pass_setup(c, sx, w, b0, Bb, K, nz, rpc, l2, inv_n, col_fold, fmask, cw, roww, &d_fold)) return 1;
     if (lbfgs_init(c, w.lb, d_fold, nullptr, nullptr, tol, max_iter)) return 1;
     if (lbfgs_run(c, w.lb, Bb, fit_intercept, max_iter, nullptr, nullptr,
                   [&](int n_act, long, int*) { return multi_eval(c, w, n_act); }, nullptr))
@@ -235,8 +237,8 @@ int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const
 // Objective and gradient at caller points w_in [B][K][d+1] (float64): the passes, set-up, evaluation and
 // gather of multi_fit's first round, with every candidate active in column order.
 int multi_loss_grad(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold,
-                    int fit_intercept, const uint8_t* fmask, const float* cw, const double* w_in, double* loss_out,
-                    double* grad_out) {
+                    int fit_intercept, const uint8_t* fmask, const float* cw, const float* roww, const double* w_in,
+                    double* loss_out, double* grad_out) {
   const int dp = (int)c->d + 1;
   int nz;
   int64_t rpc;
@@ -247,7 +249,7 @@ int multi_loss_grad(Ctx* c, int B, int K, const double* l2, const double* inv_n,
     Scratch sx(c);
     MultiWork w;
     int32_t* d_fold;
-    if (multi_pass_setup(c, sx, w, b0, Bb, K, nz, rpc, l2, inv_n, col_fold, fmask, cw, &d_fold)) return 1;
+    if (multi_pass_setup(c, sx, w, b0, Bb, K, nz, rpc, l2, inv_n, col_fold, fmask, cw, roww, &d_fold)) return 1;
     std::vector<SlotMeta> hc(Bb);
     for (int j = 0; j < Bb; ++j) { hc[j].col = j; hc[j].fold = col_fold[b0 + j]; hc[j].pos = 0; hc[j].pad = 0; }
     double *dx, *df, *dg;

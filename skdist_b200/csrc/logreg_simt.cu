@@ -54,7 +54,8 @@ fwd_kernel(const float* __restrict__ X, int64_t n, int ldx, const float* __restr
            double* __restrict__ gsump, int64_t* __restrict__ correct, int64_t* __restrict__ count,
            float* __restrict__ dec, int ldd, const float* __restrict__ yreal,
            const uint32_t* __restrict__ ybits = nullptr, const uint32_t* __restrict__ mbits = nullptr,
-           long long rb_words = 0, const float2* __restrict__ cw = nullptr) {
+           long long rb_words = 0, const float2* __restrict__ cw = nullptr,
+           const float* __restrict__ roww = nullptr) {
   __shared__ float As[TK][TM + 4];
   __shared__ float Bs[TK][TN + 4];
   __shared__ double red[16][TN + 1];
@@ -147,9 +148,11 @@ fwd_kernel(const float* __restrict__ X, int64_t n, int ldx, const float* __restr
             double y = ypos ? 1.0 : 0.0;
             double l, g;
             loss_grad_half_binomial(y, (double)raw, l, g);
-            if (cw) {   // the row's class weight times the double results (SK/_loss/_loss.pyx.tp:1083-1084)
+            if (cw) {   // the row's weight times the double results (SK/_loss/_loss.pyx.tp:1083-1084): its class
+                        // weight times its sample weight, a float32 product as SK/linear_model/_logistic.py:436 forms it
               const float2 wc = cw[scol[j]];
-              const double sw = (double)(ypos ? wc.y : wc.x);
+              const float cwl = ypos ? wc.y : wc.x;
+              const double sw = (double)(roww ? cwl * roww[gr] : cwl);
               l *= sw;
               g *= sw;
             }
@@ -307,7 +310,7 @@ int simt_eval(Ctx* c, LogregWork& w, int n_act, int* nz_used) {
   fwd_kernel<MODE_FIT><<<gf, 256, 0, c->stream>>>(
       c->X, c->n, ldx, w.lb.W, w.lb.W + (size_t)w.lb.B * ldx /*bias block*/, w.lb.slot, n_act, c->ycls,
       c->fold, rpc, w.G, w.ldg, w.lb.lossp, w.lb.gsump, nullptr, nullptr, nullptr, 0, nullptr, w.ybits, w.mbits,
-      (long long)w.rb_words, w.cw);
+      (long long)w.rb_words, w.cw, w.cw ? w.roww : nullptr);
   dim3 gb((ldx + 63) / 64, (n_act + TN - 1) / TN, nz);
   bwd_kernel<<<gb, 256, 0, c->stream>>>(c->X, c->n, ldx, w.G, w.ldg, n_act, rpc, w.lb.gradp);
   c->launches += 2;

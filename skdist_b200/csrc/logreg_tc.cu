@@ -37,7 +37,6 @@
 namespace skd {
 
 constexpr int TC_BC = 128;       // slots per group
-constexpr int TC_R = 64;         // rows per tile (the unit of the tile lists and row bit matrices)
 constexpr int TC_SUB = 32;       // rows per ring sub-tile (wgmma N of GEMM1, K of GEMM2)
 constexpr int TC_NCH = 132;      // fixed row chunks per group (one partial sum per (chunk, slot)); fixing it fixes
                                  // the summation order of every result
@@ -220,13 +219,16 @@ struct TcParams {
   int32_t* deal_log;         // nullptr, or {live groups, groups whose second half is padding, CTAs, CTAs whose
                              // range spans two or more groups} of this launch (the last entry zeroed by the caller)
   const float2* cw;          // TC_FIT_W / TC_FIT_UNI_W: per-column {label-0, label-1} class weights, largest <= 1
+  const float* roww;         // TC_FIT_W / TC_FIT_UNI_W: [npad] per-row sample weights (0 on padding), or nullptr:
+                             // every row weighs 1; cw is normalised so that the largest product over a column's
+                             // training rows is <= 1
 };
 
 // TC_FIT_UNI: fit where every slot of a group shares (held-out fold, positive class): the row's
 // sign/mask comes from a precomputed per-fold array instead of being decoded per element.
 // TC_FIT_W / TC_FIT_UNI_W: the same two fits with class weights (each row's loss and gradient entry
-// times its column's weight for the row's label), separate instantiations so that the unweighted
-// ones stay as they are.
+// times its column's weight for the row's label, and times the row's sample weight when those are
+// staged), separate instantiations so that the unweighted ones stay as they are.
 enum { TC_FIT = 0, TC_SCORE = 1, TC_R2 = 2, TC_FIT_UNI = 3, TC_FIT_W = 4, TC_FIT_UNI_W = 5 };
 
 // shared memory of one CTA: W_hi, W_lo [NCHUNK][128 slots x 64 fp16] + the ring of sub-tiles
@@ -584,6 +586,20 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
       reg_fence(zf);
 
       if constexpr (IS_FIT) {
+        // weighted fits: sample weights of this thread's 8 rows (1 when none are staged), loaded once GEMM1
+        // has completed: held through it beside the row data they make the widest fit spill
+        float rw[8];
+        if constexpr (WEIGHTED) {
+#pragma unroll
+          for (int q = 0; q < 8; ++q) rw[q] = 1.f;
+          if (prm.roww) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const float2 v = __ldg(reinterpret_cast<const float2*>(prm.roww + r0 + 8 * q + cq));
+              rw[2 * q] = v.x; rw[2 * q + 1] = v.y;
+            }
+          }
+        }
         float lt[2] = {0.f, 0.f}, gt[2] = {0.f, 0.f};
         float gv[16];
 #pragma unroll
@@ -607,8 +623,11 @@ tc_eval_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant
             sg = train ? (yb ? -GSCALE : GSCALE) : 0.f;
           }
           // factor of the row's loss and gradient entry: sg times the class weight of the row's label
-          // (label 1 exactly when sg < 0); the margin below keeps the unweighted sg
-          const float sgw = WEIGHTED ? sg * (sg < 0.f ? cwt[s].y : cwt[s].x) : sg;
+          // (label 1 exactly when sg < 0) times the row's sample weight, that product taken in float32
+          // as scikit-learn forms it (sample_weight *= class_weight_[y]); the margin below keeps the
+          // unweighted sg
+          float sgw = sg;
+          if constexpr (WEIGHTED) sgw = sg * ((sg < 0.f ? cwt[s].y : cwt[s].x) * rw[rr]);
           const float zp = fmaf(zf[i], zi[s], zb0[s]);
           const float uu = sg * zp;       // = -y * z
           const float e = ex2_approx(-fabsf(uu) * 1.4426950408889634f);
@@ -793,7 +812,7 @@ int tc_prepare(Ctx* c) {
   const int64_t n = c->n;
   const int d = (int)c->d, ldx = (int)c->ldx;
   const int dpad = (d + 63) / 64 * 64;
-  const int64_t npad = (n + TC_R - 1) / TC_R * TC_R;
+  const int64_t npad = tc_padded_rows(n);
   if (!t.x_valid) {
     if (t.Xh && (t.dpad != dpad || t.npad != npad)) tc_free(c);   // same shape restaged: keep the buffers
     if (!t.Xh) {
@@ -968,6 +987,7 @@ static int tc_run(Ctx* c, LogregWork& w, int n_act, int mode, int* nz_used, unsi
   prm.n_tiles_ld = n_tiles;
   if (mode == TC_R2 && !t.yreal_pad) return fail(c, "tc_r2: targets not staged");
   prm.cw = mode == TC_FIT ? w.cw : nullptr;
+  prm.roww = prm.cw ? w.roww : nullptr;
   const bool weighted = prm.cw != nullptr;
   cudaError_t e = (uni && weighted) ? tc_launch<TC_FIT_UNI_W>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)
                   : uni ? tc_launch<TC_FIT_UNI>(nchunk, grid, c->stream, t.map_xh, t.map_xl, map_wh, map_wl, prm)

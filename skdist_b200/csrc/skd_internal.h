@@ -19,6 +19,11 @@ struct DevBuf {
   size_t bytes = 0;
 };
 
+// Rows per tile of the tensor-core path (logreg_tc.cu): the unit of its tile lists and row bit matrices.  Its
+// per-row inputs (rowmeta, rowsg, the staged row bits and sample weights) cover npad = n rounded up to TC_R rows.
+constexpr int TC_R = 64;
+inline int64_t tc_padded_rows(int64_t n) { return (n + TC_R - 1) / TC_R * TC_R; }
+
 // fp16-split copy of the staged X for the tensor-core path (logreg_tc.cu)
 struct TcData {
   void* Xh = nullptr;          // [npad x dpad] fp16, X * xscale rounded to fp16
@@ -96,6 +101,9 @@ struct StagedClassWeights {   // skd_stage_class_weights: w [cols x k] weight of
   std::vector<double> sw_sum; // over its training rows
   int32_t cols = 0, k = 0;
 };
+struct StagedSampleWeights {  // skd_stage_sample_weights: w [n] per-row weight of every staged row (empty: none)
+  std::vector<float> w;
+};
 
 struct Ctx {
   int device = 0;
@@ -121,12 +129,15 @@ struct Ctx {
   ForestData forest;
   int64_t ycls_cap = 0, yreal_cap = 0, fold_cap = 0;   // allocated rows of the staged vectors (reused when large enough)
   int64_t vec_n = 0;        // row count the staged labels / targets / folds belong to (dropped when X changes it)
-  // one-shot staged inputs: read by skd_logreg_fit_batch (all three), skd_logreg_loss_grad (class
-  // weights), skd_logreg_multinomial_fit_batch (masks, class weights) and skd_forest_fit (forest_cw,
-  // n_classes == 0: none; forest_criterion, 0: Gini / MSE, 1: entropy)
+  // one-shot staged inputs: read by skd_logreg_fit_batch (all four), skd_logreg_loss_grad (class and
+  // sample weights), skd_logreg_multinomial_fit_batch (masks, class and sample weights) and skd_forest_fit
+  // (forest_cw, n_classes == 0: none; forest_criterion, 0: Gini / MSE, 1: entropy)
   StagedMasks fmask;
   StagedRowBits row_bits;
   StagedClassWeights cw;
+  StagedSampleWeights sw;
+  float* roww = nullptr;    // device copy of the sample weights a call consumes, [cap] zero padded (reused)
+  int64_t roww_cap = 0;
   ForestClassWeights forest_cw;
   int32_t forest_criterion = 0;
   // scratch pool: device blocks released by finished calls, reused by the next ones (Scratch below)
@@ -281,6 +292,9 @@ struct LogregWork {
   int64_t rb_words = 0;
   const float2* cw = nullptr;  // [B] or nullptr: {label-0, label-1} weights of column j, largest <= 1
                                // (the power of two that normalised them is folded into inv_n)
+  const float* roww = nullptr; // [npad] or nullptr: per-row sample weights, 0 on padding rows (only with cw;
+                               // cw is then normalised so that the largest product over a column's training
+                               // rows is <= 1)
   float* G = nullptr;          // [n x ldg] pointwise gradients (SIMT path)
   // tensor-core path (logreg_tc.cu)
   bool use_tc = false;
@@ -337,14 +351,15 @@ struct MultiWork {
   int32_t ldg = 0;               // leading dimension of G
   float* G = nullptr;            // [n x ldg] raw predictions, overwritten by the pointwise gradients
   const float* cw = nullptr;     // [B x K] or nullptr: weight of each class in the candidate's fit
+  const float* roww = nullptr;   // [n] or nullptr (device): sample weight of each row (only with cw)
 };
 int multi_fit(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold, int fit_intercept,
               double tol, int max_iter, const uint8_t* fmask /*[B x d] or nullptr*/,
-              const float* cw /*[B x K] or nullptr*/, float* coef_out, int32_t* n_iter_out,
-              int32_t* status_out, double* loss_out, int32_t* n_evals_out);
+              const float* cw /*[B x K] or nullptr*/, const float* roww /*device [n] or nullptr*/, float* coef_out,
+              int32_t* n_iter_out, int32_t* status_out, double* loss_out, int32_t* n_evals_out);
 int multi_loss_grad(Ctx* c, int B, int K, const double* l2, const double* inv_n, const int32_t* col_fold,
-                    int fit_intercept, const uint8_t* fmask, const float* cw, const double* w_in, double* loss_out,
-                    double* grad_out);
+                    int fit_intercept, const uint8_t* fmask, const float* cw, const float* roww, const double* w_in,
+                    double* loss_out, double* grad_out);
 int multi_score(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold, int64_t* conf_out);
 int logloss_batch(Ctx* c, int B, int K, const float* coef, const int32_t* col_fold, const int32_t* col_pos,
                   double* loss_sum_out, int64_t* count_out);

@@ -269,15 +269,47 @@ def _metric_from_counts(kind, correct, count, pred_pos, actual_pos):
     raise ValueError(kind)
 
 
+def _fit_sample_weight(estimator, fit_params, n_samples):
+    """The float32 `sample_weight` a fit of `estimator` takes from `fit_params`, checked as LogisticRegression.fit
+    checks it (SK/utils/validation.py _check_sample_weight: length, finite values), or None.  Every other
+    key raises the TypeError that LogisticRegression.fit raises for it.  The device restriction: weights
+    must be >= 0 (ValueError).  Only LogisticRegression has a weighted device path: fit_params for any other
+    estimator raise NotImplementedError."""
+    if not fit_params:
+        return None
+    from sklearn.linear_model import LogisticRegression
+    if type(estimator) is not LogisticRegression:
+        raise NotImplementedError("fit_params %s of %s are not supported on the device path (sample_weight: "
+                                  "LogisticRegression only)" % (sorted(fit_params), type(estimator).__name__))
+    for key in fit_params:
+        if key != "sample_weight":
+            raise TypeError("LogisticRegression.fit() got an unexpected keyword argument %r" % key)
+    sw = fit_params["sample_weight"]
+    if sw is None:
+        return None
+    from sklearn.utils.validation import _check_sample_weight
+    sw = _check_sample_weight(sw, np.empty((n_samples, 0), dtype=np.float32), dtype=np.float32, copy=True)
+    if np.any(sw < 0):
+        raise ValueError("sample_weight must be >= 0 on the device path (negative weights make the logistic "
+                         "objective non-convex)")
+    return sw
+
+
 class _ClassWeights:
     """Per-column class weights of LogisticRegression(class_weight=...) fits, as
     SK/linear_model/_logistic.py:409-474 forms them: compute_class_weight on the labels of the fit's own
-    training rows (classes = the labels present there), cast to float32, and sw_sum = the float32 sum of
-    the per-row weights in the order of those rows.  Weights depend on (class_weight, held-out fold) only."""
+    training rows (classes = the labels present there; with sample weights, "balanced" counts them), cast to
+    float32, and sw_sum = the float32 sum of the per-row weights (sample weight times class weight, a float32
+    product) in the order of those rows.  Weights depend on (class_weight, held-out fold) only."""
 
     def __init__(self, classes, y_class):
         self.classes, self.y_class = classes, y_class
         self.fold, self.train_rows, self.cache = None, None, {}
+        self.sample_weight = None
+
+    def set_sample_weight(self, sample_weight):
+        """float32 sample weight of every row (None: none); each fit takes those of its training rows."""
+        self.sample_weight, self.cache = sample_weight, {}
 
     def set_folds(self, fold, train_rows=None):
         """fold ids of the staged layout; train_rows[f] = training rows of local fold f in the splitter's
@@ -295,35 +327,57 @@ class _ClassWeights:
         """(float32 weight of every class id, sw_sum) of a fit on the training rows of fold f (-1: all rows)."""
         key = (repr(class_weight), int(f))
         if key not in self.cache:
-            self.cache[key] = _fit_class_weights(class_weight, self.y_class[self._train(f)], self.classes)
+            rows = self._train(f)
+            sw = None if self.sample_weight is None else self.sample_weight[rows]
+            self.cache[key] = _fit_class_weights(class_weight, self.y_class[rows], self.classes, sw)
         return self.cache[key]
 
     def stage(self, eng, class_weights, folds):
-        """Stage the weights of columns (class_weight, held-out fold) for the next fit; nothing when no
-        column is weighted (the unweighted kernels then run)."""
-        if all(cw is None for cw in class_weights):
+        """Stage the weights of columns (class_weight, held-out fold) for the next fit, and the sample weights
+        when there are any; nothing when no column is weighted (the unweighted kernels then run)."""
+        if self.sample_weight is None and all(cw is None for cw in class_weights):
             return
-        _stage_columns(eng, [self.column(cw, f) for cw, f in zip(class_weights, folds)])
+        _stage_columns(eng, [self.column(cw, f) for cw, f in zip(class_weights, folds)], self.sample_weight)
 
 
-def _fit_class_weights(class_weight, ids, classes):
+def _fit_class_weights(class_weight, ids, classes, sw=None):
     """(float32 weight of every class id, sw_sum) of ONE fit whose training rows, in the fit's order, carry
-    the class ids `ids` (labels classes[ids]): what SK/linear_model/_logistic.py:409-474 forms from
-    class_weight (classes = the labels present in the fit, weights cast to float32, sw_sum = the float32
-    sum of the per-row weights).  Errors of compute_class_weight propagate."""
+    the class ids `ids` (labels classes[ids]) and the float32 sample weights `sw` (None: none): what
+    SK/linear_model/_logistic.py:409-474 forms from class_weight and sample_weight (classes = the labels
+    present in the fit, compute_class_weight with the fit's sample weights, weights cast to float32, sw_sum =
+    the float32 sum of the per-row weights sw * class_weight_[y]).  Errors of compute_class_weight propagate;
+    sample weights that sum to 0 over the fit's rows raise ValueError."""
     from sklearn.utils.class_weight import compute_class_weight
     w = np.ones(len(classes), dtype=np.float32)
     if class_weight is None:
-        return w, float(len(ids))
-    present = np.unique(ids)
-    w[:] = 0.0      # a class without training rows carries no weight
-    w[present] = compute_class_weight(class_weight, classes=classes[present], y=classes[ids]).astype(np.float32)
-    return w, float(np.sum(w[ids]))
+        if sw is None:
+            return w, float(len(ids))
+        rw = sw
+    else:
+        present = np.unique(ids)
+        w[:] = 0.0      # a class without training rows carries no weight
+        w[present] = compute_class_weight(class_weight, classes=classes[present], y=classes[ids],
+                                          sample_weight=sw).astype(np.float32)
+        rw = w[ids] if sw is None else sw * w[ids]
+    sw_sum = float(np.sum(rw))
+    if sw is not None and not sw_sum > 0:
+        raise ValueError("the sample weights of a fit's training rows sum to %r: a fit needs a positive sum" % sw_sum)
+    return w, sw_sum
 
 
-def _stage_columns(eng, cols):
-    """Stage [(weights, sw_sum)] of the columns of the next fit."""
-    eng.stage_class_weights(np.stack([c[0] for c in cols]), np.array([c[1] for c in cols]))
+def _stage_columns(eng, cols, sample_weight=None):
+    """Stage [(weights, sw_sum)] of the columns of the next fit, and the float32 sample weights of every staged
+    row when not None.  If a staging call fails, both are cleared: staged inputs are one-shot, and class weights
+    without the sample weights they were summed over must not reach a later fit."""
+    try:
+        eng.stage_class_weights(np.stack([c[0] for c in cols]), np.array([c[1] for c in cols]))
+        if sample_weight is not None:
+            eng.stage_sample_weights(sample_weight)
+    except Exception:
+        eng.stage_class_weights(None, None)
+        if sample_weight is not None:
+            eng.stage_sample_weights(None)
+        raise
 
 
 class _LogRegFamily:
@@ -373,6 +427,11 @@ class _LogRegFamily:
         else:
             self.pos_in_fold = np.zeros(n_splits, dtype=np.int64)
             self.total_pos = 0
+
+    def set_sample_weight(self, sample_weight):
+        """float32 sample weight of every row (None: none), indexed by each fit's training rows as the
+        reference indexes fit_params (ref search.py:208-211); the refit takes all of them."""
+        self.weights.set_sample_weight(sample_weight)
 
     def set_train_rows(self, train_rows):
         """Training rows of every fold of the staged layout in the splitter's order (None entries: the

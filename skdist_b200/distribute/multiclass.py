@@ -147,9 +147,11 @@ class DistOneVsRestClassifier(_ScParamMixin, OneVsRestClassifier):
         `mlb_override`, ref :267-274) and `max_negatives` (ref `_negatives_mask`, :76-106) give every
         column its own 0/1 label vector / training-row set: both go to the device as bit matrices
         (`Engine.stage_row_bits`), no `X[rows]` copies.  `n_splits` only cuts X into broadcast pieces in
-        the reference (`_split_X`, :35-50) and has no effect here."""
-        if fit_params:
-            raise NotImplementedError("fit_params are not supported on the device path")
+        the reference (`_split_X`, :35-50) and has no effect here.
+
+        fit_params: `sample_weight` of a LogisticRegression base.  As in the reference (:145-151), every
+        label column's fit takes the full array; with `max_negatives` dropping rows that is a fit on fewer
+        rows than weights, which raises the ValueError scikit-learn raises for it."""
         _check_estimator(self, verbose=self.verbose)
         from collections.abc import Sequence
         if (not self.mlb_override and not hasattr(y[0], "__array__") and isinstance(y[0], Sequence)
@@ -166,6 +168,8 @@ class DistOneVsRestClassifier(_ScParamMixin, OneVsRestClassifier):
         n, d = X_arr.shape
         _parse_partitions(self.partitions, K)
         base = self.estimator
+        from .logreg_family import _fit_sample_weight
+        sample_weight = _fit_sample_weight(base, fit_params, n)
         multilabel = y_arr.ndim == 2
         use_bits = multilabel or self.max_negatives is not None
         if use_bits and type(base) is not LogisticRegression:
@@ -211,16 +215,29 @@ class DistOneVsRestClassifier(_ScParamMixin, OneVsRestClassifier):
                 if self.max_negatives is not None:
                     train = np.stack([_negatives_rows(labels[i], self.max_negatives, self.random_state, self.method)
                                       for i in range(len(mine))])
-                eng.stage_row_bits(labels if multilabel else None, train)
-            if p["class_weight"] is not None and len(mine):
+            # every refusal comes before the first staging call, so that no staged input outlives a refused fit
+            if sample_weight is not None and train is not None:
+                from sklearn.utils.validation import _check_sample_weight
+                for i in range(len(mine)):
+                    if not train[i].all():     # the full-length weights of a fit on fewer rows (ref :141-151)
+                        _check_sample_weight(sample_weight, np.empty((int(train[i].sum()), 0), np.float32))
+            cols = []
+            if (p["class_weight"] is not None or sample_weight is not None) and len(mine):
                 # every column's binary fit: its 0/1 labels on its training rows (ascending), as _fit_binary
-                # hands them to the estimator (ref multiclass.py:141-151)
-                cols = []
+                # hands them to the estimator (ref multiclass.py:141-151), with the sample weights of all rows
                 for i, k in enumerate(mine):
                     y01 = labels[i] if labels is not None else ycls == k
                     rows = np.flatnonzero(train[i]) if train is not None else slice(None)
-                    cols.append(_fit_class_weights(p["class_weight"], y01[rows].astype(np.intp), np.array([0, 1])))
-                _stage_columns(eng, cols)
+                    cols.append(_fit_class_weights(p["class_weight"], y01[rows].astype(np.intp), np.array([0, 1]),
+                                                   None if sample_weight is None else sample_weight[rows]))
+            try:
+                if labels is not None:
+                    eng.stage_row_bits(labels if multilabel else None, train)
+                if cols:
+                    _stage_columns(eng, cols, sample_weight)
+            except Exception:
+                eng.stage_row_bits(None, None)     # staged inputs are one-shot: none outlives a failed staging
+                raise
             res = eng.logreg_fit_batch(np.full(len(mine), p["C"]), np.full(len(mine), -1, np.int32),
                                        mine.astype(np.int32), fit_intercept=p["fit_intercept"],
                                        tol=p["tol"], max_iter=p["max_iter"])

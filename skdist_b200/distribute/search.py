@@ -46,7 +46,7 @@ __all__ = ["DistGridSearchCV", "DistRandomizedSearchCV", "DistMultiModelSearch"]
 
 
 from .folds import _cv_fold_groups, _cv_fold_ids, _encode_target
-from .logreg_family import _check_engine_entries, _LogRegFamily, _MultinomialFamily
+from .logreg_family import _check_engine_entries, _fit_sample_weight, _LogRegFamily, _MultinomialFamily
 
 
 # ----------------------------------------------------------------------------------------
@@ -76,9 +76,12 @@ class DistBaseSearchCV(_ScParamMixin):
     """Same role as the reference's DistBaseSearchCV (search.py:291-581)."""
 
     def fit(self, X, y=None, groups=None, **fit_params):
-        """Run fit with all sets of parameters (ref search.py:315-571)."""
-        if fit_params:
-            raise NotImplementedError("fit_params are not supported on the device path")
+        """Run fit with all sets of parameters (ref search.py:315-571).
+
+        fit_params: `sample_weight` of a LogisticRegression base (any other key raises the TypeError of
+        LogisticRegression.fit; other bases raise NotImplementedError).  As in the reference, each
+        (candidate, fold) fit takes the weights of its training rows (ref search.py:208-211) and the refit
+        takes all of them (:548); the scores stay unweighted (:264)."""
         _check_estimator(self, verbose=self.verbose)
         estimator = self.estimator
         cv = check_cv(self.cv, y, classifier=is_classifier(estimator))
@@ -102,6 +105,7 @@ class DistBaseSearchCV(_ScParamMixin):
             raise ValueError("X must be a 2-d array")
         y_arr = np.asarray(y)
         n_samples, n_features = X_arr.shape
+        sample_weight = _fit_sample_weight(estimator, fit_params, n_samples)
         # the host-to-device copy of X (the C-ABI call releases the GIL) runs while the host draws the
         # candidates (ParameterSampler: one scipy rvs call per candidate), computes the cv splits and
         # validates the candidates
@@ -123,6 +127,8 @@ class DistBaseSearchCV(_ScParamMixin):
                 fold = layouts[0][0]
                 family = _pick_family(estimator, candidate_params, X_arr, y_arr, scorers, enc)
                 _check_engine_entries(family, eng)
+                if sample_weight is not None:
+                    family.set_sample_weight(sample_weight)
                 if self.refit and self.preds and not hasattr(family, "fold_proba"):
                     raise NotImplementedError("preds=True has no device path for %s" % type(estimator).__name__)
                 if hasattr(family, "prepare"):      # host-only statistics of the folds (no engine calls)

@@ -171,6 +171,17 @@ class Engine:
         assert w.ndim == 2 and sw_sum.shape == (w.shape[0],)
         check(self._lib.skd_stage_class_weights(self._h, w.shape[0], w.shape[1], ptr(w), ptr(sw_sum)), self._h)
 
+    def stage_sample_weights(self, w):
+        """[n] float32 per-row sample weights consumed by the next logreg_fit_batch / logreg_loss_grad /
+        logreg_multinomial_fit_batch / logreg_multinomial_loss_grad, together with the class weights staged for
+        that call (whose sw_sum must include them).  Scores stay unweighted.  None clears."""
+        if w is None:
+            check(self._lib.skd_stage_sample_weights(self._h, None, 0), self._h)
+            return
+        w = np.ascontiguousarray(w, dtype=np.float32)
+        assert w.ndim == 1
+        check(self._lib.skd_stage_sample_weights(self._h, ptr(w), w.shape[0]), self._h)
+
     def logreg_fit_batch(self, C, col_fold, col_pos, fit_intercept=True, tol=1e-4, max_iter=100, col_neg=None):
         """B binary lbfgs fits sharing the staged X.  col_neg[j] >= 0 restricts column j to the rows
         of class col_pos[j] / col_neg[j] (one-vs-one pair); None or < 0 = one-vs-rest."""
