@@ -253,6 +253,19 @@ static double weighted_class_sums(const T* count, int C, const double* cw, doubl
   return w;
 }
 
+// MSE impurity and value of a regression node from its own statistics s = {sum w, sum w y, sum w y^2}:
+// sq / w - (sum / w)^2 and sum / w (SK/tree/_criterion.pyx MSE node_impurity / node_value), the builder's
+// operations (fo_children_mse).  A right child's statistics are the parent's minus the left child's, and
+// w_right = w_node - w_left is the same subtraction: they are the operands the builder used for the right
+// child at the parent, so the impurity is the one it compared with EPSILON.
+static double mse(const double* s, double* value) {
+  const volatile double mean = s[1] / s[0];
+  const volatile double q = s[2] / s[0];
+  const volatile double mm = mean * mean;      // volatile: no contraction of the product into the difference
+  *value = mean;
+  return q - mm;
+}
+
 // The impurity array of a classification tree (Gini, or entropy in bits) from its integer class sums, as the
 // builders and scikit-learn form it.  A node's impurity is the one its parent's children_impurity formed: for
 // the root (node_impurity) and a left child from the node's own sums; for a right child from sum_right_c =
@@ -260,24 +273,30 @@ static double weighted_class_sums(const T* count, int C, const double* cw, doubl
 // the last bits from the right child's own sums; the tree reports the impurity the builder compared with
 // EPSILON and used in the improvement.  Entropy uses this process's libm, the one scikit-learn calls: the
 // builder ranks candidates with CUDA's log, which differs from the host's in the last bit on a few inputs.
-// sums(i): node i's C class sums; children(i, l, r): node i's children, false for a leaf.
-template <class Sums, class Children>
-static void forest_class_impurity(int m, int C, const double* cw, bool entropy, Sums sums, Children children,
-                                  double* imp) {
+// node_sums(i, s): node i's C float64 class sums into s, returns their total (weighted_class_sums);
+// children(i, l, r): node i's children, false for a leaf.
+template <class NodeSums, class Children>
+static void forest_class_impurity(int m, int C, bool entropy, NodeSums node_sums, Children children, double* imp) {
   if (m <= 0) return;
   auto impurity = [&](const double* s, double w) { return entropy ? entropy_bits(s, C, w) : gini(s, C, w); };
   std::vector<double> s(C), t(C);
-  imp[0] = impurity(s.data(), weighted_class_sums(sums(0), C, cw, s.data()));
+  imp[0] = impurity(s.data(), node_sums(0, s.data()));
   for (int i = 0; i < m; ++i) {
     int l, r;
     if (!children(i, l, r)) continue;
-    const double wn = weighted_class_sums(sums(i), C, cw, t.data());
-    const double wl = weighted_class_sums(sums(l), C, cw, s.data());
+    const double wn = node_sums(i, t.data());
+    const double wl = node_sums(l, s.data());
     imp[l] = impurity(s.data(), wl);
     for (int c = 0; c < C; ++c) { const volatile double b = t[c] - s[c]; s[c] = b; }
     const volatile double wr = wn - wl;
     imp[r] = impurity(s.data(), wr);
   }
+}
+
+// The C integer class sums of a classification node record (forest_common.h), widened to 64 bits
+static void record_class_sums(const uint32_t* r, int kind, int C, unsigned long long* s) {
+  if (kind == FOREST_REC_FAST) for (int c = 0; c < C; ++c) s[c] = r[4 + c];
+  else memcpy(s, r + 6, (size_t)C * sizeof(*s));
 }
 
 extern "C" {
@@ -1604,51 +1623,30 @@ int skd_sgd_fit_groups(skd_ctx* ctx, int32_t B, const int32_t* col_pos, const in
 
 struct skd_forest {
   struct Tree {
-    int32_t max_depth = 0, n_classes = 0, node_count = 0;
-    std::vector<int32_t> left, right, feature, nsamp;
-    std::vector<uint8_t> mgl;
-    std::vector<double> thr, imp, wn, val;
-    std::vector<uint32_t> compact;     // 8 words per node (throughput builder); expanded by skd_forest_tree_copy
-    std::vector<double> cw;            // class weights the tree was built with (compact records of a weighted fit)
+    int32_t max_depth = 0, n_classes = 0, node_count = 0, kind = 0;
+    std::vector<uint32_t> records;     // node_count node records of `kind` (forest_common.h)
+    std::vector<double> cw;            // class weights the tree was built with (weighted classification fits)
   };
   std::vector<Tree> trees;
   ForestClassWeights cw;               // staged for the fit (n_classes == 0: unweighted)
   int32_t criterion = 0;               // staged for the fit: 0 Gini / MSE, 1 entropy
-  std::vector<float> binval;           // [d][256] distinct feature values (thresholds of compact records)
+  std::vector<float> binval;           // [d][256] distinct feature values (thresholds of FOREST_REC_FAST records)
 };
 
 static void forest_sink(void* arg, int t, const SkdTreeView* v) {
   skd_forest* f = (skd_forest*)arg;
   skd_forest::Tree& tr = f->trees[t];
-  const int m = v->node_count;
-  tr.max_depth = v->max_depth; tr.n_classes = v->n_classes; tr.node_count = m;
-  // the class weights the tree was built with, for the impurity formed from its class sums
-  std::vector<double> cw;
-  if (f->cw.n_classes && m > 0 && (v->compact || v->class_sums)) {
-    cw = f->cw.w;
+  const int m = v->node_count, C = v->n_classes;
+  tr.max_depth = v->max_depth; tr.n_classes = C; tr.node_count = m; tr.kind = v->kind;
+  tr.records.assign(v->records, v->records + (size_t)m * (forest_record_bytes(v->kind, C) / 4));
+  if (f->cw.n_classes && m > 0) {
+    tr.cw = f->cw.w;
     if (f->cw.balanced_subsample) {   // the root's class sums are the bootstrap class counts
-      std::vector<uint32_t> root(v->n_classes);
-      for (int c = 0; c < v->n_classes; ++c) root[c] = v->compact ? v->compact[4 + c] : (uint32_t)v->class_sums[c];
-      cw.resize(v->n_classes);
-      forest_subsample_weights(root.data(), v->n_classes, cw.data());
+      unsigned long long root[16];
+      record_class_sums(v->records, v->kind, C, root);
+      tr.cw.resize(C);
+      forest_subsample_weights(root, C, tr.cw.data());
     }
-  }
-  if (v->compact) {
-    tr.compact.assign(v->compact, v->compact + (size_t)m * 8);
-    tr.cw = std::move(cw);
-    return;
-  }
-  tr.left.assign(v->left, v->left + m); tr.right.assign(v->right, v->right + m);
-  tr.feature.assign(v->feature, v->feature + m); tr.nsamp.assign(v->n_node_samples, v->n_node_samples + m);
-  tr.mgl.assign(v->missing_go_to_left, v->missing_go_to_left + m);
-  tr.thr.assign(v->threshold, v->threshold + m); tr.imp.assign(v->impurity, v->impurity + m);
-  tr.wn.assign(v->weighted_n_node_samples, v->weighted_n_node_samples + m);
-  tr.val.assign(v->value, v->value + (size_t)m * v->n_classes);
-  if (v->class_sums) {   // entropy trees: the builder's impurity was formed with CUDA's log
-    const int C = v->n_classes;
-    forest_class_impurity(
-        m, C, cw.empty() ? nullptr : cw.data(), true, [&](int i) { return v->class_sums + (size_t)i * C; },
-        [&](int i, int& l, int& r) { l = v->left[i]; r = v->right[i]; return l >= 0; }, tr.imp.data());
   }
 }
 
@@ -1696,71 +1694,68 @@ int skd_forest_tree_size(skd_forest* f, int32_t tree, int32_t* node_count, int32
   return 0;
 }
 
+// Expands the node records (forest_common.h) with the builders' (= scikit-learn's) operations:
+//   threshold    FOREST_REC_FAST: v[a] / 2 + v[b] / 2 of the two bins (SK/tree/_splitter.pyx:459-461); else the stored float64
+//   missing_go_to_left = n_left > n_right (best_split.missing_go_to_left with no missing values)
+//   classification: weighted_n = sum_c s_c, value_c = s_c / weighted_n with s_c = cw_c * count_c
+//                   (weighted_class_sums); impurity as forest_class_impurity forms it
+//   regression:     the node's own statistics (mse)
 int skd_forest_tree_copy(skd_forest* f, int32_t tree, int32_t* left, int32_t* right, int32_t* feature,
                          double* threshold, double* impurity, int32_t* n_node_samples,
                          double* weighted_n_node_samples, uint8_t* missing_go_to_left, double* value) {
   if (!f || tree < 0 || tree >= (int)f->trees.size()) return fail(nullptr, "skd_forest_tree_copy: bad arguments");
   const skd_forest::Tree& t = f->trees[tree];
-  if (!t.compact.empty()) {
-    // Compact records of the throughput builder: {right child, feature | bin_a << 16 | bin_b << 24,
-    // n_node_samples, depth, class sums[4]}, nodes in depth-first order (left child = id + 1).  The
-    // float64 fields are formed here with the builder's (= scikit-learn's) operations:
-    //   weighted_n = sum_c s_c;  value_c = s_c / weighted_n                     (weighted_class_sums)
-    //   impurity   = Gini, as forest_class_impurity forms it
-    //   threshold  = v[a] / 2 + v[b] / 2                                        (SK/tree/_splitter.pyx:459-461)
-    const size_t m = (size_t)t.node_count;
-    const int C = t.n_classes;
-    const uint32_t* r = t.compact.data();
-    const float* bv = f->binval.data();
-    const double* cw = t.cw.empty() ? nullptr : t.cw.data();
-    for (size_t i = 0; i < m; ++i, r += 8) {
-      const int32_t rc = (int32_t)r[0];
-      const uint32_t code = r[1];
-      const bool leaf = (code & 0xFFFFu) == 0xFFFFu;
-      if (left) left[i] = leaf ? -1 : (int32_t)i + 1;
-      if (right) right[i] = leaf ? -1 : rc;
-      if (feature) feature[i] = leaf ? -2 : (int32_t)(code & 0xFFFFu);
-      if (threshold) {
-        if (leaf) threshold[i] = -2.0;
-        else {
-          const size_t fo = (size_t)(code & 0xFFFFu) * 256;
-          const volatile double ha = (double)bv[fo + ((code >> 16) & 0xFF)] / 2.0;
-          const volatile double hb = (double)bv[fo + ((code >> 24) & 0xFF)] / 2.0;
-          threshold[i] = ha + hb;
-        }
+  const int m = t.node_count, C = t.n_classes;
+  const bool fast = t.kind == FOREST_REC_FAST, reg = t.kind == FOREST_REC_REG;
+  const size_t rw = forest_record_bytes(t.kind, C) / 4;
+  const uint32_t* rec = t.records.data();
+  const float* bv = f->binval.data();
+  const double* cw = t.cw.empty() ? nullptr : t.cw.data();
+  auto children = [&](int i, int& l, int& r) {
+    const uint32_t* p = rec + (size_t)i * rw;
+    l = i + 1;
+    r = (int32_t)p[0];
+    return (p[1] & 0xFFFFu) != 0xFFFFu && r > 0;
+  };
+  auto node_sums = [&](int i, double* s) {
+    unsigned long long cnt[16];
+    record_class_sums(rec + (size_t)i * rw, t.kind, C, cnt);
+    return weighted_class_sums(cnt, C, cw, s);
+  };
+  for (int i = 0; i < m; ++i) {
+    const uint32_t* r = rec + (size_t)i * rw;
+    int l, rc;
+    const bool split = children(i, l, rc);
+    if (left) left[i] = split ? l : -1;
+    if (right) right[i] = split ? rc : -1;
+    if (feature) feature[i] = split ? (int32_t)(r[1] & 0xFFFFu) : -2;
+    if (threshold) {
+      if (!split) threshold[i] = -2.0;
+      else if (fast) {
+        const size_t fo = (size_t)(r[1] & 0xFFFFu) * 256;
+        const volatile double ha = (double)bv[fo + ((r[1] >> 16) & 0xFF)] / 2.0;
+        const volatile double hb = (double)bv[fo + ((r[1] >> 24) & 0xFF)] / 2.0;
+        threshold[i] = ha + hb;
+      } else {
+        memcpy(&threshold[i], r + 4, sizeof(double));
       }
-      if (n_node_samples) n_node_samples[i] = (int32_t)r[2];
-      if (missing_go_to_left) missing_go_to_left[i] = 0;
-      double s[4];
-      const double w = weighted_class_sums(r + 4, C, cw, s);
-      if (weighted_n_node_samples) weighted_n_node_samples[i] = w;
-      if (value) for (int c = 0; c < C; ++c) value[i * C + c] = s[c] / w;
     }
-    const uint32_t* rec = t.compact.data();
-    auto children = [&](int i, int& l, int& rc) {
-      rc = (int32_t)rec[(size_t)i * 8];
-      l = i + 1;
-      return (rec[(size_t)i * 8 + 1] & 0xFFFFu) != 0xFFFFu && rc > 0;
-    };
-    if (impurity)
-      forest_class_impurity((int)m, C, cw, false, [&](int i) { return rec + (size_t)i * 8 + 4; }, children, impurity);
-    if (missing_go_to_left) {      // n_left > n_right (SK/tree/_splitter.pyx: best_split.missing_go_to_left with no missing values)
-      int l, rc;
-      for (size_t i = 0; i < m; ++i)
-        if (children((int)i, l, rc)) missing_go_to_left[i] = rec[(size_t)l * 8 + 2] > rec[(size_t)rc * 8 + 2] ? 1 : 0;
+    if (n_node_samples) n_node_samples[i] = (int32_t)r[2];
+    if (missing_go_to_left) missing_go_to_left[i] = split && rec[(size_t)l * rw + 2] > rec[(size_t)rc * rw + 2];
+    double s[16], w, v;
+    if (reg) {
+      memcpy(s, r + 6, 3 * sizeof(double));
+      w = s[0];
+      const double imp = mse(s, &v);
+      if (impurity) impurity[i] = imp;
+      if (value) value[i] = v;
+    } else {
+      w = node_sums(i, s);
+      if (value) for (int c = 0; c < C; ++c) value[(size_t)i * C + c] = s[c] / w;
     }
-    return 0;
+    if (weighted_n_node_samples) weighted_n_node_samples[i] = w;
   }
-  const size_t m = t.left.size();
-  if (left) memcpy(left, t.left.data(), m * 4);
-  if (right) memcpy(right, t.right.data(), m * 4);
-  if (feature) memcpy(feature, t.feature.data(), m * 4);
-  if (threshold) memcpy(threshold, t.thr.data(), m * 8);
-  if (impurity) memcpy(impurity, t.imp.data(), m * 8);
-  if (n_node_samples) memcpy(n_node_samples, t.nsamp.data(), m * 4);
-  if (weighted_n_node_samples) memcpy(weighted_n_node_samples, t.wn.data(), m * 8);
-  if (missing_go_to_left) memcpy(missing_go_to_left, t.mgl.data(), m);
-  if (value) memcpy(value, t.val.data(), t.val.size() * 8);
+  if (impurity && !reg) forest_class_impurity(m, C, f->criterion == 1, node_sums, children, impurity);
   return 0;
 }
 

@@ -41,7 +41,6 @@ constexpr int FO_THREADS = 256;
 constexpr int FO_MAXC = 16;      // classes
 constexpr int FO_BINS = 256;
 constexpr float FEATURE_THRESHOLD = 1e-7f;
-constexpr double FO_EPSILON = 2.220446049250313e-16;   // np.finfo('double').eps (SK/tree/_tree.pyx EPSILON)
 
 struct FoRecord {          // builder stack record (SK/tree/_tree.pyx StackRecord) + the node's class sums
   int32_t start, end, depth, parent, is_left, n_const;
@@ -63,43 +62,15 @@ constexpr int FO_KB_MAX = 8;
 constexpr int FO_SSTK = 128;     // builder-stack entries kept in shared memory (deeper ones spill to global)
 constexpr int FO_HIST_WORDS = 40 * FO_BINS;   // KB * (C + 1) * 256 <= this
 
-struct FoParams {
+struct FoParams : ForestParams {
   const uint8_t* xbin;        // [d][n] bin codes, feature-major (best splitter)
   const float* binval;        // [d][256] distinct values ascending
   const float* xval;          // [d][n] raw values, feature-major: random splitter on features without codes, else nullptr
-  const int32_t* ycls;        // [n] class ids (classification)
   const double* yreal;        // [n] float64 targets (regression: MSE criterion), else nullptr
-  int64_t n;
-  int d, n_classes;
-  int max_features, max_depth, min_samples_split, min_samples_leaf;
   int random_split;           // 0: node_split_best (RandomForest), 1: node_split_random (ExtraTrees)
-  double min_weight_leaf, min_impurity_decrease;
-  // per tree (wave-local index = blockIdx.x)
-  const uint8_t* counts;      // [trees_in_wave][n] bootstrap multiplicities (sample_weight)
-  const uint32_t* rand_state; // [trees_in_wave]
-  int n_trees;
-  // per slot work + output buffers
-  uint2* samp;                // [slots][n]   (sample index, (weight << 8) | class)
-  uint2* samp_tmp;            // [slots][n]
-  FoRecord* stack;            // [slots][stack_cap]
-  int stack_cap;
-  int64_t node_cap;
-  int32_t* o_left; int32_t* o_right; int32_t* o_feature; int32_t* o_nsamp; uint8_t* o_mgl;
-  double* o_thr; double* o_imp; double* o_wn; double* o_val;   // o_val [node_cap][n_classes]
-  int32_t* o_count;           // [slots] node_count
-  int32_t* o_maxdepth;        // [slots]
-  int32_t* o_status;          // [slots] 0 ok, 1 node capacity, 2 stack capacity
-  long long* o_prof;          // [slots][16] cycles per builder phase (SKDIST_B200_FOREST_PROF=1), else nullptr
-  // class weights, read only by the weighted instantiation (W): as FfParams
-  int cw_bs;
-  const double* cw;
-  double min_weight_fraction;
-  // sort-based best splitter (FO_SORT): [slots][2][n] ping-pong (key, node position) buffers of the
+  // sort-based best splitter (FO_SORT): [trees][2][n] ping-pong (key, node position) buffers of the
   // large-node radix sort, else nullptr
   uint2* srt;
-  // entropy (ENT): [slots][node_cap][n_classes] integer class sums of every node, from which the host forms
-  // the impurity with its own log (api.cu), else nullptr
-  unsigned long long* o_sums;
 };
 
 // What the general builder reads for a split (one kernel instantiation each, so that the histogram
@@ -109,17 +80,6 @@ enum FoMode : int {
   FO_RAW = 1,    // random splitter over the raw float32 values (P.xval)
   FO_SORT = 2,   // best splitter over the raw float32 values: sort the node's values, scan the runs
 };
-
-__device__ __forceinline__ uint32_t fo_rand_r(uint32_t* seed) {   // SK/utils/_random.pxd:20-34
-  if (*seed == 0) *seed = 1;
-  *seed ^= (uint32_t)(*seed << 13);
-  *seed ^= (uint32_t)(*seed >> 17);
-  *seed ^= (uint32_t)(*seed << 5);
-  return *seed % ((uint32_t)2147483647 + 1);
-}
-__device__ __forceinline__ int fo_rand_int(int low, int high, uint32_t* seed) {
-  return low + (int)(fo_rand_r(seed) % (uint32_t)(high - low));
-}
 
 // CM: compile-time bound on the class count (3 statistics when REG), so the per-class arrays of a thread live in registers.
 // W: class weights (classification only).  Histograms, records and the partition keep the integer
@@ -512,9 +472,8 @@ forest_build_kernel(const FoParams P) {
   const int64_t n = P.n;
   uint2* samp = P.samp + (size_t)slot * n;
   uint2* tmp = P.samp_tmp + (size_t)slot * n;
-  FoRecord* stack = P.stack + (size_t)slot * P.stack_cap;
+  FoRecord* stack = static_cast<FoRecord*>(P.stack) + (size_t)slot * P.stack_cap;
   const uint8_t* cnt = P.counts + (size_t)slot * n;
-  const int64_t nb = (int64_t)slot * P.node_cap;
 
   extern __shared__ int fo_sm[];
   int* features = fo_sm;                     // [d]
@@ -649,12 +608,11 @@ forest_build_kernel(const FoParams P) {
       impurity = fo_node_impurity<CM, REG, W, ENT>(rec.sums, s_cw, C, w_node);
       first = false;
     }
-    is_leaf = is_leaf || impurity <= FO_EPSILON;
+    is_leaf = is_leaf || impurity <= FOREST_EPSILON;
 
     // ------------------------------- node_split_best -------------------------------------
     int best_feature = 0, best_pos = end, best_bin = -1, n_total_constants = rec.n_const;
     double best_thr = 0.0, best_il = 0.0, best_ir = 0.0, best_improvement = 0.0;
-    int best_mgl = 0;
     if (!is_leaf) {
       const int n_known = rec.n_const;
       int f_i = d, n_visited = 0, n_found = 0, n_drawn = 0;
@@ -676,7 +634,7 @@ forest_build_kernel(const FoParams P) {
           while (nbatch < KB && s_fi > n_total_constants &&
                  (s_nv < P.max_features || s_nv <= n_found + s_nd)) {
             s_nv += 1;
-            int fj = fo_rand_int(s_nd, s_fi - n_found, &s_rs);
+            int fj = forest_rand_int(s_nd, s_fi - n_found, &s_rs);
             if (fj < n_known) {   // a known constant: move it to the drawn-constants prefix
               const int t = features[s_nd]; features[s_nd] = features[fj]; features[fj] = t;
               undo[ulen++] = make_int2(s_nd, fj);
@@ -692,7 +650,7 @@ forest_build_kernel(const FoParams P) {
             undo[ulen++] = make_int2(s_fi, fj);
             // node_split_random draws the threshold of a non-constant feature from the same stream
             // right after the feature (SK/tree/_splitter.pyx:633-637)
-            if (P.random_split) items[nbatch].rnd = fo_rand_r(&s_rs);
+            if (P.random_split) items[nbatch].rnd = forest_rand_r(&s_rs);
             nbatch += 1;
           }
           s_ctrl[0] = nbatch;
@@ -1043,7 +1001,6 @@ forest_build_kernel(const FoParams P) {
               if (R.proxy > best_proxy) {
                 best_proxy = R.proxy;
                 best_feature = items[k].f; best_pos = R.pos; best_bin = R.bin; best_thr = R.thr;
-                best_mgl = (R.pos - start) > (end - R.pos);
                 best_il = R.il; best_ir = R.ir;
                 FOR_C(c) best_sl[c] = R.sl[c];
               }
@@ -1070,7 +1027,6 @@ forest_build_kernel(const FoParams P) {
       // restore / record the constant-feature invariants (end of node_split_best)
       if (tid == 0) {
         s_ctrl[2] = best_pos; s_ctrl[3] = best_feature; s_ctrl[4] = best_bin; s_ctrl[5] = n_total_constants;
-        s_ctrl[6] = best_mgl;
         s_dbl[0] = best_thr; s_dbl[1] = best_il; s_dbl[2] = best_ir;
         if (best_pos < end) {
           const double wl = fo_weight<CM, REG, W>(best_sl, s_cw, C);
@@ -1090,9 +1046,8 @@ forest_build_kernel(const FoParams P) {
       // spread over the block; the next reader of these arrays is behind later barriers
       for (int i = tid; i < n_known; i += FO_THREADS) features[i] = constant_features[i];
       for (int i = n_known + tid; i < n_total_constants; i += FO_THREADS) constant_features[i] = features[i];
-      best_mgl = s_ctrl[6];
       best_thr = s_dbl[0]; best_il = s_dbl[1]; best_ir = s_dbl[2]; best_improvement = s_dbl[3];
-      is_leaf = is_leaf || best_pos >= end || (best_improvement + FO_EPSILON < P.min_impurity_decrease);
+      is_leaf = is_leaf || best_pos >= end || (best_improvement + FOREST_EPSILON < P.min_impurity_decrease);
 
       if (best_pos < end) {
         // --- partition_samples_final: stable partition (keeps sample indices ascending) ---
@@ -1133,33 +1088,19 @@ forest_build_kernel(const FoParams P) {
     }
 
     FO_TICK(7);
-    // ------------------------------- _add_node + node_value --------------------------------
+    // ------------------------------------- _add_node ----------------------------------------
     const int node_id = node_count;
     if (node_id >= P.node_cap) { status = 1; break; }
     if (tid == 0) {
-      if (rec.parent >= 0) {
-        if (rec.is_left) P.o_left[nb + rec.parent] = node_id; else P.o_right[nb + rec.parent] = node_id;
-      }
-      P.o_imp[nb + node_id] = impurity;
-      P.o_nsamp[nb + node_id] = n_node;
-      P.o_wn[nb + node_id] = w_node;
-      if (is_leaf) {
-        P.o_left[nb + node_id] = -1; P.o_right[nb + node_id] = -1;
-        P.o_feature[nb + node_id] = -2; P.o_thr[nb + node_id] = -2.0; P.o_mgl[nb + node_id] = 0;
-      } else {
-        P.o_feature[nb + node_id] = best_feature; P.o_thr[nb + node_id] = best_thr;
-        P.o_mgl[nb + node_id] = (uint8_t)best_mgl;
-      }
-      if constexpr (REG) {
-        P.o_val[nb + node_id] = __ddiv_rn(st_d(rec.sums[1]), w_node);               // node mean (MSE.node_value)
-      } else if constexpr (W) {
-        FOR_C(c)
-          P.o_val[(nb + node_id) * C + c] = __ddiv_rn(__dmul_rn(s_cw[c], (double)rec.sums[c]), w_node);
-      } else {
-        FOR_C(c)
-          P.o_val[(nb + node_id) * C + c] = __ddiv_rn((double)rec.sums[c], w_node);   // class fractions
-      }
-      if constexpr (ENT) { FOR_C(c) P.o_sums[(nb + node_id) * C + c] = rec.sums[c]; }
+      // node record FOREST_REC_CLASS / FOREST_REC_REG (forest_common.h): header, threshold, statistics
+      const int rw = (int)(forest_record_bytes(REG ? FOREST_REC_REG : FOREST_REC_CLASS, P.n_classes) / 4);   // words
+      uint32_t* nodes = P.o_nodes + (size_t)slot * P.node_cap * rw;
+      if (rec.parent >= 0 && !rec.is_left) nodes[(size_t)rec.parent * rw] = (uint32_t)node_id;
+      uint32_t* r = nodes + (size_t)node_id * rw;
+      r[0] = 0xFFFFFFFFu; r[1] = is_leaf ? 0xFFFFu : (uint32_t)best_feature; r[2] = (uint32_t)n_node; r[3] = (uint32_t)depth;
+      *reinterpret_cast<double*>(r + 4) = best_thr;
+      unsigned long long* sums = reinterpret_cast<unsigned long long*>(r + 6);
+      FOR_C(c) sums[c] = rec.sums[c];
     }
     node_count += 1;
     if (!is_leaf) {
@@ -1333,15 +1274,15 @@ int forest_prepare(Ctx* c, bool values) {
 }
 
 // Build `n_trees` trees.  counts: [n_trees][n] uint8 host array of bootstrap multiplicities,
-// rand_states: [n_trees] splitter seeds.  Results are delivered tree by tree through `sink`.
-// random_split: node_split_random (ExtraTrees), else node_split_best (RandomForest).  sort_split (best
-// splitter only): a feature without bin codes is split by sorting its raw values (FO_SORT) instead of
-// being refused; when every feature has codes the fit is the same as without it.  entropy: criterion
-// "entropy" (classification, general builder only); the trees come with their integer class sums.
+// rand_states: [n_trees] splitter seeds.  Results are delivered tree by tree through `sink`, as the node
+// records of forest_common.h.  random_split: node_split_random (ExtraTrees), else node_split_best
+// (RandomForest).  sort_split (best splitter only): a feature without bin codes is split by sorting its raw
+// values (FO_SORT) instead of being refused; when every feature has codes the fit is the same as without it.
+// entropy: criterion "entropy" (classification, general builder only).
 // Two builders: forest_fast.cu (classification, Gini, best splitter, <= 4 classes: seven trees per SM)
 // and the general kernel above (two per SM).  Trees are built in rounds of `slots` concurrent
-// trees; the node arrays of a slot hold `node_cap` nodes, sized from the free device memory; a tree
-// that outgrows them (status 1) is rebuilt in a later round with the worst-case capacity 2n - 1.
+// trees; the node records of a slot hold `node_cap` nodes (throughput builder: sized from the free device
+// memory); a tree that outgrows them (status 1) is rebuilt in a later round with the worst-case capacity 2n - 1.
 int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_states, int n_classes,
                int max_features, int max_depth, int min_samples_split, int min_samples_leaf,
                double min_weight_leaf, double min_impurity_decrease, bool random_split, bool sort_split,
@@ -1381,11 +1322,11 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
     if (!(hi > 0.0) || hi > 1099511627776.0 * lo) fast = false;
   }
   const int stack_cap = 4096;
-  const size_t rec_bytes = fast ? forest_fast_record_bytes(n_classes) : sizeof(FoRecord);
-  // fast builder: compact records; entropy: the class sums too
-  const size_t node_bytes = fast ? 32 : (size_t)(4 * 4 + 1 + 8 * 3 + 8 * n_classes * (entropy ? 2 : 1));
+  const size_t stack_bytes = fast ? forest_fast_stack_bytes(n_classes) : sizeof(FoRecord);
+  const int kind = fast ? FOREST_REC_FAST : reg ? FOREST_REC_REG : FOREST_REC_CLASS;
+  const size_t node_bytes = forest_record_bytes(kind, n_classes);
   // two sample buffers + counts + stack (+ the two (key, position) buffers of the sort-based splitter)
-  const size_t slot_fixed = (size_t)n * (sort_values ? 33 : 17) + (size_t)stack_cap * rec_bytes + 64;
+  const size_t slot_fixed = (size_t)n * (sort_values ? 33 : 17) + (size_t)stack_cap * stack_bytes + 64;
   const int64_t node_cap_max = std::max<int64_t>(2 * n, 16);
   int64_t node_cap = node_cap_max;
   if (const char* e = getenv("SKDIST_B200_FOREST_NODECAP")) {   // experiments / tests: smaller output arrays per tree
@@ -1428,8 +1369,6 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
   std::vector<int> pending(n_trees);
   for (int t = 0; t < n_trees; ++t) pending[t] = t;
   c->forest_kernel_ms = 0.0;
-  std::vector<int32_t> hl, hr, hf, hn; std::vector<uint8_t> hm; std::vector<double> ht, hi, hw, hv;
-  std::vector<unsigned long long> hs;
   for (int round = 0; !pending.empty(); ++round) {
     // slots: concurrent trees of this round, bounded by the resident builders and by memory
     size_t free_b = 0, total_b = 0;
@@ -1449,62 +1388,36 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
     if ((size_t)slots * per_slot > budget) slots = (int)(budget / per_slot);
     if (slots < 1) return fail(c, "forest: not enough device memory for one tree");
     Scratch sx(c);
-    FoParams P;
-    memset(&P, 0, sizeof(P));
-    uint8_t* dcounts; uint32_t* drs; void* dstack;
+    ForestParams B{};   // what both builders read
+    uint8_t* dcounts; uint32_t* drs; uint8_t* dstack;
     SKD_CUDA(c, sx.alloc(&dcounts, (size_t)slots * n));
     SKD_CUDA(c, sx.alloc(&drs, (size_t)slots));
-    SKD_CUDA(c, sx.alloc(&P.samp, (size_t)slots * n));
-    SKD_CUDA(c, sx.alloc(&P.samp_tmp, (size_t)slots * n));
-    SKD_CUDA(c, sx.alloc((uint8_t**)&dstack, (size_t)slots * stack_cap * rec_bytes));
-    uint32_t* d_nodes = nullptr;
-    if (fast) {
-      SKD_CUDA(c, sx.alloc(&d_nodes, (size_t)slots * node_cap * 8));
-    } else {
-      SKD_CUDA(c, sx.alloc(&P.o_left, (size_t)slots * node_cap));
-      SKD_CUDA(c, sx.alloc(&P.o_right, (size_t)slots * node_cap));
-      SKD_CUDA(c, sx.alloc(&P.o_feature, (size_t)slots * node_cap));
-      SKD_CUDA(c, sx.alloc(&P.o_nsamp, (size_t)slots * node_cap));
-      SKD_CUDA(c, sx.alloc(&P.o_mgl, (size_t)slots * node_cap));
-      SKD_CUDA(c, sx.alloc(&P.o_thr, (size_t)slots * node_cap));
-      SKD_CUDA(c, sx.alloc(&P.o_imp, (size_t)slots * node_cap));
-      SKD_CUDA(c, sx.alloc(&P.o_wn, (size_t)slots * node_cap));
-      SKD_CUDA(c, sx.alloc(&P.o_val, (size_t)slots * node_cap * n_classes));
-      if (entropy) SKD_CUDA(c, sx.alloc(&P.o_sums, (size_t)slots * node_cap * n_classes));
-    }
-    SKD_CUDA(c, sx.alloc(&P.o_count, (size_t)slots));
-    SKD_CUDA(c, sx.alloc(&P.o_maxdepth, (size_t)slots));
-    SKD_CUDA(c, sx.alloc(&P.o_status, (size_t)slots));
-    if (sort_values) SKD_CUDA(c, sx.alloc(&P.srt, (size_t)slots * 2 * n));
-    long long* d_prof = nullptr;
-    if (want_prof) SKD_CUDA(c, sx.alloc(&d_prof, (size_t)slots * 16));
-    P.stack = (FoRecord*)dstack;
-    P.xbin = c->forest.xbin; P.binval = c->forest.binval; P.xval = raw_values || sort_values ? c->forest.xval : nullptr; P.ycls = c->ycls; P.yreal = dy;
-    P.n = n; P.d = d; P.n_classes = n_classes;
-    P.max_features = max_features; P.max_depth = max_depth; P.min_samples_split = min_samples_split;
-    P.min_samples_leaf = min_samples_leaf; P.min_weight_leaf = min_weight_leaf;
-    P.min_impurity_decrease = min_impurity_decrease;
-    P.random_split = random_split ? 1 : 0;
-    P.counts = dcounts; P.rand_state = drs; P.stack_cap = stack_cap; P.node_cap = node_cap;
-    P.o_prof = d_prof;
+    SKD_CUDA(c, sx.alloc(&B.samp, (size_t)slots * n));
+    SKD_CUDA(c, sx.alloc(&B.samp_tmp, (size_t)slots * n));
+    SKD_CUDA(c, sx.alloc(&dstack, (size_t)slots * stack_cap * stack_bytes));
+    SKD_CUDA(c, sx.alloc(&B.o_nodes, (size_t)slots * node_cap * (node_bytes / 4)));
+    SKD_CUDA(c, sx.alloc(&B.o_count, (size_t)slots));
+    SKD_CUDA(c, sx.alloc(&B.o_maxdepth, (size_t)slots));
+    SKD_CUDA(c, sx.alloc(&B.o_status, (size_t)slots));
+    if (want_prof) SKD_CUDA(c, sx.alloc(&B.o_prof, (size_t)slots * 16));
+    B.ycls = c->ycls; B.n = n; B.d = d; B.n_classes = n_classes;
+    B.max_features = max_features; B.max_depth = max_depth; B.min_samples_split = min_samples_split;
+    B.min_samples_leaf = min_samples_leaf; B.min_weight_leaf = min_weight_leaf;
+    B.min_impurity_decrease = min_impurity_decrease;
+    B.counts = dcounts; B.rand_state = drs; B.stack = dstack; B.stack_cap = stack_cap; B.node_cap = node_cap;
     if (weighted) {
-      P.cw_bs = cw->balanced_subsample ? 1 : 0; P.cw = dcw; P.min_weight_fraction = cw->min_weight_fraction;
+      B.weighted = 1; B.cw_bs = cw->balanced_subsample ? 1 : 0; B.cw = dcw; B.min_weight_fraction = cw->min_weight_fraction;
     }
-    FfParams F;
-    memset(&F, 0, sizeof(F));
-    F.xrow = c->forest.xrow; F.ycls = c->ycls; F.n = n; F.d = d; F.dp = c->forest.dp; F.n_classes = n_classes;
-    F.max_features = max_features; F.max_depth = max_depth; F.min_samples_split = min_samples_split;
-    F.min_samples_leaf = min_samples_leaf; F.min_weight_leaf = min_weight_leaf;
-    F.min_impurity_decrease = min_impurity_decrease;
-    F.counts = dcounts; F.rand_state = drs; F.samp = P.samp; F.samp_tmp = P.samp_tmp; F.stack = dstack;
-    F.stack_cap = stack_cap; F.node_cap = node_cap;
-    F.o_nodes = d_nodes;
-    F.o_count = P.o_count; F.o_maxdepth = P.o_maxdepth; F.o_status = P.o_status; F.o_prof = d_prof;
-    F.weighted = weighted ? 1 : 0; F.cw_bs = P.cw_bs; F.cw = P.cw; F.min_weight_fraction = P.min_weight_fraction;
+    FoParams P{B};
+    P.xbin = c->forest.xbin; P.binval = c->forest.binval; P.xval = raw_values || sort_values ? c->forest.xval : nullptr;
+    P.yreal = dy;
+    P.random_split = random_split ? 1 : 0;
+    if (sort_values) SKD_CUDA(c, sx.alloc(&P.srt, (size_t)slots * 2 * n));
+    FfParams F{B};
+    F.xrow = c->forest.xrow; F.dp = c->forest.dp;
     std::vector<int32_t> hcount(slots), hdepth(slots), hstatus(slots);
     std::vector<uint32_t> hrs(slots);
     std::vector<int> failed;
-    SkdTreeView view;
     for (size_t p0 = 0; p0 < pending.size(); p0 += slots) {
       const int nt = (int)std::min<size_t>(slots, pending.size() - p0);
       const bool contiguous = pending[p0 + nt - 1] - pending[p0] == nt - 1;
@@ -1532,14 +1445,14 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
       }
       SKD_CUDA(c, cudaGetLastError());
       SKD_CUDA(c, cudaEventRecord(k1, c->stream));
-      SKD_CUDA(c, cudaMemcpyAsync(hcount.data(), P.o_count, nt * 4, cudaMemcpyDeviceToHost, c->stream));
-      SKD_CUDA(c, cudaMemcpyAsync(hdepth.data(), P.o_maxdepth, nt * 4, cudaMemcpyDeviceToHost, c->stream));
-      SKD_CUDA(c, cudaMemcpyAsync(hstatus.data(), P.o_status, nt * 4, cudaMemcpyDeviceToHost, c->stream));
+      SKD_CUDA(c, cudaMemcpyAsync(hcount.data(), B.o_count, nt * 4, cudaMemcpyDeviceToHost, c->stream));
+      SKD_CUDA(c, cudaMemcpyAsync(hdepth.data(), B.o_maxdepth, nt * 4, cudaMemcpyDeviceToHost, c->stream));
+      SKD_CUDA(c, cudaMemcpyAsync(hstatus.data(), B.o_status, nt * 4, cudaMemcpyDeviceToHost, c->stream));
       SKD_CUDA(c, cudaStreamSynchronize(c->stream));
       { float kms = 0.f; cudaEventElapsedTime(&kms, k0, k1); c->forest_kernel_ms += kms; cudaEventDestroy(k0); cudaEventDestroy(k1); }
       if (want_prof) {
         std::vector<long long> hp((size_t)nt * 16);
-        cudaMemcpy(hp.data(), d_prof, hp.size() * 8, cudaMemcpyDeviceToHost);
+        cudaMemcpy(hp.data(), B.o_prof, hp.size() * 8, cudaMemcpyDeviceToHost);
         static const char* nm_g[12] = {"pop", "speculate", "zero+stage", "histogram", "scan", "commit", "restore+improve", "partition", "add_node+push", "-", "loop barrier", "-"};
         static const char* nm_f[12] = {"pop+header", "stage subtree", "draw", "gather hist", "scan (unstaged)", "hist+scan (staged)", "rank (<=32)", "commit", "finish split", "partition", "add_node+push", "-"};
         const char** nm = fast ? nm_f : nm_g;
@@ -1549,102 +1462,69 @@ int forest_fit(Ctx* c, int n_trees, const uint8_t* counts, const uint32_t* rand_
         if (fast) fprintf(stderr, "[skd forest prof] tree 0 nodes: unstaged %lld, staged histogram %lld, staged rank %lld, leaves %lld; total %.3f Gcycles\n",
                           hp[11], hp[12], hp[13], hp[14], tot * 1e-9);
       }
-      if (fast) {
-        // compact records: trees come back through a ring of pinned buffers; the copies are issued by
-        // this thread, a few host threads wait for them and hand the trees to the consumer (which copies
-        // 12 MB per tree out of the pinned buffer: a single thread would be the bottleneck)
-        constexpr int NB = 8, NW = 4;
-        size_t max_m = 1;
-        for (int s = 0; s < nt; ++s) if (hstatus[s] == 0) max_m = std::max(max_m, (size_t)hcount[s]);
-        if (c->pin_tree_bytes < max_m * 32) {
-          for (void*& pb : c->pin_tree) { if (pb) cudaFreeHost(pb); pb = nullptr; }
-          c->pin_tree_bytes = max_m * 32 + (max_m * 32) / 8;
-          for (void*& pb : c->pin_tree) SKD_CUDA(c, cudaHostAlloc(&pb, c->pin_tree_bytes, cudaHostAllocDefault));
-        }
-        std::vector<int> ok;
-        for (int s = 0; s < nt; ++s) {
-          if (hstatus[s] == 1 && node_cap < node_cap_max) { failed.push_back(pending[p0 + s]); continue; }
-          if (hstatus[s] != 0) return fail(c, hstatus[s] == 1 ? "forest: node capacity exceeded" : "forest: builder stack capacity exceeded");
-          ok.push_back(s);
-        }
-        cudaEvent_t evc[NB];
-        for (int b = 0; b < NB; ++b) SKD_CUDA(c, cudaEventCreateWithFlags(&evc[b], cudaEventDisableTiming));
-        std::mutex mu;
-        std::condition_variable cv_job, cv_free;
-        std::deque<size_t> ready;
-        bool busy[NB] = {false}, finished = false;
-        std::atomic<int> cuda_err{0};
-        auto worker = [&]() {
-          cudaSetDevice(c->device);
-          for (;;) {
-            size_t k;
-            {
-              std::unique_lock<std::mutex> lk(mu);
-              cv_job.wait(lk, [&] { return !ready.empty() || finished; });
-              if (ready.empty()) return;
-              k = ready.front(); ready.pop_front();
-            }
-            const int b = (int)(k % NB), s = ok[k];
-            if (cudaEventSynchronize(evc[b]) != cudaSuccess) cuda_err = 1;
-            SkdTreeView v;
-            v.compact = (const uint32_t*)c->pin_tree[b];
-            v.binval = c->forest.h_binval.data();
-            v.node_count = hcount[s]; v.max_depth = hdepth[s]; v.n_classes = n_classes;
-            v.left = v.right = v.feature = v.n_node_samples = nullptr; v.missing_go_to_left = nullptr;
-            v.threshold = v.impurity = v.weighted_n_node_samples = v.value = nullptr;
-            sink(sink_arg, pending[p0 + s], &v);
-            { std::lock_guard<std::mutex> lk(mu); busy[b] = false; }
-            cv_free.notify_all();
-          }
-        };
-        std::vector<std::thread> pool;
-        for (int w = 0; w < NW; ++w) pool.emplace_back(worker);
-        for (size_t k = 0; k < ok.size(); ++k) {
-          const int b = (int)(k % NB), s = ok[k];
-          { std::unique_lock<std::mutex> lk(mu); cv_free.wait(lk, [&] { return !busy[b]; }); busy[b] = true; }
-          cudaMemcpyAsync(c->pin_tree[b], d_nodes + (size_t)s * node_cap * 8, (size_t)hcount[s] * 32, cudaMemcpyDeviceToHost, c->stream);
-          cudaEventRecord(evc[b], c->stream);
-          { std::lock_guard<std::mutex> lk(mu); ready.push_back(k); }
-          cv_job.notify_one();
-          c->d2h += (int64_t)hcount[s] * 32;
-        }
-        { std::lock_guard<std::mutex> lk(mu); finished = true; }
-        cv_job.notify_all();
-        for (auto& t : pool) t.join();
-        for (int b = 0; b < NB; ++b) cudaEventDestroy(evc[b]);
-        if (cuda_err) return fail(c, "forest: copying the trees back failed");
-        SKD_CUDA(c, cudaGetLastError());
-        continue;
+      // Trees come back through a ring of pinned buffers; the copies are issued by this thread, a few
+      // host threads wait for them and hand the trees to the consumer (which copies 12 MB per config-4
+      // tree out of the pinned buffer: a single thread would be the bottleneck)
+      constexpr int NB = 8, NW = 4;
+      size_t max_m = 1;
+      for (int s = 0; s < nt; ++s) if (hstatus[s] == 0) max_m = std::max(max_m, (size_t)hcount[s]);
+      if (c->pin_tree_bytes < max_m * node_bytes) {
+        for (void*& pb : c->pin_tree) { if (pb) cudaFreeHost(pb); pb = nullptr; }
+        c->pin_tree_bytes = max_m * node_bytes + (max_m * node_bytes) / 8;
+        for (void*& pb : c->pin_tree) SKD_CUDA(c, cudaHostAlloc(&pb, c->pin_tree_bytes, cudaHostAllocDefault));
       }
+      std::vector<int> ok;
       for (int s = 0; s < nt; ++s) {
         if (hstatus[s] == 1 && node_cap < node_cap_max) { failed.push_back(pending[p0 + s]); continue; }
         if (hstatus[s] != 0) return fail(c, hstatus[s] == 1 ? "forest: node capacity exceeded" : "forest: builder stack capacity exceeded");
-        const int m = hcount[s];
-        hl.resize(m); hr.resize(m); hf.resize(m); hn.resize(m); hm.resize(m); ht.resize(m); hi.resize(m); hw.resize(m);
-        hv.resize((size_t)m * n_classes);
-        const size_t o = (size_t)s * node_cap;
-        SKD_CUDA(c, cudaMemcpyAsync(hl.data(), P.o_left + o, m * 4, cudaMemcpyDeviceToHost, c->stream));
-        SKD_CUDA(c, cudaMemcpyAsync(hr.data(), P.o_right + o, m * 4, cudaMemcpyDeviceToHost, c->stream));
-        SKD_CUDA(c, cudaMemcpyAsync(hf.data(), P.o_feature + o, m * 4, cudaMemcpyDeviceToHost, c->stream));
-        SKD_CUDA(c, cudaMemcpyAsync(hn.data(), P.o_nsamp + o, m * 4, cudaMemcpyDeviceToHost, c->stream));
-        SKD_CUDA(c, cudaMemcpyAsync(hm.data(), P.o_mgl + o, m, cudaMemcpyDeviceToHost, c->stream));
-        SKD_CUDA(c, cudaMemcpyAsync(ht.data(), P.o_thr + o, m * 8, cudaMemcpyDeviceToHost, c->stream));
-        SKD_CUDA(c, cudaMemcpyAsync(hi.data(), P.o_imp + o, m * 8, cudaMemcpyDeviceToHost, c->stream));
-        SKD_CUDA(c, cudaMemcpyAsync(hw.data(), P.o_wn + o, m * 8, cudaMemcpyDeviceToHost, c->stream));
-        SKD_CUDA(c, cudaMemcpyAsync(hv.data(), P.o_val + o * n_classes, (size_t)m * n_classes * 8, cudaMemcpyDeviceToHost, c->stream));
-        if (entropy) {
-          hs.resize((size_t)m * n_classes);
-          SKD_CUDA(c, cudaMemcpyAsync(hs.data(), P.o_sums + o * n_classes, (size_t)m * n_classes * 8, cudaMemcpyDeviceToHost, c->stream));
-        }
-        SKD_CUDA(c, cudaStreamSynchronize(c->stream));
-        c->d2h += (int64_t)m * node_bytes;
-        view.node_count = m; view.max_depth = hdepth[s]; view.n_classes = n_classes;
-        view.left = hl.data(); view.right = hr.data(); view.feature = hf.data(); view.n_node_samples = hn.data();
-        view.missing_go_to_left = hm.data(); view.threshold = ht.data(); view.impurity = hi.data();
-        view.weighted_n_node_samples = hw.data(); view.value = hv.data();
-        view.class_sums = entropy ? hs.data() : nullptr;
-        sink(sink_arg, pending[p0 + s], &view);
+        ok.push_back(s);
       }
+      cudaEvent_t evc[NB];
+      for (int b = 0; b < NB; ++b) SKD_CUDA(c, cudaEventCreateWithFlags(&evc[b], cudaEventDisableTiming));
+      std::mutex mu;
+      std::condition_variable cv_job, cv_free;
+      std::deque<size_t> ready;
+      bool busy[NB] = {false}, finished = false;
+      std::atomic<int> cuda_err{0};
+      auto worker = [&]() {
+        cudaSetDevice(c->device);
+        for (;;) {
+          size_t k;
+          {
+            std::unique_lock<std::mutex> lk(mu);
+            cv_job.wait(lk, [&] { return !ready.empty() || finished; });
+            if (ready.empty()) return;
+            k = ready.front(); ready.pop_front();
+          }
+          const int b = (int)(k % NB), s = ok[k];
+          if (cudaEventSynchronize(evc[b]) != cudaSuccess) cuda_err = 1;
+          SkdTreeView v;
+          v.records = (const uint32_t*)c->pin_tree[b]; v.kind = kind;
+          v.node_count = hcount[s]; v.max_depth = hdepth[s]; v.n_classes = n_classes;
+          v.binval = c->forest.h_binval.data();
+          sink(sink_arg, pending[p0 + s], &v);
+          { std::lock_guard<std::mutex> lk(mu); busy[b] = false; }
+          cv_free.notify_all();
+        }
+      };
+      std::vector<std::thread> pool;
+      for (int w = 0; w < NW; ++w) pool.emplace_back(worker);
+      for (size_t k = 0; k < ok.size(); ++k) {
+        const int b = (int)(k % NB), s = ok[k];
+        { std::unique_lock<std::mutex> lk(mu); cv_free.wait(lk, [&] { return !busy[b]; }); busy[b] = true; }
+        cudaMemcpyAsync(c->pin_tree[b], (const uint8_t*)B.o_nodes + (size_t)s * node_cap * node_bytes,
+                        (size_t)hcount[s] * node_bytes, cudaMemcpyDeviceToHost, c->stream);
+        cudaEventRecord(evc[b], c->stream);
+        { std::lock_guard<std::mutex> lk(mu); ready.push_back(k); }
+        cv_job.notify_one();
+        c->d2h += (int64_t)hcount[s] * node_bytes;
+      }
+      { std::lock_guard<std::mutex> lk(mu); finished = true; }
+      cv_job.notify_all();
+      for (auto& t : pool) t.join();
+      for (int b = 0; b < NB; ++b) cudaEventDestroy(evc[b]);
+      if (cuda_err) return fail(c, "forest: copying the trees back failed");
+      SKD_CUDA(c, cudaGetLastError());
     }
     pending.swap(failed);
     node_cap = node_cap_max;      // trees that outgrew their arrays: worst-case capacity, fewer at a time

@@ -51,7 +51,6 @@ constexpr int FF_KBM = 4;         // ... for staged histogram nodes (packed hist
 constexpr int FF_SMAX = 256;      // staged rows at most (local ids are bytes, packed 16-bit sums must hold 256 x 255)
 constexpr int FF_SSTK = 64;       // builder-stack entries kept in shared memory
 constexpr int FF_SMALL = 32;      // staged nodes up to this size take the ranking path
-constexpr double FF_EPSILON = 2.220446049250313e-16;
 
 template <int CM>
 struct __align__(8) FfRec {       // builder stack record (SK/tree/_tree.pyx StackRecord) + the node's class sums
@@ -80,17 +79,6 @@ struct __align__(8) FfResult {    // best split of one feature in the current no
 // the sample count above them
 template <int CM> struct FfAcc { typedef unsigned long long T; static constexpr int CNT = 13 * CM; };
 template <> struct FfAcc<2> { typedef unsigned int T; static constexpr int CNT = 26; };
-
-__device__ __forceinline__ uint32_t ff_rand_r(uint32_t* seed) {   // SK/utils/_random.pxd:20-34
-  if (*seed == 0) *seed = 1;
-  *seed ^= (uint32_t)(*seed << 13);
-  *seed ^= (uint32_t)(*seed >> 17);
-  *seed ^= (uint32_t)(*seed << 5);
-  return *seed % ((uint32_t)2147483647 + 1);
-}
-__device__ __forceinline__ int ff_rand_int(int low, int high, uint32_t* seed) {
-  return low + (int)(ff_rand_r(seed) % (uint32_t)(high - low));
-}
 
 // The builder is latency-bound on ONE warp's instruction stream per tree (ncu: 44 % of the stall
 // samples are instruction fetch when the kernel is unrolled to 130 KB), so everything below is written
@@ -517,7 +505,7 @@ forest_fast_kernel(const FfParams P) {
       impurity = __dsub_rn(1.0, __ddiv_rn(sq, __dmul_rn(w_node, w_node)));
       first = false;
     }
-    is_leaf = is_leaf || impurity <= FF_EPSILON;
+    is_leaf = is_leaf || impurity <= FOREST_EPSILON;
     FF_TICK(0);
 
     int best_feature = 0, best_nl = -1, best_code = 0, n_total_constants = n_known;
@@ -569,7 +557,7 @@ forest_fast_kernel(const FfParams P) {
           while (nbatch < KB && s_fi > n_total_constants &&
                  (s_nv < P.max_features || s_nv <= n_found + s_nd)) {
             s_nv += 1;
-            int fj = ff_rand_int(s_nd, s_fi - n_found, &s_rs);
+            int fj = forest_rand_int(s_nd, s_fi - n_found, &s_rs);
             if (fj < n_known) {   // a known constant: move it to the drawn-constants prefix
               const uint8_t t = features[s_nd]; features[s_nd] = features[fj]; features[fj] = t;
               undo[2 * ulen] = (uint8_t)s_nd; undo[2 * ulen + 1] = (uint8_t)fj; ++ulen;
@@ -827,7 +815,7 @@ forest_fast_kernel(const FfParams P) {
       // restore / record the constant-feature prefix (the memcpy pair at the end of node_split_best)
       for (int i = tid; i < n_known; i += FF_THREADS) features[i] = constant_features[i];
       for (int i = n_known + tid; i < n_total_constants; i += FF_THREADS) constant_features[i] = features[i];
-      is_leaf = best_nl <= 0 || (s_dbl[2] + FF_EPSILON < P.min_impurity_decrease);
+      is_leaf = best_nl <= 0 || (s_dbl[2] + FOREST_EPSILON < P.min_impurity_decrease);
       FF_TICK(8);
 
       if (best_nl > 0) {
@@ -931,9 +919,7 @@ forest_fast_kernel(const FfParams P) {
     const int node_id = node_count;
     if (node_id >= P.node_cap) { status = 1; break; }
     if (tid == 0) {
-      // compact node record (32 bytes = one sector): right child | feature + the two bins around the
-      // threshold | n_node_samples | depth | class sums.  Left child = id + 1 (depth-first order); the
-      // host derives threshold, impurity, weighted_n_node_samples, value and missing_go_to_left.
+      // node record FOREST_REC_FAST (forest_common.h; 32 bytes = one sector)
       uint32_t* nodes = P.o_nodes + (size_t)slot * P.node_cap * 8;
       if (rec->parent >= 0 && !(rec->flags & (1 << 16))) nodes[(size_t)rec->parent * 8] = (uint32_t)node_id;
       const uint32_t code = is_leaf ? 0xFFFFu : ((uint32_t)best_feature | ((uint32_t)(best_code & 0xFFFF) << 16));
@@ -1010,7 +996,7 @@ bool forest_fast_supported(const Ctx* c, int n_classes, bool reg, int random_spl
 }
 
 int forest_fast_slots_per_sm() { return 7; }
-size_t forest_fast_record_bytes(int n_classes) { return n_classes <= 2 ? sizeof(FfRec<2>) : sizeof(FfRec<4>); }
+size_t forest_fast_stack_bytes(int n_classes) { return n_classes <= 2 ? sizeof(FfRec<2>) : sizeof(FfRec<4>); }
 
 int forest_fast_launch(Ctx* c, FfParams& P, int nt) {
   int ws = 0;

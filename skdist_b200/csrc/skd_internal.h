@@ -55,23 +55,17 @@ struct ForestData {
   bool well_separated = false;   // every feature's adjacent distinct values are more than 1e-7 apart
   bool all_coded = false;        // every feature has <= 256 distinct values (bin codes): the best splitter can run
   int uncoded_feature = -1, uncoded_distinct = 0;   // the first feature without codes and its distinct values
-  std::vector<float> h_binval;   // host copy of binval (thresholds of compact node records are formed on the host)
+  std::vector<float> h_binval;   // host copy of binval (thresholds of FOREST_REC_FAST records are formed on the host)
   bool valid = false;
 };
 
-// host view of one finished tree (arrays of node_count entries; value is [node_count][n_classes]).
-// compact != nullptr: the tree comes as compact 32-byte node records (forest_fast.cu) and the arrays
-// are null; `binval` ([d][256] distinct feature values) lets the consumer form the thresholds.
+// host view of one finished tree: node_count node records of `kind` (ForestRecordKind, forest_common.h);
+// `binval` ([d][256] distinct feature values) lets the consumer form the thresholds of FOREST_REC_FAST
 struct SkdTreeView {
-  const uint32_t* compact = nullptr;
-  const float* binval = nullptr;
+  const uint32_t* records;
+  int kind;
   int32_t node_count, max_depth, n_classes;
-  const int32_t *left, *right, *feature, *n_node_samples;
-  const uint8_t* missing_go_to_left;
-  const double *threshold, *impurity, *weighted_n_node_samples, *value;
-  // criterion entropy: [node_count][n_classes] integer class sums of every node, else nullptr; the
-  // consumer forms the impurity from them (`impurity` then holds the builder's ranking values)
-  const unsigned long long* class_sums = nullptr;
+  const float* binval;
 };
 typedef void (*ForestSink)(void* arg, int tree_index, const SkdTreeView* view);
 

@@ -472,8 +472,8 @@ class Engine:
             return a
 
         try:
-            # the copies (and, for the compact records of the throughput builder, the float64 fields formed
-            # from the integer class sums) run in the library without the GIL: one host thread per tree
+            # the copies (and the float64 fields formed from the node records' statistics) run in the
+            # library without the GIL: one host thread per tree
             import os
             from concurrent.futures import ThreadPoolExecutor
             nthr = max(1, min(32, T, (os.cpu_count() or 8) // 2))
