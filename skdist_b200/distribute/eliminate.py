@@ -13,11 +13,11 @@ columns (csrc/lbfgs_dev.cu gather_fg).  No column-dropped copies of X are made; 
 zero-padded coefficient rows on the full X.
 
 Base estimator with a device path: ``LogisticRegression(solver="lbfgs")`` (binary or multiclass target).  The
-(feature set, fold) fits are scored by the search's LogisticRegression families (logreg_family.py), so every
-classifier scorer the search takes for the target works here too: accuracy, balanced accuracy, precision /
-recall / f1 with any averaging the target allows (the reference's examples/eliminate/covtype.py uses
-"f1_weighted"), roc_auc, roc_auc_ovr / roc_auc_ovo [_weighted], average_precision and neg_log_loss.  Anything
-else raises NotImplementedError (no CPU fallback).
+(feature set, fold) columns are fitted and scored by the search's LogisticRegression families (logreg_family.py),
+so every classifier scorer the search takes for the target works here too: accuracy, balanced accuracy,
+precision / recall / f1 with any averaging the target allows (the reference's examples/eliminate/covtype.py
+uses "f1_weighted"), roc_auc, roc_auc_ovr / roc_auc_ovo [_weighted], average_precision and neg_log_loss.
+Anything else raises NotImplementedError (no CPU fallback).
 """
 import numpy as np
 from sklearn.utils.metaestimators import available_if
@@ -30,8 +30,9 @@ from sklearn.utils.validation import check_is_fitted
 from .. import parallel
 from ..engine import get_engine
 from .base import _clone, _parse_partitions, _ScParamMixin
+from .family import _check_engine_entries
 from .folds import _fold_ids
-from .logreg_family import _check_engine_entries, _check_logreg, _ClassWeights, _LogRegFamily, _MultinomialFamily
+from .logreg_family import _check_logreg, _LogRegFamily, _MultinomialFamily
 from .utils import _check_multimetric_scoring
 
 __all__ = ["DistFeatureEliminator"]
@@ -66,14 +67,14 @@ class DistFeatureEliminator(_ScParamMixin, ClassifierMixin, BaseEstimator):
             raise NotImplementedError(
                 "%s has no device path in DistFeatureEliminator; supported: LogisticRegression(solver='lbfgs')."
                 "  (No CPU fallback by design.)" % type(self.estimator).__name__)
-        p = _check_logreg(_clone(self.estimator), class_weight=True)
+        _check_logreg(_clone(self.estimator), class_weight=True)     # a configuration error comes first
         scorers, _ = _check_multimetric_scoring(self.estimator, scoring=self.scoring)
-        classes = np.unique(y)
-        n_classes = len(classes)
+        n_classes = len(np.unique(y))
         if n_classes < 2:
             raise ValueError("the target has a single class")
         multi = n_classes > 2          # LogisticRegression(lbfgs) is multinomial there (SK/linear_model/_logistic.py:523-547)
-        # the search's family for this target scores the fits (it raises for a scorer without a device path)
+        # the search's family for this target fits and scores the columns (it raises for a configuration or a
+        # scorer without a device path)
         family = (_MultinomialFamily if multi else _LogRegFamily)(self.estimator, [{}], X, y, scorers)
         cv = check_cv(self.cv, y, classifier=is_classifier(self.estimator))
         n_samples, n_features = X.shape
@@ -86,26 +87,19 @@ class DistFeatureEliminator(_ScParamMixin, ClassifierMixin, BaseEstimator):
         rank, world, _ = parallel.dist_info()
         eng = get_engine()
         _check_engine_entries(family, eng)
-        ycls = np.searchsorted(classes, y).astype(np.int32)
         cv_splits = list(cv.split(X, y, groups))
         n_splits = len(cv_splits)
         fold = _fold_ids(cv_splits, n_samples)
         parallel.stage_x_replicated(eng, X)
-        family.stage(eng, X, fold, n_splits, x_staged=True)      # class ids (== ycls) and fold ids
-        kw = dict(fit_intercept=p["fit_intercept"], tol=p["tol"], max_iter=p["max_iter"])
-        one = np.ones(1, np.int32)
-        weights = _ClassWeights(classes, ycls)
-        weights.set_folds(fold, [np.asarray(train) for train, _ in cv_splits])
+        family.stage(eng, X, fold, n_splits, x_staged=True)
+        family.set_train_rows([np.asarray(train) for train, _ in cv_splits])
 
-        def fit(C, folds):
-            weights.stage(eng, [p["class_weight"]] * len(C), folds)
-            if multi:
-                return eng.logreg_multinomial_fit_batch(C, folds, n_classes, **kw)
-            return eng.logreg_fit_batch(C, folds, np.ones(len(C), np.int32), **kw)
+        def fit(folds):
+            return family.fit_columns(eng, family.cands * len(folds), folds)
 
         # initial fit on every feature -> ranking by squared coefficient, summed over the class rows of a
         # multiclass model (ref :141-156)
-        res0 = fit(np.array([p["C"]]), np.array([-1], np.int32))
+        res0 = fit(np.array([-1], np.int32))
         coefs = res0["coef"][0][..., :n_features].astype(np.float64)
         ranks = np.argsort((coefs ** 2).sum(axis=0) if multi else coefs ** 2)
         ranks = np.ravel(ranks)[: (n_features - min_features_to_select)]
@@ -126,8 +120,8 @@ class DistFeatureEliminator(_ScParamMixin, ClassifierMixin, BaseEstimator):
         f_cols = (np.asarray(mine) % n_splits).astype(np.int32)
         if len(mine):
             eng.stage_column_masks(masks)
-            res = fit(np.full(len(mine), p["C"]), f_cols)
-            loc = np.asarray(family.score_columns(eng, res["coef"], f_cols)["score"], dtype=np.float64)
+            res = fit(f_cols)
+            loc = np.asarray(family.score_columns(eng, res["coef"], f_cols)[0]["score"], dtype=np.float64)
         else:
             loc = np.zeros(0)
         scores = np.asarray(parallel.all_gather_columns(loc, n_cols, rank, world), dtype=np.float64)
@@ -147,18 +141,10 @@ class DistFeatureEliminator(_ScParamMixin, ClassifierMixin, BaseEstimator):
         m = np.zeros((1, n_features), np.uint8)
         m[0, np.asarray(self.best_features_, dtype=np.int64)] = 1
         eng.stage_column_masks(m)
-        resb = fit(np.array([p["C"]]), np.array([-1], np.int32))
+        resb = fit(np.array([-1], np.int32))
         keep = np.asarray(self.best_features_, dtype=np.int64)
-        est = _clone(self.estimator)
-        dt = np.float64 if X.dtype == np.float64 else np.float32
-        rows = np.atleast_2d(resb["coef"][0])                 # (1, d+1) binary, (K, d+1) multiclass
-        est.coef_ = rows[:, :n_features][:, keep].astype(dt)
-        est.intercept_ = (rows[:, n_features].astype(dt) if est.fit_intercept
-                          else np.zeros(rows.shape[0], dtype=dt))
-        est.classes_ = classes
-        est.n_iter_ = np.array([int(resb["n_iter"][0])], dtype=np.int32)
-        est.n_features_in_ = len(keep)
-        self.best_estimator_ = est
+        rows = np.atleast_2d(resb["coef"][0])[:, np.append(keep, n_features)]      # kept features, intercept
+        self.best_estimator_ = family.make_estimator({}, rows, resb["n_iter"][0], X.dtype, len(keep))
         self.n_features_ = len(self.best_features_)
         self.__dict__.pop("sc", None)
         return self

@@ -35,6 +35,16 @@ def _train_codes(fold):
     return (-3 - fold).astype(np.int32)
 
 
+def _train_rows(fold, train_rows, f):
+    """Training rows of fold f of a layout (-1: all rows) in the order a fit takes them: train_rows[f], the
+    splitter's order, when given, else the rows outside fold f in ascending order."""
+    if f < 0:
+        return np.arange(len(fold))
+    if train_rows is not None and train_rows[f] is not None:
+        return np.asarray(train_rows[f])
+    return np.flatnonzero(fold != f)
+
+
 class _TargetCodes:
     """One hash pass over a 1-d integer / bool target: `codes` numbers the classes by order of first
     appearance (what StratifiedKFold's `_make_test_folds` works on), `classes` are the sorted labels and

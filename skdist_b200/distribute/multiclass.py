@@ -31,6 +31,7 @@ from sklearn.utils.validation import check_is_fitted
 from .. import parallel
 from ..engine import get_engine
 from .base import _clone, _Cloner, _parse_partitions, _ScParamMixin
+from .sgd_family import SGD_DIVERGED
 from .validation import _check_estimator
 
 __all__ = ["DistOneVsRestClassifier", "DistOneVsOneClassifier"]
@@ -71,9 +72,6 @@ def _binary_estimator(template, coef_row, n_features, X_dtype, **extra):
     for k, v in extra.items():
         setattr(est, k, v)
     return est
-
-
-SGD_DIVERGED = 5        # sgd_fit_batch status: a column's weights or intercept became non-finite
 
 
 def _check_sgd_status(template, status, n_iter):

@@ -4,25 +4,14 @@ Replaces, for `DistGridSearchCV/DistRandomizedSearchCV(Ridge(), ...)`, the per-t
 `Ridge.fit` + r2 scoring that the reference fans out (ref search.py:180-288): one pass over X
 gives every fold's Gram block; each (alpha, fold) is then a 256x256 Cholesky solve
 (csrc/ridge.cu) and one r2 epilogue pass scores all columns (csrc/logreg_tc.cu TC_R2)."""
-import time
-from collections import defaultdict
-
 import numpy as np
 
 from .. import parallel
-from .base import _clone, _merged_params
-from .folds import _train_codes
+from .base import _merged_params
+from .family import _Family, _resolve
 
-_RIDGE_SEARCHABLE = {"alpha", "fit_intercept"}
 # each column's packed Cholesky factor lives in one CTA's shared memory (csrc/ridge.cu RIDGE_MAX_D)
 _RIDGE_MAX_FEATURES = 338
-
-
-def _resolve(estimator, params):
-    est = _clone(estimator)
-    if params:
-        est.set_params(**params)
-    return est
 
 
 def _check_ridge(est):
@@ -39,17 +28,13 @@ def _check_ridge(est):
     return p
 
 
-class _RidgeFamily:
+class _RidgeFamily(_Family):
     name = "ridge"
+    searchable = frozenset({"alpha", "fit_intercept"})
 
     def __init__(self, estimator, candidate_params, X, y, scorers):
         self.estimator = estimator
-        for p in candidate_params:
-            extra = set(p) - _RIDGE_SEARCHABLE
-            if extra:
-                raise NotImplementedError(
-                    "searching Ridge over %s has no device path (searchable: %s)"
-                    % (sorted(extra), sorted(_RIDGE_SEARCHABLE)))
+        self._check_searchable(candidate_params)
         self.cands = [_check_ridge(q) for q in _merged_params(estimator, candidate_params)]
         if np.ndim(y) != 1:
             raise NotImplementedError("multi-target Ridge has no device path")
@@ -91,7 +76,7 @@ class _RidgeFamily:
             parallel.stage_x_replicated(eng, X)
         eng.stage_targets(self.y)
         eng.stage_folds(fold, n_splits)
-        if getattr(self, "fold", None) is not fold:
+        if self.fold is not fold:
             self.prepare(fold, n_splits)
 
     def prepare(self, fold, n_splits):
@@ -107,43 +92,21 @@ class _RidgeFamily:
             t = y64[fold != k]
             self.sst_train[k] = np.sum((t - t.mean()) ** 2)
 
-    def run_columns(self, eng, cols, n_splits, return_train_score):
-        cols = np.asarray(cols, dtype=np.int64)
-        out = {
-            "n_test": np.zeros(len(cols), dtype=np.int64),
-            "fit_time": np.zeros(len(cols)), "score_time": np.zeros(len(cols)),
-            "n_iter": np.zeros(len(cols), dtype=np.int32), "status": np.zeros(len(cols), dtype=np.int32),
-        }
-        for name in self.metrics:
-            out["test_%s" % name] = np.zeros(len(cols))
-            if return_train_score:
-                out["train_%s" % name] = np.zeros(len(cols))
-        cand = cols // n_splits
-        fold = (cols % n_splits).astype(np.int32)
-        groups = defaultdict(list)
-        for i, c in enumerate(cand):
-            groups[bool(self.cands[c]["fit_intercept"])].append(i)
-        for fi, idx in groups.items():
-            idx = np.asarray(idx)
-            alpha = np.array([self.cands[c]["alpha"] for c in cand[idx]], dtype=np.float64)
-            t0 = time.time()
-            res = eng.ridge_fit_batch(alpha, fold[idx], fit_intercept=fi)
-            t1 = time.time()
-            sse, count = eng.linear_r2_batch(res["coef"], fold[idx])
-            t2 = time.time()
-            for name, kind in self.metrics.items():
-                score = self._metric(kind, sse, count, self.sst_test[fold[idx]])
-                score[res["status"] != 1] = np.nan
-                out["test_%s" % name][idx] = score
-            out["n_test"][idx] = count
-            out["fit_time"][idx] = (t1 - t0) / len(idx)
-            out["score_time"][idx] = (t2 - t1) / len(idx)
-            out["status"][idx] = res["status"]
-            if return_train_score:
-                sse2, n2 = eng.linear_r2_batch(res["coef"], _train_codes(fold[idx]))
-                for name, kind in self.metrics.items():
-                    out["train_%s" % name][idx] = self._metric(kind, sse2, n2, self.sst_train[fold[idx]])
-        return out
+    @staticmethod
+    def _launch_key(p):
+        return bool(p["fit_intercept"])
+
+    def _launch(self, eng, cands, folds):
+        alpha = np.array([p["alpha"] for p in cands], dtype=np.float64)
+        res = eng.ridge_fit_batch(alpha, folds, fit_intercept=self._launch_key(cands[0]))
+        return res["coef"], 0, res["status"], res["status"] != 1, np.zeros(len(cands), dtype=bool)
+
+    def score_columns(self, eng, coef, codes):
+        """({scorer name: per-column value}, rows per column) on the rows the scoring codes select; r2 takes the
+        total sum of squares of those rows."""
+        sse, count = eng.linear_r2_batch(coef, codes)
+        sst = np.where(codes >= 0, self.sst_test[np.maximum(codes, 0)], self.sst_train[np.maximum(-3 - codes, 0)])
+        return {name: self._metric(kind, sse, count, sst) for name, kind in self.metrics.items()}, count
 
     def refit(self, eng, params, X_dtype, n_features):
         p = _check_ridge(_resolve(self.estimator, params))

@@ -46,11 +46,12 @@ __all__ = ["DistGridSearchCV", "DistRandomizedSearchCV", "DistMultiModelSearch"]
 
 
 from .folds import _cv_fold_groups, _cv_fold_ids, _encode_target
-from .logreg_family import _check_engine_entries, _fit_sample_weight, _LogRegFamily, _MultinomialFamily
+from .family import _check_engine_entries
+from .logreg_family import _fit_sample_weight, _LogRegFamily, _MultinomialFamily
 
 
 # ----------------------------------------------------------------------------------------
-# estimator families with a device path (logreg_family.py, ridge_family.py)
+# estimator families with a device path (family.py; logreg_family.py, sgd_family.py, ridge_family.py)
 # ----------------------------------------------------------------------------------------
 def _pick_family(estimator, candidate_params, X, y, scorers, enc=None):
     if type(estimator) is LogisticRegression:
@@ -131,8 +132,7 @@ class DistBaseSearchCV(_ScParamMixin):
                     family.set_sample_weight(sample_weight)
                 if self.refit and self.preds and not hasattr(family, "fold_proba"):
                     raise NotImplementedError("preds=True has no device path for %s" % type(estimator).__name__)
-                if hasattr(family, "prepare"):      # host-only statistics of the folds (no engine calls)
-                    family.prepare(fold, layouts[0][1])
+                family.prepare(fold, layouts[0][1])     # host-only statistics of the folds (no engine calls)
             finally:
                 staged.result()
 
@@ -147,18 +147,16 @@ class DistBaseSearchCV(_ScParamMixin):
         n_cols = n_candidates * n_splits
         full = np.zeros((n_cols, len(keys)))
         for li, (fold_l, nf_l, idx_l) in enumerate(layouts):
-            if li > 0 and hasattr(family, "prepare"):
+            if li > 0:
                 family.prepare(fold_l, nf_l)
             family.stage(eng, X_arr, fold_l, nf_l, x_staged=True)
-            if hasattr(family, "set_train_rows"):    # training rows of every local fold, in the splitter's order
-                family.set_train_rows([train_orders[s] if train_orders else None for s in idx_l])
+            # training rows of every local fold, in the splitter's order
+            family.set_train_rows([train_orders[s] if train_orders else None for s in idx_l])
             k_l = len(idx_l)
             # local columns cand * nf_l + f, f < k_l (the extra fold id of a layout is never held out).
             # Ranks are dealt blocks of 128 consecutive candidates of ONE fold (fold-major order).
             cols_l = (np.arange(n_candidates)[None, :] * nf_l + np.arange(k_l)[:, None]).ravel()
-            col_cost = None
-            if world > 1 and hasattr(family, "column_cost"):
-                col_cost = family.column_cost(nf_l)[cols_l]
+            col_cost = family.column_cost(nf_l)[cols_l] if world > 1 else None
             pick = parallel.shard_blocks(len(cols_l), rank, world, cost=col_cost)
             loc = family.run_columns(eng, cols_l[pick], nf_l, bool(self.return_train_score))
             # one collective per layout for all per-column results (counts are exact in float64)

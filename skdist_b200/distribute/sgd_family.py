@@ -17,25 +17,20 @@ binary target the ranking scorers run on the rank kernel: average_precision on t
 roc_auc_ovr / roc_auc_ovo [_weighted] (the AUC of predict_proba[:, 1], ranked as the decision values rank) when
 every candidate has loss="log_loss"."""
 import copy
-import time
 import warnings
-from collections import defaultdict
 
 import numpy as np
 
-from .. import parallel
 from ..engine import sgd_config, sgd_seed
-from .base import _clone, _merged_params
-from .folds import _classes_and_ids, _train_codes
-from .logreg_family import (_count_metric, _is_rank, _label_one, _metric_from_confusion, _metric_from_counts,
-                            _rank_entries, _RankScores)
+from .base import _merged_params
+from .family import _count_metric, _Family, _is_rank, _resolve
+from .folds import _classes_and_ids
 
 _MAX_INT = np.iinfo(np.int32).max
 # parameters that group the launches (one value per launch); alpha varies per column
 _SGD_LAUNCH = ("loss", "learning_rate", "eta0", "power_t", "max_iter", "tol", "fit_intercept", "n_iter_no_change",
                "shuffle", "random_state")
-_SGD_SEARCHABLE = {"alpha"} | set(_SGD_LAUNCH)
-SGD_DIVERGED = 5        # skd_sgd_fit_groups status: the column's weights or intercept became non-finite
+SGD_DIVERGED = 5        # sgd_fit_groups / sgd_fit_batch status: a column's weights or intercept became non-finite
 
 
 def _launch_key(p):
@@ -66,19 +61,21 @@ def sgd_class_seeds(random_state, n_classes):
     return [sgd_seed(int(s)) for s in draws]
 
 
-class _SGDFamily:
+def _warn_max_iter():
+    from sklearn.exceptions import ConvergenceWarning
+    warnings.warn("Maximum number of iteration reached before convergence. Consider increasing max_iter to improve "
+                  "the fit.", ConvergenceWarning)
+
+
+class _SGDFamily(_Family):
     """(candidate x fold) columns of SGDClassifier (hinge or log_loss, penalty l2)."""
 
     name = "sgd"
+    searchable = frozenset({"alpha"} | set(_SGD_LAUNCH))
 
     def __init__(self, estimator, candidate_params, X, y, scorers, enc=None):
         self.estimator = estimator
-        for p in candidate_params:
-            extra = set(p) - _SGD_SEARCHABLE
-            if extra:
-                raise NotImplementedError(
-                    "searching SGDClassifier over %s has no device path (searchable: %s)"
-                    % (sorted(extra), sorted(_SGD_SEARCHABLE)))
+        self._check_searchable(candidate_params)
         self.cands = _merged_params(estimator, candidate_params)
         for q in self.cands:
             sgd_config(q)
@@ -90,7 +87,7 @@ class _SGDFamily:
             raise ValueError("The number of classes has to be greater than one; got %d class" % K)
         self.n_classes = K
         self.binary = K == 2
-        self.metrics = {}
+        metrics = {}
         for name, scorer in scorers.items():
             m = _count_metric(scorer)
             ok = m is not None
@@ -109,45 +106,11 @@ class _SGDFamily:
                     "roc_auc and average_precision (binary target), neg_log_loss, roc_auc_ovr, "
                     "roc_auc_ovr_weighted, roc_auc_ovo and roc_auc_ovo_weighted (binary target, "
                     "loss='log_loss'))" % (scorer,))
-            if self.binary:
-                self.metrics[name] = m if _is_rank(m) or m[1] not in (None, "binary") else m[0]
-            else:
-                self.metrics[name] = m
-        self.needs_pred_pos = self.binary and any(
-            k not in ("accuracy", "roc_auc", "neg_log_loss") and not _is_rank(k) for k in self.metrics.values())
-        self.label_one = _label_one(self.classes_)
-        self.engine_entries = _rank_entries(self.metrics)
-        self.fold, self.train_rows = None, None
-
-    # -- layout -------------------------------------------------------------------------------------------
-    def stage(self, eng, X, fold, n_splits, x_staged=False):
-        if not x_staged:
-            parallel.stage_x_replicated(eng, X)
-        eng.stage_labels(self.y_class)
-        eng.stage_folds(fold, n_splits)
-        self.fold, self.train_rows = np.asarray(fold), None
-        if self.needs_pred_pos:
-            self.pos_in_fold = np.bincount(self.fold[self.y_class == 1], minlength=n_splits).astype(np.int64)
+            metrics[name] = m
+        if self.binary:
+            self._set_binary_metrics(metrics)
         else:
-            self.pos_in_fold = np.zeros(n_splits, dtype=np.int64)
-        self.total_pos = int(self.pos_in_fold.sum())
-
-    def set_train_rows(self, train_rows):
-        """Training rows of every fold of the staged layout in the splitter's order (None entries: the rows
-        outside the fold, ascending, as KFold / StratifiedKFold give them).  SGD walks them in this order."""
-        self.train_rows = train_rows
-
-    def _train(self, f):
-        if f < 0:
-            return np.arange(len(self.y_class))
-        if self.train_rows is not None and self.train_rows[f] is not None:
-            return np.asarray(self.train_rows[f])
-        return np.flatnonzero(self.fold != f)
-
-    def column_cost(self, n_splits):
-        """Expected relative duration of every (candidate, fold) column, for the multi-GPU block deal: one
-        warp walks the fold's rows once per epoch whatever alpha is, so every column costs the same."""
-        return np.ones(len(self.cands) * n_splits)
+            self.metrics = metrics
 
     # -- fits ---------------------------------------------------------------------------------------------
     def _fit(self, eng, p, alphas, folds):
@@ -174,104 +137,42 @@ class _SGDFamily:
         res = eng.sgd_fit_groups(p, col_pos, col_group, col_alpha, rows, np.array(seeds, dtype=np.uint32))
         return res, Kc
 
-    def _coef(self, res, Kc):
-        """float32 [B, d + 1] (binary) or [B, K, d + 1] coefficients, intercept last, for the scoring kernels."""
-        coef = np.concatenate([res["coef32"], res["intercept"].astype(np.float32)[:, None]], axis=1)
-        return coef if Kc == 1 else coef.reshape(-1, Kc, coef.shape[1])
+    _launch_key = staticmethod(_launch_key)
 
-    def _scores(self, eng, coef, codes, actual_pos):
+    def _launch(self, eng, cands, folds):
+        """One launch through `_fit`: float32 [B, d + 1] (binary) or [B, K, d + 1] coefficients, intercept last,
+        for the scoring kernels; a fit's epochs are the most of its class columns, and its status is
+        SGD_DIVERGED when a class column diverged (scikit-learn's _plain_sgd raises there), else the least of
+        theirs."""
+        res, Kc = self._fit(eng, cands[0], [p["alpha"] for p in cands], folds)
+        coef = np.concatenate([res["coef32"], res["intercept"].astype(np.float32)[:, None]], axis=1)
+        coef = coef if Kc == 1 else coef.reshape(-1, Kc, coef.shape[1])
+        status = res["status"].reshape(len(cands), Kc)
+        n_iter = res["n_iter"].reshape(len(cands), Kc).max(axis=1)
+        bad = np.any(status == SGD_DIVERGED, axis=1)
+        return coef, n_iter, np.where(bad, SGD_DIVERGED, status.min(axis=1)), bad, bad
+
+    def score_columns(self, eng, coef, codes):
         if not self.binary:
-            conf = eng.multinomial_confusion_batch(coef, codes)
-            return {name: _metric_from_confusion(kind, average, conf)
-                    for name, (kind, average) in self.metrics.items()}, conf.sum(axis=(1, 2))
-        pos = np.ones(len(codes), dtype=np.int32)
-        correct, count = eng.linear_score_batch(coef, codes, pos)
-        pred_pos = None
-        if self.needs_pred_pos:
-            neg_correct, _ = eng.linear_score_batch(coef, codes, np.full(len(pos), -7, dtype=np.int32))
-            pred_pos = count - neg_correct
-        out = {}
+            return self._multiclass_scores(eng, coef, codes)
         # binary SGDClassifier's predict_proba is expit of a float64 decision (float64 intercept_): strictly
         # increasing in z until float64 saturates (|z| > 36), so it ranks the rows as the decision values do
-        rank = _RankScores(eng, coef, codes, self.label_one, binary_proba="decision")
-        for name, kind in self.metrics.items():
-            if kind == "roc_auc":
-                out[name], _ = eng.linear_auc_batch(coef, codes, pos)
-            elif kind == "neg_log_loss":
-                out[name] = -eng.linear_logloss_batch(coef, codes, pos)[0]
-            elif _is_rank(kind):
-                out[name] = rank.value(*kind)
-            elif isinstance(kind, tuple):
-                tp = (pred_pos + actual_pos + correct - count) / 2.0
-                fp, fn = pred_pos - tp, actual_pos - tp
-                conf = np.stack([np.stack([count - tp - fp - fn, fp], -1), np.stack([fn, tp], -1)], -2)
-                out[name] = _metric_from_confusion(kind[0], kind[1], conf)
-            else:
-                out[name] = _metric_from_counts(kind, correct, count, pred_pos, actual_pos)
-        return out, count
+        return self._binary_scores(eng, coef, codes, binary_proba="decision")
 
     def run_columns(self, eng, cols, n_splits, return_train_score):
-        """Fit + score the given global column ids (col = cand * n_splits + fold).
-        Returns dict of per-column arrays aligned with `cols`."""
-        cols = np.asarray(cols, dtype=np.int64)
-        out = {
-            "n_test": np.zeros(len(cols), dtype=np.int64),
-            "fit_time": np.zeros(len(cols)), "score_time": np.zeros(len(cols)),
-            "n_iter": np.zeros(len(cols), dtype=np.int32), "status": np.zeros(len(cols), dtype=np.int32),
-        }
-        for name in self.metrics:
-            out["test_%s" % name] = np.zeros(len(cols))
-            if return_train_score:
-                out["train_%s" % name] = np.zeros(len(cols))
-        cand = cols // n_splits
-        fold = (cols % n_splits).astype(np.int32)
-        launches = defaultdict(list)
-        for i, c in enumerate(cand):
-            launches[_launch_key(self.cands[c])].append(i)
-        max_iter_hit = False
-        for idx in launches.values():
-            idx = np.asarray(idx)
-            p = self.cands[cand[idx[0]]]
-            t0 = time.time()
-            res, Kc = self._fit(eng, p, [self.cands[c]["alpha"] for c in cand[idx]], fold[idx])
-            t1 = time.time()
-            coef = self._coef(res, Kc)
-            vals, count = self._scores(eng, coef, fold[idx], self.pos_in_fold[fold[idx]])
-            t2 = time.time()
-            status = res["status"].reshape(len(idx), Kc)
-            n_iter = res["n_iter"].reshape(len(idx), Kc).max(axis=1)
-            # a diverged fit raises in scikit-learn's _plain_sgd; NaN scores let search.py apply error_score
-            bad = np.any(status == SGD_DIVERGED, axis=1)
-            if p["tol"] is not None and np.any(n_iter[~bad] == int(p["max_iter"])):
-                max_iter_hit = True
-            for name, v in vals.items():
-                v = np.asarray(v, dtype=np.float64).copy()
-                v[bad] = np.nan
-                out["test_%s" % name][idx] = v
-            out["n_test"][idx] = count
-            out["fit_time"][idx] = (t1 - t0) / len(idx)
-            out["score_time"][idx] = (t2 - t1) / len(idx)
-            out["n_iter"][idx] = n_iter
-            out["status"][idx] = np.where(bad, SGD_DIVERGED, status.min(axis=1))
-            if return_train_score:
-                vals, _ = self._scores(eng, coef, _train_codes(fold[idx]),
-                                       self.total_pos - self.pos_in_fold[fold[idx]])
-                for name, v in vals.items():
-                    v = np.asarray(v, dtype=np.float64).copy()
-                    v[bad] = np.nan
-                    out["train_%s" % name][idx] = v
-        if max_iter_hit:
-            from sklearn.exceptions import ConvergenceWarning
-            warnings.warn("Maximum number of iteration reached before convergence. Consider increasing max_iter to "
-                          "improve the fit.", ConvergenceWarning)
+        """The base loop, and scikit-learn's ConvergenceWarning once when a fit that did not diverge ran
+        max_iter epochs with tol set."""
+        out = super().run_columns(eng, cols, n_splits, return_train_score)
+        cand = np.asarray(cols, dtype=np.int64) // n_splits
+        live = out["status"] != SGD_DIVERGED
+        if any(self.cands[c]["tol"] is not None and n == int(self.cands[c]["max_iter"])
+               for c, n in zip(cand[live], out["n_iter"][live])):
+            _warn_max_iter()
         return out
 
     # -- refit --------------------------------------------------------------------------------------------
     def refit(self, eng, params, X_dtype, n_features):
-        est = _clone(self.estimator)
-        if params:
-            est.set_params(**params)
-        p = est.get_params(deep=False)
+        p = _resolve(self.estimator, params).get_params(deep=False)
         res, Kc = self._fit(eng, p, [p["alpha"]], [-1])
         status = res["status"]
         if np.any(status == SGD_DIVERGED):
@@ -280,9 +181,7 @@ class _SGDFamily:
                              % int(res["n_iter"][np.flatnonzero(status == SGD_DIVERGED)[0]]))
         n_iter = int(res["n_iter"].max())
         if p["tol"] is not None and n_iter == int(p["max_iter"]):
-            from sklearn.exceptions import ConvergenceWarning
-            warnings.warn("Maximum number of iteration reached before convergence. Consider increasing max_iter to "
-                          "improve the fit.", ConvergenceWarning)
+            _warn_max_iter()
         return self.make_estimator(params, res["coef32"], res["intercept"], n_iter, X_dtype, n_features)
 
     def make_estimator(self, params, coef32, intercept, n_iter, X_dtype, n_features):
@@ -290,9 +189,7 @@ class _SGDFamily:
         set (SK/linear_model/_stochastic_gradient.py:760-850): coef_ (1 or K, d) in X's dtype, intercept_
         float64 (binary) or in X's dtype (K > 2), n_iter_ = the largest of the binary fits' epochs and
         t_ = 1 + n_iter_ * n."""
-        est = _clone(self.estimator)
-        if params:
-            est.set_params(**params)
+        est = _resolve(self.estimator, params)
         dt = np.float64 if X_dtype == np.float64 else np.float32
         est.coef_ = np.asarray(coef32)[:, :n_features].astype(dt)
         est.intercept_ = np.asarray(intercept, dtype=np.float64).astype(np.float64 if self.binary else dt)

@@ -56,7 +56,7 @@ def case(X, y, Cs, n_splits):
         one = _MultinomialFamily(LogisticRegression(), [{}], X, y, {s: get_scorer(s)})
         one.score_columns(eng, res["coef"], f)                 # warm-up (scratch pool, cub temp sizes)
         t0 = time.perf_counter()
-        v = one.score_columns(eng, res["coef"], f)[s]
+        v = one.score_columns(eng, res["coef"], f)[0][s]
         out["score_seconds"][s] = time.perf_counter() - t0
         out.setdefault("mean_score", {})[s] = float(np.nanmean(v))
     cpu = {}
